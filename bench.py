@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — throughput of the B200-native ORB front-end on the BASELINE.json configurations; see DESIGN.md §Measurement.
+"""bench.py — throughput of the CUDA ORB front-end (H100, sm_90a) on the BASELINE.json configurations; see DESIGN.md §Measurement.
 
   python bench.py [--config 1|2|4] [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
   N>1:  python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 ... bench.py --gpus N ...
@@ -10,7 +10,7 @@
   --config 4            configs[4]: EuRoC-shaped 752x480 @1200 query frames against a 2000-keyframe resident database:
                         ComputeBoW + KeyFrameDatabase scoring + SearchByBoW against every keyframe
 One "step" = `passes_per_step` passes of the hot path over one batch of synthetic input per GPU; passes_per_step is calibrated
-after warm-up so that the K timed steps take >= 1 s whatever --steps is.
+after warm-up so that one step takes >= 55 ms, so the timed region grows with --steps (the default 20 steps take >= 1.1 s).
   value     frames/s, whole job, inputs already resident in HBM (device buffers in, counts out)
   e2e       same metric through the C-ABI call with HOST (pinned) buffers: H2D of the inputs and D2H of the results
             inside the timed region
@@ -18,7 +18,11 @@ after warm-up so that the K timed steps take >= 1 s whatever --steps is.
   cpu_baseline  the reference's own sources compiled verbatim (oracle/_ref) timed on this box's host cores on a bounded
             sample of the same workload (rank 0, N=1 only); value = all cores, one_core_value = a single core
 --impl reference: that CPU implementation alone, all host threads, same metric/config (no GPU work).
-The B200 arm asserts equality with the oracle on a sample of its own outputs before timing (outside the timed region).
+The GPU arm asserts equality with the oracle on a sample of its own outputs before timing (outside the timed region).
+--dump-outputs DIR: after the timed steps, the arrays the timed call returned in its last pass (config 1: keypoints, descriptors,
+            counts, mvuRight, mvDepth read back from HBM; config 2: SearchByProjection matches; config 4: scores and SearchByBoW
+            pairs) go to DIR/<name>.npy as float32 / float64.  Inputs depend on the arguments only, and the calibrated pass count
+            is rounded so that the last pass always sees the same input, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -72,7 +76,7 @@ def hbm_peak():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (NVIDIA H100 SXM data sheet, HBM3; not measured)"
 
 
 # ----------------------------------------------------------------------------------------------
@@ -114,6 +118,33 @@ def make_mappoints(keys, desc, scale_factors, rng, u_right=None):
         ur = np.asarray(u_right, np.float32)[sel]
         pxr = np.where(ur >= 0, ur + (px - keys["x"][sel]), pxr).astype(np.float32)
     return dict(px=px, py=py, pxr=pxr, lvl=keys["octave"][sel].astype(np.int32), vc=np.full(n, 0.9, np.float32), desc=np.ascontiguousarray(desc[sel]))
+
+
+DUMP_LIMIT = 64 << 20
+
+
+def dump_outputs(out_dir: str, arrays: dict) -> None:
+    """Writes each array as out_dir/<name>.npy: float arrays keep float32 / float64, integers become float32 when every value is
+    exact in it (|v| < 2^24) and float64 otherwise."""
+    os.makedirs(out_dir, exist_ok=True)
+    conv = {}
+    for name, a in arrays.items():
+        a = np.ascontiguousarray(a)
+        if a.dtype.kind == "f":
+            a = a.astype(np.float64 if a.dtype == np.float64 else np.float32)
+        else:
+            a = a.astype(np.float32 if a.size == 0 or np.abs(a.astype(np.int64)).max() < (1 << 24) else np.float64)
+        conv[name] = a
+    total = sum(a.nbytes for a in conv.values())
+    assert total <= DUMP_LIMIT, f"--dump-outputs: {total} bytes exceed the {DUMP_LIMIT}-byte limit"
+    for name, a in conv.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+    log(f"dumped {len(conv)} arrays ({total / 1e6:.1f} MB) to {out_dir}")
+
+
+def keypoint_columns(kps: np.ndarray) -> np.ndarray:
+    """borb_keypoint rows -> (n, 6) float32: x, y, size, angle, response, octave."""
+    return np.stack([kps[f].astype(np.float32) for f in ("x", "y", "size", "angle", "response", "octave")], axis=1).reshape(-1, 6)
 
 
 # ----------------------------------------------------------------------------------------------
@@ -328,7 +359,7 @@ class Clocks:
 
 
 class Env:
-    """torch / torch.distributed plumbing shared by the three B200 arms."""
+    """torch / torch.distributed plumbing shared by the three GPU arms."""
 
     def __init__(self, rank, world, local_rank):
         import torch
@@ -336,7 +367,7 @@ class Env:
         self.torch, self.dist = torch, dist
         self.rank, self.world, self.local_rank = rank, world, local_rank
         if not torch.cuda.is_available():
-            raise SystemExit("bench.py: no CUDA device visible - the B200 arm has no CPU fallback")
+            raise SystemExit("bench.py: no CUDA device visible - the GPU arm has no CPU fallback")
         torch.cuda.set_device(local_rank)
         self.dev = torch.device("cuda", local_rank)
         if world > 1:
@@ -356,10 +387,12 @@ class Env:
             self.dist.all_reduce(t, op=self.dist.ReduceOp.MAX)
         return float(t.item())
 
-    def passes_per_step(self, t_pass_s: float, K: int) -> int:
-        """Inner repeat so that K steps take >= ~1.1 s (same value on every rank)."""
+    def passes_per_step(self, t_pass_s: float, multiple: int) -> int:
+        """Inner repeat so that one step takes >= ~55 ms (same value on every rank), rounded up to a multiple of `multiple`
+        (the input buffers x handles cycle) so that the last pass of every step sees the same input and handle."""
         t = self.max_over_ranks(t_pass_s)
-        return int(min(100000, max(1, math.ceil(1.1 / (K * max(t, 1e-7))))))
+        n = int(min(100000, max(1, math.ceil(0.055 / max(t, 1e-7)))))
+        return -(-n // multiple) * multiple
 
     def finish(self):
         if self.world > 1:
@@ -473,12 +506,30 @@ def run_config1(args, env: Env):
     for k in range(NH * 4):
         step_resident(k)
     drain(); torch.cuda.synchronize()
-    inner = env.passes_per_step((time.perf_counter() - t0) / (NH * 4), K)
+    inner = env.passes_per_step((time.perf_counter() - t0) / (NH * 4), math.lcm(NBUF, NH))
 
     # ---- timed region 1: HBM-resident throughput
     launches0 = sum(x.launch_count() for x in exts)
     ms, _ = timed(env, step_resident, drain, K, inner)
     launches = sum(x.launch_count() for x in exts) - launches0
+    if args.dump_outputs and rank == 0:
+        # the last pass ran on handle NH-1 over buffer NBUF-1 (inner is a multiple of both); its results are still in HBM
+        from orb_slam2_b200._lib import KP_DTYPE
+        n = min(B, 64)                                        # 64 pairs x ~0.7 MB stay under the dump limit
+        kl, kr = np.zeros((n, cap), KP_DTYPE), np.zeros((n, cap), KP_DTYPE)
+        dl, dr = np.zeros((n, cap, 32), np.uint8), np.zeros((n, cap, 32), np.uint8)
+        nl, nr = np.zeros(n, np.int32), np.zeros(n, np.int32)
+        ur, dp = np.zeros((n, cap), np.float32), np.zeros((n, cap), np.float32)
+        _lib.check(lib.borb_stereo_frames_results(exts[(K * inner - 1) % NH]._h, n, kl.ctypes.data, dl.ctypes.data, nl.ctypes.data,
+                                                  kr.ctypes.data, dr.ctypes.data, nr.ctypes.data, ur.ctypes.data, dp.ctypes.data, cap),
+                   "stereo_frames_results")
+        dump_outputs(args.dump_outputs, {
+            "n_left": nl, "n_right": nr,
+            "keypoints_left": np.concatenate([keypoint_columns(kl[p, :nl[p]]) for p in range(n)]),
+            "keypoints_right": np.concatenate([keypoint_columns(kr[p, :nr[p]]) for p in range(n)]),
+            "descriptors_left": np.concatenate([dl[p, :nl[p]] for p in range(n)]),
+            "descriptors_right": np.concatenate([dr[p, :nr[p]] for p in range(n)]),
+            "u_right": np.concatenate([ur[p, :nl[p]] for p in range(n)]), "depth": np.concatenate([dp[p, :nl[p]] for p in range(n)])})
     # per-kernel device times: a short single-handle pass right after the timed region (with several batches in flight the
     # events of one stream would also count the other streams' kernels), CUDA events on the launching stream
     exts[0].set_timing(True)
@@ -535,13 +586,6 @@ def run_config1(args, env: Env):
     fast_bytes = LEVEL_PIXELS * 2 * B
     fast_ms = stage_ms["fast_nms"]
     achieved = fast_bytes / (fast_ms * 1e-3) / 1e9 if fast_ms > 0 else 0.0
-    traffic, traffic_src = None, None
-    tp = os.path.join(ROOT, "profiles", "fast_traffic.json")
-    if os.path.exists(tp):
-        tj = json.load(open(tp))
-        if tj.get("pairs_per_launch"):
-            traffic = tj["dram_bytes_per_launch"] * B / tj["pairs_per_launch"]
-            traffic_src = tj.get("source", "static ncu capture (profiles/), not measured in this run")
     cpu = None
     if world == 1 and not args.no_cpu_baseline:
         threads = host_cores()
@@ -552,12 +596,12 @@ def run_config1(args, env: Env):
             "ms_per_step": ms_max / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u8", "data": "synthetic",
             "config": {"workload": WORKLOADS[1], "pairs_per_pass_per_gpu": B, "passes_per_step": inner, "batches_in_flight": NH,
                        "parallelism": f"{world} independent camera streams, one per GPU (no data-path collective)",
-                       "cache": f"inputs larger than L2: {NBUF} rotating batches x {2 * B * W_IMG * H_IMG / 1e6:.0f} MB input + {2 * B * 2 * 1.75:.0f} MB pyramids per pass vs 126 MB L2",
+                       "cache": f"inputs larger than L2: {NBUF} rotating batches x {2 * B * W_IMG * H_IMG / 1e6:.0f} MB input + {2 * B * 2 * 1.75:.0f} MB pyramids per pass vs 50 MB L2",
                        "parity_checked": parity},
             "clocks": clk, "gpu_launches": int(launches),
             "e2e": {"value": e2e_value, "unit": "frames/s", "h2d_bytes_per_step": h2d * inner, "d2h_bytes_per_step": d2h * inner},
             "roofline": {"kernel": "fast_kernel", "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src, "algorithmic_bytes_per_launch": fast_bytes,
+                         "traffic": None, "peak_source": peak_src, "algorithmic_bytes_per_launch": fast_bytes,
                          "mean_launch_ms": fast_ms},
             "stage_ms_per_pass": stage_ms, "cpu_baseline": cpu}
     if voc_ms is not None:
@@ -721,11 +765,14 @@ def run_config2(args, env: Env):
     torch.cuda.synchronize(); t0 = time.perf_counter()
     run_passes(pass_resident, NH * 2)
     torch.cuda.synchronize()
-    inner = env.passes_per_step((time.perf_counter() - t0) / (NH * 2), K)
+    inner = env.passes_per_step((time.perf_counter() - t0) / (NH * 2), math.lcm(NBUF, NH))
     launches0 = sum(x.launch_count() for x in exts)
     ml0 = sum(_mlaunch(lib, m) for m in mats)
     ms, _ = timed(env, lambda k: None, lambda: run_passes(pass_resident, K * inner), 0, 0)
     launches = sum(x.launch_count() for x in exts) - launches0 + sum(_mlaunch(lib, m) for m in mats) - ml0
+    if args.dump_outputs and rank == 0:
+        last = hs[(K * inner - 1) % NH]                       # the last pass: handle NH-1, buffer NBUF-1 (inner is a multiple of both)
+        dump_outputs(args.dump_outputs, {"n_keypoints": last.n_out, "n_matches": last.nms, "matches": last.match_all[:, :N_MAPPOINTS]})
     ms_max = env.max_over_ranks(ms)
     value = world * B * K * inner / (ms_max * 1e-3)
     # FAST stage time (single handle, CUDA events on the library's stream)
@@ -791,7 +838,7 @@ def run_config2(args, env: Env):
             "config": {"workload": WORKLOADS[2], "frames_per_pass_per_gpu": B, "passes_per_step": inner, "batches_in_flight": NH,
                        "map_points_per_frame": N_MAPPOINTS, "camera": "TUM1.yaml (k1 = 0.2624: UndistortKeyPoints active), DepthMapFactor 5000, CV_16U depth",
                        "parallelism": f"{world} GPUs x {NH} host threads, each {B} independent RGB-D streams per pass (no data-path collective)",
-                       "cache": f"inputs larger than L2: {NBUF} rotating batches; {NH} handles x {B} x 1.9 MB of pyramids + blurred copies in flight vs 126 MB L2",
+                       "cache": f"inputs larger than L2: {NBUF} rotating batches; {NH} handles x {B} x 1.9 MB of pyramids + blurred copies in flight vs 50 MB L2",
                        "parity_checked": parity},
             "clocks": clk, "gpu_launches": int(launches),
             "e2e": {"value": e2e_value, "unit": "frames/s", "h2d_bytes_per_step": h2d * inner, "d2h_bytes_per_step": d2h * inner},
@@ -990,10 +1037,15 @@ def run_config4(args, env: Env):
     torch.cuda.synchronize(); t0 = time.perf_counter()
     run_passes(pass_resident, 8 * NH)
     torch.cuda.synchronize()
-    inner = env.passes_per_step((time.perf_counter() - t0) / (8 * NH), K)
+    inner = env.passes_per_step((time.perf_counter() - t0) / (8 * NH), math.lcm(Q, NH))
     ml0 = sum(_mlaunch(lib, x.mt) for x in qs)
     ms, _ = timed(env, lambda k: None, lambda: run_passes(pass_resident, K * inner), 0, 0)
     launches = sum(_mlaunch(lib, x.mt) for x in qs) - ml0 + K * inner       # + the vocabulary descent kernel of every ComputeBoW
+    if args.dump_outputs and rank == 0:
+        st = qs[(K * inner - 1) % NH]                         # the last pass: stream NH-1, query (K * inner - 1) % Q
+        dump_outputs(args.dump_outputs, {"bow_word": st.bw[:st.nb.value], "bow_value": st.bv[:st.nb.value], "common_words": st.cw,
+                                         "scores": st.sc, "first_word": st.fw, "n_matches": st.nm, "pair_offset": st.off,
+                                         "pairs": st.pairs[:st.npairs.value]})
     ms_max = env.max_over_ranks(ms)
     value = world * K * inner / (ms_max * 1e-3)
     # device time of the database search kernels (CUDA events on the matcher's stream), one stream alone
@@ -1017,13 +1069,6 @@ def run_config4(args, env: Env):
         return
     peak, peak_src = hbm_peak()
     achieved = db_bytes / (kernel_ms * 1e-3) / 1e9 if kernel_ms > 0 else 0.0
-    traffic, traffic_src = None, None
-    tp = os.path.join(ROOT, "profiles", "bowdb_traffic.json")
-    if os.path.exists(tp):
-        with open(tp) as f:
-            tj = json.load(f)
-        traffic = tj["dram_bytes_per_launch"] * n_kf / tj["keyframes_per_launch"]
-        traffic_src = tj.get("source", "static ncu capture (profiles/), not measured in this run")
     h2d = Q * (2 * W * H) + Q * (int(nq.mean()) * (32 + 2 + 4 + 4 + 12) + 4096)
     d2h = Q * (2 * cap * 60 + 8 * cap + n_kf * 20 + int(state["pairs"]) * 4 + int(nq.mean()) * 16)
     cpu = None
@@ -1039,12 +1084,12 @@ def run_config4(args, env: Env):
                        "vocabulary": "k=10 L=6 seeded random tree of ORBvoc's shape (1,111,111 nodes)", "query_frames": Q, "passes_per_step": inner,
                        "pairs_per_query": int(state["pairs"]), "query_streams_in_flight": NH,
                        "parallelism": f"{world} GPUs x {NH} host threads, each an independent query stream on the GPU's database (no data-path collective; NCCL: vocabulary broadcast only)",
-                       "cache": f"the database sweep reads {db_bytes / 1e6:.0f} MB per query vs 126 MB L2: successive queries do find part of it in L2 (the reference's relocalisation re-reads the same keyframes too)",
+                       "cache": f"the database sweep reads {db_bytes / 1e6:.0f} MB per query vs 50 MB L2: successive queries do find part of it in L2 (the reference's relocalisation re-reads the same keyframes too)",
                        "e2e_pass": f"{Q} query frames: stereo extraction from host images + ComputeBoW + scoring + SearchByBoW each", "parity_checked": parity},
             "clocks": clk, "gpu_launches": int(launches),
             "e2e": {"value": e2e_value, "unit": "frames/s", "h2d_bytes_per_step": h2d * inner_e, "d2h_bytes_per_step": d2h * inner_e},
             "roofline": {"kernel": "bowdb_match_kernel (+ bowdb_finalize_kernel)", "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": achieved / peak, "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+                         "frac": achieved / peak, "traffic": None, "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": db_bytes, "mean_launch_ms": kernel_ms},
             "query_latency": {"call": "ComputeBoW + KeyFrameDatabase scoring + SearchByBoW vs all keyframes, one stream alone, host buffers in and out",
                               "us_p50": query_us},
@@ -1071,7 +1116,11 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--per-frame-calls", action="store_true", help="config 2: one borb_search_by_projection call per frame instead of the batched call")
     ap.add_argument("--no-parity", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the arrays the timed call returned in its last pass to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.dump_outputs and args.per_frame_calls:
+        ap.error("--dump-outputs reads the batched matcher call's results; it cannot be combined with --per-frame-calls")
     if args.handles is None:
         args.handles = {1: 6, 2: 8, 4: 8}.get(args.config, 4)
     rank = int(os.environ.get("RANK", "0"))

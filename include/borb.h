@@ -1,4 +1,4 @@
-/* borb.h — C ABI of the B200-native ORB front-end (libborb.so).
+/* borb.h — C ABI of the CUDA ORB front-end for the H100 (libborb.so).
  *
  * Drop-in boundary for the ONE hot path of raulmur/ORB_SLAM2 (SURVEY.md §8):
  *   ORBextractor::operator()              include/ORBextractor.h:59-61, src/ORBextractor.cc:1043
@@ -170,6 +170,15 @@ BORB_API borb_status borb_stereo_frames_device_enqueue(borb_extractor* e, const 
 BORB_API borb_status borb_stereo_frames_device(borb_extractor* e, const uint8_t* d_gray, int n_pairs, int width, int height,
                                       size_t pitch, size_t image_stride, float bf, float b, int* n_left, int* n_right,
                                       float* u_right, float* depth, int cap);
+/* Copies what the last stereo call on `e` left resident in HBM — keypoints, descriptors and counts of both images and
+ * mvuRight / mvDepth of its first n_pairs pairs — into host buffers laid out as in borb_stereo_frames (any pointer may be
+ * NULL), e.g. to inspect the results of the device-resident variants.  Waits for the handle's stream.  BORB_ERR_STATE unless
+ * the last call on `e` was a stereo call over at least n_pairs pairs in the default layout (left 2p, right 2p+1: the
+ * borb_stereo_frames* calls, or borb_stereo_match without index arrays); BORB_ERR_CAPACITY, after the copies, when an image
+ * has more than `cap` keypoints. */
+BORB_API borb_status borb_stereo_frames_results(borb_extractor* e, int n_pairs, borb_keypoint* kps_left, uint8_t* desc_left,
+                                                int* n_left, borb_keypoint* kps_right, uint8_t* desc_right, int* n_right,
+                                                float* u_right, float* depth, int cap);
 
 /* ---------------------------------------------------------------- matchers ------------------- */
 /* ORB_SLAM2::ORBmatcher is a stateless stack object created at every call site on three threads
@@ -501,11 +510,11 @@ BORB_API borb_status borb_matcher_launch_count(const borb_matcher* m, uint64_t* 
 BORB_API borb_status borb_debug_candidates(borb_extractor* e, int image, int level, int32_t* xys, int cap, int* n_out);
 BORB_API borb_status borb_debug_selected(borb_extractor* e, int image, int level, int32_t* xys, int cap, int* n_out);
 BORB_API borb_status borb_debug_blurred(borb_extractor* e, int image, int level, uint8_t* dst, int* w, int* h);
-/* Ablation of fast_kernel for the speed-of-light table in profiles/ (0 = full kernel, the only mode that produces
+/* Ablation of fast_kernel for speed-of-light measurements (tools/fast_ablation.py; 0 = full kernel, the only mode that produces
  * keypoints; 1 = TMA tile load only, 2 = + packed reject pass, 3 = + exact scores without NMS / emit). */
 BORB_API borb_status borb_debug_set_fast_mode(borb_extractor* e, int mode);
 /* Distance arithmetic of the database SearchByBoW kernel: 2 (default) = three 3:2 compressors + 5 POPC per 256-bit distance,
- * 1 = full carry-save adder tree + 4 POPC, 0 = 8 POPC.  Same results; kept switchable for the measurement in profiles/. */
+ * 1 = full carry-save adder tree + 4 POPC, 0 = 8 POPC.  Same results; kept switchable for measurements. */
 BORB_API borb_status borb_debug_set_bow_csa(int mode);
 /* Work-item size of the same kernel: keyframes per item = target / (bucket width)^2, clamped to [1, 32] (default 2560); a negative
  * target selects the static item-to-warp schedule instead of the atomic work counter. */

@@ -17,6 +17,10 @@ DBoW2::BowVector make_bow(const uint32_t* w, const double* v, int n) {
     for (int i = 0; i < n; i++) b.insert(b.end(), std::make_pair((DBoW2::WordId)w[i], (DBoW2::WordValue)v[i]));
     return b;
 }
+// The tree as TemplatedVocabulary keeps it (the protected m_nodes), read through a pointer to member formed in a derived class.
+struct VocNodes : ORBVocabulary {
+    static const std::vector<Node>& of(const ORBVocabulary& v) { return v.*(&VocNodes::m_nodes); }
+};
 }  // namespace
 
 extern "C" {
@@ -28,6 +32,21 @@ void* dbowref_voc_load_text(const char* path) {
 }
 void dbowref_voc_destroy(void* h) { delete static_cast<ORBVocabulary*>(h); }
 int dbowref_voc_words(void* h) { return (int)static_cast<ORBVocabulary*>(h)->size(); }
+int dbowref_voc_nodes(void* h) { return (int)VocNodes::of(*static_cast<ORBVocabulary*>(h)).size(); }
+// Node by node: parent, leaf flag, 32-byte descriptor (zeros for the root), weight; k and L of the tree.
+void dbowref_voc_export(void* h, int32_t* parent, uint8_t* is_leaf, uint8_t* desc, double* weight, int* k, int* L) {
+    const ORBVocabulary* voc = static_cast<ORBVocabulary*>(h);
+    const auto& nodes = VocNodes::of(*voc);
+    for (size_t i = 0; i < nodes.size(); i++) {
+        parent[i] = (int32_t)nodes[i].parent;
+        is_leaf[i] = nodes[i].isLeaf() ? 1 : 0;
+        weight[i] = nodes[i].weight;
+        std::memset(desc + i * 32, 0, 32);
+        if (!nodes[i].descriptor.empty()) std::memcpy(desc + i * 32, nodes[i].descriptor.data, 32);
+    }
+    *k = voc->getBranchingFactor();
+    *L = voc->getDepthLevels();
+}
 
 // TemplatedVocabulary::transform(features, BowVector, FeatureVector, levelsup) — Frame::ComputeBoW (src/Frame.cc:395-402)
 int dbowref_transform(void* h, const uint8_t* desc, int n, int levelsup, uint32_t* bow_word, double* bow_val, int* n_bow,

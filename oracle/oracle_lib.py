@@ -10,6 +10,8 @@ from __future__ import annotations
 import ctypes as C
 import os
 import subprocess
+import tarfile
+import tempfile
 
 import numpy as np
 
@@ -35,6 +37,8 @@ def build(force: bool = False) -> None:
     if force:
         subprocess.check_call(["make", "-C", HERE, "clean"], stdout=subprocess.DEVNULL)
     subprocess.check_call(["make", "-C", HERE] + targets, stdout=subprocess.DEVNULL)
+    if "ref" in targets:
+        build_voc_arrays()
 
 
 def have_ref() -> bool:
@@ -901,6 +905,16 @@ class RefVocabulary:
             self._lib.dbowref_voc_destroy(self._h)
             self._h = None
 
+    def export(self):
+        """The loaded tree node by node, in the layout of PortVocabulary.export (word ids excepted)."""
+        self._lib.dbowref_voc_nodes.argtypes = [C.c_void_p]
+        n = self._lib.dbowref_voc_nodes(self._h)
+        parent = np.zeros(n, np.int32); leaf = np.zeros(n, np.uint8); desc = np.zeros((n, 32), np.uint8); weight = np.zeros(n, np.float64)
+        k, L = C.c_int(), C.c_int()
+        self._lib.dbowref_voc_export.argtypes = [C.c_void_p] * 5 + [C.POINTER(C.c_int), C.POINTER(C.c_int)]
+        self._lib.dbowref_voc_export(self._h, _ptr(parent), _ptr(leaf), _ptr(desc), _ptr(weight), C.byref(k), C.byref(L))
+        return dict(parent=parent, is_leaf=leaf, desc=desc, weight=weight, k=k.value, L=L.value)
+
     def transform(self, desc, levelsup):
         """-> (bow {word: value}, fv_node, fv_start, fv_idx)"""
         d = _a(desc, np.uint8)
@@ -1131,3 +1145,43 @@ class RefBowSweep:
                 self.lib.matchref_kf_destroy(h)
         except Exception:
             pass
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# The reference's real vocabulary as arrays (oracle/_ref/orbvoc_arrays.npz, 1,082,073 nodes): tests/test_gpu_voc_real.py pushes it
+# through the CUDA library.  Written by build() where the reference tree exists; like the libraries it travels with oracle/_ref.
+VOC_ARRAYS = os.path.join(HERE, "_ref", "orbvoc_arrays.npz")
+
+
+def build_voc_arrays() -> None:
+    """Parses Vocabulary/ORBvoc.txt.tar.gz with the reference's own DBoW2 loadFromTextFile (libdbowref.so), checks the tree node
+    for node against the restated loader, and writes the arrays.  loadFromTextFile loops `while(!f.eof())`
+    (TemplatedVocabulary.h:1379-1420), so a trailing newline would give it an extra node with uninitialised fields: it reads a
+    copy without that newline, where it is well defined (tests/test_oracle_dbow_ref.py shows the quirk)."""
+    tar = os.path.join(REFERENCE_ROOT, "Vocabulary", "ORBvoc.txt.tar.gz")
+    if not (os.path.exists(tar) and have_dbowref()):
+        return
+    if os.path.exists(VOC_ARRAYS) and os.path.getmtime(VOC_ARRAYS) >= max(os.path.getmtime(tar), os.path.getmtime(DBOWREF_SO)):
+        return
+    with tempfile.TemporaryDirectory() as tmp:
+        with tarfile.open(tar) as t:
+            t.extract("ORBvoc.txt", tmp, filter="data")
+        txt, nonl = os.path.join(tmp, "ORBvoc.txt"), os.path.join(tmp, "ORBvoc_nonl.txt")
+        with open(txt, "rb") as f:
+            raw = f.read()
+        with open(nonl, "wb") as f:
+            f.write(raw.rstrip(b"\n"))
+        del raw
+        ref = RefVocabulary(nonl)
+        e = ref.export()
+        assert int(e["is_leaf"].sum()) == ref.words
+        del ref
+        port = PortVocabulary.load_text(txt).export()
+    for key in ("is_leaf", "desc", "weight", "k", "L"):
+        assert np.array_equal(e[key], port[key]), f"restated vocabulary loader differs from DBoW2 in {key}"
+    assert np.array_equal(e["parent"][1:], port["parent"][1:]), "restated vocabulary loader differs from DBoW2 in parent"
+    e["parent"][0] = port["parent"][0]                     # the root's parent is undefined in DBoW2; keep the restatement's marker
+    part = VOC_ARRAYS[:-len(".npz")] + ".part.npz"
+    np.savez_compressed(part, parent=e["parent"], is_leaf=e["is_leaf"], desc=e["desc"], weight=e["weight"],
+                        k=np.array([e["k"]]), L=np.array([e["L"]]))
+    os.replace(part, VOC_ARRAYS)

@@ -66,6 +66,7 @@ _SIGNATURES = {
                                             C.c_float, vp, vp, vp, vp, C.c_int]),
     "borb_stereo_frames_device_enqueue": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, C.c_size_t, C.c_size_t, C.c_float,
                                                     C.c_float, vp, vp, vp, vp, C.c_int]),
+    "borb_stereo_frames_results": (C.c_int, [vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, C.c_int]),
     "borb_stage_times_total": (C.c_int, [vp, C.POINTER(C.c_double), C.POINTER(C.c_uint64)]),
     "borb_extractor_stream": (C.c_int, [vp, C.POINTER(vp)]),
     "borb_matcher_create": (C.c_int, [C.c_int, C.POINTER(vp)]),

@@ -226,6 +226,7 @@ borb_status ensure(borb_extractor* e, int w, int h, int n_images) {
     std::vector<int16_t> tabs;
     e->have_geom = false;
     e->last_n_images = 0;
+    e->last_stereo_pairs = 0;
     borb_status st = build_geometry(e, w, h, tabs);
     if (st != BORB_OK) return st;
     size_t n = (size_t)(n_images > 2 ? n_images : 2);
@@ -324,6 +325,7 @@ borb_status enqueue_extract(borb_extractor* e, int n) {
     mark(e, 6);
     BORB_CUDA(cudaGetLastError());
     e->last_n_images = n;
+    e->last_stereo_pairs = 0;
     return BORB_OK;
 }
 
@@ -470,6 +472,8 @@ borb_status enqueue_stereo(borb_extractor* eL, borb_extractor* eR, int n_pairs, 
     e->launches += launch_stereo(g, L, R, e->ws.pair_idx, n_pairs, bf, b, e->ws.u_right, e->ws.depth, e->ws.sad, g.sel_image_stride, e->ws.st_bins, e->ws.st_recs, e->stream);
     mark(e, 7);
     BORB_CUDA(cudaGetLastError());
+    // borb_stereo_frames_results reads pairs in the default layout (left 2p, right 2p+1 of this handle's batch) only
+    e->last_stereo_pairs = (eL == eR && !left_idx && !right_idx) ? n_pairs : 0;
     return BORB_OK;
 }
 
@@ -896,6 +900,28 @@ borb_status borb_stereo_frames_device(borb_extractor* e, const uint8_t* d_gray, 
                                                        u_right, depth, cap);
     if (st != BORB_OK || n_pairs == 0) return st;
     return borb_sync(e);
+}
+
+borb_status borb_stereo_frames_results(borb_extractor* e, int n_pairs, borb_keypoint* kps_left, uint8_t* desc_left, int* n_left,
+                                       borb_keypoint* kps_right, uint8_t* desc_right, int* n_right, float* u_right, float* depth,
+                                       int cap) {
+    if (!e || n_pairs < 0 || cap < 0) { set_error("bad arguments"); return BORB_ERR_INVALID_ARG; }
+    if (n_pairs == 0) return BORB_OK;
+    if (!e->have_geom || n_pairs > e->last_stereo_pairs) {
+        set_error("the last call on this handle left stereo results for %d pairs, %d requested", e->last_stereo_pairs, n_pairs);
+        return BORB_ERR_STATE;
+    }
+    BORB_CUDA(cudaSetDevice(e->device));
+    borb_status st;
+    if ((st = download_kps(e, 0, n_pairs, 2, kps_left, desc_left, cap, n_left)) != BORB_OK) return st;
+    if ((st = download_kps(e, 1, n_pairs, 2, kps_right, desc_right, cap, n_right)) != BORB_OK) return st;
+    if ((st = download_stereo(e, n_pairs, u_right, depth, cap)) != BORB_OK) return st;
+    if ((st = borb_sync(e)) != BORB_OK) return st;
+    std::vector<int> counts(2 * (size_t)n_pairs);
+    BORB_CUDA(cudaMemcpy(counts.data(), e->ws.nkp, counts.size() * sizeof(int), cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < counts.size(); i++)
+        if (counts[i] > cap) { set_error("pair %d exceeds capacity %d", (int)(i / 2), cap); return BORB_ERR_CAPACITY; }
+    return BORB_OK;
 }
 
 }  // extern "C"

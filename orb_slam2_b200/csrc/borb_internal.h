@@ -1,4 +1,4 @@
-// Internal declarations of libborb (B200 / sm_100a ORB front-end).  Not part of the C ABI.
+// Internal declarations of libborb (H100 / sm_90a ORB front-end).  Not part of the C ABI.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -156,6 +156,7 @@ struct borb_extractor {
     borb::Geometry geom;
     borb::Workspace ws;
     int last_n_images = 0;       // images of the last batch (0: none)
+    int last_stereo_pairs = 0;   // pairs (2p, 2p+1) of the last batch associated by a stereo call on this handle (0: none)
     int in_channels = 1;         // host input pixel format (borb_extractor_set_input_format): 1 gray, 3 RGB/BGR, 4 RGBA/BGRA
     int in_rgb = 1;              // 1: R first (mbRGB), 0: B first
     // rectification maps (borb_extractor_set_rectify_maps): set 0 = mono / left, set 1 = right; device float maps

@@ -197,7 +197,7 @@ int launch_projection_last(const LastArgs& L, const ProjArgs& A, int32_t* state_
 int launch_initialization(const ProjArgs& A, const borb_keypoint* keys1, int n1, int32_t* match12, int32_t* ev_idx, uint8_t* ev_bin,
                           float* prev, int* n_matches, cudaStream_t s);
 int launch_kfdb_score(const BowDev* table, int n_slots, const uint32_t* qword, const double* qvalue, int nq, int32_t* common, float* score,
-                      uint32_t* first_word, cudaStream_t s);
+                      uint32_t* first_word, int n_sm, cudaStream_t s);
 int launch_distinctive(const uint8_t* desc, const int32_t* offsets, int n_points, int32_t* best_idx, cudaStream_t s);
 int launch_frustum_projection(const LastArgs& L, const ProjArgs& A, int32_t* match_feat, int* n_matches, cudaStream_t s);
 int launch_projection_argmin(const LastArgs& L, const ProjArgs& A, int32_t* best_idx, int* n_found, cudaStream_t s);

@@ -1310,7 +1310,7 @@ borb_status borb_kfdb_query(borb_matcher* m, borb_kfdb* db, const uint32_t* bow_
         // the three result arrays are written by the kernel straight into the pinned landing buffer (device-addressable, UVA)
         uint8_t* ho = m->h_out;
         m->launches += launch_kfdb_score(db->d_table, n, (const uint32_t*)(b + o_w), (const double*)(b + o_v), n_bow, (int32_t*)ho,
-                                         (float*)(ho + (size_t)n * 4), (uint32_t*)(ho + (size_t)n * 8), m->stream);
+                                         (float*)(ho + (size_t)n * 4), (uint32_t*)(ho + (size_t)n * 8), db->n_sm, m->stream);
         BORB_CUDA(cudaGetLastError());
     }
     BORB_CUDA(cudaStreamSynchronize(m->stream));

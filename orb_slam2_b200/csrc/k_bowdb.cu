@@ -20,9 +20,8 @@
 // keyframe) applies ComputeThreeMaxima (:267-285) and compacts the survivors into (frame feature, keyframe feature) pairs in
 // (node, frame feature) order — deterministic output.
 //
-// Bound (profiles/r02_bowdb_ncu_summary.md): not HBM (96 MB per 2000-keyframe sweep in 0.105 ms) and no longer the POPC
-// pipe (ham256<MODE>: 8 POPC, 4 POPC + carry-save tree, or 5 POPC + three 3:2 compressors run the sweep in the same time);
-// 40 % of the instructions are per-item / per-batch bookkeeping around the column loop.
+// Bound: not HBM (96 MB of keyframe records per 2000-keyframe sweep) but the integer pipes and the per-item / per-batch
+// bookkeeping around the column loop (ham256<MODE>: 8 POPC, 4 POPC + carry-save tree, or 5 POPC + three 3:2 compressors).
 #include "borb_match.h"
 
 namespace borb {
@@ -39,9 +38,9 @@ constexpr int HISTO_LENGTH = 30;
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 // 256-bit Hamming distance.  MODE 0: 8 POPC.  MODE 1: full carry-save adder tree, 4 POPC + 17 LOP3.  MODE 2 (default): three
-// 3:2 compressors, 5 POPC + 6 LOP3.  On sm_100 POPC issues on the XU pipe at 4 lanes/clk per SM sub-partition (8 cycles per
-// warp instruction) and LOP3 on the ALU pipe at 16 lanes/clk (2 cycles): per distance MODE 0 costs 64 XU cycles, MODE 1
-// 32 XU + ~60 ALU cycles (ALU-bound: ncu showed alu 73 %, xu 40 %), MODE 2 40 XU + ~34 ALU cycles - the balanced point.
+// 3:2 compressors, 5 POPC + 6 LOP3.  POPC issues at a quarter of LOP3's rate (16 vs 64 results per clock per SM on sm_90,
+// CUDA C++ Programming Guide throughput table): per distance MODE 0 is all POPC, MODE 1 shifts most of the work to LOP3,
+// MODE 2 balances the two.
 template <int MODE>
 __device__ __forceinline__ int ham256(const uint4 a0, const uint4 a1, const uint4 b0, const uint4 b1) {
     const uint32_t x0 = a0.x ^ b0.x, x1 = a0.y ^ b0.y, x2 = a0.z ^ b0.z, x3 = a0.w ^ b0.w;

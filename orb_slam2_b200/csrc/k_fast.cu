@@ -30,8 +30,8 @@
 // Output: unordered candidate list per (image, level) of packed (x,y,score); consumers break ties with
 // the reference's emission order key (cell row, cell col, y, x), never with list position.
 //
-// Bound (target): HBM read of the level pixels, once — sum_l w_l*h_l bytes per image.  Measured on B200: the
-// integer ALU pipe (LOP3/PRMT/VABSDIFF4/VIMNMX3 all issue at 64 lanes/clk/SM, tools/ubench*.cu) — see DESIGN.md.
+// Bound (target): HBM read of the level pixels, once — sum_l w_l*h_l bytes per image.  In practice the integer ALU pipe
+// (LOP3/PRMT/VABSDIFF4/VIMNMX3) bounds it: a bit-exact FAST-9 needs tens of integer operations per pixel — see DESIGN.md.
 #include <cuda.h>
 
 #include <cstring>

@@ -768,13 +768,13 @@ int launch_initialization(const ProjArgs& A, const borb_keypoint* keys1, int n1,
     return 2;
 }
 int launch_kfdb_score(const BowDev* table, int n_slots, const uint32_t* qword, const double* qvalue, int nq, int32_t* common, float* score,
-                      uint32_t* first_word, cudaStream_t s) {
+                      uint32_t* first_word, int n_sm, cudaStream_t s) {
     if (n_slots > 0) {
         const size_t smem = (size_t)nq * 12 + 16;
         const int in_smem = smem <= 160 * 1024;
         if (in_smem) allow_max_smem((const void*)kfdb_score_kernel);
         int ctas = (n_slots + 3) / 4;                                 // 4 keyframes (warps) per CTA: 2000 keyframes spread over all SMs
-        if (ctas > 148 * 8) ctas = 148 * 8;                           // persistent: the query is staged once per CTA
+        if (ctas > n_sm * 8) ctas = n_sm * 8;                         // persistent: the query is staged once per CTA
         kfdb_score_kernel<<<ctas, 128, in_smem ? smem : 0, s>>>(table, n_slots, qword, qvalue, nq, in_smem, common, score, first_word);
     }
     return 1;

@@ -2,7 +2,7 @@
 
 Same constructor arguments, call operator, getters and the public ``mvImagePyramid`` member as the
 reference class, so parity tests read like calls into the reference; plus the batched entry points
-(many independent frames per launch) that the B200 design is built around.  All compute happens in
+(many independent frames per launch) that the design is built around.  All compute happens in
 the CUDA library; this module only marshals numpy buffers through the C ABI.
 """
 from __future__ import annotations

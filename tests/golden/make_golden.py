@@ -21,6 +21,7 @@ CASES = {  # name: (w, h, nfeatures, iniTh, minTh, seed)   — BASELINE.json con
     "tum_1000": (640, 480, 1000, 20, 7, 102),
     "euroc_1200": (752, 480, 1200, 20, 7, 103),
     "tum_mono_init_2000": (640, 480, 2000, 20, 7, 104),  # Tracking.cc:125 mpIniORBextractor = 2*nFeatures
+    "kitti_seed21_2000": (1242, 375, 2000, 20, 7, 21),   # test_gpu_extract.py::test_matches_verbatim_reference_build
 }
 
 

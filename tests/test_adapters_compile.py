@@ -156,7 +156,7 @@ def test_keyframe_database_drop_in_compiles_with_resident_features(tmp_path):
 def test_multistream_host_example_builds_and_fails_loudly_without_a_gpu(tmp_path):
     """integration/example_multistream_host.cc — a C++ host written against the C ABI only (batched extraction, device-resident
     frames, one batched SearchByProjection for all streams, self-checking) — compiles and links; without a GPU it must stop at the
-    first library call with the library's error (exit code 3), with one it runs its self-check (verified on the B200: every point
+    first library call with the library's error (exit code 3), with one it runs its self-check (verified on the GPU: every point
     of every stream matched to its own feature)."""
     so = os.path.join(ROOT, "orb_slam2_b200", "libborb.so")
     exe = tmp_path / "example_host"

@@ -1,5 +1,5 @@
 """CPU: the `--impl reference` arm of bench.py (the reference's own CPU implementation, oracle/_ref when it compiles here,
-else the oracle port) runs without a GPU and prints ONE JSON line with the contract's keys; the B200 arm must refuse to
+else the oracle port) runs without a GPU and prints ONE JSON line with the contract's keys; the GPU arm must refuse to
 produce a number without a GPU (no CPU fallback)."""
 import json
 import os
@@ -43,7 +43,7 @@ def test_b200_arm_needs_a_gpu():
 
 
 def test_reference_arm_under_torchrun_prints_on_rank_0_only():
-    """The driver launches the reference arm like the B200 arm (torchrun, one process per GPU): rank 0 alone runs and prints
+    """The reference arm is launched like the GPU arm (torchrun, one process per GPU): rank 0 alone runs and prints
     the line, the other ranks exit 0 without output and without work."""
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",
            "--master-port", "29577", os.path.join(ROOT, "bench.py"), "--impl", "reference", "--gpus", "2", "--steps", "1", "--warmup", "1",

@@ -23,7 +23,7 @@ def test_port_reproduces_golden(oracle, path):
     assert np.array_equal(k, g["keypoints"]) and np.array_equal(d, g["descriptors"])
 
 
-@pytest.mark.parametrize("path", golden_extract_cases()[:2], ids=os.path.basename)
+@pytest.mark.parametrize("path", golden_extract_cases()[:2] + [os.path.join(GOLD, "extract_kitti_seed21_2000.npz")], ids=os.path.basename)
 def test_verbatim_reference_reproduces_golden(oracle_ref, path):
     g = np.load(path)
     w, h, nf, ini, mn, seed = g["meta"].tolist()
@@ -80,7 +80,7 @@ def test_matcher_restatement_reproduces_golden(oracle, name):
 
 
 def test_gpu_side_of_the_golden_cases_binds_to_the_product_api(oracle):
-    """The `gpu` half of every golden case (run on the B200 by tests/test_gpu_match.py) is exercised here without a GPU: a
+    """The `gpu` half of every golden case (run on the GPU by tests/test_gpu_match.py) is exercised here without a GPU: a
     stand-in ORBmatcher checks each call against the real method's signature (inspect.signature(...).bind) and answers with the
     restatement, so a mistake in the call plumbing cannot hide until the GPU run."""
     import inspect

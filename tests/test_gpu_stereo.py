@@ -74,6 +74,51 @@ def test_two_handle_path_equals_batched_path(X, oracle):
     assert np.array_equal(ur[:len(kl)], our) and np.array_equal(dp[:len(kl)], odp)
 
 
+def test_results_of_the_device_resident_call_read_back_equal_the_host_call(X):
+    """borb_stereo_frames_device leaves keypoints, descriptors and the association in HBM; borb_stereo_frames_results copies
+    them out afterwards and they equal what borb_stereo_frames returns for the same pairs."""
+    import torch
+    from orb_slam2_b200 import _lib
+    from orb_slam2_b200._lib import KP_DTYPE
+    lib = _lib.load()
+    w, h = synth.KITTI
+    pairs = [synth.stereo_pair(500 + i, 0, 0, w, h) for i in range(2)]
+    G = X(2000)
+    cap = G.capacity(w, h)
+    d_img = torch.from_numpy(np.stack([im for p in pairs for im in p[:2]])).cuda()
+    b = float(np.float32(BF) / np.float32(FX))
+    nl, nr = np.zeros(2, np.int32), np.zeros(2, np.int32)
+    _lib.check(lib.borb_stereo_frames_device(G._h, d_img.data_ptr(), 2, w, h, w, w * h, BF, b, _lib.ptr(nl), _lib.ptr(nr), None, None, cap),
+               "borb_stereo_frames_device")
+    kl, kr = np.zeros((2, cap), KP_DTYPE), np.zeros((2, cap), KP_DTYPE)
+    dl, dr = np.zeros((2, cap, 32), np.uint8), np.zeros((2, cap, 32), np.uint8)
+    ml, mr = np.zeros(2, np.int32), np.zeros(2, np.int32)
+    ur, dp = np.zeros((2, cap), np.float32), np.zeros((2, cap), np.float32)
+    _lib.check(lib.borb_stereo_frames_results(G._h, 2, kl.ctypes.data, dl.ctypes.data, ml.ctypes.data, kr.ctypes.data, dr.ctypes.data,
+                                              mr.ctypes.data, ur.ctypes.data, dp.ctypes.data, cap), "borb_stereo_frames_results")
+    assert np.array_equal(ml, nl) and np.array_equal(mr, nr)
+    want = X(2000).stereo_frames([p[0] for p in pairs], [p[1] for p in pairs], BF, FX)
+    for p, o in enumerate(want):
+        n, m = nl[p], nr[p]
+        assert np.array_equal(kl[p, :n], o["mvKeys"]) and np.array_equal(dl[p, :n], o["mDescriptors"])
+        assert np.array_equal(kr[p, :m], o["mvKeysRight"]) and np.array_equal(dr[p, :m], o["mDescriptorsRight"])
+        assert np.array_equal(ur[p, :n], o["mvuRight"]) and np.array_equal(dp[p, :n], o["mvDepth"])
+    # a buffer smaller than a pair's keypoint count is reported, as borb_stereo_frames does
+    small = int(min(nl.min(), nr.min())) - 1
+    with pytest.raises(_lib.BorbError) as ex:
+        _lib.check(lib.borb_stereo_frames_results(G._h, 1, kl.ctypes.data, dl.ctypes.data, ml.ctypes.data, kr.ctypes.data,
+                                                  dr.ctypes.data, mr.ctypes.data, ur.ctypes.data, dp.ctypes.data, small), "results")
+    assert ex.value.status == 5                                                    # BORB_ERR_CAPACITY
+    with pytest.raises(_lib.BorbError) as ex:                                      # more pairs than the stereo call associated
+        _lib.check(lib.borb_stereo_frames_results(G._h, 3, None, None, None, None, None, None, None, None, cap), "results")
+    assert ex.value.status == 6                                                    # BORB_ERR_STATE
+    G(pairs[0][0])                                                                 # a mono extraction replaces the batch
+    with pytest.raises(_lib.BorbError) as ex:
+        _lib.check(lib.borb_stereo_frames_results(G._h, 1, None, None, None, None, None, None, ur.ctypes.data, dp.ctypes.data, cap),
+                   "results")
+    assert ex.value.status == 6
+
+
 def test_explicit_pair_indices_and_no_match_cases(X, oracle):
     G = X(1000)
     L, R, _ = synth.stereo_pair(500, 0, 0, 640, 480)

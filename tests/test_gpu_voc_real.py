@@ -1,7 +1,7 @@
 """The REAL vocabulary (reference Vocabulary/ORBvoc.txt.tar.gz: k=10, L=6, 1,082,073 nodes, 971,814 words) through the product:
 tests/golden/voc_real.npz holds BowVector / FeatureVector of three golden descriptor sets as the reference's own DBoW2 (compiled
-verbatim) computes them; oracle/_ref/orbvoc_arrays.npz (git-ignored, written by tools/make_golden_voc.py, travels to the GPU box)
-holds the parsed tree.  Checked here: borb_voc_create + borb_compute_bow on the real tree, the text loader on a text file rebuilt
+verbatim) computes them; oracle/_ref/orbvoc_arrays.npz (git-ignored, written by build() with the reference's own DBoW2 loader,
+oracle_lib.build_voc_arrays, and kept with the other oracle/_ref builds) holds the parsed tree.  Checked here: borb_voc_create + borb_compute_bow on the real tree, the text loader on a text file rebuilt
 in ORBvoc.txt's format (with its trailing newline), the packed blob round trip; load / upload times are printed."""
 import os
 import time
@@ -19,7 +19,7 @@ SETS = ["extract_kitti_2000", "extract_euroc_1200", "extract_tum_1000"]
 @pytest.fixture(scope="module")
 def real():
     if not os.path.exists(ARR):
-        pytest.skip("oracle/_ref/orbvoc_arrays.npz absent (run tools/make_golden_voc.py where /root/reference exists)")
+        pytest.skip("oracle/_ref/orbvoc_arrays.npz absent (build() writes it where the reference tree is present)")
     a = np.load(ARR)
     return dict(parent=a["parent"], is_leaf=a["is_leaf"], desc=a["desc"], weight=a["weight"], k=int(a["k"][0]), L=int(a["L"][0]))
 

@@ -1,4 +1,4 @@
-"""Stage-by-stage GPU-vs-oracle diagnostic (run on the B200 box). Prints mismatch counts; never asserts.
+"""Stage-by-stage GPU-vs-oracle diagnostic (run on a machine with the GPU). Prints mismatch counts; never asserts.
 Test tooling: uses the oracle as the checker."""
 import os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

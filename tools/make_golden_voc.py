@@ -6,9 +6,8 @@
    bogus extra node with uninitialised fields; the pin loads a copy without that newline, where the reference is well defined;
 3. transforms the committed golden descriptor sets (tests/golden/extract_*.npz) with the VERBATIM DBoW2 (levelsup 4, what
    Frame::ComputeBoW asks for) and stores BowVector + FeatureVector in tests/golden/voc_real.npz (small, committed);
-4. checks that the oracle port's loader + transform reproduce them, and writes the parsed tree as arrays to
-   oracle/_ref/orbvoc_arrays.npz (git-ignored, travels to the GPU box) so that tests/test_gpu_voc_real.py can rebuild the
-   text file there and push the REAL vocabulary through borb_voc_load_text / borb_voc_create / borb_compute_bow."""
+4. checks that the oracle port's loader + transform reproduce them.  The parsed tree itself (oracle/_ref/orbvoc_arrays.npz,
+   what tests/test_gpu_voc_real.py pushes through the CUDA library) is written by build(): oracle_lib.build_voc_arrays."""
 import os
 import subprocess
 import sys
@@ -58,9 +57,7 @@ def main():
         print(f"{name}: {len(desc)} descriptors -> {len(bow)} words, {len(fn)} nodes (port == verbatim DBoW2)")
     out["n_nodes"] = np.array([len(e["parent"])]); out["n_words"] = np.array([ref.words])
     np.savez_compressed(os.path.join(ROOT, "tests", "golden", "voc_real.npz"), **out)
-    np.savez_compressed(os.path.join(ROOT, "oracle", "_ref", "orbvoc_arrays.npz"), parent=e["parent"], is_leaf=e["is_leaf"], desc=e["desc"],
-                        weight=e["weight"], k=np.array([e["k"]]), L=np.array([e["L"]]))
-    print("wrote tests/golden/voc_real.npz and oracle/_ref/orbvoc_arrays.npz")
+    print("wrote tests/golden/voc_real.npz")
 
 
 if __name__ == "__main__":

@@ -19,7 +19,7 @@ UNIT_SCALE = {"ns": 1e-3, "us": 1.0, "usecond": 1.0, "ms": 1e3, "msecond": 1e3, 
               "byte": 1e-6, "Kbyte": 1e-3, "Mbyte": 1.0, "Gbyte": 1e3}
 
 
-PEAK = 6574.1     # GB/s, MEASURED_PEAKS.json hbm_gbs (burst copy bandwidth of this pool's B200s)
+PEAK = 3350.0     # GB/s, HBM3 bandwidth of the H100 SXM data sheet (not a measured figure)
 
 
 def main():
