@@ -369,6 +369,54 @@ BORB_API borb_status borb_search_local_points(borb_matcher* m, const borb_frame_
                                               float nnratio, uint8_t* in_view, float* proj_x, float* proj_y, float* proj_xr,
                                               int32_t* level, float* view_cos, int32_t* match_feat, int32_t* n_matches);
 
+/* One camera stream's Tracking::SearchLocalPoints (src/Tracking.cc:1148-1194): the per-frame arguments of
+ * borb_search_local_points. */
+typedef struct borb_local_points_job {
+    borb_frame_view frame;         /* frame.resident must be set; frame.occupied is read per job (NULL: none) */
+    borb_worldpoints_view pts;     /* as for borb_search_local_points: valid[i] = the point reaches isInFrustum (:1171-1175) */
+    const uint8_t* has_obs;        /* Observations()>0 (NULL: all) */
+    float Tcw[12];                 /* mCurrentFrame.mTcw rows 0..2 = [mRcw | mtcw] */
+    float Ow[3];                   /* mCurrentFrame.mOw = -mRcw.t()*mtcw (src/Frame.cc:266) */
+    float fx, fy, cx, cy, mbf;     /* Frame::fx, fy, cx, cy, mbf (isInFrustum, src/Frame.cc:288,319) */
+    float log_scale_factor;        /* mfLogScaleFactor (PredictScale, src/MapPoint.cc:402-417) */
+    float th;                      /* 1, 3 (RGB-D) or 5 (just relocalised) at the call site, src/Tracking.cc:1185-1191 */
+    uint8_t* in_view;              /* outputs, pts.n entries each, as in borb_search_local_points; proj_* / level / view_cos may be NULL */
+    float* proj_x;
+    float* proj_y;
+    float* proj_xr;
+    int32_t* level;
+    float* view_cos;
+    int32_t* match_feat;
+} borb_local_points_job;
+/* borb_search_local_points for n_jobs independent camera streams in one launch sequence (projection, candidates, resolve) and one
+ * synchronisation.  Every job's outputs and n_matches[j] are bit-identical to what the single call returns for the same inputs.
+ * Frames must be device-resident; a host view, and every per-job argument error (more than BORB_MATCH_MAX_FEATURES valid points,
+ * log_scale_factor <= 0, incomplete views), is refused with BORB_ERR_INVALID_ARG before anything is launched, the error text naming
+ * the job.  A job with no points or no valid points gets the single call's defaults (in_view and track fields 0, match_feat -1,
+ * n_matches 0); a frame with 0 features still gets isInFrustum's in_view and track fields, with every match_feat -1. */
+BORB_API borb_status borb_search_local_points_batch(borb_matcher* m, const borb_local_points_job* jobs, int n_jobs, float viewing_cos_limit,
+                                                    float nnratio, int32_t* n_matches);
+
+/* One camera stream's ORBmatcher::SearchByProjection(CurrentFrame, LastFrame, th, bMono) (src/ORBmatcher.cc:1328-1470): the
+ * per-frame arguments of borb_search_by_projection_last. */
+typedef struct borb_last_frame_job {
+    borb_frame_view cur;           /* cur.resident must be set; cur.occupied is read per job (NULL: none) */
+    borb_lastframe_view last;
+    float Tcw[12];                 /* CurrentFrame.mTcw rows 0..2 = mVelocity*mLastFrame.mTcw (src/Tracking.cc:874) */
+    float fx, fy, cx, cy, bf;      /* CurrentFrame.fx, fy, cx, cy, mbf (src/ORBmatcher.cc:1370-1371,1409) */
+    float th;                      /* 15 (monocular / RGB-D) or 7 (stereo), doubled on the retry, src/Tracking.cc:880-891 */
+    int32_t forward, backward;     /* bForward / bBackward (src/ORBmatcher.cc:1348-1349) */
+    int32_t* state_cur;            /* output, cur n entries, as in borb_search_by_projection_last */
+} borb_last_frame_job;
+/* borb_search_by_projection_last for n_jobs independent camera streams in one launch sequence (projection, candidates, resolve
+ * with a rotation histogram per job) and one synchronisation.  check_orientation applies to every job.  Every job's state_cur and
+ * n_matches[j] are bit-identical to the single call's.  Frames must be device-resident; a host view and every per-job argument
+ * error (more than BORB_MATCH_MAX_FEATURES last-frame points, last-frame octaves outside the frame's levels, incomplete views) are
+ * refused with BORB_ERR_INVALID_ARG before anything is launched, the error text naming the job.  A job with an empty last frame or
+ * a frame with 0 features gets state_cur -1 and n_matches 0. */
+BORB_API borb_status borb_search_by_projection_last_batch(borb_matcher* m, const borb_last_frame_job* jobs, int n_jobs, int check_orientation,
+                                                          int32_t* n_matches);
+
 /* ORBmatcher::SearchForInitialization(Frame &F1, Frame &F2, vector<cv::Point2f> &vbPrevMatched, vector<int> &vnMatches12,
  * int windowSize) — src/ORBmatcher.cc:405-520 (Tracking::MonocularInitialization, src/Tracking.cc:599).
  * f1/f2: keys_un, desc (and f2's grid bounds) are read; prev_matched = vbPrevMatched as f1->n x 2 floats, updated in

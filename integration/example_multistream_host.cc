@@ -6,10 +6,15 @@
 //   per tick:  borb_extract_batch            one launch sequence for the N images            (ORBextractor::operator() x N)
 //              borb_frames_from_extractor    N device-resident frames, keypoints stay in HBM  (Frame constructor tail x N)
 //              borb_search_by_projection_batch   one launch pair for the N matcher calls      (SearchByProjection x N)
+//              borb_search_by_projection_last_batch   motion-model search of the N streams    (TrackWithMotionModel x N)
+//              (pose optimisation on the host)
+//              borb_search_local_points_batch    isInFrustum + local-map search of the N streams   (SearchLocalPoints x N)
 //
 // The program self-checks: the "local map" of every stream is made of that stream's own keypoints (projected where they were
 // seen, with their own descriptors, predicted at their own octave), so SearchByProjection must give (almost) every point back to
-// a feature — bar the few points whose twin at a neighbouring level wins the ratio test.
+// a feature — bar the few points whose twin at a neighbouring level wins the ratio test.  For the two Tracking-thread searches
+// the keypoints are back-projected to a per-point depth with the identity pose: as the last frame's MapPoints they must land on
+// their own features, and as world points (normal = viewing ray, distances that predict the keypoint's octave) as well.
 // Build:  g++ -std=c++14 -Iinclude integration/example_multistream_host.cc orb_slam2_b200/libborb.so -Wl,-rpath,$PWD/orb_slam2_b200
 // Exit code 0 = ran and checked, 3 = the library reported an error (e.g. no CUDA device: there is no CPU fallback).
 #include <cmath>
@@ -66,7 +71,8 @@ int main(int argc, char** argv) {
     std::vector<borb_frame*> frames(N, nullptr);
     const borb_camera cam = {517.3f, 516.5f, 318.6f, 255.3f, 0.f, 0.f, 0.f, 0.f, 0.f, 40.f};      // k1 = 0: mvKeysUn = mvKeys
     float bounds[4];
-    long total_points = 0, total_matches = 0;
+    long total_points = 0, total_matches = 0, last_self = 0, local_self = 0;
+    const float log_scale = std::log(cfg.scale_factor);     // Frame::mfLogScaleFactor
 
     for (int t = 0; t < ticks; t++) {
         for (int i = 0; i < N; i++) { make_image(imgs[i], W, H, i + 100 * t); img_ptr[i] = imgs[i].data(); image_idx[i] = i; }
@@ -97,11 +103,54 @@ int main(int argc, char** argv) {
             match_ptr[i] = match[i].data();
         }
         CHECK(borb_search_by_projection_batch(mat, fv.data(), mps.data(), N, 3.0f, 0.8f, match_ptr.data(), n_matches.data()));
+        // ---- the Tracking thread's two per-frame searches on the same resident frames: every keypoint back-projected to a
+        //      depth z with the identity pose is the "last frame"'s MapPoint of that feature, and a local MapPoint as well
+        std::vector<std::vector<float> > wpos(N), maxd(N), mind(N), nrm(N);
+        std::vector<std::vector<int32_t> > state(N), lmatch(N);
+        std::vector<std::vector<uint8_t> > in_view(N);
+        std::vector<borb_last_frame_job> ljobs(N);
+        std::vector<borb_local_points_job> pjobs(N);
+        std::vector<int32_t> n_last(N), n_local(N);
+        for (int i = 0; i < N; i++) {
+            const int n = n_out[i];
+            const borb_keypoint* k = &kps[(size_t)i * cap];
+            wpos[i].resize((size_t)n * 3); maxd[i].resize(n); mind[i].resize(n); nrm[i].resize((size_t)n * 3);
+            state[i].assign(n > 0 ? n : 1, -1); lmatch[i].assign(n > 0 ? n : 1, -1); in_view[i].assign(n > 0 ? n : 1, 0);
+            for (int j = 0; j < n; j++) {
+                const float z = 2.0f + 0.5f * (float)(j % 17);
+                float* P = &wpos[i][(size_t)j * 3];
+                P[0] = (k[j].x - cam.cx) * z / cam.fx; P[1] = (k[j].y - cam.cy) * z / cam.fy; P[2] = z;
+                const float d = std::sqrt(P[0] * P[0] + P[1] * P[1] + P[2] * P[2]);
+                for (int c = 0; c < 3; c++) nrm[i][(size_t)j * 3 + c] = P[c] / d;
+                maxd[i][j] = d * scale[k[j].octave] * 0.95f;          // PredictScale: ceil(octave - 0.28) = octave
+                mind[i][j] = maxd[i][j] / scale[cfg.n_levels - 1];
+            }
+            const float I34[12] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0};
+            borb_last_frame_job& L = ljobs[i];
+            L = borb_last_frame_job();
+            L.cur.resident = frames[i];
+            L.last.n = n; L.last.keys_un = k; L.last.world_pos = wpos[i].data(); L.last.desc = &desc[(size_t)i * cap * 32];
+            for (int c = 0; c < 12; c++) L.Tcw[c] = I34[c];
+            L.fx = cam.fx; L.fy = cam.fy; L.cx = cam.cx; L.cy = cam.cy; L.bf = cam.bf; L.th = 15.0f;
+            L.state_cur = state[i].data();
+            borb_local_points_job& J = pjobs[i];
+            J = borb_local_points_job();
+            J.frame.resident = frames[i];
+            J.pts.n = n; J.pts.world_pos = wpos[i].data(); J.pts.desc = &desc[(size_t)i * cap * 32];
+            J.pts.max_distance = maxd[i].data(); J.pts.min_distance = mind[i].data(); J.pts.normal = nrm[i].data();
+            for (int c = 0; c < 12; c++) J.Tcw[c] = I34[c];
+            J.fx = cam.fx; J.fy = cam.fy; J.cx = cam.cx; J.cy = cam.cy; J.mbf = cam.bf; J.log_scale_factor = log_scale; J.th = 1.0f;
+            J.in_view = in_view[i].data(); J.match_feat = lmatch[i].data();
+        }
+        CHECK(borb_search_by_projection_last_batch(mat, ljobs.data(), N, 1, n_last.data()));
+        CHECK(borb_search_local_points_batch(mat, pjobs.data(), N, 0.5f, 0.8f, n_local.data()));
         for (int i = 0; i < N; i++) {
             total_points += n_out[i]; total_matches += n_matches[i];
-            int self = 0;
-            for (int j = 0; j < n_out[i]; j++) self += match[i][j] == j;
-            std::printf("tick %d stream %d: %d keypoints, %d matches (%d to themselves)\n", t, i, n_out[i], n_matches[i], self);
+            int self = 0, sl = 0, sp = 0;
+            for (int j = 0; j < n_out[i]; j++) { self += match[i][j] == j; sl += state[i][j] == j; sp += lmatch[i][j] == j; }
+            last_self += sl; local_self += sp;
+            std::printf("tick %d stream %d: %d keypoints, %d matches (%d to themselves); motion model %d (%d); local map %d (%d)\n", t, i,
+                        n_out[i], n_matches[i], self, n_last[i], sl, n_local[i], sp);
             CHECK(borb_frame_destroy(frames[i]));
             frames[i] = nullptr;
         }
@@ -109,7 +158,13 @@ int main(int argc, char** argv) {
     CHECK(borb_matcher_destroy(mat));
     CHECK(borb_extractor_destroy(ext));
     std::printf("%ld points, %ld matched\n", total_points, total_matches);
-    if (total_points < 100L * N * ticks || total_matches < total_points * 8 / 10) { std::printf("self-check failed\n"); return 1; }
+    std::printf("motion-model search: %ld of %ld features matched to their own last-frame point\n", last_self, total_points);
+    std::printf("local-map search: %ld of %ld points matched to their own feature\n", local_self, total_points);
+    if (total_points < 100L * N * ticks || total_matches < total_points * 8 / 10 || last_self < total_points * 8 / 10 ||
+        local_self < total_points * 8 / 10) {
+        std::printf("self-check failed\n");
+        return 1;
+    }
     std::printf("ok\n");
     return 0;
 }

@@ -65,8 +65,11 @@ struct ProjArgs {                 // device pointers
     int chi2;                     // 1: Fuse(pKF, vpMapPoints, th) reprojection gates per candidate (:907-931)
     const float* inv_sigma2;      // chi2: mvInvLevelSigma2
     uint8_t* q_valid_out;         // mode 1: validity written by project_points_kernel (aliases mp_valid)
-    // batched launches (borb_search_by_projection_batch): where this job's results go
-    int32_t* out_match;           // n_mp entries, then the match count
+    // batched launches (borb_search_by_projection_batch, borb_search_local_points_batch, borb_search_by_projection_last_batch):
+    // where this job's results go
+    int32_t* out_match;           // n_mp entries (mode 1: the per-feature state, n entries), then the match count
+    int32_t* ev_idx;              // mode 1: match events of the rotation histogram, n_mp entries
+    uint8_t* ev_bin;
 };
 
 struct LastArgs {                 // inputs of project_points_kernel
@@ -189,7 +192,10 @@ struct VocDev {                   // views into the packed blob
 int launch_grid_sort(const borb_keypoint* keys, int n, float minX, float minY, float invW, float invH, int* cell_start, int* cell_idx,
                      cudaStream_t s);
 void launch_candidates(const ProjArgs& A, cudaStream_t s);
-int launch_projection_batch(const ProjArgs* d_jobs, int n_jobs, int max_n, int max_n_mp, cudaStream_t s);
+int launch_projection_batch(const ProjArgs* d_jobs, int n_jobs, int max_n, int max_n_mp, cudaStream_t s, bool last = false);
+// project_points over a LastArgs table, then the batched candidates and resolve (last: resolve<true>) over a ProjArgs table
+int launch_point_projection_batch(const LastArgs* d_last, const ProjArgs* d_jobs, int n_jobs, int max_nq, int max_n, int max_n_mp, bool last,
+                                  cudaStream_t s);
 void launch_resolve(const ProjArgs& A, bool last, int32_t* out, int32_t* ev_idx, uint8_t* ev_bin, int* n_matches, cudaStream_t s);
 int launch_projection(const ProjArgs& A, int32_t* match_feat, int* n_matches, cudaStream_t s);
 int launch_projection_last(const LastArgs& L, const ProjArgs& A, int32_t* state_cur, int32_t* hist_idx, uint8_t* hist_bin, int* n_matches,

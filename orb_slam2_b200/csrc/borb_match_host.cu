@@ -962,6 +962,300 @@ borb_status borb_search_local_points(borb_matcher* m, const borb_frame_view* F, 
     return BORB_OK;
 }
 
+// ---- the two per-frame searches of the Tracking thread for many camera streams at once.  The per-job arguments go to device
+// tables (LastArgs for the projection, ProjArgs for candidates and resolve), every job's results to one region of the arena that
+// comes back with ONE device-to-host copy.  The last-frame state stays in the arena (not in mapped host memory): resolve<true>
+// writes it with atomicMax.
+namespace {
+borb_status job_error(int j, borb_status s) {      // prefixes the error text a shared check left with the job index
+    const std::string e = borb_last_error();
+    set_error("job %d: %s", j, e.c_str());
+    return s;
+}
+void bind_resident(const borb_frame* rf, ProjArgs& A) {
+    A.n = rf->n;
+    A.minX = rf->min_x; A.minY = rf->min_y;
+    A.invW = (float)GRID_COLS / (float)(rf->max_x - rf->min_x);      // as bind_frame
+    A.invH = (float)GRID_ROWS / (float)(rf->max_y - rf->min_y);
+    A.keys = rf->keys; A.desc = rf->desc; A.u_right = rf->u_right; A.scale_factors = rf->sf;
+    A.cell_start = rf->cell_start; A.cell_idx = rf->cell_idx;
+}
+}  // namespace
+
+borb_status borb_search_local_points_batch(borb_matcher* m, const borb_local_points_job* jobs, int n_jobs, float viewing_cos_limit,
+                                           float nnratio, int32_t* n_matches) {
+    if (!m || n_jobs < 0 || (n_jobs > 0 && (!jobs || !n_matches))) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+    if (n_jobs == 0) return BORB_OK;
+    // nq = valid points (m->sel[sel0 .. sel0 + nq)); search = nq > 0 on a frame with features (otherwise only isInFrustum runs)
+    struct JobOff { size_t sel0, wp, md, obs, mx, mn, nr, occ, rad, ang, minl, maxl, cand, cc, res; int nq; bool gather, search; };
+    std::vector<JobOff> J(n_jobs);
+    std::vector<int32_t>& sel = m->sel;
+    sel.clear();
+    int max_nq = 0, max_n = 1, max_n_mp = 0;
+    for (int j = 0; j < n_jobs; j++) {
+        const borb_local_points_job& B = jobs[j];
+        const borb_frame_view* F = &B.frame;
+        const borb_worldpoints_view& P = B.pts;
+        J[j] = JobOff{};
+        J[j].sel0 = sel.size();
+        n_matches[j] = 0;
+        if (!F->resident) { set_error("job %d: borb_search_local_points_batch needs device-resident frames (borb_frame_view::resident)", j); return BORB_ERR_INVALID_ARG; }
+        const FrameInfo I = frame_info(F);
+        borb_status s = check_frame(F, I, m);
+        if (s != BORB_OK) return job_error(j, s);
+        if (!B.in_view || !B.match_feat) { set_error("job %d: null output", j); return BORB_ERR_INVALID_ARG; }
+        const int n_all = P.n;
+        if (n_all < 0) { set_error("job %d: negative point count", j); return BORB_ERR_INVALID_ARG; }
+        for (int i = 0; i < n_all; i++) {
+            B.in_view[i] = 0; B.match_feat[i] = -1;
+            if (B.proj_x) B.proj_x[i] = 0.f;
+            if (B.proj_y) B.proj_y[i] = 0.f;
+            if (B.proj_xr) B.proj_xr[i] = 0.f;
+            if (B.level) B.level[i] = 0;
+            if (B.view_cos) B.view_cos[i] = 0.f;
+        }
+        if (n_all == 0) continue;
+        if (!P.world_pos || !P.desc || !P.max_distance || !P.min_distance || !P.normal) { set_error("job %d: incomplete world-points view", j); return BORB_ERR_INVALID_ARG; }
+        if (!(B.log_scale_factor > 0.f)) { set_error("job %d: log_scale_factor must be positive (Frame::mfLogScaleFactor)", j); return BORB_ERR_INVALID_ARG; }
+        for (int i = 0; i < n_all; i++)
+            if (!P.valid || P.valid[i]) sel.push_back(i);
+        const int nq = (int)(sel.size() - J[j].sel0);
+        if (nq > MATCH_MAX_FEATURES) { set_error("job %d: %d valid local map points (limit %d per call)", j, nq, MATCH_MAX_FEATURES); return BORB_ERR_INVALID_ARG; }
+        J[j].nq = nq; J[j].gather = nq != n_all; J[j].search = nq > 0 && I.n > 0;
+        if (nq > max_nq) max_nq = nq;
+        if (J[j].search) { max_n = std::max(max_n, I.n); max_n_mp = std::max(max_n_mp, nq); }
+    }
+    if (max_nq == 0) return BORB_OK;
+    BORB_CUDA(cudaSetDevice(m->device));
+    Stager st(m);
+    for (int j = 0; j < n_jobs; j++) {
+        const borb_local_points_job& B = jobs[j];
+        const borb_worldpoints_view& P = B.pts;
+        const size_t nq = (size_t)J[j].nq;
+        if (nq == 0) continue;
+        const bool g = J[j].gather;                 // gathered inputs are written into the staging buffer once the layout is known
+        J[j].wp = st.add(g ? nullptr : P.world_pos, nq * 12); J[j].md = st.add(g ? nullptr : P.desc, nq * 32);
+        J[j].obs = B.has_obs ? st.add(g ? nullptr : B.has_obs, nq) : 0;
+        J[j].mx = st.add(g ? nullptr : P.max_distance, nq * 4); J[j].mn = st.add(g ? nullptr : P.min_distance, nq * 4);
+        J[j].nr = st.add(g ? nullptr : P.normal, nq * 12);
+        J[j].occ = (J[j].search && B.frame.occupied) ? st.add(B.frame.occupied, (size_t)B.frame.resident->n) : 0;
+    }
+    const size_t o_last = st.add(nullptr, (size_t)n_jobs * sizeof(LastArgs)), o_jobs = st.add(nullptr, (size_t)n_jobs * sizeof(ProjArgs));
+    const size_t input_end = st.off;
+    // results of every job in one region, per job as in borb_search_local_points: px | py | pxr | level | viewcos | match | nm | valid
+    size_t res_bytes = 0;
+    for (int j = 0; j < n_jobs; j++) {
+        const size_t nq = (size_t)J[j].nq;
+        if (nq == 0) continue;
+        J[j].rad = st.reserve(nq * 4); J[j].ang = st.reserve(nq * 4); J[j].minl = st.reserve(nq * 4); J[j].maxl = st.reserve(nq * 4);
+        if (J[j].search) { J[j].cand = st.reserve(nq * (size_t)jobs[j].frame.resident->n * 4); J[j].cc = st.reserve(nq * 4); }
+        J[j].res = res_bytes; res_bytes += (nq * 25 + 16 + 15) & ~size_t(15);
+    }
+    const size_t o_res = st.reserve(res_bytes);
+    const size_t total = st.off;
+    st.off = input_end;
+    borb_status s;
+    if ((s = ensure_host(m, input_end)) != BORB_OK) return s;
+    if ((s = ensure_arena(m, total)) != BORB_OK) return s;
+    if ((s = ensure_out(m, res_bytes)) != BORB_OK) return s;
+    BORB_CUDA(cudaStreamSynchronize(m->stream));       // the staging buffer may still feed an earlier copy
+    uint8_t* b = m->arena;
+    uint8_t* h = m->h_stage;
+    LastArgs* hl = reinterpret_cast<LastArgs*>(h + o_last);
+    ProjArgs* hj = reinterpret_cast<ProjArgs*>(h + o_jobs);
+    for (int j = 0; j < n_jobs; j++) {
+        const borb_local_points_job& B = jobs[j];
+        const borb_worldpoints_view& P = B.pts;
+        const int nq = J[j].nq;
+        LastArgs L{};
+        ProjArgs A{};
+        if (nq > 0) {
+            const JobOff& O = J[j];
+            if (O.gather)
+                for (int k = 0; k < nq; k++) {
+                    const int i = sel[O.sel0 + k];
+                    std::memcpy(h + O.wp + (size_t)k * 12, P.world_pos + (size_t)i * 3, 12);
+                    std::memcpy(h + O.md + (size_t)k * 32, P.desc + (size_t)i * 32, 32);
+                    if (B.has_obs) h[O.obs + k] = B.has_obs[i];
+                    std::memcpy(h + O.mx + (size_t)k * 4, P.max_distance + i, 4);
+                    std::memcpy(h + O.mn + (size_t)k * 4, P.min_distance + i, 4);
+                    std::memcpy(h + O.nr + (size_t)k * 12, P.normal + (size_t)i * 3, 12);
+                }
+            const borb_frame* rf = B.frame.resident;
+            uint8_t* r = b + o_res + O.res;
+            L.variant = 3; L.n_last = nq; L.world_pos = (const float*)(b + O.wp);
+            L.max_distance = (const float*)(b + O.mx); L.min_distance = (const float*)(b + O.mn); L.normal = (const float*)(b + O.nr);
+            for (int i = 0; i < 3; i++) L.Ow[i] = B.Ow[i];
+            L.log_scale = B.log_scale_factor; L.n_levels = rf->n_levels; L.view_cos_limit = viewing_cos_limit;
+            L.valid_in = nullptr;
+            for (int i = 0; i < 12; i++) L.T[i] = B.Tcw[i];
+            L.fx = B.fx; L.fy = B.fy; L.cx = B.cx; L.cy = B.cy; L.bf = B.mbf; L.th = B.th;
+            L.minX = rf->min_x; L.minY = rf->min_y; L.maxX = rf->max_x; L.maxY = rf->max_y;
+            L.scale_factors = rf->sf;
+            L.proj_x = (float*)r; L.proj_y = L.proj_x + nq; L.proj_xr = L.proj_y + nq;
+            L.level_out = (int32_t*)(L.proj_xr + nq); L.viewcos_out = (float*)(L.level_out + nq);
+            L.valid_out = r + (size_t)nq * 24 + 16;
+            L.radius = (float*)(b + O.rad); L.angle = (float*)(b + O.ang); L.minl = (int32_t*)(b + O.minl); L.maxl = (int32_t*)(b + O.maxl);
+            if (O.search) {
+                bind_resident(rf, A);
+                A.occupied = B.frame.occupied ? b + O.occ : nullptr;
+                A.n_mp = nq; A.proj_x = L.proj_x; A.proj_y = L.proj_y; A.proj_xr = L.proj_xr; A.view_cos = L.viewcos_out; A.level = L.level_out;
+                A.mp_desc = b + O.md; A.mp_valid = L.valid_out; A.mp_has_obs = B.has_obs ? b + O.obs : nullptr;
+                A.th = B.th; A.nnratio = nnratio; A.th_dist = TH_HIGH;
+                A.cand = (uint32_t*)(b + O.cand); A.cand_cnt = (int*)(b + O.cc);
+                A.mode = 0;
+                A.out_match = (int32_t*)(L.viewcos_out + nq);
+            }                                        // a frame without features keeps n_mp = 0: candidates and resolve skip it
+        }                                            // a job without valid points keeps n_last = 0 as well
+        hl[j] = L;
+        hj[j] = A;
+    }
+    if ((s = commit(st, total)) != BORB_OK) return s;
+    BORB_CUDA(cudaMemsetAsync(b + o_res, 0, res_bytes, m->stream));     // level | viewcos of points outside the frustum read as 0
+    for (int j = 0; j < n_jobs; j++) BORB_CUDA(cudaStreamWaitEvent(m->stream, jobs[j].frame.resident->ready, 0));
+    m->launches += launch_point_projection_batch((const LastArgs*)(b + o_last), (const ProjArgs*)(b + o_jobs), n_jobs, max_nq, max_n, max_n_mp,
+                                                 false, m->stream);
+    BORB_CUDA(cudaGetLastError());
+    BORB_CUDA(cudaMemcpyAsync(m->h_out, b + o_res, res_bytes, cudaMemcpyDeviceToHost, m->stream));
+    BORB_CUDA(cudaStreamSynchronize(m->stream));
+    for (int j = 0; j < n_jobs; j++) {
+        const borb_local_points_job& B = jobs[j];
+        const int nq = J[j].nq;
+        if (nq == 0) continue;
+        const uint8_t* r = m->h_out + J[j].res;
+        const float* rpx = (const float*)r; const float* rpy = rpx + nq; const float* rpxr = rpy + nq;
+        const int32_t* rlvl = (const int32_t*)(rpxr + nq); const float* rvc = (const float*)(rlvl + nq);
+        const int32_t* rmatch = (const int32_t*)(rvc + nq);
+        const uint8_t* rval = r + (size_t)nq * 24 + 16;
+        const bool search = J[j].search;
+        if (search) n_matches[j] = *(const int32_t*)(rmatch + nq);
+        for (int k = 0; k < nq; k++) {
+            const int i = sel[J[j].sel0 + k];
+            B.in_view[i] = rval[k];
+            if (search) B.match_feat[i] = rmatch[k];
+            if (B.proj_x) B.proj_x[i] = rpx[k];
+            if (B.proj_y) B.proj_y[i] = rpy[k];
+            if (B.proj_xr) B.proj_xr[i] = rpxr[k];
+            if (B.level) B.level[i] = rlvl[k];
+            if (B.view_cos) B.view_cos[i] = rvc[k];
+        }
+    }
+    return BORB_OK;
+}
+
+borb_status borb_search_by_projection_last_batch(borb_matcher* m, const borb_last_frame_job* jobs, int n_jobs, int check_orientation,
+                                                 int32_t* n_matches) {
+    if (!m || n_jobs < 0 || (n_jobs > 0 && (!jobs || !n_matches))) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+    if (n_jobs == 0) return BORB_OK;
+    struct JobOff { size_t lk, wp, md, vin, obs, occ, px, py, pxr, rad, ang, minl, maxl, val, cand, cc, evi, evb, res; int n, nq; };
+    std::vector<JobOff> J(n_jobs);
+    int max_n = 1, max_nq = 0;
+    for (int j = 0; j < n_jobs; j++) {
+        const borb_last_frame_job& B = jobs[j];
+        const borb_frame_view* F = &B.cur;
+        const borb_lastframe_view& Lf = B.last;
+        J[j] = JobOff{};
+        n_matches[j] = 0;
+        if (!F->resident) { set_error("job %d: borb_search_by_projection_last_batch needs device-resident frames (borb_frame_view::resident)", j); return BORB_ERR_INVALID_ARG; }
+        const FrameInfo I = frame_info(F);
+        borb_status s = check_frame(F, I, m);
+        if (s != BORB_OK) return job_error(j, s);
+        if (!B.state_cur) { set_error("job %d: null output", j); return BORB_ERR_INVALID_ARG; }
+        if (Lf.n < 0 || Lf.n > MATCH_MAX_FEATURES) { set_error("job %d: %d query points (limit %d per call)", j, Lf.n, MATCH_MAX_FEATURES); return BORB_ERR_INVALID_ARG; }
+        for (int i = 0; i < I.n; i++) B.state_cur[i] = -1;
+        if (I.n == 0 || Lf.n == 0) continue;
+        if (!Lf.world_pos || !Lf.desc) { set_error("job %d: incomplete query view", j); return BORB_ERR_INVALID_ARG; }
+        if (!Lf.keys_un) { set_error("job %d: incomplete last-frame view", j); return BORB_ERR_INVALID_ARG; }
+        for (int i = 0; i < Lf.n; i++)
+            if (Lf.keys_un[i].octave < 0 || Lf.keys_un[i].octave >= I.n_levels) { set_error("job %d: last-frame keypoint %d: octave out of range", j, i); return BORB_ERR_INVALID_ARG; }
+        J[j].n = I.n; J[j].nq = Lf.n;
+        max_n = std::max(max_n, I.n); max_nq = std::max(max_nq, Lf.n);
+    }
+    if (max_nq == 0) return BORB_OK;
+    BORB_CUDA(cudaSetDevice(m->device));
+    Stager st(m);
+    for (int j = 0; j < n_jobs; j++) {
+        const borb_last_frame_job& B = jobs[j];
+        const size_t nq = (size_t)J[j].nq;
+        if (nq == 0) continue;
+        J[j].lk = st.add(B.last.keys_un, nq * sizeof(borb_keypoint)); J[j].wp = st.add(B.last.world_pos, nq * 12);
+        J[j].md = st.add(B.last.desc, nq * 32);
+        J[j].vin = B.last.valid ? st.add(B.last.valid, nq) : 0;
+        J[j].obs = B.last.has_obs ? st.add(B.last.has_obs, nq) : 0;
+        J[j].occ = B.cur.occupied ? st.add(B.cur.occupied, (size_t)J[j].n) : 0;
+    }
+    const size_t o_last = st.add(nullptr, (size_t)n_jobs * sizeof(LastArgs)), o_jobs = st.add(nullptr, (size_t)n_jobs * sizeof(ProjArgs));
+    const size_t input_end = st.off;
+    size_t res_bytes = 0;                        // every job's state (cur n entries) and match count, in one region
+    for (int j = 0; j < n_jobs; j++) {
+        const size_t nq = (size_t)J[j].nq;
+        if (nq == 0) continue;
+        J[j].px = st.reserve(nq * 4); J[j].py = st.reserve(nq * 4); J[j].pxr = st.reserve(nq * 4); J[j].rad = st.reserve(nq * 4);
+        J[j].ang = st.reserve(nq * 4); J[j].minl = st.reserve(nq * 4); J[j].maxl = st.reserve(nq * 4); J[j].val = st.reserve(nq);
+        J[j].cand = st.reserve(nq * (size_t)J[j].n * 4); J[j].cc = st.reserve(nq * 4);
+        J[j].evi = st.reserve(nq * 4); J[j].evb = st.reserve(nq);
+        J[j].res = res_bytes; res_bytes += ((size_t)J[j].n * 4 + 4 + 15) & ~size_t(15);
+    }
+    const size_t o_res = st.reserve(res_bytes);
+    const size_t total = st.off;
+    st.off = input_end;
+    borb_status s;
+    if ((s = ensure_host(m, input_end)) != BORB_OK) return s;
+    if ((s = ensure_arena(m, total)) != BORB_OK) return s;
+    if ((s = ensure_out(m, res_bytes)) != BORB_OK) return s;
+    BORB_CUDA(cudaStreamSynchronize(m->stream));
+    uint8_t* b = m->arena;
+    LastArgs* hl = reinterpret_cast<LastArgs*>(m->h_stage + o_last);
+    ProjArgs* hj = reinterpret_cast<ProjArgs*>(m->h_stage + o_jobs);
+    for (int j = 0; j < n_jobs; j++) {
+        const borb_last_frame_job& B = jobs[j];
+        const JobOff& O = J[j];
+        LastArgs L{};
+        ProjArgs A{};
+        if (O.nq > 0) {                              // as run_point_projection, variant 0
+            const borb_frame* rf = B.cur.resident;
+            L.variant = 0;
+            L.n_last = O.nq; L.last_keys = (const borb_keypoint*)(b + O.lk); L.world_pos = (const float*)(b + O.wp);
+            L.n_levels = rf->n_levels;
+            L.valid_in = B.last.valid ? b + O.vin : nullptr;
+            for (int i = 0; i < 12; i++) L.T[i] = B.Tcw[i];
+            L.fx = B.fx; L.fy = B.fy; L.cx = B.cx; L.cy = B.cy; L.bf = B.bf; L.th = B.th;
+            L.minX = rf->min_x; L.minY = rf->min_y; L.maxX = rf->max_x; L.maxY = rf->max_y;
+            L.scale_factors = rf->sf;
+            L.forward = B.forward; L.backward = B.backward;
+            L.proj_x = (float*)(b + O.px); L.proj_y = (float*)(b + O.py); L.proj_xr = (float*)(b + O.pxr); L.radius = (float*)(b + O.rad);
+            L.angle = (float*)(b + O.ang); L.minl = (int32_t*)(b + O.minl); L.maxl = (int32_t*)(b + O.maxl); L.valid_out = b + O.val;
+            bind_resident(rf, A);
+            A.occupied = B.cur.occupied ? b + O.occ : nullptr;
+            A.n_mp = O.nq; A.proj_x = L.proj_x; A.proj_y = L.proj_y; A.proj_xr = L.proj_xr;
+            A.mp_desc = b + O.md; A.mp_valid = L.valid_out; A.mp_has_obs = B.last.has_obs ? b + O.obs : nullptr;
+            A.th = B.th; A.nnratio = 0.f;
+            A.cand = (uint32_t*)(b + O.cand); A.cand_cnt = (int*)(b + O.cc);
+            A.q_radius = L.radius; A.q_minl = L.minl; A.q_maxl = L.maxl; A.mode = 1; A.check_ori = check_orientation; A.q_angle = L.angle;
+            A.th_dist = 100;                                                   // TH_HIGH (:1426)
+            A.q_valid_out = L.valid_out;
+            A.out_match = (int32_t*)(b + o_res + O.res);
+            A.ev_idx = (int32_t*)(b + O.evi); A.ev_bin = b + O.evb;
+        }                                            // a job without work keeps n_last = n_mp = 0: every kernel skips it
+        hl[j] = L;
+        hj[j] = A;
+    }
+    if ((s = commit(st, total)) != BORB_OK) return s;
+    for (int j = 0; j < n_jobs; j++) BORB_CUDA(cudaStreamWaitEvent(m->stream, jobs[j].cur.resident->ready, 0));
+    m->launches += launch_point_projection_batch((const LastArgs*)(b + o_last), (const ProjArgs*)(b + o_jobs), n_jobs, max_nq, max_n, max_nq,
+                                                 true, m->stream);
+    BORB_CUDA(cudaGetLastError());
+    BORB_CUDA(cudaMemcpyAsync(m->h_out, b + o_res, res_bytes, cudaMemcpyDeviceToHost, m->stream));
+    BORB_CUDA(cudaStreamSynchronize(m->stream));
+    for (int j = 0; j < n_jobs; j++) {
+        const JobOff& O = J[j];
+        if (O.nq == 0) continue;
+        std::memcpy(jobs[j].state_cur, m->h_out + O.res, (size_t)O.n * 4);
+        std::memcpy(&n_matches[j], m->h_out + O.res + (size_t)O.n * 4, 4);
+    }
+    return BORB_OK;
+}
+
 borb_status borb_search_for_initialization(borb_matcher* m, const borb_frame_view* f1, const borb_frame_view* f2, float* prev_matched,
                                            int window_size, float nnratio, int check_orientation, int32_t* matches12, int32_t* n_matches) {
     if (!m || !f1 || !f2 || !prev_matched || !matches12 || !n_matches) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }

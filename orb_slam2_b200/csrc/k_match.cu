@@ -146,10 +146,9 @@ __device__ __forceinline__ int predict_scale(float max_distance, float dist, flo
     return nScale;
 }
 
-// Projection of the query points with the 3x4 pose, for the three SearchByProjection overloads that take world points.
-__global__ void __launch_bounds__(256) project_points_kernel(LastArgs L) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= L.n_last) return;
+// Projection of query point i with the 3x4 pose, for the three SearchByProjection overloads that take world points and for
+// Frame::isInFrustum.
+__device__ __forceinline__ void project_point(const LastArgs& L, int i) {
     bool ok = L.valid_in == nullptr || L.valid_in[i] != 0;
     float u = 0.f, v = 0.f, ur = 0.f, radius = 0.f, ang = 0.f;
     int minl = 0, maxl = -1;
@@ -233,6 +232,18 @@ __global__ void __launch_bounds__(256) project_points_kernel(LastArgs L) {
     L.proj_x[i] = u; L.proj_y[i] = v; L.proj_xr[i] = ur; L.radius[i] = radius; L.minl[i] = minl; L.maxl[i] = maxl;
     L.angle[i] = ang;
     L.valid_out[i] = ok ? 1 : 0;
+}
+
+__global__ void __launch_bounds__(256) project_points_kernel(LastArgs L) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < L.n_last) project_point(L, i);
+}
+// one launch for many independent jobs (borb_search_local_points_batch / borb_search_by_projection_last_batch): grid.y = job,
+// the job's arguments come from device memory; a job without points has n_last = 0
+__global__ void __launch_bounds__(256) project_points_batch_kernel(const LastArgs* __restrict__ jobs) {
+    const LastArgs& L = jobs[blockIdx.y];
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < L.n_last) project_point(L, i);
 }
 
 // SearchForInitialization (:405-520): one warp replays F1's level-0 features in order.  A candidate i2 is skipped
@@ -786,6 +797,12 @@ int launch_distinctive(const uint8_t* desc, const int32_t* offsets, int n_points
 int launch_frustum_projection(const LastArgs& L, const ProjArgs& A, int32_t* match_feat, int* n_matches, cudaStream_t s) {
     if (L.n_last > 0) project_points_kernel<<<(L.n_last + 255) / 256, 256, 0, s>>>(L);
     return 1 + launch_projection(A, match_feat, n_matches, s);
+}
+int launch_point_projection_batch(const LastArgs* d_last, const ProjArgs* d_jobs, int n_jobs, int max_nq, int max_n, int max_n_mp, bool last,
+                                  cudaStream_t s) {
+    if (n_jobs <= 0 || max_nq <= 0) return 0;
+    project_points_batch_kernel<<<dim3((max_nq + 255) / 256, n_jobs), 256, 0, s>>>(d_last);
+    return 1 + launch_projection_batch(d_jobs, n_jobs, max_n, max_n_mp, s, last);
 }
 int launch_projection_argmin(const LastArgs& L, const ProjArgs& A, int32_t* best_idx, int* n_found, cudaStream_t s) {
     cudaMemsetAsync(n_found, 0, sizeof(int), s);

@@ -331,24 +331,32 @@ __global__ void __launch_bounds__(1024) proj_resolve_kernel(ProjArgs A, const bo
                                                            int32_t* __restrict__ ev_idx, uint8_t* __restrict__ ev_bin, int* __restrict__ n_matches) {
     resolve_body<LAST>(A, cur_keys, out, ev_idx, ev_bin, n_matches);
 }
-// a CTA per job (SearchByProjection(F, vpMapPoints) of many independent frames in one launch)
+// a CTA per job (SearchByProjection(F, vpMapPoints) or (CurrentFrame, LastFrame) of many independent frames in one launch);
+// the block size follows the largest job, and the wave fixpoint is the sequential result for any block size
+template <bool LAST>
 __global__ void __launch_bounds__(1024) proj_resolve_batch_kernel(const ProjArgs* __restrict__ jobs) {
     const ProjArgs& A = jobs[blockIdx.x];
     if (A.n_mp <= 0) return;                        // a job without work (no MapPoints / empty frame) carries null pointers
-    resolve_body<false>(A, A.keys, A.out_match, nullptr, nullptr, reinterpret_cast<int*>(A.out_match + A.n_mp));
+    const int n_out = LAST ? A.n : A.n_mp;          // out_match: the per-feature state (LAST) or per-query match, then the count
+    resolve_body<LAST>(A, A.keys, A.out_match, A.ev_idx, A.ev_bin, reinterpret_cast<int*>(A.out_match + n_out));
 }
 
 void launch_candidates(const ProjArgs& A, cudaStream_t s) {
     if (A.n_mp > 0) proj_candidates_kernel<<<(A.n_mp + 7) / 8, 256, 0, s>>>(A);
 }
 
-int launch_projection_batch(const ProjArgs* d_jobs, int n_jobs, int max_n, int max_n_mp, cudaStream_t s) {
+int launch_projection_batch(const ProjArgs* d_jobs, int n_jobs, int max_n, int max_n_mp, cudaStream_t s, bool last) {
     if (n_jobs <= 0 || max_n_mp <= 0) return 0;
     proj_candidates_batch_kernel<<<dim3((max_n_mp + 7) / 8, n_jobs), 256, 0, s>>>(d_jobs);
     const size_t smem = resolve_smem_bytes(max_n, max_n_mp);
     const int threads = max_n_mp > 512 ? 1024 : (max_n_mp > 256 ? 512 : 256);
-    allow_max_smem((const void*)proj_resolve_batch_kernel);
-    proj_resolve_batch_kernel<<<n_jobs, threads, smem, s>>>(d_jobs);
+    if (last) {
+        allow_max_smem((const void*)proj_resolve_batch_kernel<true>);
+        proj_resolve_batch_kernel<true><<<n_jobs, threads, smem, s>>>(d_jobs);
+    } else {
+        allow_max_smem((const void*)proj_resolve_batch_kernel<false>);
+        proj_resolve_batch_kernel<false><<<n_jobs, threads, smem, s>>>(d_jobs);
+    }
     return 2;
 }
 

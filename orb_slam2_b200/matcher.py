@@ -49,8 +49,29 @@ class _KeyFrameViewC(C.Structure):
                 ("fv", _FeatVecC), ("n_levels", C.c_int32), ("scale_factors", C.c_void_p), ("level_sigma2", C.c_void_p)]
 
 
+class _LocalPointsJobC(C.Structure):               # borb_local_points_job
+    _fields_ = [("frame", _FrameViewC), ("pts", _WorldPointsViewC), ("has_obs", C.c_void_p), ("Tcw", C.c_float * 12), ("Ow", C.c_float * 3)] + \
+               [(n, C.c_float) for n in ("fx", "fy", "cx", "cy", "mbf", "log_scale_factor", "th")] + \
+               [(n, C.c_void_p) for n in ("in_view", "proj_x", "proj_y", "proj_xr", "level", "view_cos", "match_feat")]
+
+
+class _LastFrameJobC(C.Structure):                 # borb_last_frame_job
+    _fields_ = [("cur", _FrameViewC), ("last", _LastFrameViewC), ("Tcw", C.c_float * 12)] + \
+               [(n, C.c_float) for n in ("fx", "fy", "cx", "cy", "bf", "th")] + \
+               [("forward", C.c_int32), ("backward", C.c_int32), ("state_cur", C.c_void_p)]
+
+
 def _p(a):
     return a.ctypes.data if a is not None else None
+
+
+def _per_job(x, n, ndim=0):
+    """A per-job sequence, or one value (of `ndim` dimensions) for every job."""
+    return list(x) if np.ndim(x) > ndim else [x] * n
+
+
+def _pose12(Tcw):
+    return (C.c_float * 12)(*np.asarray(Tcw, np.float32)[:3, :4].reshape(12).tolist())
 
 
 @dataclass
@@ -396,6 +417,74 @@ class ORBmatcher:
         out = {k: v[:nq] for k, v in out.items()}
         out["nmatches"] = nm.value
         return out
+
+    def SearchLocalPointsBatch(self, frames: Sequence[FrameView], points: Sequence[WorldPointsView], poses, K, mbf, th=1.0,
+                               has_obs=None, viewingCosLimit: float = 0.5):
+        """borb_search_local_points_batch: SearchLocalPoints of many independent camera streams (device-resident frames) in one
+        launch sequence.  poses[j] = (Tcw, Ow); K (fx, fy, cx, cy), mbf and th are one value for every job or one per job; has_obs is
+        None or a per-job list (entries may be None).  Returns one dict per job, equal to what SearchLocalPoints returns."""
+        n = len(frames)
+        assert n == len(points) == len(poses)
+        Ks, bfs, ths = _per_job(K, n, 1), _per_job(mbf, n), _per_job(th, n)
+        obs = list(has_obs) if has_obs is not None else [None] * n
+        jobs = (_LocalPointsJobC * max(n, 1))()
+        keep, outs = [], []
+        for j in range(n):
+            fv, pv, logs, _, k = self._points_call(frames[j], points[j], with_stereo=True)
+            ho = np.ascontiguousarray(obs[j], np.uint8) if obs[j] is not None else None
+            nq = len(points[j].world_pos)
+            m1 = max(nq, 1)
+            out = dict(in_view=np.zeros(m1, np.uint8), proj_x=np.zeros(m1, np.float32), proj_y=np.zeros(m1, np.float32),
+                       proj_xr=np.zeros(m1, np.float32), level=np.zeros(m1, np.int32), view_cos=np.zeros(m1, np.float32),
+                       match=np.full(m1, -1, np.int32))
+            Tcw, Ow = poses[j]
+            J = jobs[j]
+            J.frame, J.pts, J.has_obs, J.Tcw = fv, pv, _p(ho), _pose12(Tcw)
+            J.Ow = (C.c_float * 3)(*np.asarray(Ow, np.float32).reshape(3).tolist())
+            J.fx, J.fy, J.cx, J.cy = [float(x) for x in Ks[j]]
+            J.mbf, J.log_scale_factor, J.th = float(bfs[j]), logs, float(ths[j])
+            J.in_view, J.proj_x, J.proj_y, J.proj_xr = _p(out["in_view"]), _p(out["proj_x"]), _p(out["proj_y"]), _p(out["proj_xr"])
+            J.level, J.view_cos, J.match_feat = _p(out["level"]), _p(out["view_cos"]), _p(out["match"])
+            keep.append((k, ho)); outs.append((nq, out))
+        nm = np.zeros(max(n, 1), np.int32)
+        check(self._lib.borb_search_local_points_batch(self._h, jobs, n, float(viewingCosLimit), self.mfNNratio, _p(nm)),
+              "borb_search_local_points_batch")
+        res = []
+        for j, (nq, out) in enumerate(outs):
+            r = {k: v[:nq] for k, v in out.items()}
+            r["nmatches"] = int(nm[j])
+            res.append(r)
+        return res
+
+    def SearchByProjectionLastBatch(self, curs: Sequence[FrameView], lasts: Sequence[LastFrameView], poses, K, bf, th,
+                                    forward=False, backward=False):
+        """borb_search_by_projection_last_batch: SearchByProjection(CurrentFrame, LastFrame, th, bMono) of many independent camera
+        streams (device-resident current frames) in one launch sequence.  poses[j] = Tcw; K, bf, th, forward and backward are one
+        value for every job or one per job.  Returns [(nmatches, state)] per job, equal to what SearchByProjectionLast returns."""
+        n = len(curs)
+        assert n == len(lasts) == len(poses)
+        Ks, bfs, ths = _per_job(K, n, 1), _per_job(bf, n), _per_job(th, n)
+        fws, bws = _per_job(forward, n), _per_job(backward, n)
+        jobs = (_LastFrameJobC * max(n, 1))()
+        keep, outs = [], []
+        for j in range(n):
+            fv, k = curs[j]._view()
+            L = lasts[j]
+            lk = np.ascontiguousarray(L.mvKeysUn, KP_DTYPE); wp = np.ascontiguousarray(L.world_pos, np.float32)
+            ld = np.ascontiguousarray(L.descriptors, np.uint8)
+            va = np.ascontiguousarray(L.valid, np.uint8) if L.valid is not None else None
+            ho = np.ascontiguousarray(L.has_obs, np.uint8) if L.has_obs is not None else None
+            n_cur = len(curs[j].mvKeysUn)
+            state = np.full(max(n_cur, 1), -1, np.int32)
+            J = jobs[j]
+            J.cur, J.last, J.Tcw = fv, _LastFrameViewC(len(lk), _p(lk), _p(wp), _p(ld), _p(va), _p(ho)), _pose12(poses[j])
+            J.fx, J.fy, J.cx, J.cy = [float(x) for x in Ks[j]]
+            J.bf, J.th, J.forward, J.backward, J.state_cur = float(bfs[j]), float(ths[j]), int(fws[j]), int(bws[j]), _p(state)
+            keep.append((k, lk, wp, ld, va, ho)); outs.append((n_cur, state))
+        nm = np.zeros(max(n, 1), np.int32)
+        check(self._lib.borb_search_by_projection_last_batch(self._h, jobs, n, int(self.mbCheckOrientation), _p(nm)),
+              "borb_search_by_projection_last_batch")
+        return [(int(nm[j]), state[:n_cur]) for j, (n_cur, state) in enumerate(outs)]
 
     def SearchForInitialization(self, F1: FrameView, F2: FrameView, vbPrevMatched: np.ndarray, windowSize: int = 10):
         """SearchForInitialization(F1, F2, vbPrevMatched, vnMatches12, windowSize) — src/ORBmatcher.cc:405-520.

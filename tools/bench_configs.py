@@ -2,13 +2,17 @@
    config 2: RGB-D TUM-shaped 640x480 extract + SearchByProjection against 300 local MapPoints — us per call;
    config 4: EuRoC-shaped 752x480 @1200 features, loop-closure / relocalisation against a 2000-keyframe database:
              one KeyFrameDatabase query (shared words + L1 score for all keyframes) and SearchByBoW against all
-             2000 resident keyframes.
+             2000 resident keyframes;
+   tracking tick of N streams: the motion-model search (SearchByProjection(CurrentFrame, LastFrame)) plus the local-map search
+             (Tracking::SearchLocalPoints) of N TUM-shaped 640x480 @1000 streams with a few hundred to ~2000 local MapPoints each,
+             as N single calls of each search and as one batched call of each, for N in 1, 8, 32.
 All times are wall-clock around the public Python call (host buffers in, results out), median of `--reps`, taken right
 after a burst of extraction work so that the SM clocks are where a running tracker keeps them.
 usage: python tools/bench_configs.py [--kfs 2000] [--reps 20]  -> one JSON line per config on stdout."""
 import argparse
 import json
 import os
+import subprocess
 import sys
 import time
 
@@ -113,6 +117,69 @@ def config4(n_kf, reps):
             "search_by_bow_top20_us": t_bow20 * 1e6}
 
 
+def gpu_name_and_power_limit():
+    """Read-only query of the card the numbers were measured on."""
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True,
+                             timeout=30).stdout.strip().splitlines()
+        return out[0] if out else "unknown"
+    except (OSError, subprocess.SubprocessError):
+        return "unknown"
+
+
+def track_streams(reps, ns=(1, 8, 32)):
+    X = ORBextractor(1000)
+    n_max = max(ns)
+    outs = X.extract_batch([synth.mono_frame(200 + i, 0, 0, 640, 480) for i in range(n_max)])
+    sf = np.asarray(X.GetScaleFactors(), np.float32)
+    K, bf = (525.0, 525.0, 319.5, 239.5), 40.0
+    T = np.eye(4, dtype=np.float32)[:3]
+    Ow = np.zeros(3, np.float32)
+    mt = M.ORBmatcher(0.8, True)
+    rng = np.random.default_rng(2)
+    frames, lasts, points = [], [], []
+    for i, (k, d) in enumerate(outs):
+        n = len(k)
+        z = rng.uniform(2.0, 20.0, n).astype(np.float32)
+        Pw = np.stack([(k["x"] - K[2]) * z / K[0], (k["y"] - K[3]) * z / K[1], z], 1).astype(np.float32)
+        frames.append(M.FrameView(k, d, sf, (0.0, 0.0, 640.0, 480.0)).make_resident(mt))
+        lasts.append(M.LastFrameView(mvKeysUn=k, world_pos=Pw, descriptors=d))
+        # local map: the frame's own points (in view) and, for the larger maps, points beside the view that isInFrustum rejects
+        n_lp = 300 + (i * 389) % 1700
+        n_in = min(n_lp, n)
+        extra = n_lp - n_in
+        side = np.stack([rng.uniform(30, 60, extra), rng.uniform(-5, 5, extra), rng.uniform(2, 20, extra)], 1).astype(np.float32)
+        Pl = np.concatenate([Pw[:n_in], side]).astype(np.float32)
+        dist = np.linalg.norm(Pl.astype(np.float64), axis=1)
+        octv = np.concatenate([k["octave"][:n_in], np.zeros(extra, np.int32)])
+        maxd = (dist * sf[octv] * 0.95).astype(np.float32)
+        desc = np.concatenate([d[:n_in], d[:extra] if extra <= n else np.resize(d, (extra, 32))]).astype(np.uint8)
+        points.append(M.WorldPointsView(world_pos=Pl, descriptors=desc, max_distance=maxd, min_distance=(maxd / sf[-1]).astype(np.float32),
+                                        normal=(Pl / dist[:, None]).astype(np.float32)))
+    res = {}
+    for n in ns:
+        F, L, P = frames[:n], lasts[:n], points[:n]
+
+        def single():
+            m = 0
+            for j in range(n):
+                m += mt.SearchByProjectionLast(F[j], L[j], T, K, bf, 15.0)[0]
+                m += mt.SearchLocalPoints(F[j], P[j], T, Ow, K, bf, 1.0)["nmatches"]
+            return m
+
+        def batched():
+            m = sum(r[0] for r in mt.SearchByProjectionLastBatch(F, L, [T] * n, K, bf, 15.0))
+            return m + sum(r["nmatches"] for r in mt.SearchLocalPointsBatch(F, P, [(T, Ow)] * n, K, bf, 1.0))
+
+        assert single() == batched()
+        t_single, t_batch = med(single, reps), med(batched, reps)
+        res[str(n)] = {"single_calls_us": t_single * 1e6, "batched_us": t_batch * 1e6, "matches": int(batched()),
+                       "local_points": int(sum(len(p.world_pos) for p in P))}
+    return {"config": "tracking tick of N TUM-shaped 640x480 @1000 streams: SearchByProjection(CurrentFrame, LastFrame) + "
+                      "SearchLocalPoints (300-1999 local MapPoints per stream), per-tick host time of N single calls of each search vs "
+                      "one batched call of each", "gpu": gpu_name_and_power_limit(), "streams": res}
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--kfs", type=int, default=2000)
@@ -120,3 +187,4 @@ if __name__ == "__main__":
     a = ap.parse_args()
     print(json.dumps(config2(a.reps)), flush=True)
     print(json.dumps(config4(a.kfs, a.reps)), flush=True)
+    print(json.dumps(track_streams(a.reps)), flush=True)
