@@ -194,7 +194,7 @@ borb_status build_geometry(borb_extractor* e, int w, int h, std::vector<int16_t>
             v.x_windowed = resize_window_table(tabs, (size_t)v.xtab_off * 4, wpad, win) ? 1 : 0;
             tabs.insert(tabs.end(), win.begin(), win.end());
         }
-        if (quadtree_smem_bytes(v.node_cap) > 200 * 1024) {
+        if (quadtree_smem_bytes(v.node_cap) > 200 * 1024) {   // also keeps node_cap < 2^14, which the kernel's 16-bit node ids need
             set_error("per-level quota %d exceeds the quadtree kernel's shared-memory envelope", v.quota);
             return BORB_ERR_UNSUPPORTED;
         }
