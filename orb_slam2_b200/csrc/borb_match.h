@@ -64,10 +64,8 @@ struct ProjArgs {                 // device pointers
     int th_dist;                  // mode 1: accept bestDist <= th_dist (TH_HIGH / ORBdist / TH_LOW)
     int chi2;                     // 1: Fuse(pKF, vpMapPoints, th) reprojection gates per candidate (:907-931)
     const float* inv_sigma2;      // chi2: mvInvLevelSigma2
-    uint8_t* q_valid_out;         // mode 1: validity written by project_points_kernel (aliases mp_valid)
-    // batched launches (borb_search_by_projection_batch, borb_search_local_points_batch, borb_search_by_projection_last_batch):
-    // where this job's results go
-    int32_t* out_match;           // n_mp entries (mode 1: the per-feature state, n entries), then the match count
+    // where the resolve / argmin kernels write the results
+    int32_t* out_match;           // n_mp entries (mode 1 resolve: the per-feature state, n entries), then the match count
     int32_t* ev_idx;              // mode 1: match events of the rotation histogram, n_mp entries
     uint8_t* ev_bin;
 };
@@ -196,17 +194,16 @@ int launch_projection_batch(const ProjArgs* d_jobs, int n_jobs, int max_n, int m
 // project_points over a LastArgs table, then the batched candidates and resolve (last: resolve<true>) over a ProjArgs table
 int launch_point_projection_batch(const LastArgs* d_last, const ProjArgs* d_jobs, int n_jobs, int max_nq, int max_n, int max_n_mp, bool last,
                                   cudaStream_t s);
-void launch_resolve(const ProjArgs& A, bool last, int32_t* out, int32_t* ev_idx, uint8_t* ev_bin, int* n_matches, cudaStream_t s);
-int launch_projection(const ProjArgs& A, int32_t* match_feat, int* n_matches, cudaStream_t s);
-int launch_projection_last(const LastArgs& L, const ProjArgs& A, int32_t* state_cur, int32_t* hist_idx, uint8_t* hist_bin, int* n_matches,
-                           cudaStream_t s);
+void launch_resolve(const ProjArgs& A, bool last, cudaStream_t s);
+int launch_projection(const ProjArgs& A, cudaStream_t s);
+int launch_projection_last(const LastArgs& L, const ProjArgs& A, cudaStream_t s);
 int launch_initialization(const ProjArgs& A, const borb_keypoint* keys1, int n1, int32_t* match12, int32_t* ev_idx, uint8_t* ev_bin,
                           float* prev, int* n_matches, cudaStream_t s);
 int launch_kfdb_score(const BowDev* table, int n_slots, const uint32_t* qword, const double* qvalue, int nq, int32_t* common, float* score,
                       uint32_t* first_word, int n_sm, cudaStream_t s);
 int launch_distinctive(const uint8_t* desc, const int32_t* offsets, int n_points, int32_t* best_idx, cudaStream_t s);
-int launch_frustum_projection(const LastArgs& L, const ProjArgs& A, int32_t* match_feat, int* n_matches, cudaStream_t s);
-int launch_projection_argmin(const LastArgs& L, const ProjArgs& A, int32_t* best_idx, int* n_found, cudaStream_t s);
+int launch_frustum_projection(const LastArgs& L, const ProjArgs& A, cudaStream_t s);
+int launch_projection_argmin(const LastArgs& L, const ProjArgs& A, cudaStream_t s);
 int launch_sim3_agree(const int32_t* match1, const int32_t* match2, int n1, int n2, int32_t* match12, int* n_found, cudaStream_t s);
 int launch_bow_match(const KfDev* qs, const KfDev* ts, int n_pairs, int mode, float nnratio, int check_ori, int32_t* match,
                      int out_stride, uint8_t* bins, int32_t* n_matches, int max_t, cudaStream_t s);

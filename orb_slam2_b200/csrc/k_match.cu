@@ -323,7 +323,10 @@ __global__ void __launch_bounds__(32) init_resolve_kernel(ProjArgs A, const borb
 
 // Order-independent overloads (Fuse x2, the two directions of SearchBySim3): a warp per query point takes the
 // first minimum of its candidate list (dist < bestDist scan == lexicographic min of (distance, list position)).
-__global__ void __launch_bounds__(256) proj_argmin_kernel(ProjArgs A, int32_t* __restrict__ best_idx, int* __restrict__ n_found) {
+// out_match: the feature per query, then the count
+__global__ void __launch_bounds__(256) proj_argmin_kernel(ProjArgs A) {
+    int32_t* __restrict__ best_idx = A.out_match;
+    int* __restrict__ n_found = reinterpret_cast<int*>(A.out_match + A.n_mp);
     const int lane = threadIdx.x & 31;
     const int iq = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (iq >= A.n_mp) return;
@@ -757,18 +760,17 @@ int launch_grid_sort(const borb_keypoint* keys, int n, float minX, float minY, f
     grid_sort_kernel<<<1, 1024, K * 4, s>>>(keys, n, minX, minY, invW, invH, K, cell_start, cell_idx);
     return 1;
 }
-int launch_projection(const ProjArgs& A, int32_t* match_feat, int* n_matches, cudaStream_t s) {
+int launch_projection(const ProjArgs& A, cudaStream_t s) {
     launch_candidates(A, s);
-    launch_resolve(A, false, match_feat, nullptr, nullptr, n_matches, s);
+    launch_resolve(A, false, s);
     return 2;
 }
-int launch_projection_last(const LastArgs& L, const ProjArgs& A, int32_t* state_cur, int32_t* ev_idx, uint8_t* ev_bin, int* n_matches,
-                           cudaStream_t s) {
+int launch_projection_last(const LastArgs& L, const ProjArgs& A, cudaStream_t s) {
     if (L.n_last > 0) {
         project_points_kernel<<<(L.n_last + 255) / 256, 256, 0, s>>>(L);
         launch_candidates(A, s);
     }
-    launch_resolve(A, true, state_cur, ev_idx, ev_bin, n_matches, s);
+    launch_resolve(A, true, s);
     return 3;
 }
 int launch_initialization(const ProjArgs& A, const borb_keypoint* keys1, int n1, int32_t* match12, int32_t* ev_idx, uint8_t* ev_bin,
@@ -794,9 +796,9 @@ int launch_distinctive(const uint8_t* desc, const int32_t* offsets, int n_points
     if (n_points > 0) distinctive_kernel<<<(n_points + 3) / 4, 128, 0, s>>>(desc, offsets, n_points, best_idx);
     return 1;
 }
-int launch_frustum_projection(const LastArgs& L, const ProjArgs& A, int32_t* match_feat, int* n_matches, cudaStream_t s) {
+int launch_frustum_projection(const LastArgs& L, const ProjArgs& A, cudaStream_t s) {
     if (L.n_last > 0) project_points_kernel<<<(L.n_last + 255) / 256, 256, 0, s>>>(L);
-    return 1 + launch_projection(A, match_feat, n_matches, s);
+    return 1 + launch_projection(A, s);
 }
 int launch_point_projection_batch(const LastArgs* d_last, const ProjArgs* d_jobs, int n_jobs, int max_nq, int max_n, int max_n_mp, bool last,
                                   cudaStream_t s) {
@@ -804,12 +806,12 @@ int launch_point_projection_batch(const LastArgs* d_last, const ProjArgs* d_jobs
     project_points_batch_kernel<<<dim3((max_nq + 255) / 256, n_jobs), 256, 0, s>>>(d_last);
     return 1 + launch_projection_batch(d_jobs, n_jobs, max_n, max_n_mp, s, last);
 }
-int launch_projection_argmin(const LastArgs& L, const ProjArgs& A, int32_t* best_idx, int* n_found, cudaStream_t s) {
-    cudaMemsetAsync(n_found, 0, sizeof(int), s);
+int launch_projection_argmin(const LastArgs& L, const ProjArgs& A, cudaStream_t s) {
+    cudaMemsetAsync(A.out_match + A.n_mp, 0, sizeof(int), s);
     if (A.n_mp > 0) {
         project_points_kernel<<<(L.n_last + 255) / 256, 256, 0, s>>>(L);
         launch_candidates(A, s);
-        proj_argmin_kernel<<<(A.n_mp + 7) / 8, 256, 0, s>>>(A, best_idx, n_found);
+        proj_argmin_kernel<<<(A.n_mp + 7) / 8, 256, 0, s>>>(A);
     }
     return 3;
 }

@@ -194,9 +194,14 @@ size_t resolve_smem_bytes(int n, int n_mp) {
     return ((size_t)(n + 31) / 32 + (size_t)n + (size_t)n_mp * RES_K + (size_t)n_mp) * 4 + (size_t)n_mp + 64;
 }
 
+// out_match: the per-feature state (LAST) or the per-query match, then the match count
 template <bool LAST>
-__device__ __forceinline__ void resolve_body(const ProjArgs& A, const borb_keypoint* __restrict__ cur_keys, int32_t* __restrict__ out,
-                                             int32_t* __restrict__ ev_idx, uint8_t* __restrict__ ev_bin, int* __restrict__ n_matches) {
+__device__ __forceinline__ void resolve_body(const ProjArgs& A) {
+    const borb_keypoint* __restrict__ cur_keys = A.keys;
+    int32_t* __restrict__ out = A.out_match;
+    int32_t* __restrict__ ev_idx = A.ev_idx;
+    uint8_t* __restrict__ ev_bin = A.ev_bin;
+    int* __restrict__ n_matches = reinterpret_cast<int*>(A.out_match + (LAST ? A.n : A.n_mp));
     extern __shared__ uint32_t rsm[];
     __shared__ int hist[32];
     __shared__ int cnt_nm, cnt_ev, cnt_rm;
@@ -327,18 +332,14 @@ __device__ __forceinline__ void resolve_body(const ProjArgs& A, const borb_keypo
 }
 
 template <bool LAST>
-__global__ void __launch_bounds__(1024) proj_resolve_kernel(ProjArgs A, const borb_keypoint* __restrict__ cur_keys, int32_t* __restrict__ out,
-                                                           int32_t* __restrict__ ev_idx, uint8_t* __restrict__ ev_bin, int* __restrict__ n_matches) {
-    resolve_body<LAST>(A, cur_keys, out, ev_idx, ev_bin, n_matches);
-}
+__global__ void __launch_bounds__(1024) proj_resolve_kernel(ProjArgs A) { resolve_body<LAST>(A); }
 // a CTA per job (SearchByProjection(F, vpMapPoints) or (CurrentFrame, LastFrame) of many independent frames in one launch);
 // the block size follows the largest job, and the wave fixpoint is the sequential result for any block size
 template <bool LAST>
 __global__ void __launch_bounds__(1024) proj_resolve_batch_kernel(const ProjArgs* __restrict__ jobs) {
     const ProjArgs& A = jobs[blockIdx.x];
     if (A.n_mp <= 0) return;                        // a job without work (no MapPoints / empty frame) carries null pointers
-    const int n_out = LAST ? A.n : A.n_mp;          // out_match: the per-feature state (LAST) or per-query match, then the count
-    resolve_body<LAST>(A, A.keys, A.out_match, A.ev_idx, A.ev_bin, reinterpret_cast<int*>(A.out_match + n_out));
+    resolve_body<LAST>(A);
 }
 
 void launch_candidates(const ProjArgs& A, cudaStream_t s) {
@@ -360,15 +361,15 @@ int launch_projection_batch(const ProjArgs* d_jobs, int n_jobs, int max_n, int m
     return 2;
 }
 
-void launch_resolve(const ProjArgs& A, bool last, int32_t* out, int32_t* ev_idx, uint8_t* ev_bin, int* n_matches, cudaStream_t s) {
+void launch_resolve(const ProjArgs& A, bool last, cudaStream_t s) {
     const size_t smem = resolve_smem_bytes(A.n, A.n_mp);
     const int threads = A.n_mp > 512 ? 1024 : (A.n_mp > 256 ? 512 : 256);     // one wave covers the whole call when it can
     if (last) {
         allow_max_smem((const void*)proj_resolve_kernel<true>);
-        proj_resolve_kernel<true><<<1, threads, smem, s>>>(A, A.keys, out, ev_idx, ev_bin, n_matches);
+        proj_resolve_kernel<true><<<1, threads, smem, s>>>(A);
     } else {
         allow_max_smem((const void*)proj_resolve_kernel<false>);
-        proj_resolve_kernel<false><<<1, threads, smem, s>>>(A, A.keys, out, ev_idx, ev_bin, n_matches);
+        proj_resolve_kernel<false><<<1, threads, smem, s>>>(A);
     }
 }
 

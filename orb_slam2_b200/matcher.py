@@ -74,6 +74,34 @@ def _pose12(Tcw):
     return (C.c_float * 12)(*np.asarray(Tcw, np.float32)[:3, :4].reshape(12).tolist())
 
 
+def _c_arrays(*pairs):
+    """Contiguous copies of (array, dtype) pairs; None stays None."""
+    return [np.ascontiguousarray(a, dt) if a is not None else None for a, dt in pairs]
+
+
+def _mappoints_c(mps: "MapPointsView"):
+    """(borb_mappoint_view, arrays to keep alive)."""
+    arrs = _c_arrays((mps.mTrackProjX, np.float32), (mps.mTrackProjY, np.float32), (mps.mTrackProjXR, np.float32),
+                     (mps.mnTrackScaleLevel, np.int32), (mps.mTrackViewCos, np.float32), (mps.descriptors, np.uint8), (mps.valid, np.uint8),
+                     (mps.has_obs, np.uint8))
+    return _MapPointViewC(len(arrs[0]), *[_p(a) for a in arrs]), arrs
+
+
+def _lastframe_c(Last: "LastFrameView"):
+    """(borb_lastframe_view, arrays to keep alive)."""
+    arrs = _c_arrays((Last.mvKeysUn, KP_DTYPE), (Last.world_pos, np.float32), (Last.descriptors, np.uint8), (Last.valid, np.uint8),
+                     (Last.has_obs, np.uint8))
+    return _LastFrameViewC(len(arrs[0]), *[_p(a) for a in arrs]), arrs
+
+
+def _local_points_outputs(nq: int):
+    """The output arrays of SearchLocalPoints for nq points (at least one entry each, so that every pointer is valid)."""
+    m1 = max(nq, 1)
+    return dict(in_view=np.zeros(m1, np.uint8), proj_x=np.zeros(m1, np.float32), proj_y=np.zeros(m1, np.float32),
+                proj_xr=np.zeros(m1, np.float32), level=np.zeros(m1, np.int32), view_cos=np.zeros(m1, np.float32),
+                match=np.full(m1, -1, np.int32))
+
+
 @dataclass
 class FeatureVector:
     """DBoW2::FeatureVector as CSR: node ids ascending, feature indices ascending inside a node."""
@@ -300,17 +328,12 @@ class ORBmatcher:
     def SearchByProjection(self, F: FrameView, mps: MapPointsView, th: float = 3.0) -> Tuple[int, np.ndarray]:
         """src/ORBmatcher.cc:45-129.  Returns (nmatches, match_feat[n_mp]): frame feature that received map point i, or -1."""
         fv, keep = F._view()
-        px = np.ascontiguousarray(mps.mTrackProjX, np.float32); py = np.ascontiguousarray(mps.mTrackProjY, np.float32)
-        pxr = np.ascontiguousarray(mps.mTrackProjXR, np.float32); lv = np.ascontiguousarray(mps.mnTrackScaleLevel, np.int32)
-        vc = np.ascontiguousarray(mps.mTrackViewCos, np.float32); md = np.ascontiguousarray(mps.descriptors, np.uint8)
-        va = np.ascontiguousarray(mps.valid, np.uint8) if mps.valid is not None else None
-        ho = np.ascontiguousarray(mps.has_obs, np.uint8) if mps.has_obs is not None else None
-        mv = _MapPointViewC(len(px), _p(px), _p(py), _p(pxr), _p(lv), _p(vc), _p(md), _p(va), _p(ho))
-        match = np.full(max(len(px), 1), -1, np.int32)
+        mv, arrs = _mappoints_c(mps)
+        match = np.full(max(mv.n, 1), -1, np.int32)
         n = C.c_int32(0)
         check(self._lib.borb_search_by_projection(self._h, C.byref(fv), C.byref(mv), float(th), self.mfNNratio, _p(match), C.byref(n)),
               "borb_search_by_projection")
-        return n.value, match[:len(px)]
+        return n.value, match[:mv.n]
 
     def SearchByProjectionBatch(self, frames: Sequence[FrameView], mps_list: Sequence[MapPointsView], th: float = 3.0):
         """borb_search_by_projection_batch: SearchByProjection(F, vpMapPoints, th) of many independent device-resident frames in one
@@ -321,16 +344,9 @@ class ORBmatcher:
         MV = (_MapPointViewC * n)()
         keep, outs = [], []
         for j, (F, mps) in enumerate(zip(frames, mps_list)):
-            fv, k = F._view()
-            FV[j] = fv
-            px = np.ascontiguousarray(mps.mTrackProjX, np.float32); py = np.ascontiguousarray(mps.mTrackProjY, np.float32)
-            pxr = np.ascontiguousarray(mps.mTrackProjXR, np.float32); lv = np.ascontiguousarray(mps.mnTrackScaleLevel, np.int32)
-            vc = np.ascontiguousarray(mps.mTrackViewCos, np.float32); md = np.ascontiguousarray(mps.descriptors, np.uint8)
-            va = np.ascontiguousarray(mps.valid, np.uint8) if mps.valid is not None else None
-            ho = np.ascontiguousarray(mps.has_obs, np.uint8) if mps.has_obs is not None else None
-            MV[j] = _MapPointViewC(len(px), _p(px), _p(py), _p(pxr), _p(lv), _p(vc), _p(md), _p(va), _p(ho))
-            out = np.full(max(len(px), 1), -1, np.int32)
-            keep.append((k, px, py, pxr, lv, vc, md, va, ho)); outs.append(out)
+            FV[j], k = F._view()
+            MV[j], arrs = _mappoints_c(mps)
+            keep.append((k, arrs)); outs.append(np.full(max(MV[j].n, 1), -1, np.int32))
         ptrs = (C.c_void_p * n)(*[o.ctypes.data for o in outs])
         nm = np.zeros(max(n, 1), np.int32)
         check(self._lib.borb_search_by_projection_batch(self._h, FV, MV, n, float(th), self.mfNNratio, ptrs, _p(nm)), "borb_search_by_projection_batch")
@@ -342,11 +358,7 @@ class ORBmatcher:
         K = (fx, fy, cx, cy).  Returns (nmatches, state[cur.N]): >=0 last-frame index now matched, -1 untouched, -2 culled."""
         fv, keep = Cur._view()
         k = Cur.mvKeysUn
-        lk = np.ascontiguousarray(Last.mvKeysUn, KP_DTYPE); wp = np.ascontiguousarray(Last.world_pos, np.float32)
-        ld = np.ascontiguousarray(Last.descriptors, np.uint8)
-        va = np.ascontiguousarray(Last.valid, np.uint8) if Last.valid is not None else None
-        ho = np.ascontiguousarray(Last.has_obs, np.uint8) if Last.has_obs is not None else None
-        lv = _LastFrameViewC(len(lk), _p(lk), _p(wp), _p(ld), _p(va), _p(ho))
+        lv, arrs = _lastframe_c(Last)
         T = np.ascontiguousarray(np.asarray(Tcw, np.float32)[:3, :4]).reshape(12)
         state = np.full(max(len(k), 1), -1, np.int32)
         n = C.c_int32(0)
@@ -359,10 +371,8 @@ class ORBmatcher:
         fv, keep = F._view(with_stereo)
         k = F.mvKeysUn
         sf = np.ascontiguousarray(F.mvScaleFactors, np.float32)
-        arrs = []
-        for a, dt in ((P.world_pos, np.float32), (P.descriptors, np.uint8), (P.max_distance, np.float32), (P.min_distance, np.float32),
-                      (P.normal, np.float32), (P.angle, np.float32), (P.valid, np.uint8)):
-            arrs.append(np.ascontiguousarray(a, dt) if a is not None else None)
+        arrs = _c_arrays((P.world_pos, np.float32), (P.descriptors, np.uint8), (P.max_distance, np.float32), (P.min_distance, np.float32),
+                         (P.normal, np.float32), (P.angle, np.float32), (P.valid, np.uint8))
         pv = _WorldPointsViewC(len(arrs[0]), *[_p(a) for a in arrs])
         logs = F.mfLogScaleFactor if F.mfLogScaleFactor is not None else _libm_logf(sf[1] if len(sf) > 1 else 1.2)
         return fv, pv, float(logs), len(k), keep + arrs
@@ -405,10 +415,7 @@ class ORBmatcher:
         ow = np.ascontiguousarray(np.asarray(Ow, np.float32).reshape(3))
         ho = np.ascontiguousarray(has_obs, np.uint8) if has_obs is not None else None
         nq = len(P.world_pos)
-        m1 = max(nq, 1)
-        out = dict(in_view=np.zeros(m1, np.uint8), proj_x=np.zeros(m1, np.float32), proj_y=np.zeros(m1, np.float32),
-                   proj_xr=np.zeros(m1, np.float32), level=np.zeros(m1, np.int32), view_cos=np.zeros(m1, np.float32),
-                   match=np.full(m1, -1, np.int32))
+        out = _local_points_outputs(nq)
         nm = C.c_int32(0)
         check(self._lib.borb_search_local_points(self._h, C.byref(fv), C.byref(pv), _p(ho), _p(T), _p(ow), float(K[0]), float(K[1]), float(K[2]),
                                                  float(K[3]), float(mbf), float(viewingCosLimit), logs, float(th), self.mfNNratio,
@@ -433,10 +440,7 @@ class ORBmatcher:
             fv, pv, logs, _, k = self._points_call(frames[j], points[j], with_stereo=True)
             ho = np.ascontiguousarray(obs[j], np.uint8) if obs[j] is not None else None
             nq = len(points[j].world_pos)
-            m1 = max(nq, 1)
-            out = dict(in_view=np.zeros(m1, np.uint8), proj_x=np.zeros(m1, np.float32), proj_y=np.zeros(m1, np.float32),
-                       proj_xr=np.zeros(m1, np.float32), level=np.zeros(m1, np.int32), view_cos=np.zeros(m1, np.float32),
-                       match=np.full(m1, -1, np.int32))
+            out = _local_points_outputs(nq)
             Tcw, Ow = poses[j]
             J = jobs[j]
             J.frame, J.pts, J.has_obs, J.Tcw = fv, pv, _p(ho), _pose12(Tcw)
@@ -469,18 +473,14 @@ class ORBmatcher:
         keep, outs = [], []
         for j in range(n):
             fv, k = curs[j]._view()
-            L = lasts[j]
-            lk = np.ascontiguousarray(L.mvKeysUn, KP_DTYPE); wp = np.ascontiguousarray(L.world_pos, np.float32)
-            ld = np.ascontiguousarray(L.descriptors, np.uint8)
-            va = np.ascontiguousarray(L.valid, np.uint8) if L.valid is not None else None
-            ho = np.ascontiguousarray(L.has_obs, np.uint8) if L.has_obs is not None else None
+            lv, arrs = _lastframe_c(lasts[j])
             n_cur = len(curs[j].mvKeysUn)
             state = np.full(max(n_cur, 1), -1, np.int32)
             J = jobs[j]
-            J.cur, J.last, J.Tcw = fv, _LastFrameViewC(len(lk), _p(lk), _p(wp), _p(ld), _p(va), _p(ho)), _pose12(poses[j])
+            J.cur, J.last, J.Tcw = fv, lv, _pose12(poses[j])
             J.fx, J.fy, J.cx, J.cy = [float(x) for x in Ks[j]]
             J.bf, J.th, J.forward, J.backward, J.state_cur = float(bfs[j]), float(ths[j]), int(fws[j]), int(bws[j]), _p(state)
-            keep.append((k, lk, wp, ld, va, ho)); outs.append((n_cur, state))
+            keep.append((k, arrs)); outs.append((n_cur, state))
         nm = np.zeros(max(n, 1), np.int32)
         check(self._lib.borb_search_by_projection_last_batch(self._h, jobs, n, int(self.mbCheckOrientation), _p(nm)),
               "borb_search_by_projection_last_batch")

@@ -233,6 +233,14 @@ def test_argument_errors_name_the_job_and_launch_nothing(M, oracle, views):
     bad = Last.mvKeysUn.copy()
     bad["octave"][5] = len(Cur.mvScaleFactors)
     refused(lambda: mt.SearchByProjectionLastBatch([CR, CR, CR], [Last, Last, dataclasses.replace(Last, mvKeysUn=bad)], [T] * 3, K2, BF, 15.0), 2)
+    # SearchByProjection(F, vpMapPoints): host view, predicted level outside the frame's levels
+    PF, mps = mf.projection_case(views[7], 100, n_mp=50)
+    PR = PF.make_resident(mt)
+    refused(lambda: mt.SearchByProjectionBatch([PR, PF], [mps, mps], 3.0), 1)
+    lvl = mps.mnTrackScaleLevel.copy()
+    lvl[3] = len(PF.mvScaleFactors)
+    bad_mps = dataclasses.replace(mps, mnTrackScaleLevel=lvl, valid=None)
+    refused(lambda: mt.SearchByProjectionBatch([PR, PR, PR], [mps, mps, bad_mps], 3.0), 2)
     # the handle still works after the refusals
     got = mt.SearchLocalPointsBatch([FR], [P], [pose], K, BF, 3.0, has_obs=[ho])[0]
     single = mt.SearchLocalPoints(FR, P, pose[0], pose[1], K, BF, 3.0, has_obs=ho)
