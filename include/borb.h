@@ -462,6 +462,24 @@ BORB_API borb_status borb_search_by_bow(borb_matcher* m, const borb_keyframe_vie
  * match12[i] = index in kf2 of the MapPoint matched to feature i of kf1, or -1. */
 BORB_API borb_status borb_search_by_bow_kf(borb_matcher* m, const borb_keyframe_view* kf1, const borb_keyframe_view* kf2,
                                            float nnratio, int check_orientation, int32_t* match12, int32_t* n_matches);
+
+/* One camera stream's TrackReferenceKeyFrame search, ORBmatcher::SearchByBoW(KeyFrame*, Frame&) (src/ORBmatcher.cc:159-288). */
+typedef struct borb_bow_job {
+    const borb_frame* frame;       /* current frame: resident, BoW computed */
+    borb_keyframe_view kf;         /* reference keyframe as a host view; kf.has_mp is always read from here */
+    const borb_frame* kf_frame;    /* NULL, or the resident frame the keyframe was made from (BoW computed): then kf.n, keys_un,
+                                      desc and fv are taken from it and only kf.has_mp crosses PCIe */
+    int32_t* match;                /* output, frame n entries: as borb_search_by_bow */
+} borb_bow_job;
+/* borb_search_by_bow (one keyframe against one frame) for n_jobs independent camera streams in one launch and one synchronisation
+ * (Tracking::TrackReferenceKeyFrame, src/Tracking.cc:757-799, runs it whenever the motion model has no velocity or finds too few
+ * matches).  Frames come with the BoW of borb_frames_compute_bow, so nothing of the current frame crosses PCIe.  match and n_matches[j]
+ * are bit-identical to borb_search_by_bow on host views of the same data.  A NULL frame, a frame without BoW (every frame comes from
+ * borb_frame_create / borb_frames_from_extractor without one, recycled ones included), a frame on another device and an incomplete
+ * host view are refused with BORB_ERR_INVALID_ARG before anything is launched, the error text naming the job.  A frame with 0 features
+ * or a keyframe with an empty FeatureVector gives 0 matches (match all -1). */
+BORB_API borb_status borb_search_by_bow_batch(borb_matcher* m, const borb_bow_job* jobs, int n_jobs, float nnratio,
+                                              int check_orientation, int32_t* n_matches);
 /* ORBmatcher::SearchForTriangulation — src/ORBmatcher.cc:657-823.  F12 row-major 3x3; (ex,ey) = projection of
  * kf1's camera centre into kf2 (:663-670, computed by the caller).  pairs: 2*cap ints (idx1, idx2), ascending idx1. */
 BORB_API borb_status borb_search_for_triangulation(borb_matcher* m, const borb_keyframe_view* kf1, const borb_keyframe_view* kf2,
@@ -547,6 +565,17 @@ BORB_API borb_status borb_bow_transform(borb_voc* v, const uint8_t* desc, int n,
  * (capacities n, n + 1, n), *n_nodes nodes — the layout borb_featvec_view and borb_kfdb_add take. */
 BORB_API borb_status borb_compute_bow(borb_voc* v, const uint8_t* desc, int n, int levelsup, uint32_t* bow_word, double* bow_value,
                                       int32_t* n_bow, uint32_t* fv_node, int32_t* fv_start, uint32_t* fv_idx, int32_t* n_nodes);
+
+/* Frame::ComputeBoW (src/Frame.cc:395-402) for n_frames resident frames: tree descent and the BowVector / FeatureVector
+ * bookkeeping of TemplatedVocabulary::transform (:1127-1194) on the device, kept with the frame (borb_search_by_bow_batch reads
+ * it).  Bit-identical to borb_compute_bow on the frame's descriptors.  Host copies are optional (NULL tables: device only; a NULL
+ * entry skips that frame's copy; n_bow / n_nodes may be NULL); capacities per frame as borb_compute_bow (n, n, n, n + 1, n).
+ * 2 launches whatever n_frames, one synchronisation.  The vocabulary, the frames and the matcher must live on the same device; a
+ * frame with 0 features or only stop words gets empty vectors (fv_start[0] = 0). */
+BORB_API borb_status borb_frames_compute_bow(borb_matcher* m, borb_voc* v, borb_frame* const* frames, int n_frames, int levelsup,
+                                             uint32_t* const* bow_word, double* const* bow_value, int32_t* n_bow,
+                                             uint32_t* const* fv_node, int32_t* const* fv_start, uint32_t* const* fv_idx,
+                                             int32_t* n_nodes);
 
 /* ---------------------------------------------------------------- introspection -------------- */
 /* Device time (CUDA events on the matcher's stream) of the kernels of the last borb_search_by_bow_db* call on this handle. */

@@ -7,6 +7,8 @@
 //              borb_frames_from_extractor    N device-resident frames, keypoints stay in HBM  (Frame constructor tail x N)
 //              borb_search_by_projection_batch   one launch pair for the N matcher calls      (SearchByProjection x N)
 //              borb_search_by_projection_last_batch   motion-model search of the N streams    (TrackWithMotionModel x N)
+//              borb_frames_compute_bow       BowVector / FeatureVector of the N frames, kept in HBM   (Frame::ComputeBoW x N)
+//              borb_search_by_bow_batch      reference-keyframe search of the N streams   (TrackReferenceKeyFrame x N)
 //              (pose optimisation on the host)
 //              borb_search_local_points_batch    isInFrustum + local-map search of the N streams   (SearchLocalPoints x N)
 //
@@ -14,7 +16,9 @@
 // seen, with their own descriptors, predicted at their own octave), so SearchByProjection must give (almost) every point back to
 // a feature — bar the few points whose twin at a neighbouring level wins the ratio test.  For the two Tracking-thread searches
 // the keypoints are back-projected to a per-point depth with the identity pose: as the last frame's MapPoints they must land on
-// their own features, and as world points (normal = viewing ray, distances that predict the keypoint's octave) as well.
+// their own features, and as world points (normal = viewing ray, distances that predict the keypoint's octave) as well.  For the
+// reference-keyframe search every stream's frame is its own reference keyframe, every feature with a MapPoint: a feature can only
+// match itself (a duplicate descriptor fails the ratio test), so every match[j] is j or -1.  The vocabulary is a small seeded tree.
 // Build:  g++ -std=c++14 -Iinclude integration/example_multistream_host.cc orb_slam2_b200/libborb.so -Wl,-rpath,$PWD/orb_slam2_b200
 // Exit code 0 = ran and checked, 3 = the library reported an error (e.g. no CUDA device: there is no CPU fallback).
 #include <cmath>
@@ -48,6 +52,30 @@ static void make_image(std::vector<uint8_t>& img, int w, int h, int stream) {
     }
 }
 
+// a seeded vocabulary (k = 10, depth 3: 1000 words, idf weights in [1, 2)); with levelsup 2 the FeatureVector has the 10 nodes of
+// level 1, so every bucket holds many features
+static borb_status make_vocabulary(borb_voc** out) {
+    const int k = 10, L = 3;
+    std::vector<int32_t> parent(1, 0);
+    std::vector<uint8_t> leaf(1, 0), desc(32, 0);
+    std::vector<double> weight(1, 0.0);
+    uint32_t rng = 424242u;
+    int first = 0, count = 1;                                // the nodes of the level above
+    for (int l = 1; l <= L; l++) {
+        const int start = (int)parent.size();
+        for (int p = first; p < first + count; p++)
+            for (int c = 0; c < k; c++) {
+                parent.push_back(p);
+                leaf.push_back(l == L ? 1 : 0);
+                for (int b = 0; b < 32; b++) { rng = rng * 1664525u + 1013904223u; desc.push_back((uint8_t)(rng >> 24)); }
+                weight.push_back(l == L ? 1.0 + (double)(parent.size() % 7) / 7.0 : 0.0);
+            }
+        first = start;
+        count *= k;
+    }
+    return borb_voc_create(parent.data(), leaf.data(), desc.data(), weight.data(), (int)parent.size(), k, L, 0, out);
+}
+
 int main(int argc, char** argv) {
     const int N = argc > 1 ? std::atoi(argv[1]) : 8, W = 640, H = 480, ticks = 3;
     int ndev = 0;
@@ -57,6 +85,8 @@ int main(int argc, char** argv) {
     borb_matcher* mat = nullptr;
     CHECK(borb_extractor_create(&cfg, 0, &ext));
     CHECK(borb_matcher_create(0, &mat));
+    borb_voc* voc = nullptr;
+    CHECK(make_vocabulary(&voc));
     int cap = 0;
     CHECK(borb_extractor_capacity(ext, W, H, &cap));
     std::vector<float> scale(cfg.n_levels);
@@ -71,7 +101,7 @@ int main(int argc, char** argv) {
     std::vector<borb_frame*> frames(N, nullptr);
     const borb_camera cam = {517.3f, 516.5f, 318.6f, 255.3f, 0.f, 0.f, 0.f, 0.f, 0.f, 40.f};      // k1 = 0: mvKeysUn = mvKeys
     float bounds[4];
-    long total_points = 0, total_matches = 0, last_self = 0, local_self = 0;
+    long total_points = 0, total_matches = 0, last_self = 0, local_self = 0, ref_self = 0, ref_other = 0;
     const float log_scale = std::log(cfg.scale_factor);     // Frame::mfLogScaleFactor
 
     for (int t = 0; t < ticks; t++) {
@@ -143,25 +173,50 @@ int main(int argc, char** argv) {
             J.in_view = in_view[i].data(); J.match_feat = lmatch[i].data();
         }
         CHECK(borb_search_by_projection_last_batch(mat, ljobs.data(), N, 1, n_last.data()));
+        // ---- the reference-keyframe search (Tracking::TrackReferenceKeyFrame, the fallback of a motion-model search that finds too
+        //      few matches): the frames' BoW on the device, then SearchByBoW with each frame as its own reference keyframe (kf_frame:
+        //      only has_mp crosses PCIe)
+        CHECK(borb_frames_compute_bow(mat, voc, frames.data(), N, 2, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr));
+        std::vector<borb_bow_job> bjobs(N);
+        std::vector<std::vector<uint8_t> > has_mp(N);
+        std::vector<std::vector<int32_t> > bmatch(N);
+        std::vector<int32_t> n_ref(N);
+        for (int i = 0; i < N; i++) {
+            const int n = n_out[i];
+            has_mp[i].assign(n > 0 ? n : 1, 1);
+            bmatch[i].assign(n > 0 ? n : 1, -1);
+            borb_bow_job& B = bjobs[i];
+            B = borb_bow_job();
+            B.frame = frames[i];
+            B.kf_frame = frames[i];
+            B.kf.has_mp = has_mp[i].data();
+            B.match = bmatch[i].data();
+        }
+        CHECK(borb_search_by_bow_batch(mat, bjobs.data(), N, 0.7f, 1, n_ref.data()));
         CHECK(borb_search_local_points_batch(mat, pjobs.data(), N, 0.5f, 0.8f, n_local.data()));
         for (int i = 0; i < N; i++) {
             total_points += n_out[i]; total_matches += n_matches[i];
-            int self = 0, sl = 0, sp = 0;
-            for (int j = 0; j < n_out[i]; j++) { self += match[i][j] == j; sl += state[i][j] == j; sp += lmatch[i][j] == j; }
-            last_self += sl; local_self += sp;
-            std::printf("tick %d stream %d: %d keypoints, %d matches (%d to themselves); motion model %d (%d); local map %d (%d)\n", t, i,
-                        n_out[i], n_matches[i], self, n_last[i], sl, n_local[i], sp);
+            int self = 0, sl = 0, sp = 0, sr = 0;
+            for (int j = 0; j < n_out[i]; j++) {
+                self += match[i][j] == j; sl += state[i][j] == j; sp += lmatch[i][j] == j; sr += bmatch[i][j] == j;
+                ref_other += bmatch[i][j] != j && bmatch[i][j] != -1;
+            }
+            last_self += sl; local_self += sp; ref_self += sr;
+            std::printf("tick %d stream %d: %d keypoints, %d matches (%d to themselves); motion model %d (%d); reference keyframe %d (%d); "
+                        "local map %d (%d)\n", t, i, n_out[i], n_matches[i], self, n_last[i], sl, n_ref[i], sr, n_local[i], sp);
             CHECK(borb_frame_destroy(frames[i]));
             frames[i] = nullptr;
         }
     }
+    CHECK(borb_voc_destroy(voc));
     CHECK(borb_matcher_destroy(mat));
     CHECK(borb_extractor_destroy(ext));
     std::printf("%ld points, %ld matched\n", total_points, total_matches);
     std::printf("motion-model search: %ld of %ld features matched to their own last-frame point\n", last_self, total_points);
+    std::printf("reference-keyframe search: %ld of %ld features matched to themselves, %ld elsewhere\n", ref_self, total_points, ref_other);
     std::printf("local-map search: %ld of %ld points matched to their own feature\n", local_self, total_points);
     if (total_points < 100L * N * ticks || total_matches < total_points * 8 / 10 || last_self < total_points * 8 / 10 ||
-        local_self < total_points * 8 / 10) {
+        ref_self < total_points * 8 / 10 || ref_other != 0 || local_self < total_points * 8 / 10) {
         std::printf("self-check failed\n");
         return 1;
     }

@@ -106,6 +106,8 @@ _SIGNATURES = {
                                       C.c_float, vp, i32p]),
     "borb_search_by_bow": (C.c_int, [vp, vp, C.c_int, vp, C.c_float, C.c_int, vp, vp]),
     "borb_search_by_bow_kf": (C.c_int, [vp, vp, vp, C.c_float, C.c_int, vp, i32p]),
+    "borb_search_by_bow_batch": (C.c_int, [vp, vp, C.c_int, C.c_float, C.c_int, vp]),
+    "borb_frames_compute_bow": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp]),
     "borb_search_for_triangulation": (C.c_int, [vp, vp, vp, vp, C.c_float, C.c_float, C.c_int, C.c_int, vp, C.c_int, i32p]),
     "borb_voc_create": (C.c_int, [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(vp)]),
     "borb_voc_load_text": (C.c_int, [C.c_char_p, C.c_int, C.POINTER(vp)]),

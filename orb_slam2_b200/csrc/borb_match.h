@@ -9,7 +9,8 @@ struct borb_frame {
     int device = 0;
     int n = 0, n_levels = 0;
     float min_x = 0, min_y = 0, max_x = 0, max_y = 0;
-    uint8_t* block = nullptr;       // one allocation: keys | desc | u_right | depth | scale factors | cell_start | cell_idx
+    uint8_t* block = nullptr;       // one allocation: keys | desc | u_right | depth | scale factors | cell_start | cell_idx |
+                                    //                 bow_value | bow_word | fv_node | fv_start | fv_idx
     size_t block_bytes = 0;
     int cap = 0;                    // features the block can hold
     borb_keypoint* keys = nullptr;
@@ -21,6 +22,15 @@ struct borb_frame {
     float* sf = nullptr;
     int* cell_start = nullptr;
     int* cell_idx = nullptr;
+    // Frame::mBowVec / mFeatVec (borb_frames_compute_bow): BowVector in word order, FeatureVector as CSR (cap entries each,
+    // fv_start cap + 1); valid only while has_bow, which frame_alloc clears
+    double* bow_value = nullptr;
+    uint32_t* bow_word = nullptr;
+    uint32_t* fv_node = nullptr;
+    int32_t* fv_start = nullptr;
+    uint32_t* fv_idx = nullptr;
+    bool has_bow = false;
+    int n_bow = 0, n_nodes = 0;
     cudaEvent_t ready = nullptr;    // recorded after the last kernel that writes the block
 };
 
@@ -178,6 +188,25 @@ struct FrameJob {                 // one frame of borb_frames_from_extractor (k_
 
 struct TriArgs { float F[9]; float ex, ey; int only_stereo, check_ori; };
 
+struct BowTables {                // a BowVector (word order) and a FeatureVector (CSR); word == null: not written
+    uint32_t* word;
+    double* value;
+    uint32_t* node;
+    int32_t* start;               // n_nodes + 1
+    uint32_t* idx;
+};
+
+struct BowFrameJob {              // one frame of borb_frames_compute_bow (bow_transform_batch_kernel, bow_build_kernel)
+    const uint8_t* desc;          // the resident frame's descriptors
+    int n;
+    int32_t* word;                // scratch: word id, word weight, node id per feature (the descent's output)
+    double* weight;
+    int32_t* node;
+    BowTables dst;                // the frame's storage
+    BowTables copy;               // the same tables again, for the host (may be unset)
+    int32_t* counts;              // n_bow, n_nodes
+};
+
 struct VocDev {                   // views into the packed blob
     int n_nodes, k, L;
     const uint8_t* desc;          // n_nodes x 32
@@ -205,8 +234,9 @@ int launch_distinctive(const uint8_t* desc, const int32_t* offsets, int n_points
 int launch_frustum_projection(const LastArgs& L, const ProjArgs& A, cudaStream_t s);
 int launch_projection_argmin(const LastArgs& L, const ProjArgs& A, cudaStream_t s);
 int launch_sim3_agree(const int32_t* match1, const int32_t* match2, int n1, int n2, int32_t* match12, int* n_found, cudaStream_t s);
+// out_off: null (every pair against ts[0], output p at match + p * out_stride) or, mode 0, one target and output offset per pair
 int launch_bow_match(const KfDev* qs, const KfDev* ts, int n_pairs, int mode, float nnratio, int check_ori, int32_t* match,
-                     int out_stride, uint8_t* bins, int32_t* n_matches, int max_t, cudaStream_t s);
+                     int out_stride, const size_t* out_off, uint8_t* bins, int32_t* n_matches, int max_t, cudaStream_t s);
 void host_image_bounds(int w, int h, const borb_camera& c, float* b4);
 int launch_frame_build(const FrameJob* d_jobs, int n_jobs, int max_n, const borb_camera& cam, int mode, int depth_type, float depth_factor, int w,
                        int h, int out_cap, borb_keypoint* keys_out, float* ur_out, float* depth_out, cudaStream_t s);
@@ -216,5 +246,7 @@ int launch_triangulation(const KfDev& q, const KfDev& t, const TriArgs& T, int32
                          int32_t* n_pairs, cudaStream_t s);
 int launch_bow_transform(const VocDev& V, const uint8_t* desc, int n, int levelsup, int32_t* word, double* weight, int32_t* node,
                          cudaStream_t s);
+// descent + bookkeeping for n_frames frames (a job table in device memory): 2 launches
+int launch_bow_frames(const VocDev& V, const BowFrameJob* d_jobs, int n_frames, int max_n, int levelsup, cudaStream_t s);
 
 }  // namespace borb

@@ -321,13 +321,19 @@ borb_status frame_alloc(int device, int n, int n_levels, bool stereo, borb_frame
         auto put = [&](size_t bytes) { off = (off + 255) & ~size_t(255); const size_t o = off; off += bytes; return o; };
         const size_t o_k = put((size_t)f->cap * sizeof(borb_keypoint)), o_d = put((size_t)f->cap * 32), o_u = put((size_t)f->cap * 4), o_z = put((size_t)f->cap * 4);
         const size_t o_s = put(BORB_MAX_LEVELS * 4), o_cs = put((size_t)(GRID_CELLS + 1) * 4), o_ci = put((size_t)MATCH_MAX_FEATURES * 4 + 16);
+        const size_t o_bv = put((size_t)f->cap * 8), o_bw = put((size_t)f->cap * 4), o_fn = put((size_t)f->cap * 4);
+        const size_t o_fs = put((size_t)(f->cap + 1) * 4), o_fi = put((size_t)f->cap * 4);
         cudaError_t e = cudaMalloc(&f->block, off + 256);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&f->ready, cudaEventDisableTiming);
         if (e != cudaSuccess) { set_error("frame allocation failed: %s", cudaGetErrorString(e)); cudaFree(f->block); delete f; return BORB_ERR_CUDA; }
         f->block_bytes = off + 256;
         f->keys = (borb_keypoint*)(f->block + o_k); f->desc = f->block + o_d; f->ur_store = (float*)(f->block + o_u); f->depth_store = (float*)(f->block + o_z);
         f->sf = (float*)(f->block + o_s); f->cell_start = (int*)(f->block + o_cs); f->cell_idx = (int*)(f->block + o_ci);
+        f->bow_value = (double*)(f->block + o_bv); f->bow_word = (uint32_t*)(f->block + o_bw); f->fv_node = (uint32_t*)(f->block + o_fn);
+        f->fv_start = (int32_t*)(f->block + o_fs); f->fv_idx = (uint32_t*)(f->block + o_fi);
     }
+    f->has_bow = false;                 // a new frame, or a recycled block that still holds another frame's vectors
+    f->n_bow = f->n_nodes = 0;
     // u_right / depth storage always exists; the pointers are nulled for a monocular frame
     f->u_right = stereo ? f->ur_store : nullptr;
     f->depth = stereo ? f->depth_store : nullptr;
@@ -375,7 +381,7 @@ borb_status borb_frame_create(borb_matcher* m, const borb_frame_view* v, borb_fr
 borb_status borb_frame_destroy(borb_frame* f) {
     if (!f) return BORB_OK;
     std::lock_guard<std::mutex> lk(g_frame_pool_mu);
-    if (g_frame_pool.size() < 1024) { g_frame_pool.push_back(f); return BORB_OK; }     // ~170 KB each; a multi-stream server keeps hundreds alive
+    if (g_frame_pool.size() < 1024) { g_frame_pool.push_back(f); return BORB_OK; }     // ~235 KB each (2048 features); a multi-stream server keeps hundreds alive
     cudaSetDevice(f->device);
     cudaEventSynchronize(f->ready);
     cudaFree(f->block);
@@ -1323,7 +1329,7 @@ static borb_status bow_common(borb_matcher* m, const borb_keyframe_view* qs, int
     if ((s = commit(st, total)) != BORB_OK) return s;
     uint8_t* b = m->arena;
     m->launches += launch_bow_match((const KfDev*)(b + o_qd), (const KfDev*)(b + o_td), n_q, mode, nnratio, check_ori, (int32_t*)(b + o_match),
-                                    out_stride, b + o_bins, (int32_t*)(b + o_nm), t->n, m->stream);
+                                    out_stride, nullptr, b + o_bins, (int32_t*)(b + o_nm), t->n, m->stream);
     BORB_CUDA(cudaGetLastError());
     if (out_stride > 0) BORB_CUDA(cudaMemcpyAsync(match, b + o_match, (size_t)n_q * out_stride * 4, cudaMemcpyDeviceToHost, m->stream));
     BORB_CUDA(cudaMemcpyAsync(n_matches, b + o_nm, (size_t)n_q * 4, cudaMemcpyDeviceToHost, m->stream));
@@ -1348,6 +1354,96 @@ borb_status borb_search_by_bow_kf(borb_matcher* m, const borb_keyframe_view* kf1
     if (s == BORB_OK) s = check_kf(kf2, "borb_search_by_bow_kf(kf2)");
     if (s != BORB_OK) return s;
     return bow_common(m, kf1, 1, kf2, 1, nnratio, check_orientation, match12, n_matches);
+}
+
+// ---- TrackReferenceKeyFrame's SearchByBoW(KeyFrame*, Frame&) for many camera streams in one launch: each job's frame is resident
+// with its BoW (borb_frames_compute_bow); its keyframe is a host view, or a resident frame of which only has_mp crosses PCIe.
+namespace {
+borb_status check_resident_bow(const borb_frame* f, const borb_matcher* m, int j, const char* what) {
+    if (!f) { set_error("job %d: %s is not a device-resident frame", j, what); return BORB_ERR_INVALID_ARG; }
+    if (f->device != m->device) { set_error("job %d: %s and matcher live on different devices", j, what); return BORB_ERR_INVALID_ARG; }
+    if (!f->has_bow) { set_error("job %d: %s has no BoW (borb_frames_compute_bow)", j, what); return BORB_ERR_INVALID_ARG; }
+    if (f->n > MATCH_MAX_FEATURES) { set_error("job %d: %s has %d features (limit %d)", j, what, f->n, MATCH_MAX_FEATURES); return BORB_ERR_INVALID_ARG; }
+    return BORB_OK;
+}
+// a resident frame as the SearchByBoW side of a KfDev (has_mp from the caller)
+KfDev resident_kf_dev(const borb_frame* f, const uint8_t* has_mp) {
+    KfDev d{};
+    d.n = f->n; d.nn = f->n_nodes;
+    d.keys = f->keys; d.desc = f->desc; d.has_mp = has_mp; d.u_right = f->u_right;
+    d.node = f->fv_node; d.start = f->fv_start; d.idx = f->fv_idx;
+    d.scale_factors = f->sf;
+    return d;
+}
+}  // namespace
+
+borb_status borb_search_by_bow_batch(borb_matcher* m, const borb_bow_job* jobs, int n_jobs, float nnratio, int check_orientation,
+                                     int32_t* n_matches) {
+    if (!m || n_jobs < 0 || (n_jobs > 0 && (!jobs || !n_matches))) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+    if (n_jobs == 0) return BORB_OK;
+    int max_t = 0;
+    std::vector<size_t> off(n_jobs);                  // each job's matches in the result block (frames differ in n)
+    size_t total_n = 0;
+    for (int j = 0; j < n_jobs; j++) {
+        const borb_bow_job& B = jobs[j];
+        n_matches[j] = 0;
+        borb_status s = check_resident_bow(B.frame, m, j, "frame");
+        if (s != BORB_OK) return s;
+        if (!B.match) { set_error("job %d: null output", j); return BORB_ERR_INVALID_ARG; }
+        if (B.kf_frame) {
+            if ((s = check_resident_bow(B.kf_frame, m, j, "kf_frame")) != BORB_OK) return s;
+        } else if ((s = check_kf(&B.kf, "keyframe")) != BORB_OK) return job_error(j, s);
+        max_t = std::max(max_t, B.frame->n);
+        off[j] = total_n; total_n += (size_t)B.frame->n;
+    }
+    BORB_CUDA(cudaSetDevice(m->device));
+    Stager st(m);
+    std::vector<KfOffsets> ko(n_jobs);
+    std::vector<size_t> o_hm(n_jobs, 0);
+    for (int j = 0; j < n_jobs; j++) {
+        const borb_bow_job& B = jobs[j];
+        if (!B.kf_frame) ko[j] = stage_kf(st, &B.kf);
+        else if (B.kf.has_mp) o_hm[j] = st.add(B.kf.has_mp, (size_t)B.kf_frame->n);
+    }
+    const size_t o_q = st.add(nullptr, (size_t)n_jobs * sizeof(KfDev)), o_t = st.add(nullptr, (size_t)n_jobs * sizeof(KfDev));   // filled in place
+    const size_t o_off = st.add(nullptr, (size_t)n_jobs * sizeof(size_t));
+    const size_t input_end = st.off;
+    const size_t cnt_bytes = ((size_t)n_jobs * 4 + 15) & ~size_t(15);
+    const size_t res_bytes = cnt_bytes + total_n * 4;                  // n_matches of every job, then every job's matches: one D2H
+    const size_t o_res = st.reserve(res_bytes), o_bins = st.reserve(total_n + 16);
+    const size_t total = st.off;
+    st.off = input_end;
+    borb_status s;
+    if ((s = ensure_host(m, input_end)) != BORB_OK) return s;
+    if ((s = ensure_arena(m, total)) != BORB_OK) return s;
+    if ((s = ensure_out(m, res_bytes)) != BORB_OK) return s;
+    BORB_CUDA(cudaStreamSynchronize(m->stream));
+    uint8_t* b = m->arena;
+    KfDev* hq = reinterpret_cast<KfDev*>(m->h_stage + o_q);
+    KfDev* ht = reinterpret_cast<KfDev*>(m->h_stage + o_t);
+    size_t* hoff = reinterpret_cast<size_t*>(m->h_stage + o_off);
+    for (int j = 0; j < n_jobs; j++) {
+        const borb_bow_job& B = jobs[j];
+        hq[j] = B.kf_frame ? resident_kf_dev(B.kf_frame, B.kf.has_mp ? b + o_hm[j] : nullptr) : kf_dev(m, &B.kf, ko[j]);
+        ht[j] = resident_kf_dev(B.frame, nullptr);
+        hoff[j] = off[j];
+    }
+    if ((s = commit(st, total)) != BORB_OK) return s;
+    for (int j = 0; j < n_jobs; j++) {
+        BORB_CUDA(cudaStreamWaitEvent(m->stream, jobs[j].frame->ready, 0));
+        if (jobs[j].kf_frame) BORB_CUDA(cudaStreamWaitEvent(m->stream, jobs[j].kf_frame->ready, 0));
+    }
+    m->launches += launch_bow_match((const KfDev*)(b + o_q), (const KfDev*)(b + o_t), n_jobs, 0, nnratio, check_orientation,
+                                    (int32_t*)(b + o_res + cnt_bytes), 0, (const size_t*)(b + o_off), b + o_bins, (int32_t*)(b + o_res), max_t,
+                                    m->stream);
+    BORB_CUDA(cudaGetLastError());
+    BORB_CUDA(cudaMemcpyAsync(m->h_out, b + o_res, res_bytes, cudaMemcpyDeviceToHost, m->stream));
+    BORB_CUDA(cudaStreamSynchronize(m->stream));
+    for (int j = 0; j < n_jobs; j++) {
+        std::memcpy(&n_matches[j], m->h_out + (size_t)j * 4, 4);
+        std::memcpy(jobs[j].match, m->h_out + cnt_bytes + off[j] * 4, (size_t)jobs[j].frame->n * 4);
+    }
+    return BORB_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1955,6 +2051,91 @@ borb_status borb_compute_bow(borb_voc* v, const uint8_t* desc, int n, int levels
     }
     fv_start[nn] = (int32_t)byn.size();
     *n_bow = nb; *n_nodes = nn;
+    return BORB_OK;
+}
+
+// Frame::ComputeBoW for many resident frames: borb_compute_bow's descent and bookkeeping both on the device (bow_transform_batch_kernel,
+// bow_build_kernel), two launches and one synchronisation; the vectors stay with the frames for borb_search_by_bow_batch.
+borb_status borb_frames_compute_bow(borb_matcher* m, borb_voc* v, borb_frame* const* frames, int n_frames, int levelsup,
+                                    uint32_t* const* bow_word, double* const* bow_value, int32_t* n_bow, uint32_t* const* fv_node,
+                                    int32_t* const* fv_start, uint32_t* const* fv_idx, int32_t* n_nodes) {
+    if (!m || !v || n_frames < 0 || (n_frames > 0 && !frames)) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+    if (n_frames == 0) return BORB_OK;
+    if (v->device != m->device) { set_error("vocabulary and matcher live on different devices"); return BORB_ERR_INVALID_ARG; }
+    int max_n = 0;
+    for (int i = 0; i < n_frames; i++) {
+        const borb_frame* f = frames[i];
+        if (!f) { set_error("frame %d: not a device-resident frame", i); return BORB_ERR_INVALID_ARG; }
+        if (f->device != m->device) { set_error("frame %d: frame and matcher live on different devices", i); return BORB_ERR_INVALID_ARG; }
+        if (f->n < 0 || f->n > MATCH_MAX_FEATURES) { set_error("frame %d: %d features (limit %d)", i, f->n, MATCH_MAX_FEATURES); return BORB_ERR_INVALID_ARG; }
+        max_n = std::max(max_n, f->n);
+    }
+    auto wants = [&](int i) {
+        return (bow_word && bow_word[i]) || (bow_value && bow_value[i]) || (fv_node && fv_node[i]) || (fv_start && fv_start[i]) || (fv_idx && fv_idx[i]);
+    };
+    BORB_CUDA(cudaSetDevice(m->device));
+    Stager st(m);
+    const size_t o_jobs = st.add(nullptr, (size_t)n_frames * sizeof(BowFrameJob));     // filled in place
+    const size_t input_end = st.off;
+    std::vector<size_t> o_scr(n_frames), o_copy(n_frames, 0);
+    const size_t cnt_bytes = ((size_t)n_frames * 8 + 15) & ~size_t(15);
+    size_t res_bytes = cnt_bytes;                       // (n_bow, n_nodes) of every frame, then the host copies: one D2H
+    for (int i = 0; i < n_frames; i++) {
+        const size_t n = (size_t)frames[i]->n;
+        o_scr[i] = st.reserve(n * 16);                  // weight f64 | word i32 | node i32
+        if (wants(i)) { o_copy[i] = res_bytes; res_bytes += (n * 24 + 4 + 15) & ~size_t(15); }   // value | word | node | start | idx
+    }
+    const size_t o_res = st.reserve(res_bytes);
+    const size_t total = st.off;
+    st.off = input_end;
+    borb_status s;
+    if ((s = ensure_host(m, input_end)) != BORB_OK) return s;
+    if ((s = ensure_arena(m, total)) != BORB_OK) return s;
+    if ((s = ensure_out(m, res_bytes)) != BORB_OK) return s;
+    BORB_CUDA(cudaStreamSynchronize(m->stream));
+    uint8_t* b = m->arena;
+    BowFrameJob* hj = reinterpret_cast<BowFrameJob*>(m->h_stage + o_jobs);
+    for (int i = 0; i < n_frames; i++) {
+        borb_frame* f = frames[i];
+        const size_t n = (size_t)f->n;
+        BowFrameJob J{};
+        J.desc = f->desc; J.n = f->n;
+        J.weight = (double*)(b + o_scr[i]); J.word = (int32_t*)(b + o_scr[i] + n * 8); J.node = (int32_t*)(b + o_scr[i] + n * 12);
+        J.dst = BowTables{f->bow_word, f->bow_value, f->fv_node, f->fv_start, f->fv_idx};
+        if (wants(i)) {
+            uint8_t* c = b + o_res + o_copy[i];
+            J.copy = BowTables{(uint32_t*)(c + n * 8), (double*)c, (uint32_t*)(c + n * 12), (int32_t*)(c + n * 16), (uint32_t*)(c + n * 20 + 4)};
+        }
+        J.counts = (int32_t*)(b + o_res) + 2 * i;
+        hj[i] = J;
+        f->has_bow = false;                             // the storage is rewritten from here on
+    }
+    if ((s = commit(st, total)) != BORB_OK) return s;
+    for (int i = 0; i < n_frames; i++) BORB_CUDA(cudaStreamWaitEvent(m->stream, frames[i]->ready, 0));
+    m->launches += launch_bow_frames(v->dev, (const BowFrameJob*)(b + o_jobs), n_frames, max_n, levelsup, m->stream);
+    BORB_CUDA(cudaGetLastError());
+    for (int i = 0; i < n_frames; i++) BORB_CUDA(cudaEventRecord(frames[i]->ready, m->stream));
+    BORB_CUDA(cudaMemcpyAsync(m->h_out, b + o_res, res_bytes, cudaMemcpyDeviceToHost, m->stream));
+    BORB_CUDA(cudaStreamSynchronize(m->stream));
+    const uint8_t* h = m->h_out;
+    for (int i = 0; i < n_frames; i++) {
+        borb_frame* f = frames[i];
+        int32_t cnt[2];
+        std::memcpy(cnt, h + (size_t)i * 8, 8);
+        f->n_bow = cnt[0]; f->n_nodes = cnt[1]; f->has_bow = true;
+        if (n_bow) n_bow[i] = cnt[0];
+        if (n_nodes) n_nodes[i] = cnt[1];
+        if (!wants(i)) continue;
+        const size_t n = (size_t)f->n;
+        const uint8_t* c = h + o_copy[i];
+        int32_t kept = 0;
+        std::memcpy(&kept, c + n * 16 + (size_t)cnt[1] * 4, 4);        // fv_start[n_nodes]
+        if (bow_value && bow_value[i]) std::memcpy(bow_value[i], c, (size_t)cnt[0] * 8);
+        if (bow_word && bow_word[i]) std::memcpy(bow_word[i], c + n * 8, (size_t)cnt[0] * 4);
+        if (fv_node && fv_node[i]) std::memcpy(fv_node[i], c + n * 12, (size_t)cnt[1] * 4);
+        if (fv_start && fv_start[i]) std::memcpy(fv_start[i], c + n * 16, (size_t)(cnt[1] + 1) * 4);
+        if (fv_idx && fv_idx[i]) std::memcpy(fv_idx[i], c + n * 20 + 4, (size_t)kept * 4);
+    }
     return BORB_OK;
 }
 

@@ -11,7 +11,9 @@
 //   triangulation_kernel  SearchForTriangulation (:657-823): no sequential dependence (vbMatched2 is never set in
 //       the reference), "dist<=bestDist, later wins" == min over (distance, -position); epipolar tests as :140-157.
 //   bow_transform_kernel  TemplatedVocabulary::transform (Thirdparty/DBoW2/DBoW2/TemplatedVocabulary.h:1218-1259):
-//       a warp per descriptor descends the tree, lanes = children, first-wins argmin.
+//       a warp per descriptor descends the tree, lanes = children, first-wins argmin (bow_transform_batch_kernel: the same
+//       descent for many resident frames, grid.y = frame).
+//   bow_build_kernel      the BowVector / FeatureVector bookkeeping of transform (:1150-1194) on the device, a CTA per frame.
 // All float tests use _rn intrinsics (no FMA contraction) so comparisons match the reference bit for bit.
 //
 // Bound: latency / POPC issue (15 thread-ops/clk/SM measured); the batch (map points, keyframes) supplies parallelism.
@@ -483,9 +485,11 @@ constexpr int BOW_JCAP = 1024;      // widest target bucket the matrix path hand
 constexpr int BOW_RCAP = 256;       // rows per chunk
 constexpr int BOW_WARP_WORDS = BOW_DCAP / 2 + BOW_JCAP / 2 + BOW_RCAP / 2;
 
+// out_off (mode 0 only, may be null): pair p searches its own frame ts[p] and writes at match + out_off[p] (borb_search_by_bow_batch);
+// null: every pair searches ts[0] and writes at match + p * out_stride.
 __global__ void __launch_bounds__(32 * BOW_WARPS) bow_match_kernel(const KfDev* __restrict__ qs, const KfDev* __restrict__ ts, int n_pairs,
                                                                    int mode, float nnratio, int check_ori, int32_t* __restrict__ match,
-                                                                   int out_stride, uint8_t* __restrict__ bins,
+                                                                   int out_stride, const size_t* __restrict__ out_off, uint8_t* __restrict__ bins,
                                                                    int32_t* __restrict__ n_matches, int max_t) {
     extern __shared__ uint32_t sm[];
     __shared__ int hist[32];
@@ -498,9 +502,10 @@ __global__ void __launch_bounds__(32 * BOW_WARPS) bow_match_kernel(const KfDev* 
     uint16_t* J = D + BOW_DCAP;                                                  // target feature per column (0xFFFF = unusable)
     uint16_t* R = J + BOW_JCAP;                                                  // query feature per row of the chunk
     const KfDev q = qs[pair];
-    const KfDev t = ts[mode == 0 ? 0 : pair];
-    int32_t* out = match + (size_t)pair * out_stride;
-    uint8_t* bin = bins + (size_t)pair * out_stride;
+    const KfDev t = ts[(mode == 0 && out_off == nullptr) ? 0 : pair];
+    const size_t o0 = out_off != nullptr ? out_off[pair] : (size_t)pair * out_stride;
+    int32_t* out = match + o0;
+    uint8_t* bin = bins + o0;
     const int nout = mode == 0 ? t.n : q.n;
     for (int i = tid; i < nout; i += 32 * BOW_WARPS) out[i] = -1;
     for (int w = tid; w < words; w += 32 * BOW_WARPS) claimed[w] = 0;
@@ -719,12 +724,10 @@ __global__ void __launch_bounds__(256) triangulation_kernel(KfDev q, KfDev t, Tr
 }
 
 // ------------------------------------------------------------------------------------------------ vocabulary
-__global__ void __launch_bounds__(256) bow_transform_kernel(VocDev V, const uint8_t* __restrict__ desc, int n, int levelsup,
-                                                            int32_t* __restrict__ word, double* __restrict__ weight,
-                                                            int32_t* __restrict__ node) {
+// descent of feature f (a warp)
+__device__ __forceinline__ void bow_descend(const VocDev& V, const uint8_t* __restrict__ desc, int f, int levelsup, int32_t* __restrict__ word,
+                                            double* __restrict__ weight, int32_t* __restrict__ node) {
     const int lane = threadIdx.x & 31;
-    const int f = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    if (f >= n) return;
     // the descriptor is read ONCE into registers: `desc` may be pinned host memory (borb_bow_transform reads it in place)
     const uint4 f0 = reinterpret_cast<const uint4*>(desc)[(size_t)f * 2], f1 = reinterpret_cast<const uint4*>(desc)[(size_t)f * 2 + 1];
     const uint32_t feat[8] = {f0.x, f0.y, f0.z, f0.w, f1.x, f1.y, f1.z, f1.w};
@@ -748,6 +751,140 @@ __global__ void __launch_bounds__(256) bow_transform_kernel(VocDev V, const uint
         word[f] = V.word_id[final_id];
         weight[f] = V.weight[final_id];
         node[f] = nid;
+    }
+}
+
+__global__ void __launch_bounds__(256) bow_transform_kernel(VocDev V, const uint8_t* __restrict__ desc, int n, int levelsup,
+                                                            int32_t* __restrict__ word, double* __restrict__ weight,
+                                                            int32_t* __restrict__ node) {
+    const int f = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (f < n) bow_descend(V, desc, f, levelsup, word, weight, node);
+}
+// many resident frames in one launch (borb_frames_compute_bow): grid.y = frame, results in the frame's device scratch
+__global__ void __launch_bounds__(256) bow_transform_batch_kernel(VocDev V, const BowFrameJob* __restrict__ jobs, int levelsup) {
+    const BowFrameJob& J = jobs[blockIdx.y];
+    const int f = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (f < J.n) bow_descend(V, J.desc, f, levelsup, J.word, J.weight, J.node);
+}
+
+namespace {
+// ascending bitonic sort of K (a power of two) 64-bit keys in shared memory by the whole CTA; ends with a barrier
+__device__ void bitonic_sort_u64(uint64_t* k, int K) {
+    const int half = K >> 1;
+    for (int kk = 2; kk <= K; kk <<= 1)
+        for (int j = kk >> 1; j > 0; j >>= 1) {
+            for (int p = threadIdx.x; p < half; p += blockDim.x) {
+                const int i = ((p & ~(j - 1)) << 1) | (p & (j - 1));          // lower element of the p-th compare pair
+                const uint64_t a = k[i], b = k[i + j];
+                if ((a > b) == ((i & kk) == 0)) { k[i] = b; k[i + j] = a; }
+            }
+            __syncthreads();
+        }
+}
+
+// Exclusive prefix count of the run heads among sorted keys [0, m): a head is the first key of a run of equal high words.
+// Each thread owns the contiguous chunk [c0, c1); returns the number of heads before c0, and the total in *total.
+__device__ int count_heads_before(const uint64_t* k, int m, int c0, int c1, int* warp_sums, int* total) {
+    int c = 0;
+    for (int r = c0; r < c1; r++) c += (r == 0 || (k[r] >> 32) != (k[r - 1] >> 32)) ? 1 : 0;
+    const int lane = threadIdx.x & 31, wrp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    int incl = c;
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+        const int v = __shfl_up_sync(0xFFFFFFFFu, incl, off);
+        if (lane >= off) incl += v;
+    }
+    if (lane == 31) warp_sums[wrp] = incl;
+    __syncthreads();
+    int before = incl - c, all = 0;
+    for (int w = 0; w < nw; w++) {
+        const int s = warp_sums[w];
+        if (w < wrp) before += s;
+        all += s;
+    }
+    *total = all;
+    __syncthreads();                                                     // warp_sums is reused by the next call
+    return before;
+}
+}  // namespace
+
+// The bookkeeping half of TemplatedVocabulary::transform (TemplatedVocabulary.h:1150-1194) for one frame per CTA, from the
+// per-feature (word, weight, node) of the descent — what borb_compute_bow does on the host, bit for bit:
+//   kept features (weight > 0: stop words drop out of both vectors, :1157) sorted by (word, feature) and by (node, feature);
+//   per word run the weights summed in feature order (BowVector::addWeight, `vit->second += v`); the L1 norm summed in word order
+//   (BowVector::normalize, BowVector.cpp:62-83) as one sequential chain of double adds (a tree reduction would round differently);
+//   every value divided by it when it is > 0; the FeatureVector as CSR from the node order.
+// Shared memory: 16 B per key slot (K = next power of two >= n, at least 32): the sort keys, then the run values.
+__global__ void __launch_bounds__(1024) bow_build_kernel(const BowFrameJob* __restrict__ jobs) {
+    extern __shared__ __align__(16) uint64_t bb_sm[];
+    __shared__ int warp_sums[32];
+    __shared__ int s_m;
+    __shared__ double s_norm;
+    const BowFrameJob& J = jobs[blockIdx.x];
+    const int n = J.n, tid = threadIdx.x, T = blockDim.x;
+    int K = 32;
+    while (K < n) K <<= 1;
+    uint64_t* keys = bb_sm;
+    double* vals = reinterpret_cast<double*>(bb_sm + K);
+    constexpr uint64_t NONE = ~0ull;                                     // dropped feature / padding: sorts last
+    const int chunk = (K + T - 1) / T;                                   // the contiguous slice of sorted keys a thread scans
+    const int c0 = min(K, tid * chunk), c1 = min(K, c0 + chunk);
+    if (tid == 0) s_m = 0;
+    // ---- BowVector: (word, feature) order
+    for (int i = tid; i < K; i += T) keys[i] = (i < n && J.weight[i] > 0.0) ? ((uint64_t)(uint32_t)J.word[i] << 32) | (uint32_t)i : NONE;
+    __syncthreads();
+    bitonic_sort_u64(keys, K);
+    for (int r = c0; r < c1; r++)                                        // m = number of kept features = first NONE
+        if (keys[r] != NONE && (r + 1 == K || keys[r + 1] == NONE)) s_m = r + 1;
+    __syncthreads();
+    const int m = s_m;
+    int nb = 0;
+    int q = count_heads_before(keys, m, c0, min(c1, m), warp_sums, &nb);
+    for (int r = c0; r < min(c1, m); r++) {
+        const uint32_t w = (uint32_t)(keys[r] >> 32);
+        if (r > 0 && (uint32_t)(keys[r - 1] >> 32) == w) continue;
+        double v = J.weight[(uint32_t)keys[r]];
+        for (int e = r + 1; e < m && (uint32_t)(keys[e] >> 32) == w; e++) v = __dadd_rn(v, J.weight[(uint32_t)keys[e]]);   // in feature order
+        vals[q] = v;
+        J.dst.word[q] = w;
+        if (J.copy.word) J.copy.word[q] = w;
+        q++;
+    }
+    __syncthreads();
+    if (tid == 0) {                                                      // the serial chain of BowVector::normalize
+        double norm = 0.0;
+#pragma unroll 8
+        for (int k = 0; k < nb; k++) norm = __dadd_rn(norm, fabs(vals[k]));
+        s_norm = norm;
+    }
+    __syncthreads();
+    const double norm = s_norm;
+    for (int k = tid; k < nb; k += T) {
+        const double v = norm > 0.0 ? __ddiv_rn(vals[k], norm) : vals[k];
+        J.dst.value[k] = v;
+        if (J.copy.word) J.copy.value[k] = v;
+    }
+    // ---- FeatureVector: (node, feature) order; the kept set is the same
+    for (int i = tid; i < K; i += T) keys[i] = (i < n && J.weight[i] > 0.0) ? ((uint64_t)(uint32_t)J.node[i] << 32) | (uint32_t)i : NONE;
+    __syncthreads();
+    bitonic_sort_u64(keys, K);
+    int nn = 0;
+    q = count_heads_before(keys, m, c0, min(c1, m), warp_sums, &nn);
+    for (int r = c0; r < min(c1, m); r++) {
+        const uint32_t nd = (uint32_t)(keys[r] >> 32), f = (uint32_t)keys[r];
+        if (r == 0 || (uint32_t)(keys[r - 1] >> 32) != nd) {
+            J.dst.node[q] = nd; J.dst.start[q] = r;
+            if (J.copy.word) { J.copy.node[q] = nd; J.copy.start[q] = r; }
+            q++;
+        }
+        J.dst.idx[r] = f;
+        if (J.copy.word) J.copy.idx[r] = f;
+    }
+    if (tid == 0) {
+        J.dst.start[nn] = m;
+        if (J.copy.word) J.copy.start[nn] = m;
+        J.counts[0] = nb;
+        J.counts[1] = nn;
     }
 }
 
@@ -821,11 +958,12 @@ int launch_sim3_agree(const int32_t* match1, const int32_t* match2, int n1, int 
     return 1;
 }
 int launch_bow_match(const KfDev* qs, const KfDev* ts, int n_pairs, int mode, float nnratio, int check_ori, int32_t* match,
-                     int out_stride, uint8_t* bins, int32_t* n_matches, int max_t, cudaStream_t s) {
+                     int out_stride, const size_t* out_off, uint8_t* bins, int32_t* n_matches, int max_t, cudaStream_t s) {
     const int words = (max_t + 31) / 32;
     const size_t smem = (size_t)(words + BOW_WARPS * BOW_WARP_WORDS) * 4;
     allow_max_smem((const void*)bow_match_kernel);
-    bow_match_kernel<<<n_pairs, 32 * BOW_WARPS, smem, s>>>(qs, ts, n_pairs, mode, nnratio, check_ori, match, out_stride, bins, n_matches, max_t);
+    bow_match_kernel<<<n_pairs, 32 * BOW_WARPS, smem, s>>>(qs, ts, n_pairs, mode, nnratio, check_ori, match, out_stride, out_off, bins, n_matches,
+                                                         max_t);
     return 1;
 }
 int launch_triangulation(const KfDev& q, const KfDev& t, const TriArgs& T, int32_t* vmatch, uint8_t* bins, int32_t* pairs, int cap,
@@ -837,6 +975,15 @@ int launch_bow_transform(const VocDev& V, const uint8_t* desc, int n, int levels
                          cudaStream_t s) {
     if (n > 0) bow_transform_kernel<<<(n + 7) / 8, 256, 0, s>>>(V, desc, n, levelsup, word, weight, node);
     return 1;
+}
+int launch_bow_frames(const VocDev& V, const BowFrameJob* d_jobs, int n_frames, int max_n, int levelsup, cudaStream_t s) {
+    if (n_frames <= 0) return 0;
+    bow_transform_batch_kernel<<<dim3((max(max_n, 1) + 7) / 8, n_frames), 256, 0, s>>>(V, d_jobs, levelsup);
+    int K = 32;
+    while (K < max_n) K <<= 1;
+    allow_max_smem((const void*)bow_build_kernel);
+    bow_build_kernel<<<n_frames, 1024, (size_t)K * 16, s>>>(d_jobs);
+    return 2;
 }
 
 }  // namespace borb

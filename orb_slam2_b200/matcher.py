@@ -49,6 +49,10 @@ class _KeyFrameViewC(C.Structure):
                 ("fv", _FeatVecC), ("n_levels", C.c_int32), ("scale_factors", C.c_void_p), ("level_sigma2", C.c_void_p)]
 
 
+class _BowJobC(C.Structure):                       # borb_bow_job
+    _fields_ = [("frame", C.c_void_p), ("kf", _KeyFrameViewC), ("kf_frame", C.c_void_p), ("match", C.c_void_p)]
+
+
 class _LocalPointsJobC(C.Structure):               # borb_local_points_job
     _fields_ = [("frame", _FrameViewC), ("pts", _WorldPointsViewC), ("has_obs", C.c_void_p), ("Tcw", C.c_float * 12), ("Ow", C.c_float * 3)] + \
                [(n, C.c_float) for n in ("fx", "fy", "cx", "cy", "mbf", "log_scale_factor", "th")] + \
@@ -138,6 +142,7 @@ class FrameView:
     mfLogScaleFactor: Optional[float] = None              # Frame::mfLogScaleFactor; default logf(mvScaleFactors[1])
     mvInvLevelSigma2: Optional[np.ndarray] = None         # only read by Fuse(pKF, vpMapPoints, th)
     resident: Optional["ResidentFrame"] = None            # device-resident copy (borb_frame): only `occupied` travels per call
+    has_mp: Optional[np.ndarray] = None                   # as a reference keyframe of SearchByBoWBatch: MapPoint present && !isBad()
 
     def _view(self, with_ur: bool = True):
         """(ctypes view, arrays to keep alive).  With a resident frame only `occupied` is read from the host."""
@@ -571,6 +576,58 @@ class ORBmatcher:
         check(self._lib.borb_search_by_bow_kf(self._h, C.byref(c1), C.byref(c2), self.mfNNratio, int(self.mbCheckOrientation), _p(match), C.byref(nm)),
               "borb_search_by_bow_kf")
         return nm.value, match[:n1]
+
+    def ComputeBoWBatch(self, voc: "ORBVocabulary", frames: Sequence[FrameView], levelsup: int = 4, want_host: bool = True):
+        """borb_frames_compute_bow: Frame::ComputeBoW (src/Frame.cc:395-402) of many device-resident frames in one launch pair.  The
+        vectors stay with the frames (SearchByBoWBatch reads them).  Returns [(mBowVec as {word: value}, mFeatVec)] per frame, equal to
+        what ORBVocabulary.ComputeBoW returns for the frame's descriptors; with want_host=False nothing is copied back and the result
+        is None."""
+        n = len(frames)
+        hs = (C.c_void_p * max(n, 1))(*[F.resident._h.value if F.resident is not None else None for F in frames])
+        sizes = [F.resident.n if F.resident is not None else len(F.mvKeysUn) for F in frames]
+        outs = [(np.zeros(max(k, 1), np.uint32), np.zeros(max(k, 1), np.float64), np.zeros(max(k, 1), np.uint32), np.zeros(k + 1, np.int32),
+                 np.zeros(max(k, 1), np.uint32)) for k in sizes]
+        tables = [(C.c_void_p * max(n, 1))(*[o[t].ctypes.data for o in outs]) if want_host else None for t in range(5)]
+        nb, nn = np.zeros(max(n, 1), np.int32), np.zeros(max(n, 1), np.int32)
+        check(self._lib.borb_frames_compute_bow(self._h, voc._h, hs, n, int(levelsup), tables[0], tables[1], _p(nb), tables[2], tables[3],
+                                                tables[4], _p(nn)), "borb_frames_compute_bow")
+        if not want_host:
+            return None
+        res = []
+        for j, (bw, bv, fn, fs, fi) in enumerate(outs):
+            b, a = int(nb[j]), int(nn[j])
+            res.append((dict(zip(bw[:b].tolist(), bv[:b].tolist())), FeatureVector(fn[:a].copy(), fs[:a + 1].copy(), fi[:fs[a]].copy())))
+        return res
+
+    def SearchByBoWBatch(self, kfs, frames: Sequence[FrameView]):
+        """borb_search_by_bow_batch: TrackReferenceKeyFrame's SearchByBoW(KeyFrame*, Frame&) (src/ORBmatcher.cc:159-288) of many
+        independent camera streams in one launch.  frames[j] = device-resident FrameView whose BoW ComputeBoWBatch computed; kfs[j] =
+        a KeyFrameView, or a resident FrameView with BoW and has_mp (then only has_mp crosses PCIe).  Returns [(nmatches, match)] per
+        job, equal to what SearchByBoW returns on host views of the same data."""
+        n = len(frames)
+        assert n == len(kfs)
+        jobs = (_BowJobC * max(n, 1))()
+        keep, outs = [], []
+        for j, (kf, F) in enumerate(zip(kfs, frames)):
+            nF = F.resident.n if F.resident is not None else len(F.mvKeysUn)
+            match = np.full(max(nF, 1), -1, np.int32)
+            J = jobs[j]
+            J.frame = F.resident._h.value if F.resident is not None else None
+            if isinstance(kf, KeyFrameView):
+                J.kf = kf._c()
+                keep.append(list(kf._keep))              # the same view may serve several jobs: _c() replaces kf._keep
+            elif isinstance(kf, FrameView) and kf.resident is not None:
+                hm = np.ascontiguousarray(kf.has_mp, np.uint8) if kf.has_mp is not None else None
+                J.kf = _KeyFrameViewC(0, None, None, _p(hm))
+                J.kf_frame = kf.resident._h.value
+                keep.append(hm)
+            else:
+                raise ValueError(f"kfs[{j}]: a KeyFrameView or a device-resident FrameView")
+            J.match = _p(match)
+            outs.append((nF, match))
+        nm = np.zeros(max(n, 1), np.int32)
+        check(self._lib.borb_search_by_bow_batch(self._h, jobs, n, self.mfNNratio, int(self.mbCheckOrientation), _p(nm)), "borb_search_by_bow_batch")
+        return [(int(nm[j]), match[:nF]) for j, (nF, match) in enumerate(outs)]
 
     def SearchForTriangulation(self, pKF1: KeyFrameView, pKF2: KeyFrameView, F12: np.ndarray, epipole: Tuple[float, float],
                                bOnlyStereo: bool = False) -> np.ndarray:
