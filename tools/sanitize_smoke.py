@@ -15,6 +15,14 @@ print("stereo", len(out[0]["mvKeys"]), int((out[0]["mvuRight"] >= 0).sum()))
 G2 = ORBextractor(500)
 k, d = G2(synth.white_noise(1, 400, 300))
 print("noise", len(k))
+# geometry edges (tests/extract_geometry.py): the smallest accepted frame, a frame whose level-0 pitch is exactly its width + 8
+# (no slack after the padding), and a level 0 one candidate over the quadtree's on-chip limit
+from tests import extract_geometry as EG
+print("smallest", len(ORBextractor(1000)(synth.mono_frame(2, 0, 0, 221, 221))[0]))
+print("tight pitch", len(ORBextractor(1000)(synth.white_noise(3, 376, 240))[0]))
+G3 = ORBextractor(EG.DOT_NFEATURES)
+k = G3(EG.dot_image(5121, *synth.KITTI, 1))[0]
+print("5121 candidates", len(G3.debug_candidates(0)), len(k))
 v = mf.two_views(O, 7)
 F, mps = mf.projection_case(v, 1)
 mt = M.ORBmatcher(0.8, True)
