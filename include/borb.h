@@ -590,6 +590,10 @@ BORB_API borb_status borb_debug_blurred(borb_extractor* e, int image, int level,
 /* Ablation of fast_kernel for speed-of-light measurements (tools/fast_ablation.py; 0 = full kernel, the only mode that produces
  * keypoints; 1 = TMA tile load only, 2 = + packed reject pass, 3 = + exact scores without NMS / emit). */
 BORB_API borb_status borb_debug_set_fast_mode(borb_extractor* e, int mode);
+/* The rBRIEF tap order of the descriptor kernel (host table, no device needed): *n_bins orientation bins of 512 entries each,
+ * entry = (x + 128) | (y + 128) << 8 | point << 16 for pattern point `point` (= 2 * test + 0/1) at (x, y); the first
+ * min(cap, 512 * *n_bins) entries go to dst (may be NULL). */
+BORB_API borb_status borb_debug_brief_slots(uint32_t* dst, int cap, int* n_bins);
 /* Distance arithmetic of the database SearchByBoW kernel: 2 (default) = three 3:2 compressors + 5 POPC per 256-bit distance,
  * 1 = full carry-save adder tree + 4 POPC, 0 = 8 POPC.  Same results; kept switchable for measurements. */
 BORB_API borb_status borb_debug_set_bow_csa(int mode);

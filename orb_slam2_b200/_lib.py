@@ -129,6 +129,7 @@ _SIGNATURES = {
     "borb_debug_set_bow_csa": (C.c_int, [C.c_int]),
     "borb_debug_set_bow_item_target": (C.c_int, [C.c_int]),
     "borb_debug_set_fast_mode": (C.c_int, [vp, C.c_int]),
+    "borb_debug_brief_slots": (C.c_int, [vp, C.c_int, i32p]),
     "borb_launch_count": (C.c_int, [vp, C.POINTER(C.c_uint64)]),
     "borb_stage_times": (C.c_int, [vp, f32p]),
     "borb_set_timing": (C.c_int, [vp, C.c_int]),

@@ -135,6 +135,10 @@ bool resize_window_table(const std::vector<int16_t>& tabs, size_t xtab_first, in
     return ok;
 }
 
+const int8_t kPattern[1024] = {          // bit_pattern_31_: (x0, y0, x1, y1) per test
+#include "orb_pattern.inc"
+};
+
 borb_status build_geometry(borb_extractor* e, int w, int h, std::vector<int16_t>& tabs) {
     Geometry& g = e->geom;
     std::memset(&g, 0, sizeof(g));
@@ -212,7 +216,7 @@ borb_status build_geometry(borb_extractor* e, int w, int h, std::vector<int16_t>
 void free_workspace(Workspace& ws) {
     cudaFree(ws.pyr); cudaFree(ws.blur); cudaFree(ws.cand); cudaFree(ws.cand_cnt); cudaFree(ws.pnode); cudaFree(ws.sel);
     cudaFree(ws.sel_cnt); cudaFree(ws.kps); cudaFree(ws.desc); cudaFree(ws.nkp); cudaFree(ws.u_right); cudaFree(ws.depth);
-    cudaFree(ws.sad); cudaFree(ws.tabs); cudaFree(ws.pair_idx); cudaFree(ws.st_bins); cudaFree(ws.st_recs); cudaFree(ws.stage);
+    cudaFree(ws.sad); cudaFree(ws.tabs); cudaFree(ws.brief_slots); cudaFree(ws.pair_idx); cudaFree(ws.st_bins); cudaFree(ws.st_recs); cudaFree(ws.stage);
     free(ws.fast_tmaps); cudaFree(ws.fast_tiles);
     ws = Workspace();
 }
@@ -254,6 +258,9 @@ borb_status ensure(borb_extractor* e, int w, int h, int n_images) {
     BORB_CUDA(cudaMalloc(&ws.st_recs, n * (size_t)stereo_rec_stride(g) * stereo_rec_bytes()));
     BORB_CUDA(cudaMalloc(&ws.tabs, (tabs.size() + 4) * sizeof(int16_t)));
     BORB_CUDA(cudaMemcpy(ws.tabs, tabs.data(), tabs.size() * sizeof(int16_t), cudaMemcpyHostToDevice));
+    const std::vector<uint32_t>& slots = brief_slot_table();
+    BORB_CUDA(cudaMalloc(&ws.brief_slots, slots.size() * sizeof(uint32_t)));
+    BORB_CUDA(cudaMemcpy(ws.brief_slots, slots.data(), slots.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
     BORB_CUDA(cudaMemset(ws.nkp, 0, n * sizeof(int)));
     BORB_CUDA(cudaMallocHost(&e->h_counts, n * 2 * sizeof(int)));
     ws.max_images = (int)n;
@@ -493,6 +500,34 @@ borb_status finish_timing(borb_extractor* e) {
 }
 
 }  // namespace
+
+// Plain double math is enough here: the order only groups the taps, every order gives the same descriptor.
+const std::vector<uint32_t>& brief_slot_table() {
+    static const std::vector<uint32_t> table = [] {
+        std::vector<uint32_t> t((size_t)BRIEF_BINS * 512);
+        int row[512], col[512], order[512];
+        for (int b = 0; b < BRIEF_BINS; b++) {
+            const double th = (b + 0.5) * (2.0 * 3.14159265358979323846 / BRIEF_BINS);
+            const double a = std::cos(th), s = std::sin(th);
+            for (int p = 0; p < 512; p++) {
+                const int x = kPattern[2 * p], y = kPattern[2 * p + 1];
+                row[p] = (int)std::lround(x * s + y * a);
+                col[p] = (int)std::lround(x * a - y * s);
+                order[p] = p;
+            }
+            std::sort(order, order + 512, [&](int i, int j) {
+                return row[i] != row[j] ? row[i] < row[j] : (col[i] != col[j] ? col[i] < col[j] : i < j);
+            });
+            for (int k = 0; k < 512; k++) {
+                const int p = order[k];
+                t[(size_t)b * 512 + k] = (uint32_t)(kPattern[2 * p] + 128) | (uint32_t)(kPattern[2 * p + 1] + 128) << 8 | (uint32_t)p << 16;
+            }
+        }
+        return t;
+    }();
+    return table;
+}
+
 }  // namespace borb
 
 using namespace borb;
@@ -768,6 +803,14 @@ borb_status borb_debug_set_fast_mode(borb_extractor* e, int mode) {
     if (!e || mode < 0 || mode > 3) { set_error("fast mode must be 0..3"); return BORB_ERR_INVALID_ARG; }
     e->fast_mode = mode;
     if (e->have_geom) e->geom.fast_mode = mode;
+    return BORB_OK;
+}
+
+borb_status borb_debug_brief_slots(uint32_t* dst, int cap, int* n_bins) {
+    if (!n_bins) { set_error("n_bins is NULL"); return BORB_ERR_INVALID_ARG; }
+    const std::vector<uint32_t>& t = brief_slot_table();
+    *n_bins = BRIEF_BINS;
+    if (dst) std::memcpy(dst, t.data(), std::min((size_t)(cap > 0 ? cap : 0), t.size()) * sizeof(uint32_t));
     return BORB_OK;
 }
 

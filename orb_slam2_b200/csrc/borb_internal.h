@@ -84,6 +84,7 @@ struct Workspace {
     float* depth = nullptr;
     int* sad = nullptr;            // SAD distance per left keypoint (-1: none)
     int16_t* tabs = nullptr;       // resize tables
+    uint32_t* brief_slots = nullptr;   // rBRIEF tap order, brief_slot_table()
     int* pair_idx = nullptr;       // 2 * max_pairs (left,right image indices)
     int* st_bins = nullptr;        // stereo row-bin offsets, per pair
     void* st_recs = nullptr;       // stereo binned right-keypoint records, per pair
@@ -93,6 +94,14 @@ struct Workspace {
     void* fast_tiles = nullptr;    // DEVICE: one 16-byte descriptor per FAST CTA of an image (k_fast.cu: FastTile), n = fast_n_tiles
     int fast_n_tiles = 0;
 };
+
+// rBRIEF tap order of describe_kernel.  The circle is split into BRIEF_BINS orientation bins; a keypoint whose angle falls in
+// bin b fetches its 512 pattern points (point 2t + i = point i of test t) in the order of entries [b * 512, b * 512 + 512):
+// the points sorted by (row, column) of their rotated position at the bin's centre angle, so that the 32 lanes of one gather
+// touch a few adjacent rows of the patch.  Entry = x + 128 | (y + 128) << 8 | point << 16 (x, y: pattern coordinates).
+// Any order gives the same descriptor: the order only decides which lane fetches which point.
+constexpr int BRIEF_BINS = 32;
+const std::vector<uint32_t>& brief_slot_table();
 
 void set_error(const char* fmt, ...);
 // Raises `func`'s dynamic shared-memory limit to the device's opt-in maximum (minus the kernel's static shared memory),

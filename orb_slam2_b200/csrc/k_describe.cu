@@ -9,19 +9,21 @@
 //   operator() tail (:1059-1104) — levels concatenated 0..n-1, pt *= mvScaleFactor[level], size, octave.
 // sinf/cosf: device port (double arithmetic) of the glibc >= 2.28 single-precision kernels the
 // reference binary calls on x86-64 (ARM optimized-routines sincosf); checked exhaustively on the CPU
-// against glibc for every float in [0, 2*pi] (DESIGN.md).  Lane t%32 evaluates test t; a warp ballot
-// IS the packed little-endian uint32 of 4 descriptor bytes, so a descriptor is 8 ballots.
+// against glibc for every float in [0, 2*pi] (DESIGN.md).  The 512 taps are fetched in the order of the keypoint's
+// orientation bin (brief_slot_table, borb_internal.h): one gather instruction then touches a few adjacent rows of the
+// patch (~4 128-byte lines) instead of points spread over the whole 37 x 37 window (~20 lines).  Each tap byte goes to
+// its canonical place 2*test + which in the warp's 512 B of shared memory; lane t%32 then reads test t's two bytes as one
+// u16 and a warp ballot IS the packed little-endian uint32 of 4 descriptor bytes, so a descriptor is 8 ballots.
 //
-// Bound: L2 gather latency (512 blurred taps + 749 disc pixels per keypoint).
+// Bound: not the tap gathers' L1 wavefronts: cutting their lines from ~20 to ~4 per instruction left the kernel's own time
+// unchanged (DESIGN.md §5), and prefetching the blurred window into L1 made it 25 % slower.  What remains is filling the
+// 37 x 37 blurred and 31 x 31 level windows of every keypoint from L2 (which of their traffic or latency binds: not
+// measured).  The shorter tap instructions do raise the throughput of the whole pipeline with several streams in flight.
 #include "borb_internal.h"
 
 namespace borb {
 
 namespace {
-
-__device__ const float d_pattern[1024] = {      // bit_pattern_31_ as float: (x0, y0, x1, y1) per test, 4 KB, L1 resident
-#include "orb_pattern.inc"
-};
 
 // glibc sinf/cosf kernels for |x| < 120 (reduce_fast + degree-8/7 polynomials in double)
 struct SinCosTab { double sign[4]; double hpi_inv, hpi, c0, c1, c2, c3, c4, s1, s2, s3; };
@@ -92,9 +94,11 @@ __device__ __forceinline__ float fast_atan2_deg(float y, float x) {
 
 // 32 registers (8 CTAs/SM): the kernel is bound by gather latency and L1 wavefronts, occupancy pays (0.173 -> 0.150 ms)
 __global__ void __launch_bounds__(256, 8) describe_kernel(const __grid_constant__ Geometry g, const uint8_t* __restrict__ pyr,
-                                                       const uint8_t* __restrict__ blur, const uint32_t* __restrict__ sel,
-                                                       const int* __restrict__ sel_cnt, borb_keypoint* __restrict__ kps,
-                                                       uint8_t* __restrict__ desc, int* __restrict__ nkp) {
+                                                       const uint8_t* __restrict__ blur, const uint32_t* __restrict__ slots,
+                                                       const uint32_t* __restrict__ sel, const int* __restrict__ sel_cnt,
+                                                       borb_keypoint* __restrict__ kps, uint8_t* __restrict__ desc,
+                                                       int* __restrict__ nkp) {
+    __shared__ __align__(4) uint8_t taps[8][512];
     const int img = blockIdx.y;
     const int lane = threadIdx.x & 31;
     const int idx = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -144,18 +148,25 @@ __global__ void __launch_bounds__(256, 8) describe_kernel(const __grid_constant_
     const float t = __fmul_rn(angle, factorPI);
     const float a = glibc_sincosf(t, 1), b = glibc_sincosf(t, 0);
     const uint8_t* cb = blur + lvl_off + (size_t)py * pitch + px;
+    const int bin = min((int)(angle * (float)(BRIEF_BINS / 360.0)), BRIEF_BINS - 1);    // fast_atan2_deg may return 360
+    const uint32_t* slot = slots + bin * 512 + lane;
+    uint8_t* tw = taps[threadIdx.x >> 5];
+#pragma unroll
+    for (int k = 0; k < 16; k++) {
+        const uint32_t s = __ldg(slot + k * 32);
+        // x + 128 and y + 128 as the low mantissa bits of 2^23: one PRMT and one exact FADD per coordinate
+        const float x = __fsub_rn(__uint_as_float(__byte_perm(s, 0x4B000000u, 0x7440)), 8388736.f);
+        const float y = __fsub_rn(__uint_as_float(__byte_perm(s, 0x4B000000u, 0x7441)), 8388736.f);
+        const int r = __float2int_rn(__fadd_rn(__fmul_rn(x, b), __fmul_rn(y, a)));
+        const int q = __float2int_rn(__fsub_rn(__fmul_rn(x, a), __fmul_rn(y, b)));
+        tw[s >> 16] = cb[r * pitch + q];
+    }
+    __syncwarp();
     unsigned mine = 0;
 #pragma unroll
     for (int j = 0; j < 8; j++) {
-        const int tI = j * 32 + lane;
-        const float4 pp = __ldg(reinterpret_cast<const float4*>(d_pattern) + tI);
-        const float x0 = pp.x, y0 = pp.y, x1 = pp.z, y1 = pp.w;
-        const int r0 = __float2int_rn(__fadd_rn(__fmul_rn(x0, b), __fmul_rn(y0, a)));
-        const int q0 = __float2int_rn(__fsub_rn(__fmul_rn(x0, a), __fmul_rn(y0, b)));
-        const int r1 = __float2int_rn(__fadd_rn(__fmul_rn(x1, b), __fmul_rn(y1, a)));
-        const int q1 = __float2int_rn(__fsub_rn(__fmul_rn(x1, a), __fmul_rn(y1, b)));
-        const int t0 = cb[r0 * pitch + q0], t1 = cb[r1 * pitch + q1];
-        const unsigned word = __ballot_sync(0xFFFFFFFFu, t0 < t1);
+        const unsigned t01 = reinterpret_cast<const uint16_t*>(tw)[j * 32 + lane];    // test 32j + lane: tap 0 low, tap 1 high
+        const unsigned word = __ballot_sync(0xFFFFFFFFu, (t01 & 0xFFu) < (t01 >> 8));
         if (lane == j) mine = word;
     }
     const size_t o = (size_t)img * g.sel_image_stride + idx;
@@ -175,7 +186,7 @@ __global__ void __launch_bounds__(256, 8) describe_kernel(const __grid_constant_
 
 int launch_describe(const Geometry& g, const Workspace& ws, int n_images, cudaStream_t s) {
     dim3 grid((g.sel_image_stride + 7) / 8, n_images);
-    describe_kernel<<<grid, 256, 0, s>>>(g, ws.pyr, ws.blur, ws.sel, ws.sel_cnt, ws.kps, ws.desc, ws.nkp);
+    describe_kernel<<<grid, 256, 0, s>>>(g, ws.pyr, ws.blur, ws.brief_slots, ws.sel, ws.sel_cnt, ws.kps, ws.desc, ws.nkp);
     return 1;
 }
 
