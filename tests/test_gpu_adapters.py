@@ -57,6 +57,11 @@ test_search_for_initialization = T.test_search_for_initialization
 test_search_by_sim3 = T.test_search_by_sim3
 test_fuse_both = T.test_fuse_both
 
+# the size-envelope cases (8192-feature frames, contested claim chains, ties, wide FeatureVector nodes) through the adapters
+from tests import test_oracle_match_envelope as TE      # noqa: E402
+
+test_envelope_port_equals_reference = TE.test_port_equals_reference
+
 
 def test_adapters_reproduce_the_reference_golden_vectors(O):
     """tests/golden/match_ref.npz = outputs of the verbatim src/ORBmatcher.cc; the adapter library, driven through the same

@@ -49,6 +49,13 @@ bow2, _ = voc.transform(v["dr"], 1)
 db.add(kf1, bow1); db.add(kf2, bow2)
 print("kfdb", db.query(bow1)[0], db.SearchByBoW([0, 1], kf2)[0])
 print("distinctive", mt.ComputeDistinctiveDescriptors([v["dl"][:9], v["dl"][:1], v["dl"][:0], v["dl"][:70]]))
+# matcher envelope (tests/match_envelope.py): 8192 x 8192 SearchByProjection, and a SearchByBoW whose one node is wider than
+# the distance-matrix path
+from tests import match_envelope as ME
+c8 = ME.case(O, "self_kitti_8192")
+print("proj 8192", mt.SearchByProjection(c8["F"], c8["mps"], c8["th"])[0])
+cb = ME.case(O, "bow_one_node_8192")
+print("bow wide node", mt.SearchByBoW(cb["kf1"], cb["kf2"])[0], mt.SearchByBoW_KF(cb["kf1"], cb["kf2"])[0])
 
 # ---- round 2 kernels: device-side Frame tail (RGB-D), resident frames + in-place (pinned) inputs/outputs of the small calls,
 # CTA-wide claim resolution, database SearchByBoW (node-major items, compact pairs), ComputeBoW, persistent scoring kernel
