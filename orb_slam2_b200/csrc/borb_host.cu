@@ -168,9 +168,10 @@ borb_status build_geometry(borb_extractor* e, int w, int h, std::vector<int16_t>
         v.pyr_off = pyr_off;
         pyr_off += (unsigned)v.pitch * v.h;
         v.cellsPerBlk = FAST_TILE_W / v.wCell > 0 ? FAST_TILE_W / v.wCell : 1;
+        v.rowsPerBlk = fast_rows_per_blk(v.nRows, v.hCell);
         v.blkCols = (v.nCols + v.cellsPerBlk - 1) / v.cellsPerBlk;
         v.blkBase = blk;
-        blk += v.blkCols * v.nRows;
+        blk += v.blkCols * ((v.nRows + v.rowsPerBlk - 1) / v.rowsPerBlk);
         v.cand_off = cand_off;
         v.cand_cap = v.nCols * v.nRows * ((v.wCell + 1) / 2) * ((v.hCell + 1) / 2);   // strict 3x3 NMS: <=1 per 2x2
         cand_off += (unsigned)align_up(v.cand_cap, 32);

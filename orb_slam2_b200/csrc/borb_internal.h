@@ -20,6 +20,18 @@ constexpr int TH_LOW = 50;        // ORBmatcher.cc:38
 constexpr int BLUR_TILE_W = 120;  // blur strip: 30 output words per warp + one halo word each side
 constexpr int BLUR_TILE_H = 64;   // rows per blur CTA
 constexpr int FAST_TILE_W = 124;  // max detection-domain width of one FAST CTA (<= 32 aligned words incl. misalignment)
+constexpr int FAST_H_BAND = 64;   // max detection-domain height of one FAST CTA: a band of max(1, 64 / hCell) cell rows
+                                  // (hCell < 60, so a one-row band always fits too).  96 (3 cell rows, 3 CTAs/SM) measured
+                                  // slower than 64 (2 cell rows, 4 CTAs/SM): DESIGN.md §5
+
+// Cell rows per FAST CTA of a level whose cell grid has nRows rows of hCell pixels
+__host__ __device__ inline int fast_rows_per_blk(int nRows, int hCell) {
+    const int r = FAST_H_BAND / hCell;
+    return r < 1 ? 1 : (r > nRows ? nRows : r);
+}
+// Rows of a FAST CTA's TMA box (its cell rows + 3 halo rows above and below).  Both the tensor map's box and the CTA's
+// expect_tx byte count derive from this one expression: TMA counts the out-of-bounds-filled bytes of a short last band too.
+__host__ __device__ inline int fast_box_rows(int rowsPerBlk, int hCell) { return rowsPerBlk * hCell + 6; }
 
 // Candidate / selected-keypoint record: x | y<<12 | score<<24   (x,y <= 4095, score <= 255)
 __host__ __device__ inline uint32_t pack_xys(int x, int y, int s) { return (uint32_t)x | ((uint32_t)y << 12) | ((uint32_t)s << 24); }
@@ -34,7 +46,8 @@ struct LevelGeom {
     // FAST cell grid (ORBextractor.cc:781-787)
     int nCols, nRows, wCell, hCell;
     int cellsPerBlk;        // cells per FAST CTA along x
-    int blkCols;            // CTAs per cell row
+    int rowsPerBlk;         // cell rows per FAST CTA (fast_rows_per_blk)
+    int blkCols;            // CTAs per band of cell rows
     int blkBase;            // first CTA of this level inside one image's FAST grid
     unsigned cand_off;      // entry offset of this level's candidate list inside one image's block
     int cand_cap;

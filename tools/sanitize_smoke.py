@@ -20,6 +20,13 @@ print("noise", len(k))
 from tests import extract_geometry as EG
 print("smallest", len(ORBextractor(1000)(synth.mono_frame(2, 0, 0, 221, 221))[0]))
 print("tight pitch", len(ORBextractor(1000)(synth.white_noise(3, 376, 240))[0]))
+# FAST bands (tests/test_gpu_fast_bands.py): KITTI-shaped, R = 2/2/1/2/1/1/2/1 with a last band of one cell row on level 0
+# (11 rows, R = 2); 221x221, whose top levels have a one-row cell grid (R = 1)
+from tests import test_gpu_fast_bands as FB
+for (bw, bh), nf in (((1242, 375), 2000), ((221, 221), 1000)):
+    lv = EG.geometry(bw, bh, nfeatures=nf)[0]
+    print("bands", (bw, bh), [FB.rows_per_blk(v) for v in lv], [FB.bands(v)[-1][1] for v in lv],
+          len(ORBextractor(nf)(synth.mono_frame(6, 0, 0, bw, bh))[0]))
 G3 = ORBextractor(EG.DOT_NFEATURES)
 k = G3(EG.dot_image(5121, *synth.KITTI, 1))[0]
 print("5121 candidates", len(G3.debug_candidates(0)), len(k))
