@@ -527,6 +527,49 @@ BORB_API borb_status borb_search_by_bow_db_pairs(borb_matcher* m, borb_kfdb* db,
                                                  int32_t* n_matches, int32_t* pair_offset, uint32_t* pairs, int pairs_cap,
                                                  int32_t* n_pairs_total);
 
+/* Relocalisation (Tracking::Relocalization, src/Tracking.cc:1341-1470) and loop-closure queries of many camera streams on resident
+ * frames: the database query and the SearchByBoW of every lost stream, one call each, with nothing of the frames crossing PCIe.
+ * Frames come with the BoW of borb_frames_compute_bow.  Each job names its own database: many streams with their own maps, or many
+ * queries on one.  Every distinct database is locked for the table sync and the enqueue, in address order, so two concurrent
+ * batches cannot deadlock; borb_kfdb_erase and borb_kfdb_set_has_mp keep their guarantees.  Argument errors are refused with
+ * BORB_ERR_INVALID_ARG before anything is launched, the error text starting "job j:": a NULL database or frame, a frame without BoW
+ * (recycled frames included), a frame, database and matcher on different devices, a slot that is not a live keyframe, slots == NULL
+ * with n_kf different from the slot count, pairs without pair_offset.  A job with n_kf == 0, a database without slots, or a frame
+ * with 0 features or only stop words gives zeros. */
+typedef struct borb_kfdb_query_job {
+    borb_kfdb* db;
+    const borb_frame* frame;       /* resident, BoW computed by borb_frames_compute_bow */
+    int32_t* common_words;         /* outputs, one entry per slot, as borb_kfdb_query */
+    float* score;
+    uint32_t* first_word;
+    int32_t cap;                   /* entries of each output; fewer than the database's slots => BORB_ERR_CAPACITY before any launch */
+    int32_t* n_slots;
+} borb_kfdb_query_job;
+/* borb_kfdb_query for n_jobs frames: job j returns exactly what borb_kfdb_query returns for the frame's BowVector.
+ * 1 launch whatever n_jobs (0 when no database has a slot), one synchronisation. */
+BORB_API borb_status borb_kfdb_query_batch(borb_matcher* m, const borb_kfdb_query_job* jobs, int n_jobs);
+
+typedef struct borb_bow_db_job {
+    borb_kfdb* db;
+    const borb_frame* frame;       /* resident, BoW computed */
+    const int32_t* slots;          /* candidate keyframes (repeats allowed); NULL: every slot, n_kf must be the slot count */
+    int32_t n_kf;
+    int32_t* n_matches;            /* outputs as borb_search_by_bow_db_pairs; pair_offset indexes this job's own pairs */
+    int32_t* pair_offset;
+    uint32_t* pairs;
+    int32_t pairs_cap;
+    int32_t* n_pairs_total;
+} borb_bow_db_job;
+/* borb_search_by_bow_db_pairs for n_jobs frames: job j returns for every keyframe the same count and the same pair block as
+ * borb_search_by_bow_db_pairs on a host view of the frame; only the placement of the blocks inside the job's pairs differs.  The
+ * caller's duty, as for the single call: the frame's FeatureVector (borb_frames_compute_bow's levelsup) must be at the same level
+ * as the FeatureVectors of the database's keyframes.  Pairs beyond a job's pairs_cap give BORB_ERR_CAPACITY after the run; counts
+ * and offsets are still valid for every job, and the error names the first job that overflowed.  3 launches whatever n_jobs (the
+ * device packer of the frame blocks, the match kernel, the rotation cull; 0 when no job has work), one synchronisation.  The
+ * single calls are the one-job case of the same launches. */
+BORB_API borb_status borb_search_by_bow_db_batch(borb_matcher* m, const borb_bow_db_job* jobs, int n_jobs, float nnratio,
+                                                 int check_orientation);
+
 /* ---------------------------------------------------------------- vocabulary (BoW feeder) ---- */
 /* ORBVocabulary = DBoW2::TemplatedVocabulary<FORB> (Thirdparty/DBoW2/DBoW2/TemplatedVocabulary.h).  The tree lives
  * in HBM as one packed blob (so it can be broadcast over NCCL once and shared by every stream of a GPU). */

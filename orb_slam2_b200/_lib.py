@@ -97,6 +97,8 @@ _SIGNATURES = {
     "borb_kfdb_query": (C.c_int, [vp, vp, vp, vp, C.c_int, vp, vp, vp, C.c_int, i32p]),
     "borb_search_by_bow_db": (C.c_int, [vp, vp, vp, C.c_int, vp, C.c_float, C.c_int, vp, vp]),
     "borb_search_by_bow_db_pairs": (C.c_int, [vp, vp, vp, C.c_int, vp, C.c_float, C.c_int, vp, vp, vp, C.c_int, i32p]),
+    "borb_kfdb_query_batch": (C.c_int, [vp, vp, C.c_int]),
+    "borb_search_by_bow_db_batch": (C.c_int, [vp, vp, C.c_int, C.c_float, C.c_int]),
     "borb_search_local_points": (C.c_int, [vp, vp, vp, vp, vp, vp] + [C.c_float] * 9 + [vp] * 7 + [i32p]),
     "borb_search_local_points_batch": (C.c_int, [vp, vp, C.c_int, C.c_float, C.c_float, vp]),
     "borb_search_by_projection_last_batch": (C.c_int, [vp, vp, C.c_int, C.c_int, vp]),

@@ -30,7 +30,7 @@ struct borb_frame {
     int32_t* fv_start = nullptr;
     uint32_t* fv_idx = nullptr;
     bool has_bow = false;
-    int n_bow = 0, n_nodes = 0;
+    int n_bow = 0, n_nodes = 0, n_fv = 0;   // n_fv = fv_start[n_nodes]: features inside the FeatureVector's nodes
     cudaEvent_t ready = nullptr;    // recorded after the last kernel that writes the block
 };
 
@@ -142,33 +142,85 @@ struct KfStream {                  // one keyframe of the device-resident databa
     const void* pad2[2];
 };
 
-struct BowDbArgs {                // bowdb_match_kernel (k_bowdb.cu)
-    const KfStream* table;        // one entry per database slot (nn = 0: erased)
-    const int32_t* slots;         // n_kf slots to search, or null = slots 0..n_kf-1
-    int n_kf, n_items;            // keyframes to search; work items (frame node x keyframe range, the work list inside frame_block)
-    const uint8_t* frame_block;   // packed query frame (FrameBlockHdr + sections), 16-byte aligned, frame_bytes % 16 == 0
-    int frame_bytes, frame_in_smem;
-    int static_sched;             // 1: item i -> warp i mod (warps), 0: atomic work counter
-    float nnratio;
-    int check_ori;
-    uint32_t* table_out;          // n_kf x m_frame, preset to 0xFFFFFFFF
-    int* hist_out;                // n_kf x 32 rotation-histogram counters, preset to 0
-    int* work_counter;            // preset to 0
-};
+// Packed query frame of the database search (k_bowdb.cu), built on the device by bowdb_pack_kernel: header, then 16-byte
+// aligned sections
+//   node[nn] u32 ascending | start[nn+1] i32 | orig[m] u16 | angle[m] f32 | desc[m][32]     (m = features inside nodes)
+//   work list (np = non-empty frame nodes, widest bucket first): pnode[np] i32 node index | pcs[np] i32 keyframes per item |
+//   pstart[np+1] i32 cumulative item count
+struct FrameBlockHdr { int32_t nn, m, n, off_node, off_start, off_orig, off_angle, off_desc, bytes, np, off_pnode, off_pcs, off_pstart, pad[3]; };
 
-struct BowDbFinal {               // bowdb_finalize_kernel
-    const uint32_t* table_out;
-    const int* hist;              // n_kf x 32 (BowDbArgs::hist_out)
-    int n_kf, mf, check_ori;
-    const uint16_t* forig;        // frame feature index per frame position
+// The section offsets and the size of the block of a frame with nn FeatureVector nodes holding m of its n features.
+__host__ __device__ inline FrameBlockHdr frame_block_layout(int nn, int m, int n) {
+    FrameBlockHdr h{};
+    int off = (int)sizeof(FrameBlockHdr);
+    auto put = [&](int bytes) { off = (off + 15) & ~15; const int o = off; off += bytes; return o; };
+    h.nn = nn; h.m = m; h.n = n;
+    h.off_node = put(nn * 4); h.off_start = put((nn + 1) * 4); h.off_orig = put(m * 2);
+    h.off_angle = put(m * 4); h.off_desc = put(m * 32);
+    h.off_pnode = put(nn * 4); h.off_pcs = put(nn * 4); h.off_pstart = put((nn + 1) * 4);
+    h.bytes = (off + 15) & ~15;
+    return h;
+}
+
+// One frame of the database search (borb_search_by_bow_db*, borb_search_by_bow_db_batch): read by bowdb_pack_kernel,
+// bowdb_match_kernel and bowdb_finalize_kernel (k_bowdb.cu).
+struct BowDbJob {
+    // the frame: FeatureVector (CSR), keypoints (angle) and descriptors, resident or staged from a host view
+    const uint32_t* fv_node;
+    const int32_t* fv_start;      // nn + 1
+    const uint32_t* fv_idx;       // m
+    const borb_keypoint* keys;
+    const uint8_t* desc;          // n x 32, 16-byte aligned
+    int nn, m, n, item_target;    // item_target: keyframes per work item = item_target / nt^2, clamped to 1..32
+    uint8_t* frame_block;         // FrameBlockHdr + sections, 128-byte aligned, frame_bytes = frame_block_layout(nn, m, n).bytes
+    int frame_bytes, frame_in_smem;
+    // the keyframes
+    const KfStream* table;        // the job's database, one entry per slot (nn = 0: erased)
+    const int32_t* slots;         // n_kf slots to search, or null = slots 0..n_kf-1
+    int n_kf, kf_base;            // kf_base: the job's first finalize CTA (sum of n_kf of the jobs before it)
+    int* ctr;                     // [0] work counter, [1] work items (written by the packer), [2] pair cursor
+    uint32_t* table_out;          // n_kf x m, preset to 0xFFFFFFFF
+    int* hist_out;                // n_kf x 32 rotation-histogram counters, preset to 0
+    // results
     int32_t* n_matches;           // n_kf
     int32_t* pair_off;            // n_kf (may be null)
-    uint32_t* pairs;              // frame feature | keyframe feature << 16 (may be null)
+    uint32_t* pairs;              // frame feature | keyframe feature << 16 (may be null), pairs_cap entries
     int pairs_cap;
-    int* cursor;                  // preset to 0
-    int32_t* dense;               // n_kf x dense_stride preset to -1 (may be null): match[k][frame feature] = keyframe feature
     int dense_stride;
+    int32_t* dense;               // n_kf x dense_stride preset to -1 (may be null): match[k][frame feature] = keyframe feature
 };
+
+struct BowDbArgs {                // the launch sequence of the database search over a job table in device memory
+    const BowDbJob* jobs;
+    int n_jobs;
+    int static_sched;             // 1: item i of every job -> warp i mod (warps), 0: atomic work counter per job
+    float nnratio;
+    int check_ori;
+};
+
+struct KfdbQueryJob {             // one query of kfdb_score_kernel (k_match.cu)
+    const BowDev* table;          // the job's database, one entry per slot
+    int n_slots, nq;
+    const uint32_t* qword;        // the query BowVector, ascending words
+    const double* qvalue;
+    int32_t* common;              // n_slots entries each
+    float* score;
+    uint32_t* first_word;
+};
+
+// ascending bitonic sort of K (a power of two) 64-bit keys in shared memory by the whole CTA; ends with a barrier
+__device__ inline void bitonic_sort_u64(uint64_t* k, int K) {
+    const int half = K >> 1;
+    for (int kk = 2; kk <= K; kk <<= 1)
+        for (int j = kk >> 1; j > 0; j >>= 1) {
+            for (int p = threadIdx.x; p < half; p += blockDim.x) {
+                const int i = ((p & ~(j - 1)) << 1) | (p & (j - 1));          // lower element of the p-th compare pair
+                const uint64_t a = k[i], b = k[i + j];
+                if ((a > b) == ((i & kk) == 0)) { k[i] = b; k[i + j] = a; }
+            }
+            __syncthreads();
+        }
+}
 
 struct FrameJob {                 // one frame of borb_frames_from_extractor (k_frame.cu)
     const borb_keypoint* src_keys;   // the extractor's mvKeys of that image
@@ -204,7 +256,7 @@ struct BowFrameJob {              // one frame of borb_frames_compute_bow (bow_t
     int32_t* node;
     BowTables dst;                // the frame's storage
     BowTables copy;               // the same tables again, for the host (may be unset)
-    int32_t* counts;              // n_bow, n_nodes
+    int32_t* counts;              // n_bow, n_nodes, fv_start[n_nodes]
 };
 
 struct VocDev {                   // views into the packed blob
@@ -228,8 +280,8 @@ int launch_projection(const ProjArgs& A, cudaStream_t s);
 int launch_projection_last(const LastArgs& L, const ProjArgs& A, cudaStream_t s);
 int launch_initialization(const ProjArgs& A, const borb_keypoint* keys1, int n1, int32_t* match12, int32_t* ev_idx, uint8_t* ev_bin,
                           float* prev, int* n_matches, cudaStream_t s);
-int launch_kfdb_score(const BowDev* table, int n_slots, const uint32_t* qword, const double* qvalue, int nq, int32_t* common, float* score,
-                      uint32_t* first_word, int n_sm, cudaStream_t s);
+// n_jobs queries (a job table in device memory) in one launch; max_slots / max_nq: the largest n_slots / nq of the jobs
+int launch_kfdb_score(const KfdbQueryJob* d_jobs, int n_jobs, int max_slots, int max_nq, int n_sm, cudaStream_t s);
 int launch_distinctive(const uint8_t* desc, const int32_t* offsets, int n_points, int32_t* best_idx, cudaStream_t s);
 int launch_frustum_projection(const LastArgs& L, const ProjArgs& A, cudaStream_t s);
 int launch_projection_argmin(const LastArgs& L, const ProjArgs& A, cudaStream_t s);
@@ -240,7 +292,10 @@ int launch_bow_match(const KfDev* qs, const KfDev* ts, int n_pairs, int mode, fl
 void host_image_bounds(int w, int h, const borb_camera& c, float* b4);
 int launch_frame_build(const FrameJob* d_jobs, int n_jobs, int max_n, const borb_camera& cam, int mode, int depth_type, float depth_factor, int w,
                        int h, int out_cap, borb_keypoint* keys_out, float* ur_out, float* depth_out, cudaStream_t s);
-int launch_bowdb(const BowDbArgs& A, const BowDbFinal& F, int csa, int n_sm, cudaStream_t s);
+// pack + match + finalize over A.jobs (3 launches): one = a host copy of job 0 (what the match kernel reads of a single job),
+// max_smem_frame = largest frame_bytes of the jobs with frame_in_smem, max_items = an upper bound of the work items of all jobs,
+// total_kf = sum of their n_kf
+int launch_bowdb(const BowDbArgs& A, const BowDbJob& one, int max_smem_frame, long long max_items, int total_kf, int max_nn, int csa, int n_sm, cudaStream_t s);
 bool bowdb_frame_fits_smem(int frame_bytes);
 int launch_triangulation(const KfDev& q, const KfDev& t, const TriArgs& T, int32_t* vmatch, uint8_t* bins, int32_t* pairs, int cap,
                          int32_t* n_pairs, cudaStream_t s);

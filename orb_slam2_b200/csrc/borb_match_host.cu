@@ -333,7 +333,7 @@ borb_status frame_alloc(int device, int n, int n_levels, bool stereo, borb_frame
         f->fv_start = (int32_t*)(f->block + o_fs); f->fv_idx = (uint32_t*)(f->block + o_fi);
     }
     f->has_bow = false;                 // a new frame, or a recycled block that still holds another frame's vectors
-    f->n_bow = f->n_nodes = 0;
+    f->n_bow = f->n_nodes = f->n_fv = 0;
     // u_right / depth storage always exists; the pointers are nulled for a monocular frame
     f->u_right = stereo ? f->ur_store : nullptr;
     f->depth = stereo ? f->depth_store : nullptr;
@@ -1628,44 +1628,6 @@ static borb_status kfdb_sync_table(borb_kfdb* db, cudaStream_t stream) {
     return BORB_OK;
 }
 
-borb_status borb_kfdb_query(borb_matcher* m, borb_kfdb* db, const uint32_t* bow_word, const double* bow_value, int n_bow,
-                            int32_t* common_words, float* score, uint32_t* first_word, int cap, int32_t* n_slots) {
-    if (!m || !db || !common_words || !score || !first_word || !n_slots || n_bow < 0 || (n_bow > 0 && (!bow_word || !bow_value))) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
-    if (m->device != db->device) { set_error("matcher and keyframe database live on different devices"); return BORB_ERR_INVALID_ARG; }
-    for (int i = 1; i < n_bow; i++)
-        if (bow_word[i] <= bow_word[i - 1]) { set_error("BowVector words must ascend (std::map order)"); return BORB_ERR_INVALID_ARG; }
-    uint8_t* b = nullptr;
-    int n = 0;
-    {
-        std::lock_guard<std::mutex> lk(db->mu);       // held across the table sync and the kernel enqueue (erase() synchronises the device before freeing)
-        n = (int)db->entries.size();
-        *n_slots = n;
-        if (cap < n) { set_error("output capacity %d < %d database slots", cap, n); return BORB_ERR_CAPACITY; }
-        if (n == 0) return BORB_OK;
-        BORB_CUDA(cudaSetDevice(m->device));
-        borb_status s = kfdb_sync_table(db, m->stream);
-        if (s != BORB_OK) return s;
-        Stager st(m);
-        const size_t o_w = st.add(bow_word, (size_t)n_bow * 4), o_v = st.add(bow_value, (size_t)n_bow * 8);
-        const size_t input_end = st.off;
-        const size_t total = st.off;
-        st.off = input_end;
-        if ((s = ensure_out(m, (size_t)n * 12 + 64)) != BORB_OK) return s;
-        if ((s = commit(st, total)) != BORB_OK) return s;
-        b = m->arena;
-        // the three result arrays are written by the kernel straight into the pinned landing buffer (device-addressable, UVA)
-        uint8_t* ho = m->h_out;
-        m->launches += launch_kfdb_score(db->d_table, n, (const uint32_t*)(b + o_w), (const double*)(b + o_v), n_bow, (int32_t*)ho,
-                                         (float*)(ho + (size_t)n * 4), (uint32_t*)(ho + (size_t)n * 8), db->n_sm, m->stream);
-        BORB_CUDA(cudaGetLastError());
-    }
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
-    std::memcpy(common_words, m->h_out, (size_t)n * 4);
-    std::memcpy(score, m->h_out + (size_t)n * 4, (size_t)n * 4);
-    std::memcpy(first_word, m->h_out + (size_t)n * 8, (size_t)n * 4);
-    return BORB_OK;
-}
-
 static std::atomic<int> g_bow_csa{2};
 static std::atomic<int> g_bow_item_target{8192};   // keyframes per work item = target / nt^2 (tuning knob of the measurement scripts)
 static std::atomic<int> g_bow_static{0};
@@ -1674,169 +1636,332 @@ borb_status borb_debug_set_bow_csa(int mode) { g_bow_csa.store(mode < 0 ? 0 : (m
 
 namespace {
 
-struct FrameBlockHdrHost { int32_t nn, m, n, off_node, off_start, off_orig, off_angle, off_desc, bytes, np, off_pnode, off_pcs, off_pstart, pad[3]; };   // == FrameBlockHdr (k_bowdb.cu)
-
-// Packs the query frame into FeatureVector order (k_bowdb.cu: FrameBlockHdr + sections) inside `dst` (16-byte aligned).
-size_t frame_block_bytes(const borb_keyframe_view* f) {
-    const int nn = f->fv.n_nodes, m = nn > 0 ? f->fv.start[nn] : 0;
-    size_t off = sizeof(FrameBlockHdrHost);
-    auto put = [&](size_t bytes) { off = (off + 15) & ~size_t(15); off += bytes; };
-    put((size_t)nn * 4); put((size_t)(nn + 1) * 4); put((size_t)m * 2); put((size_t)m * 4); put((size_t)m * 32);
-    put((size_t)nn * 4); put((size_t)nn * 4); put((size_t)(nn + 1) * 4);
-    return (off + 15) & ~size_t(15);
-}
-// Returns the number of work items of the sweep over n_kf keyframes (k_bowdb.cu: an item = one frame node x a range of keyframes).
-int pack_frame_block(const borb_keyframe_view* f, int n_kf, uint8_t* dst) {
-    const int nn = f->fv.n_nodes, m = nn > 0 ? f->fv.start[nn] : 0;
-    FrameBlockHdrHost h{};
-    size_t off = sizeof(FrameBlockHdrHost);
-    auto put = [&](size_t bytes) { off = (off + 15) & ~size_t(15); const size_t o = off; off += bytes; return o; };
-    h.nn = nn; h.m = m; h.n = f->n;
-    h.off_node = (int32_t)put((size_t)nn * 4); h.off_start = (int32_t)put((size_t)(nn + 1) * 4); h.off_orig = (int32_t)put((size_t)m * 2);
-    h.off_angle = (int32_t)put((size_t)m * 4); h.off_desc = (int32_t)put((size_t)m * 32);
-    h.off_pnode = (int32_t)put((size_t)nn * 4); h.off_pcs = (int32_t)put((size_t)nn * 4); h.off_pstart = (int32_t)put((size_t)(nn + 1) * 4);
-    h.bytes = (int32_t)((off + 15) & ~size_t(15));
-    if (nn) std::memcpy(dst + h.off_node, f->fv.node_id, (size_t)nn * 4);
-    if (nn) std::memcpy(dst + h.off_start, f->fv.start, (size_t)(nn + 1) * 4);
-    else { const int32_t z = 0; std::memcpy(dst + h.off_start, &z, 4); }
-    uint16_t* orig = reinterpret_cast<uint16_t*>(dst + h.off_orig);
-    float* ang = reinterpret_cast<float*>(dst + h.off_angle);
-    for (int r = 0; r < m; r++) {
-        const uint32_t j = f->fv.feat_idx[r];
-        orig[r] = (uint16_t)j;
-        ang[r] = f->keys_un[j].angle;
-        std::memcpy(dst + h.off_desc + (size_t)r * 32, f->desc + (size_t)j * 32, 32);
+// Every distinct database of a call, locked in address order (two concurrent batches over the same databases cannot deadlock),
+// held across the table sync and the kernel enqueue (erase() and set_has_mp() synchronise the device before they touch a block).
+struct DbLocks {
+    std::vector<borb_kfdb*> dbs;
+    std::vector<std::unique_lock<std::mutex>> held;
+    explicit DbLocks(std::vector<borb_kfdb*> all) : dbs(std::move(all)) {
+        std::sort(dbs.begin(), dbs.end(), std::less<borb_kfdb*>());
+        dbs.erase(std::unique(dbs.begin(), dbs.end()), dbs.end());
+        for (borb_kfdb* db : dbs) held.emplace_back(db->mu);
     }
-    // work list: non-empty nodes, widest bucket first (the long items start first); keyframes per item ~ 1 / nt^2 so that an
-    // item is a few hundred column-loop iterations whatever the bucket width (a keyframe's bucket of the node is about as
-    // full as the frame's)
-    int32_t* pnode = reinterpret_cast<int32_t*>(dst + h.off_pnode);
-    int32_t* pcs = reinterpret_cast<int32_t*>(dst + h.off_pcs);
-    int32_t* pstart = reinterpret_cast<int32_t*>(dst + h.off_pstart);
-    int np = 0;
-    for (int a = 0; a < nn; a++)
-        if (f->fv.start[a + 1] > f->fv.start[a]) pnode[np++] = a;
-    std::stable_sort(pnode, pnode + np, [&](int32_t x, int32_t y) { return f->fv.start[x + 1] - f->fv.start[x] > f->fv.start[y + 1] - f->fv.start[y]; });
-    int items = 0;
-    for (int p = 0; p < np; p++) {
-        const long long nt = f->fv.start[pnode[p] + 1] - f->fv.start[pnode[p]];
-        long long cs = g_bow_item_target.load() / (nt * nt);
-        cs = cs < 1 ? 1 : (cs > 32 ? 32 : cs);            // one 32-lane batch of keyframes per item at most
-        pcs[p] = (int32_t)cs;
-        pstart[p] = items;
-        items += (int)((n_kf + cs - 1) / cs);
+    borb_status sync(cudaStream_t s) {
+        for (borb_kfdb* db : dbs) { borb_status st = kfdb_sync_table(db, s); if (st != BORB_OK) return st; }
+        return BORB_OK;
     }
-    pstart[np] = items;
-    h.np = np;
-    std::memcpy(dst, &h, sizeof(h));
-    return items;
+};
+
+// error text of a check shared by the single calls and the batches: the batches name the job
+borb_status job_fail(bool batch, int j, borb_status s) { return batch ? job_error(j, s) : s; }
+
+// One query of the database score: the BowVector comes from the host (word / value) or from a resident frame.
+struct QueryJob {
+    borb_kfdb* db;
+    const borb_frame* frame;
+    const uint32_t* word; const double* value; int n_bow;
+    int32_t* common; float* score; uint32_t* first_word;
+    int cap; int32_t* n_slots;
+};
+
+// Shared body of borb_kfdb_query and borb_kfdb_query_batch: one launch of kfdb_score_kernel for every job (none when no database
+// has a slot) and one synchronisation.  The arguments are checked by the callers.
+borb_status kfdb_query_jobs(borb_matcher* m, const QueryJob* q, int n_jobs, bool batch) {
+    std::vector<int> ns(n_jobs);
+    std::vector<size_t> o_w(n_jobs, 0), o_v(n_jobs, 0), ho(n_jobs, 0);
+    int max_slots = 0, max_nq = 0;
+    {
+        std::vector<borb_kfdb*> dbs(n_jobs);
+        for (int j = 0; j < n_jobs; j++) dbs[j] = q[j].db;
+        DbLocks lk(std::move(dbs));
+        size_t out_bytes = 0;
+        for (int j = 0; j < n_jobs; j++) {
+            ns[j] = (int)q[j].db->entries.size();
+            *q[j].n_slots = ns[j];
+        }
+        for (int j = 0; j < n_jobs; j++)
+            if (q[j].cap < ns[j]) { set_error("output capacity %d < %d database slots", q[j].cap, ns[j]); return job_fail(batch, j, BORB_ERR_CAPACITY); }
+        for (int j = 0; j < n_jobs; j++) {
+            ho[j] = out_bytes; out_bytes += ((size_t)ns[j] * 12 + 15) & ~size_t(15);
+            max_slots = std::max(max_slots, ns[j]);
+            max_nq = std::max(max_nq, q[j].frame ? q[j].frame->n_bow : q[j].n_bow);
+        }
+        if (max_slots == 0) return BORB_OK;
+        BORB_CUDA(cudaSetDevice(m->device));
+        borb_status s = lk.sync(m->stream);
+        if (s != BORB_OK) return s;
+        Stager st(m);
+        for (int j = 0; j < n_jobs; j++)
+            if (!q[j].frame) { o_w[j] = st.add(q[j].word, (size_t)q[j].n_bow * 4); o_v[j] = st.add(q[j].value, (size_t)q[j].n_bow * 8); }
+        const size_t o_jobs = st.add(nullptr, (size_t)n_jobs * sizeof(KfdbQueryJob));     // filled in place
+        const size_t total = st.off;
+        if ((s = ensure_host(m, total)) != BORB_OK) return s;
+        if ((s = ensure_arena(m, total)) != BORB_OK) return s;
+        if ((s = ensure_out(m, out_bytes + 64)) != BORB_OK) return s;
+        BORB_CUDA(cudaStreamSynchronize(m->stream));
+        uint8_t* b = m->arena;
+        KfdbQueryJob* hj = reinterpret_cast<KfdbQueryJob*>(m->h_stage + o_jobs);
+        for (int j = 0; j < n_jobs; j++) {
+            // the three result arrays are written by the kernel straight into the pinned landing buffer (device-addressable, UVA)
+            uint8_t* o = m->h_out + ho[j];
+            KfdbQueryJob J{};
+            J.table = q[j].db->d_table; J.n_slots = ns[j];
+            if (q[j].frame) { J.qword = q[j].frame->bow_word; J.qvalue = q[j].frame->bow_value; J.nq = q[j].frame->n_bow; }
+            else { J.qword = (const uint32_t*)(b + o_w[j]); J.qvalue = (const double*)(b + o_v[j]); J.nq = q[j].n_bow; }
+            J.common = (int32_t*)o; J.score = (float*)(o + (size_t)ns[j] * 4); J.first_word = (uint32_t*)(o + (size_t)ns[j] * 8);
+            hj[j] = J;
+        }
+        if ((s = commit(st, total)) != BORB_OK) return s;
+        for (int j = 0; j < n_jobs; j++)
+            if (q[j].frame) BORB_CUDA(cudaStreamWaitEvent(m->stream, q[j].frame->ready, 0));
+        m->launches += launch_kfdb_score((const KfdbQueryJob*)(b + o_jobs), n_jobs, max_slots, max_nq, q[0].db->n_sm, m->stream);
+        BORB_CUDA(cudaGetLastError());
+    }
+    BORB_CUDA(cudaStreamSynchronize(m->stream));
+    for (int j = 0; j < n_jobs; j++) {
+        const uint8_t* o = m->h_out + ho[j];
+        std::memcpy(q[j].common, o, (size_t)ns[j] * 4);
+        std::memcpy(q[j].score, o + (size_t)ns[j] * 4, (size_t)ns[j] * 4);
+        std::memcpy(q[j].first_word, o + (size_t)ns[j] * 8, (size_t)ns[j] * 4);
+    }
+    return BORB_OK;
 }
 
-// Shared body of the two database searches.  dense != null: match[k * frame->n + j]; pairs != null: compact list.
-borb_status bowdb_search(borb_matcher* m, borb_kfdb* db, const int32_t* slots, int n_kf, const borb_keyframe_view* frame, float nnratio,
-                         int check_ori, int32_t* dense, int32_t* n_matches, int32_t* pair_offset, uint32_t* pairs, int pairs_cap,
-                         int32_t* n_pairs_total) {
+// One frame of the database search: a resident frame with its BoW, or a host view.
+struct SearchJob {
+    borb_kfdb* db;
+    const borb_frame* frame;
+    const borb_keyframe_view* view;
+    const int32_t* slots; int n_kf;
+    int32_t* dense;                    // borb_search_by_bow_db: match[k * n + j]
+    int32_t* n_matches; int32_t* pair_offset; uint32_t* pairs; int pairs_cap; int32_t* n_pairs_total;
+};
+
+// Shared body of borb_search_by_bow_db, _db_pairs and _db_batch: pack, match and finalize over the job table (3 launches; none when
+// no job has a keyframe and a feature inside a node) and one synchronisation.  The arguments are checked by the callers, except the
+// slot lists, which are checked here under the database locks (a batch checks every job with keyframes, a single call only one
+// that has work, as before).
+borb_status bowdb_jobs(borb_matcher* m, const SearchJob* J, int n_jobs, float nnratio, int check_ori, bool batch) {
+    struct Plan { int nn, m, n; bool work; FrameBlockHdr h; size_t o_node, o_start, o_idx, o_keys, o_desc, o_fb, o_sl, o_ctr, o_hist, o_tab, o_dense, ho; };
+    std::vector<Plan> P(n_jobs);
+    for (int j = 0; j < n_jobs; j++) {
+        const SearchJob& S = J[j];
+        Plan& p = P[j];
+        if (S.frame) { p.nn = S.frame->n_nodes; p.m = S.frame->n_fv; p.n = S.frame->n; }
+        else { p.nn = S.view->fv.n_nodes; p.m = p.nn > 0 ? S.view->fv.start[p.nn] : 0; p.n = S.view->n; }
+        p.work = S.n_kf > 0 && p.m > 0;
+        if (S.n_pairs_total) *S.n_pairs_total = 0;
+        if (S.dense) for (size_t i = 0; i < (size_t)S.n_kf * p.n; i++) S.dense[i] = -1;
+        for (int i = 0; i < S.n_kf; i++) { S.n_matches[i] = 0; if (S.pair_offset) S.pair_offset[i] = 0; }
+    }
+    std::vector<int> work;
+    for (int j = 0; j < n_jobs; j++) if (P[j].work) work.push_back(j);
+    const int nw = (int)work.size();
+    {
+        std::vector<borb_kfdb*> dbs(n_jobs);
+        for (int j = 0; j < n_jobs; j++) dbs[j] = J[j].db;
+        DbLocks lk(std::move(dbs));
+        for (int j = 0; j < n_jobs; j++) {
+            const SearchJob& S = J[j];
+            if (S.n_kf == 0 || (!batch && !P[j].work)) continue;      // the single calls return zeros before looking at the slots
+            const int n_slots = (int)S.db->entries.size();
+            if (!S.slots && S.n_kf != n_slots) { set_error("slots == NULL searches every slot: n_kf must be %d", n_slots); return job_fail(batch, j, BORB_ERR_INVALID_ARG); }
+            if (S.slots)
+                for (int i = 0; i < S.n_kf; i++)
+                    if (S.slots[i] < 0 || S.slots[i] >= n_slots || !S.db->entries[S.slots[i]].alive) { set_error("slot %d is not a live keyframe", S.slots[i]); return job_fail(batch, j, BORB_ERR_INVALID_ARG); }
+        }
+        if (nw == 0) return BORB_OK;
+        BORB_CUDA(cudaSetDevice(m->device));
+        borb_status s = lk.sync(m->stream);
+        if (s != BORB_OK) return s;
+        Stager st(m);
+        for (int j : work) {
+            const SearchJob& S = J[j];
+            Plan& p = P[j];
+            if (!S.frame) {                                            // a host view: its raw arrays, packed on the device like a resident frame
+                const borb_keyframe_view* v = S.view;
+                p.o_node = st.add(v->fv.node_id, (size_t)p.nn * 4); p.o_start = st.add(v->fv.start, (size_t)(p.nn + 1) * 4);
+                p.o_idx = st.add(v->fv.feat_idx, (size_t)p.m * 4);
+                p.o_keys = st.add(v->keys_un, (size_t)p.n * sizeof(borb_keypoint)); p.o_desc = st.add(v->desc, (size_t)p.n * 32);
+            }
+            p.o_sl = S.slots ? st.add(S.slots, (size_t)S.n_kf * 4) : 0;
+        }
+        const size_t o_jobs = st.add(nullptr, (size_t)nw * sizeof(BowDbJob));       // filled in place
+        const size_t input_end = st.off;
+        size_t hist_bytes = 0, tab_bytes = 0, out_bytes = 0;
+        for (int j : work) { hist_bytes += (size_t)J[j].n_kf * 32 * 4; tab_bytes += (size_t)J[j].n_kf * P[j].m * 4; }
+        const size_t o_hist = st.reserve(hist_bytes), o_tab = st.reserve(tab_bytes);
+        size_t hist_off = o_hist, tab_off = o_tab;
+        int max_smem_frame = 0, max_nn = 0, total_kf = 0;
+        long long max_items = 0;
+        for (int j : work) {
+            const SearchJob& S = J[j];
+            Plan& p = P[j];
+            p.h = frame_block_layout(p.nn, p.m, p.n);
+            p.o_fb = st.reserve((size_t)p.h.bytes);
+            p.o_ctr = st.reserve(16);
+            p.o_hist = hist_off; hist_off += (size_t)S.n_kf * 32 * 4;
+            p.o_tab = tab_off; tab_off += (size_t)S.n_kf * p.m * 4;
+            p.o_dense = S.dense ? st.reserve((size_t)S.n_kf * p.n * 4) : 0;
+            p.ho = out_bytes; out_bytes += ((size_t)S.n_kf * 8 + (S.pairs ? (size_t)S.pairs_cap * 4 : 0) + 15) & ~size_t(15);
+            if (bowdb_frame_fits_smem(p.h.bytes)) max_smem_frame = std::max(max_smem_frame, p.h.bytes);
+            max_nn = std::max(max_nn, p.nn);
+            max_items += (long long)std::min(p.nn, p.m) * S.n_kf;
+            total_kf += S.n_kf;
+        }
+        const size_t total = st.off;
+        st.off = input_end;
+        if ((s = ensure_host(m, input_end)) != BORB_OK) return s;
+        if ((s = ensure_arena(m, total)) != BORB_OK) return s;
+        if ((s = ensure_out(m, out_bytes + 64)) != BORB_OK) return s;
+        BORB_CUDA(cudaStreamSynchronize(m->stream));
+        uint8_t* b = m->arena;
+        BowDbJob* hj = reinterpret_cast<BowDbJob*>(m->h_stage + o_jobs);
+        int kf_base = 0;
+        for (int w = 0; w < nw; w++) {
+            const SearchJob& S = J[work[w]];
+            const Plan& p = P[work[w]];
+            BowDbJob D{};
+            if (S.frame) {
+                D.fv_node = S.frame->fv_node; D.fv_start = S.frame->fv_start; D.fv_idx = S.frame->fv_idx;
+                D.keys = S.frame->keys; D.desc = S.frame->desc;
+            } else {
+                D.fv_node = (const uint32_t*)(b + p.o_node); D.fv_start = (const int32_t*)(b + p.o_start); D.fv_idx = (const uint32_t*)(b + p.o_idx);
+                D.keys = (const borb_keypoint*)(b + p.o_keys); D.desc = b + p.o_desc;
+            }
+            D.nn = p.nn; D.m = p.m; D.n = p.n; D.item_target = g_bow_item_target.load();
+            D.frame_block = b + p.o_fb; D.frame_bytes = p.h.bytes; D.frame_in_smem = bowdb_frame_fits_smem(p.h.bytes) ? 1 : 0;
+            D.table = S.db->d_stream; D.slots = S.slots ? (const int32_t*)(b + p.o_sl) : nullptr;
+            D.n_kf = S.n_kf; D.kf_base = kf_base; kf_base += S.n_kf;
+            D.ctr = (int*)(b + p.o_ctr);
+            D.table_out = (uint32_t*)(b + p.o_tab); D.hist_out = (int*)(b + p.o_hist);
+            // counts, offsets and the compact pair list are written by the finalize kernel straight into the pinned landing buffer
+            // (device-addressable, UVA) - no device-to-host copies; the dense table (MBs) still goes through one copy
+            uint8_t* o = m->h_out + p.ho;
+            D.n_matches = (int32_t*)o; D.pair_off = (int32_t*)(o + (size_t)S.n_kf * 4);
+            D.pairs = S.pairs ? (uint32_t*)(o + (size_t)S.n_kf * 8) : nullptr; D.pairs_cap = S.pairs_cap;
+            D.dense = S.dense ? (int32_t*)(b + p.o_dense) : nullptr; D.dense_stride = p.n;
+            hj[w] = D;
+        }
+        if ((s = commit(st, total)) != BORB_OK) return s;
+        BORB_CUDA(cudaMemsetAsync(b + o_hist, 0, hist_bytes, m->stream));
+        BORB_CUDA(cudaMemsetAsync(b + o_tab, 0xFF, tab_bytes, m->stream));
+        for (int j : work) {
+            if (J[j].dense) BORB_CUDA(cudaMemsetAsync(b + P[j].o_dense, 0xFF, (size_t)J[j].n_kf * P[j].n * 4, m->stream));
+            if (J[j].frame) BORB_CUDA(cudaStreamWaitEvent(m->stream, J[j].frame->ready, 0));
+        }
+        BowDbArgs A{};
+        A.jobs = (const BowDbJob*)(b + o_jobs); A.n_jobs = nw; A.static_sched = g_bow_static.load();
+        A.nnratio = nnratio; A.check_ori = check_ori;
+        if (m->timing) BORB_CUDA(cudaEventRecord(m->t0, m->stream));
+        m->launches += launch_bowdb(A, hj[0], max_smem_frame, max_items, total_kf, max_nn, g_bow_csa.load(), J[work[0]].db->n_sm, m->stream);
+        if (m->timing) BORB_CUDA(cudaEventRecord(m->t1, m->stream));
+        BORB_CUDA(cudaGetLastError());
+        for (int j : work)
+            if (J[j].dense) BORB_CUDA(cudaMemcpyAsync(J[j].dense, b + P[j].o_dense, (size_t)J[j].n_kf * P[j].n * 4, cudaMemcpyDeviceToHost, m->stream));
+    }
+    BORB_CUDA(cudaStreamSynchronize(m->stream));
+    if (m->timing) { float ms = 0.f; if (cudaEventElapsedTime(&ms, m->t0, m->t1) == cudaSuccess) m->last_ms = ms; else cudaGetLastError(); }
+    int overflow = -1;
+    long long over_total = 0;
+    for (int j : work) {
+        const SearchJob& S = J[j];
+        const uint8_t* o = m->h_out + P[j].ho;
+        std::memcpy(S.n_matches, o, (size_t)S.n_kf * 4);
+        if (S.pair_offset) std::memcpy(S.pair_offset, o + (size_t)S.n_kf * 4, (size_t)S.n_kf * 4);
+        if (!S.pairs) continue;
+        long long total_pairs = 0;
+        for (int i = 0; i < S.n_kf; i++) total_pairs += S.n_matches[i];
+        if (S.n_pairs_total) *S.n_pairs_total = (int32_t)total_pairs;
+        const long long ncopy = total_pairs < S.pairs_cap ? total_pairs : S.pairs_cap;
+        if (ncopy > 0) std::memcpy(S.pairs, o + (size_t)S.n_kf * 8, (size_t)ncopy * 4);
+        if (total_pairs > S.pairs_cap && overflow < 0) { overflow = j; over_total = total_pairs; }
+    }
+    if (overflow >= 0) {
+        set_error("%lld matched pairs, capacity %d", over_total, J[overflow].pairs_cap);
+        return job_fail(batch, overflow, BORB_ERR_CAPACITY);
+    }
+    return BORB_OK;
+}
+
+// the checks of the single database searches on their host view
+borb_status check_db_view(borb_matcher* m, borb_kfdb* db, const borb_keyframe_view* frame, int n_kf) {
     if (m->device != db->device) { set_error("matcher and keyframe database live on different devices"); return BORB_ERR_INVALID_ARG; }
     borb_status s = check_kf(frame, "SearchByBoW(database, frame)");
-    if (s != BORB_OK) return s;
-    if (n_pairs_total) *n_pairs_total = 0;
-    if (n_kf == 0) return BORB_OK;
+    if (s != BORB_OK || n_kf == 0) return s;
     const int nn = frame->fv.n_nodes, mf = nn > 0 ? frame->fv.start[nn] : 0;
     for (int a = 0; a < nn; a++)
         if (frame->fv.start[a + 1] < frame->fv.start[a] || (a > 0 && frame->fv.node_id[a] <= frame->fv.node_id[a - 1])) { set_error("FeatureVector nodes must ascend"); return BORB_ERR_INVALID_ARG; }
     for (int r = 0; r < mf; r++)
         if (frame->fv.feat_idx[r] >= (uint32_t)frame->n) { set_error("FeatureVector index outside the frame's features"); return BORB_ERR_INVALID_ARG; }
-    if (dense) for (size_t i = 0; i < (size_t)n_kf * frame->n; i++) dense[i] = -1;
-    for (int i = 0; i < n_kf; i++) { n_matches[i] = 0; if (pair_offset) pair_offset[i] = 0; }
-    if (mf == 0) return BORB_OK;
-    uint8_t* b = nullptr;
-    size_t o_nm = 0, o_po = 0, o_pairs = 0, o_dense = 0, o_ctr = 0;
-    const size_t fbytes = frame_block_bytes(frame);
-    int dense_stride = frame->n;
-    {
-        std::lock_guard<std::mutex> lk(db->mu);
-        const int n_slots = (int)db->entries.size();
-        if (!slots && n_kf != n_slots) { set_error("slots == NULL searches every slot: n_kf must be %d", n_slots); return BORB_ERR_INVALID_ARG; }
-        if (slots)
-            for (int i = 0; i < n_kf; i++)
-                if (slots[i] < 0 || slots[i] >= n_slots || !db->entries[slots[i]].alive) { set_error("slot %d is not a live keyframe", slots[i]); return BORB_ERR_INVALID_ARG; }
-        BORB_CUDA(cudaSetDevice(m->device));
-        if ((s = kfdb_sync_table(db, m->stream)) != BORB_OK) return s;
-        Stager st(m);
-        const size_t o_fb = st.reserve(fbytes);                                  // filled in place below
-        const size_t o_sl = slots ? st.add(slots, (size_t)n_kf * 4) : 0;
-        const size_t input_end = st.off;
-        o_ctr = st.reserve(256);                                                   // work counter | pair cursor
-        o_nm = st.reserve((size_t)n_kf * 4); o_po = st.reserve((size_t)n_kf * 4);
-        const size_t o_hist = st.reserve((size_t)n_kf * 32 * 4);
-        const size_t o_tab = st.reserve((size_t)n_kf * mf * 4);
-        o_pairs = pairs ? st.reserve((size_t)pairs_cap * 4 + 16) : 0;
-        o_dense = dense ? st.reserve((size_t)n_kf * dense_stride * 4) : 0;
-        const size_t total = st.off;
-        st.off = input_end;
-        if ((s = ensure_host(m, input_end)) != BORB_OK) return s;
-        if ((s = ensure_arena(m, total)) != BORB_OK) return s;
-        BORB_CUDA(cudaStreamSynchronize(m->stream));
-        const int n_items = pack_frame_block(frame, n_kf, m->h_stage + o_fb);
-        if ((s = commit(st, total)) != BORB_OK) return s;
-        b = m->arena;
-        BORB_CUDA(cudaMemsetAsync(b + o_ctr, 0, 256, m->stream));
-        BORB_CUDA(cudaMemsetAsync(b + o_hist, 0, (size_t)n_kf * 32 * 4, m->stream));
-        BORB_CUDA(cudaMemsetAsync(b + o_tab, 0xFF, (size_t)n_kf * mf * 4, m->stream));
-        if (dense) BORB_CUDA(cudaMemsetAsync(b + o_dense, 0xFF, (size_t)n_kf * dense_stride * 4, m->stream));
-        BowDbArgs A{};
-        A.table = db->d_stream; A.slots = slots ? (const int32_t*)(b + o_sl) : nullptr; A.n_kf = n_kf;
-        A.n_items = n_items; A.static_sched = g_bow_static.load();
-        A.frame_block = b + o_fb; A.frame_bytes = (int)fbytes;
-        A.frame_in_smem = bowdb_frame_fits_smem((int)fbytes) ? 1 : 0;
-        A.nnratio = nnratio; A.check_ori = check_ori;
-        A.table_out = (uint32_t*)(b + o_tab); A.work_counter = (int*)(b + o_ctr); A.hist_out = (int*)(b + o_hist);
-        // results: counts, offsets and the compact pair list are written by the finalize kernel straight into the pinned landing
-        // buffer (device-addressable, UVA) - no device-to-host copies; the dense table (MBs) still goes through one copy
-        const size_t ho_nm = 0, ho_po = (size_t)n_kf * 4, ho_pairs = (size_t)n_kf * 8;
-        if ((s = ensure_out(m, (size_t)n_kf * 8 + (size_t)pairs_cap * 4 + 64)) != BORB_OK) return s;
-        uint8_t* ho = m->h_out;
-        BowDbFinal F{};
-        F.table_out = A.table_out; F.hist = A.hist_out; F.n_kf = n_kf; F.mf = mf; F.check_ori = check_ori;
-        F.forig = (const uint16_t*)(b + o_fb + reinterpret_cast<const FrameBlockHdrHost*>(m->h_stage + o_fb)->off_orig);
-        F.n_matches = (int32_t*)(ho + ho_nm); F.pair_off = (int32_t*)(ho + ho_po);
-        F.pairs = pairs ? (uint32_t*)(ho + ho_pairs) : nullptr; F.pairs_cap = pairs_cap; F.cursor = (int*)(b + o_ctr + 64);
-        F.dense = dense ? (int32_t*)(b + o_dense) : nullptr; F.dense_stride = dense_stride;
-        if (m->timing) BORB_CUDA(cudaEventRecord(m->t0, m->stream));
-        m->launches += launch_bowdb(A, F, g_bow_csa.load(), db->n_sm, m->stream);
-        if (m->timing) BORB_CUDA(cudaEventRecord(m->t1, m->stream));
-        BORB_CUDA(cudaGetLastError());
-    }
-    if (dense) BORB_CUDA(cudaMemcpyAsync(dense, b + o_dense, (size_t)n_kf * dense_stride * 4, cudaMemcpyDeviceToHost, m->stream));
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
-    if (m->timing) { float ms = 0.f; if (cudaEventElapsedTime(&ms, m->t0, m->t1) == cudaSuccess) m->last_ms = ms; else cudaGetLastError(); }
-    const uint8_t* ho = m->h_out;
-    std::memcpy(n_matches, ho, (size_t)n_kf * 4);
-    if (pair_offset) std::memcpy(pair_offset, ho + (size_t)n_kf * 4, (size_t)n_kf * 4);
-    if (pairs) {
-        long long total_pairs = 0;
-        for (int i = 0; i < n_kf; i++) total_pairs += n_matches[i];
-        if (n_pairs_total) *n_pairs_total = (int32_t)total_pairs;
-        const long long ncopy = total_pairs < pairs_cap ? total_pairs : pairs_cap;
-        if (ncopy > 0) std::memcpy(pairs, ho + (size_t)n_kf * 8, (size_t)ncopy * 4);
-        if (total_pairs > pairs_cap) { set_error("%lld matched pairs, capacity %d", total_pairs, pairs_cap); return BORB_ERR_CAPACITY; }
-    }
     return BORB_OK;
+}
+
+// the checks of a batch job's database and resident frame
+borb_status check_db_job(borb_matcher* m, borb_kfdb* db, const borb_frame* f, int j) {
+    if (!db) { set_error("job %d: null database", j); return BORB_ERR_INVALID_ARG; }
+    if (db->device != m->device) { set_error("job %d: database and matcher live on different devices", j); return BORB_ERR_INVALID_ARG; }
+    return check_resident_bow(f, m, j, "frame");
 }
 
 }  // namespace
 
+borb_status borb_kfdb_query(borb_matcher* m, borb_kfdb* db, const uint32_t* bow_word, const double* bow_value, int n_bow,
+                            int32_t* common_words, float* score, uint32_t* first_word, int cap, int32_t* n_slots) {
+    if (!m || !db || !common_words || !score || !first_word || !n_slots || n_bow < 0 || (n_bow > 0 && (!bow_word || !bow_value))) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+    if (m->device != db->device) { set_error("matcher and keyframe database live on different devices"); return BORB_ERR_INVALID_ARG; }
+    for (int i = 1; i < n_bow; i++)
+        if (bow_word[i] <= bow_word[i - 1]) { set_error("BowVector words must ascend (std::map order)"); return BORB_ERR_INVALID_ARG; }
+    const QueryJob q{db, nullptr, bow_word, bow_value, n_bow, common_words, score, first_word, cap, n_slots};
+    return kfdb_query_jobs(m, &q, 1, false);
+}
+
+borb_status borb_kfdb_query_batch(borb_matcher* m, const borb_kfdb_query_job* jobs, int n_jobs) {
+    if (!m || n_jobs < 0 || (n_jobs > 0 && !jobs)) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+    if (n_jobs == 0) return BORB_OK;
+    std::vector<QueryJob> q(n_jobs);
+    for (int j = 0; j < n_jobs; j++) {
+        const borb_kfdb_query_job& B = jobs[j];
+        borb_status s = check_db_job(m, B.db, B.frame, j);
+        if (s != BORB_OK) return s;
+        if (!B.common_words || !B.score || !B.first_word || !B.n_slots) { set_error("job %d: null output", j); return BORB_ERR_INVALID_ARG; }
+        q[j] = QueryJob{B.db, B.frame, nullptr, nullptr, 0, B.common_words, B.score, B.first_word, B.cap, B.n_slots};
+    }
+    return kfdb_query_jobs(m, q.data(), n_jobs, true);
+}
+
 borb_status borb_search_by_bow_db(borb_matcher* m, borb_kfdb* db, const int32_t* slots, int n_kf, const borb_keyframe_view* frame,
                                   float nnratio, int check_orientation, int32_t* match, int32_t* n_matches) {
     if (!m || !db || !frame || !match || !n_matches || n_kf < 0) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
-    return bowdb_search(m, db, slots, n_kf, frame, nnratio, check_orientation, match, n_matches, nullptr, nullptr, 0, nullptr);
+    borb_status s = check_db_view(m, db, frame, n_kf);
+    if (s != BORB_OK) return s;
+    const SearchJob J{db, nullptr, frame, slots, n_kf, match, n_matches, nullptr, nullptr, 0, nullptr};
+    return bowdb_jobs(m, &J, 1, nnratio, check_orientation, false);
 }
 
 borb_status borb_search_by_bow_db_pairs(borb_matcher* m, borb_kfdb* db, const int32_t* slots, int n_kf, const borb_keyframe_view* frame,
                                         float nnratio, int check_orientation, int32_t* n_matches, int32_t* pair_offset, uint32_t* pairs,
                                         int pairs_cap, int32_t* n_pairs_total) {
     if (!m || !db || !frame || !n_matches || n_kf < 0 || pairs_cap < 0 || (pairs && !pair_offset)) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
-    return bowdb_search(m, db, slots, n_kf, frame, nnratio, check_orientation, nullptr, n_matches, pair_offset, pairs, pairs_cap, n_pairs_total);
+    borb_status s = check_db_view(m, db, frame, n_kf);
+    if (s != BORB_OK) return s;
+    const SearchJob J{db, nullptr, frame, slots, n_kf, nullptr, n_matches, pair_offset, pairs, pairs_cap, n_pairs_total};
+    return bowdb_jobs(m, &J, 1, nnratio, check_orientation, false);
+}
+
+borb_status borb_search_by_bow_db_batch(borb_matcher* m, const borb_bow_db_job* jobs, int n_jobs, float nnratio, int check_orientation) {
+    if (!m || n_jobs < 0 || (n_jobs > 0 && !jobs)) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+    if (n_jobs == 0) return BORB_OK;
+    std::vector<SearchJob> S(n_jobs);
+    for (int j = 0; j < n_jobs; j++) {
+        const borb_bow_db_job& B = jobs[j];
+        borb_status s = check_db_job(m, B.db, B.frame, j);
+        if (s != BORB_OK) return s;
+        if (B.n_kf < 0 || B.pairs_cap < 0 || (B.n_kf > 0 && !B.n_matches)) { set_error("job %d: null output or negative count", j); return BORB_ERR_INVALID_ARG; }
+        if (B.pairs && !B.pair_offset) { set_error("job %d: pairs without pair_offset", j); return BORB_ERR_INVALID_ARG; }
+        S[j] = SearchJob{B.db, B.frame, nullptr, B.slots, B.n_kf, nullptr, B.n_matches, B.pair_offset, B.pairs, B.pairs_cap, B.n_pairs_total};
+    }
+    return bowdb_jobs(m, S.data(), n_jobs, nnratio, check_orientation, true);
 }
 
 borb_status borb_search_for_triangulation(borb_matcher* m, const borb_keyframe_view* kf1, const borb_keyframe_view* kf2, const float* F12,
@@ -2078,8 +2203,8 @@ borb_status borb_frames_compute_bow(borb_matcher* m, borb_voc* v, borb_frame* co
     const size_t o_jobs = st.add(nullptr, (size_t)n_frames * sizeof(BowFrameJob));     // filled in place
     const size_t input_end = st.off;
     std::vector<size_t> o_scr(n_frames), o_copy(n_frames, 0);
-    const size_t cnt_bytes = ((size_t)n_frames * 8 + 15) & ~size_t(15);
-    size_t res_bytes = cnt_bytes;                       // (n_bow, n_nodes) of every frame, then the host copies: one D2H
+    const size_t cnt_bytes = ((size_t)n_frames * 12 + 15) & ~size_t(15);
+    size_t res_bytes = cnt_bytes;                       // (n_bow, n_nodes, fv_start[n_nodes]) of every frame, then the host copies: one D2H
     for (int i = 0; i < n_frames; i++) {
         const size_t n = (size_t)frames[i]->n;
         o_scr[i] = st.reserve(n * 16);                  // weight f64 | word i32 | node i32
@@ -2106,7 +2231,7 @@ borb_status borb_frames_compute_bow(borb_matcher* m, borb_voc* v, borb_frame* co
             uint8_t* c = b + o_res + o_copy[i];
             J.copy = BowTables{(uint32_t*)(c + n * 8), (double*)c, (uint32_t*)(c + n * 12), (int32_t*)(c + n * 16), (uint32_t*)(c + n * 20 + 4)};
         }
-        J.counts = (int32_t*)(b + o_res) + 2 * i;
+        J.counts = (int32_t*)(b + o_res) + 3 * i;
         hj[i] = J;
         f->has_bow = false;                             // the storage is rewritten from here on
     }
@@ -2120,21 +2245,19 @@ borb_status borb_frames_compute_bow(borb_matcher* m, borb_voc* v, borb_frame* co
     const uint8_t* h = m->h_out;
     for (int i = 0; i < n_frames; i++) {
         borb_frame* f = frames[i];
-        int32_t cnt[2];
-        std::memcpy(cnt, h + (size_t)i * 8, 8);
-        f->n_bow = cnt[0]; f->n_nodes = cnt[1]; f->has_bow = true;
+        int32_t cnt[3];
+        std::memcpy(cnt, h + (size_t)i * 12, 12);
+        f->n_bow = cnt[0]; f->n_nodes = cnt[1]; f->n_fv = cnt[2]; f->has_bow = true;
         if (n_bow) n_bow[i] = cnt[0];
         if (n_nodes) n_nodes[i] = cnt[1];
         if (!wants(i)) continue;
         const size_t n = (size_t)f->n;
         const uint8_t* c = h + o_copy[i];
-        int32_t kept = 0;
-        std::memcpy(&kept, c + n * 16 + (size_t)cnt[1] * 4, 4);        // fv_start[n_nodes]
         if (bow_value && bow_value[i]) std::memcpy(bow_value[i], c, (size_t)cnt[0] * 8);
         if (bow_word && bow_word[i]) std::memcpy(bow_word[i], c + n * 8, (size_t)cnt[0] * 4);
         if (fv_node && fv_node[i]) std::memcpy(fv_node[i], c + n * 12, (size_t)cnt[1] * 4);
         if (fv_start && fv_start[i]) std::memcpy(fv_start[i], c + n * 16, (size_t)(cnt[1] + 1) * 4);
-        if (fv_idx && fv_idx[i]) std::memcpy(fv_idx[i], c + n * 20 + 4, (size_t)kept * 4);
+        if (fv_idx && fv_idx[i]) std::memcpy(fv_idx[i], c + n * 20 + 4, (size_t)cnt[2] * 4);
     }
     return BORB_OK;
 }

@@ -5,8 +5,12 @@
 // Layout.  A keyframe is stored in the database as a STREAM RECORD: its features permuted into FeatureVector order (node id
 // ascending, feature index ascending inside a node — the order of the reference's two nested loops, :180-205), so that the
 // descriptors of a node are consecutive 32-byte rows and every keyframe byte is read exactly once.  The query frame is packed
-// the same way by the host (plus a work list), fetched into shared memory ONCE per (persistent, one per SM) CTA with a 1-D TMA
-// bulk copy (cp.async.bulk + mbarrier) and reused for every keyframe.
+// the same way on the device (bowdb_pack_kernel, plus a work list), fetched into shared memory ONCE per (persistent, one per SM)
+// CTA with a 1-D TMA bulk copy (cp.async.bulk + mbarrier) and reused for every keyframe.
+//
+// Jobs.  One launch sequence (pack, match, finalize) serves many frames, each against its own database and keyframe list
+// (borb_search_by_bow_db_batch; a single call is the one-job case): every job has its own block, work counter, match table,
+// histograms and pair cursor.
 //
 // Work decomposition.  A frame feature lives in exactly one node, so the greedy "frame feature already claimed" skip (:209)
 // never crosses nodes: a (keyframe, node) bucket is an independent claim scope.  An ITEM is (one node of the query frame, a
@@ -81,49 +85,14 @@ __device__ __forceinline__ void three_maxima(const int* cnt, int& ind1, int& ind
 
 }  // namespace
 
-// Packed query frame (built by the host, borb_match_host.cu:pack_frame_block): header, then 16-byte aligned sections.
-//   node[nn] u32 ascending | start[nn+1] i32 | orig[m] u16 | angle[m] f32 | desc[m][32]     (m = features inside nodes)
-//   work list (np = non-empty frame nodes, widest bucket first): pnode[np] i32 node index | pcs[np] i32 keyframes per item |
-//   pstart[np+1] i32 cumulative item count
-struct FrameBlockHdr { int32_t nn, m, n, off_node, off_start, off_orig, off_angle, off_desc, bytes, np, off_pnode, off_pcs, off_pstart, pad[3]; };
-
 struct KfRun { const uint2* meta; const uint4* desc; int rs, off; };     // rows rs.. of one keyframe's bucket; off = first row's rank in the batch
 
-// Work decomposition.  An ITEM is (frame node b, a range of keyframes): every row of the item's batch is matched against the
-// SAME nt columns (the frame features of node b), so the column loop has a warp-uniform trip count and warp-uniform
-// shared-memory addresses (one broadcast wavefront per load), and all 32 lanes hold a live row.  The number of keyframes per
-// item shrinks with nt^2 (the host's work list), widest buckets first, so the items are of similar cost.
+// The items of one job, taken by this CTA's warps until the job's work counter is exhausted.  fb: the job's frame block, in
+// shared memory (FSM) or in global memory; ws: the warp's scratch.
 template <int CSA, bool FSM>
-__global__ void __launch_bounds__(32 * BDB_WARPS, BDB_CTAS) bowdb_match_kernel(BowDbArgs A) {
-    extern __shared__ __align__(128) uint8_t sm[];
-    __shared__ __align__(8) unsigned long long bar;
-    const int tid = threadIdx.x, lane = tid & 31, wrp = tid >> 5;
+__device__ __forceinline__ void bowdb_job_items(const BowDbArgs& A, const BowDbJob& J, const uint8_t* fb, uint8_t* ws) {
+    const int lane = threadIdx.x & 31, wrp = threadIdx.x >> 5;
     const unsigned lt_mask = (1u << lane) - 1u;
-
-    // ---- the query frame: one bulk copy per CTA, reused for every item this CTA processes
-    const uint8_t* fb = FSM ? sm : A.frame_block;
-    const size_t scratch0 = FSM ? (((size_t)A.frame_bytes + 127) & ~size_t(127)) : 0;
-    if (FSM) {
-        if (tid == 0) {
-            asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(&bar)));
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(&bar)), "r"((uint32_t)A.frame_bytes) : "memory");
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                         ::"r"(smem_u32(sm)), "l"(reinterpret_cast<uint64_t>(A.frame_block)), "r"((uint32_t)A.frame_bytes), "r"(smem_u32(&bar))
-                         : "memory");
-        }
-        __syncthreads();
-        asm volatile(
-            "{\n"
-            ".reg .pred p;\n"
-            "BOWDB_WAIT:\n"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], 0;\n"
-            "@p bra BOWDB_DONE;\n"
-            "bra BOWDB_WAIT;\n"
-            "BOWDB_DONE:\n"
-            "}\n" ::"r"(smem_u32(&bar))
-            : "memory");
-    }
     const FrameBlockHdr* H = reinterpret_cast<const FrameBlockHdr*>(fb);
     const int mf = H->m, np = H->np;
     const uint32_t* fnode = reinterpret_cast<const uint32_t*>(fb + H->off_node);
@@ -134,7 +103,6 @@ __global__ void __launch_bounds__(32 * BDB_WARPS, BDB_CTAS) bowdb_match_kernel(B
     const int32_t* pcs = reinterpret_cast<const int32_t*>(fb + H->off_pcs);
     const int32_t* pstart = reinterpret_cast<const int32_t*>(fb + H->off_pstart);
 
-    uint8_t* ws = sm + scratch0 + (size_t)wrp * BDB_WARP_BYTES;
     uint32_t* claim = reinterpret_cast<uint32_t*>(ws);                                   // claimed columns when the bucket is wider than 32
     KfRun* run = reinterpret_cast<KfRun*>(ws + BDB_CLAIM_WORDS * 4);                      // the <= 32 keyframes of the current batch
     // ring of pending rows with a good MapPoint: descriptor halves and {row, run, meta.x, meta.y}
@@ -149,14 +117,14 @@ __global__ void __launch_bounds__(32 * BDB_WARPS, BDB_CTAS) bowdb_match_kernel(B
         int it = 0;
         if (A.static_sched) { it = it_static; it_static += warps_total; }
         else {
-            if (lane == 0) it = atomicAdd(A.work_counter, 1);
+            if (lane == 0) it = atomicAdd(J.ctr, 1);
             it = __shfl_sync(0xFFFFFFFFu, it, 0);
         }
         if (it >= items) break;
         int lo = 0, hi = np;                                      // largest p with pstart[p] <= it
         while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (pstart[mid] <= it) lo = mid; else hi = mid; }
         const int bf = pnode[lo], cs = pcs[lo];
-        const int k0 = (it - pstart[lo]) * cs, k1 = min(A.n_kf, k0 + cs);
+        const int k0 = (it - pstart[lo]) * cs, k1 = min(J.n_kf, k0 + cs);
         const uint32_t node = fnode[bf];
         const int ts = fstart[bf], nt = fstart[bf + 1] - ts;       // nt > 0 by construction of the work list
         const bool wide = nt > 32;
@@ -169,7 +137,7 @@ __global__ void __launch_bounds__(32 * BDB_WARPS, BDB_CTAS) bowdb_match_kernel(B
             int rs = 0, cnt = 0;
             const uint2* kmeta = nullptr; const uint4* kdesc = nullptr;
             if (k < k1) {
-                const KfStream* Kp = A.table + (A.slots ? A.slots[k] : k);
+                const KfStream* Kp = J.table + (J.slots ? J.slots[k] : k);
                 const int nn = Kp->nn;
                 if (nn > 0) {
                     const uint32_t* kn = Kp->node;
@@ -254,8 +222,8 @@ __global__ void __launch_bounds__(32 * BDB_WARPS, BDB_CTAS) bowdb_match_kernel(B
                     const uint32_t mx = (uint32_t)__shfl_sync(0xFFFFFFFFu, e.z, L), my = (uint32_t)__shfl_sync(0xFFFFFFFFu, e.w, L);
                     if (lane == 0) {
                         const int bin = A.check_ori ? rot_bin(__uint_as_float(my), fangle[ts + pb]) : 0;
-                        A.table_out[(size_t)(kb + rL) * mf + ts + pb] = (mx & 0xFFFFu) | ((uint32_t)bin << 16);   // vpMapPointMatches[bestIdxF] = pMP (:232)
-                        atomicAdd(&A.hist_out[(size_t)(kb + rL) * 32 + bin], 1);                                     // rotHist[bin].push_back (:241)
+                        J.table_out[(size_t)(kb + rL) * mf + ts + pb] = (mx & 0xFFFFu) | ((uint32_t)bin << 16);   // vpMapPointMatches[bestIdxF] = pMP (:232)
+                        atomicAdd(&J.hist_out[(size_t)(kb + rL) * 32 + bin], 1);                                     // rotHist[bin].push_back (:241)
                     }
                 }
             };
@@ -298,24 +266,117 @@ __global__ void __launch_bounds__(32 * BDB_WARPS, BDB_CTAS) bowdb_match_kernel(B
     }
 }
 
+// Job scheduling.  A call with one job (every single call) passes it as a kernel parameter (ONE_SMEM / ONE_GLOBAL): its fields stay
+// in the constant bank instead of registers, which keeps the item loop at the register budget of 64.  A job table (TABLE):
+// a CTA works on one job at a time: its warps take the job's items from the job's counter, and only when that
+// counter is exhausted (for every warp: a barrier) does the CTA move on, to the next job (in job order, wrapping) that still has
+// items.  So a CTA visits a job at most once, and fetches a shared-memory frame block (one 1-D TMA bulk copy) only for a job it
+// is about to work on.  CTAs start at jobs spread over the job table, so many small jobs are taken by different CTAs.  Blocks
+// that do not fit next to the warp scratch are read through L1 from global memory (FSM = false), in the same launch.
+enum { ONE_SMEM = 0, ONE_GLOBAL = 1, TABLE = 2 };
+template <int CSA, int KIND>
+__global__ void __launch_bounds__(32 * BDB_WARPS, BDB_CTAS) bowdb_match_kernel(BowDbArgs A, int smem_frame, const __grid_constant__ BowDbJob J0) {
+    extern __shared__ __align__(128) uint8_t sm[];
+    __shared__ __align__(8) unsigned long long bar;
+    __shared__ BowDbJob sJ;
+    __shared__ int s_job, s_next, s_left, s_loads;     // the job cursor (the next job to look at, jobs not looked at) and the block loads so far
+    const int tid = threadIdx.x;
+    if (KIND == ONE_GLOBAL) { bowdb_job_items<CSA, false>(A, J0, J0.frame_block, sm + (size_t)(tid >> 5) * BDB_WARP_BYTES); return; }
+    if (KIND == ONE_SMEM) {
+        if (tid == 0) {
+            asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(&bar)));
+            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(&bar)), "r"((uint32_t)J0.frame_bytes) : "memory");
+            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                         ::"r"(smem_u32(sm)), "l"(reinterpret_cast<uint64_t>(J0.frame_block)), "r"((uint32_t)J0.frame_bytes), "r"(smem_u32(&bar))
+                         : "memory");
+        }
+        __syncthreads();
+        asm volatile(
+            "{\n"
+            ".reg .pred p;\n"
+            "BOWDB_WAIT1:\n"
+            "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], 0;\n"
+            "@p bra BOWDB_DONE1;\n"
+            "bra BOWDB_WAIT1;\n"
+            "BOWDB_DONE1:\n"
+            "}\n" ::"r"(smem_u32(&bar))
+            : "memory");
+        bowdb_job_items<CSA, true>(A, J0, sm, sm + (((size_t)smem_frame + 127) & ~size_t(127)) + (size_t)(tid >> 5) * BDB_WARP_BYTES);
+        return;
+    }
+    if (tid == 0) {
+        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(&bar)));
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        s_next = A.static_sched ? 0 : (int)((long long)blockIdx.x * A.n_jobs / gridDim.x); s_left = A.n_jobs; s_loads = 0;
+    }
+    while (true) {
+        if (tid == 0) {
+            int pick = -1, next = s_next, left = s_left;
+            for (; left > 0 && pick < 0; left--) {
+                const int* c = A.jobs[next].ctr;
+                if (A.static_sched || *(volatile const int*)c < *(volatile const int*)(c + 1)) pick = next;
+                next = next + 1 == A.n_jobs ? 0 : next + 1;
+            }
+            s_next = next; s_left = left; s_job = pick;
+            if (pick >= 0) sJ = A.jobs[pick];
+        }
+        __syncthreads();
+        uint8_t* ws = sm + (((size_t)smem_frame + 127) & ~size_t(127)) + (size_t)(tid >> 5) * BDB_WARP_BYTES;
+        if (s_job < 0) break;
+        if (sJ.frame_in_smem) {
+            if (tid == 0) {
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");          // the previous block was read through the generic proxy
+                asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(&bar)), "r"((uint32_t)sJ.frame_bytes) : "memory");
+                asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                             ::"r"(smem_u32(sm)), "l"(reinterpret_cast<uint64_t>(sJ.frame_block)), "r"((uint32_t)sJ.frame_bytes), "r"(smem_u32(&bar))
+                             : "memory");
+            }
+            asm volatile(
+                "{\n"
+                ".reg .pred p;\n"
+                "BOWDB_WAIT:\n"
+                "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
+                "@p bra BOWDB_DONE;\n"
+                "bra BOWDB_WAIT;\n"
+                "BOWDB_DONE:\n"
+                "}\n" ::"r"(smem_u32(&bar)), "r"((uint32_t)s_loads & 1u)
+                : "memory");
+            bowdb_job_items<CSA, true>(A, sJ, sm, ws);
+        } else {
+            bowdb_job_items<CSA, false>(A, sJ, sJ.frame_block, ws);
+        }
+        __syncthreads();                                          // every warp is done with this job's block
+        if (tid == 0 && sJ.frame_in_smem) s_loads++;
+    }
+}
+
 // Rotation-consistency cull and compaction, a 128-thread CTA per keyframe.  table_out row: one u32 per frame position
 // (FeatureVector order): keyframe feature | bin << 16, or 0xFFFFFFFF.  Survivors are written in frame-position order.
 // A warp owns a contiguous quarter of the row (its entries stay in registers between the passes when the row has at most
 // FIN_THREADS * FIN_REG positions), so the ordered compaction needs ballots and ONE block-level exchange of the warp totals.
 constexpr int FIN_THREADS = 128;
 constexpr int FIN_REG = 16;
-__global__ void __launch_bounds__(FIN_THREADS) bowdb_finalize_kernel(BowDbFinal F) {
+__global__ void __launch_bounds__(FIN_THREADS) bowdb_finalize_kernel(BowDbArgs A) {
     __shared__ int hist[32];
     __shared__ int warp_cnt[FIN_THREADS / 32];
-    __shared__ int s_off, s_i1, s_i2, s_i3;
+    __shared__ int s_off, s_i1, s_i2, s_i3, s_job;
     const int tid = threadIdx.x, lane = tid & 31, wrp = tid >> 5;
-    const int k = blockIdx.x;
-    if (tid < 32) hist[tid] = F.hist[(size_t)k * 32 + tid];              // rotation histogram accumulated by the match kernel
-    const uint32_t* row = F.table_out + (size_t)k * F.mf;
-    const int per_warp = (((F.mf + FIN_THREADS / 32 - 1) / (FIN_THREADS / 32)) + 31) & ~31;      // positions per warp, whole 32-steps
-    const int w0 = wrp * per_warp, w1 = min(F.mf, w0 + per_warp);
+    if (tid == 0) {                                                       // the job of this CTA: largest j with kf_base <= blockIdx.x
+        int lo = 0, hi = A.n_jobs;
+        while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (A.jobs[mid].kf_base <= (int)blockIdx.x) lo = mid; else hi = mid; }
+        s_job = lo;
+    }
+    __syncthreads();
+    const BowDbJob& J = A.jobs[s_job];
+    const int k = blockIdx.x - J.kf_base, mf = J.m;
+    const uint16_t* forig = reinterpret_cast<const uint16_t*>(J.frame_block + frame_block_layout(J.nn, mf, J.n).off_orig);
+    if (tid < 32) hist[tid] = J.hist_out[(size_t)k * 32 + tid];              // rotation histogram accumulated by the match kernel
+    const uint32_t* row = J.table_out + (size_t)k * mf;
+    const int per_warp = (((mf + FIN_THREADS / 32 - 1) / (FIN_THREADS / 32)) + 31) & ~31;      // positions per warp, whole 32-steps
+    const int w0 = wrp * per_warp, w1 = min(mf, w0 + per_warp);
     const bool in_regs = per_warp <= 32 * FIN_REG;
-    const bool need_rows = F.pairs != nullptr || F.dense != nullptr;
+    const bool need_rows = J.pairs != nullptr || J.dense != nullptr;
     uint32_t e[FIN_REG];
 #pragma unroll
     for (int t = 0; t < FIN_REG; t++) {
@@ -325,23 +386,23 @@ __global__ void __launch_bounds__(FIN_THREADS) bowdb_finalize_kernel(BowDbFinal 
     __syncthreads();
     if (tid == 0) {
         int i1 = -1, i2 = -1, i3 = -1, kept = 0;
-        if (F.check_ori) {
+        if (A.check_ori) {
             three_maxima(hist, i1, i2, i3);
             for (int b = 0; b < HISTO_LENGTH; b++) if (b == i1 || b == i2 || b == i3) kept += hist[b];
         } else {
             for (int b = 0; b < 32; b++) kept += hist[b];
         }
-        const int off = F.pairs ? atomicAdd(F.cursor, kept) : 0;
-        F.n_matches[k] = kept;                                           // nmatches after the cull (:267-285)
-        if (F.pair_off) F.pair_off[k] = off;
+        const int off = J.pairs ? atomicAdd(J.ctr + 2, kept) : 0;
+        J.n_matches[k] = kept;                                           // nmatches after the cull (:267-285)
+        if (J.pair_off) J.pair_off[k] = off;
         s_off = off; s_i1 = i1; s_i2 = i2; s_i3 = i3;
     }
     __syncthreads();
-    if (!F.pairs && !F.dense) return;
+    if (!J.pairs && !J.dense) return;
     const int i1 = s_i1, i2 = s_i2, i3 = s_i3;
     auto kept_entry = [&](uint32_t v) -> bool {
         if (v == 0xFFFFFFFFu) return false;
-        if (!F.check_ori) return true;
+        if (!A.check_ori) return true;
         const int b = (int)((v >> 16) & 31);
         return b == i1 || b == i2 || b == i3;
     };
@@ -363,9 +424,9 @@ __global__ void __launch_bounds__(FIN_THREADS) bowdb_finalize_kernel(BowDbFinal 
         const bool keep = kept_entry(v);
         const unsigned bal = __ballot_sync(0xFFFFFFFFu, keep);
         if (keep) {
-            const int j = (int)F.forig[i], r = (int)(v & 0xFFFFu);
-            if (F.pairs) { const int pos = run + __popc(bal & ((1u << lane) - 1)); if (pos < F.pairs_cap) F.pairs[pos] = (uint32_t)j | ((uint32_t)r << 16); }
-            if (F.dense) F.dense[(size_t)k * F.dense_stride + j] = r;
+            const int j = (int)forig[i], r = (int)(v & 0xFFFFu);
+            if (J.pairs) { const int pos = run + __popc(bal & ((1u << lane) - 1)); if (pos < J.pairs_cap) J.pairs[pos] = (uint32_t)j | ((uint32_t)r << 16); }
+            if (J.dense) J.dense[(size_t)k * J.dense_stride + j] = r;
         }
         run += __popc(bal);
     };
@@ -388,23 +449,110 @@ static int bowdb_warps(int frame_bytes, bool fsm) {
 
 bool bowdb_frame_fits_smem(int frame_bytes) { return bowdb_warps(frame_bytes, true) >= 8; }
 
-int launch_bowdb(const BowDbArgs& A, const BowDbFinal& F, int csa, int n_sm, cudaStream_t s) {
-    const bool fsm = A.frame_in_smem != 0;
-    const int warps = bowdb_warps(A.frame_bytes, fsm);
-    const size_t smem = (fsm ? (((size_t)A.frame_bytes + 127) & ~size_t(127)) : 0) + (size_t)warps * BDB_WARP_BYTES;
-    int ctas = (A.n_items + warps - 1) / warps;
+// The query frame's block (FrameBlockHdr + sections), one CTA per job: the FeatureVector's node and start arrays; orig, angle and
+// desc of every feature inside a node in FeatureVector order; and the work list - the non-empty nodes stable-sorted widest first
+// (the long items start first), keyframes per item cs = clamp(item_target / nt^2, 1, 32) so that an item is a few hundred
+// column-loop iterations whatever the bucket width (a keyframe's bucket of the node is about as full as the frame's), and the
+// item prefix pstart.  Also resets the job's work counter and pair cursor and stores its item count next to them.
+// Shared memory: 8 B per sort key (next power of two >= nn, at least 32).
+constexpr int PACK_THREADS = 512;
+__global__ void __launch_bounds__(PACK_THREADS) bowdb_pack_kernel(const BowDbJob* __restrict__ jobs) {
+    extern __shared__ __align__(16) uint64_t pk_sm[];
+    __shared__ int warp_sums[PACK_THREADS / 32];
+    __shared__ int s_np;
+    const BowDbJob& J = jobs[blockIdx.x];
+    const int tid = threadIdx.x, T = blockDim.x, lane = tid & 31, wrp = tid >> 5;
+    const int nn = J.nn, m = J.m;
+    FrameBlockHdr h = frame_block_layout(nn, m, J.n);
+    uint8_t* dst = J.frame_block;
+    uint32_t* node = reinterpret_cast<uint32_t*>(dst + h.off_node);
+    int32_t* start = reinterpret_cast<int32_t*>(dst + h.off_start);
+    uint16_t* orig = reinterpret_cast<uint16_t*>(dst + h.off_orig);
+    float* angle = reinterpret_cast<float*>(dst + h.off_angle);
+    uint4* desc = reinterpret_cast<uint4*>(dst + h.off_desc);
+    const uint4* src = reinterpret_cast<const uint4*>(J.desc);
+    for (int i = tid; i < nn; i += T) node[i] = J.fv_node[i];
+    for (int i = tid; i <= nn; i += T) start[i] = nn > 0 ? J.fv_start[i] : 0;
+    for (int t = tid; t < 2 * m; t += T) {                                // a thread per descriptor half
+        const int r = t >> 1;
+        const uint32_t j = J.fv_idx[r];
+        desc[t] = src[(size_t)j * 2 + (t & 1)];
+        if ((t & 1) == 0) { orig[r] = (uint16_t)j; angle[r] = J.keys[j].angle; }
+    }
+    // work list: (widest first, then node index) as one ascending 64-bit key; empty nodes sort last
+    int K = 32;
+    while (K < nn) K <<= 1;
+    uint64_t* keys = pk_sm;
+    int mine = 0;
+    for (int i = tid; i < K; i += T) {
+        const int w = i < nn ? J.fv_start[i + 1] - J.fv_start[i] : 0;
+        keys[i] = w > 0 ? ((uint64_t)(0xFFFFFFFFu - (uint32_t)w) << 32) | (uint32_t)i : ~0ull;
+        mine += w > 0;
+    }
+    for (int o = 16; o > 0; o >>= 1) mine += __shfl_xor_sync(0xFFFFFFFFu, mine, o);
+    if (lane == 0) warp_sums[wrp] = mine;
+    __syncthreads();
+    if (tid == 0) { int a = 0; for (int w = 0; w < T / 32; w++) a += warp_sums[w]; s_np = a; }
+    bitonic_sort_u64(keys, K);                                            // starts and ends with a barrier: s_np is visible
+    const int np = s_np;                                                  // non-empty nodes
+    int32_t* pnode = reinterpret_cast<int32_t*>(dst + h.off_pnode);
+    int32_t* pcs = reinterpret_cast<int32_t*>(dst + h.off_pcs);
+    int32_t* pstart = reinterpret_cast<int32_t*>(dst + h.off_pstart);
+    // each thread owns a contiguous chunk of the list: its item count, then an exclusive scan of the chunk totals
+    const int chunk = (np + T - 1) / T, c0 = min(np, tid * chunk), c1 = min(np, c0 + chunk);
+    int items = 0;
+    for (int p = c0; p < c1; p++) {
+        const int a = (int)(uint32_t)keys[p];
+        const long long nt = J.fv_start[a + 1] - J.fv_start[a];
+        long long cs = J.item_target / (nt * nt);
+        cs = cs < 1 ? 1 : (cs > 32 ? 32 : cs);                            // one 32-lane batch of keyframes per item at most
+        pnode[p] = a; pcs[p] = (int32_t)cs;
+        items += (int)((J.n_kf + cs - 1) / cs);
+    }
+    int incl = items;
+    for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xFFFFFFFFu, incl, o); if (lane >= o) incl += t; }
+    if (lane == 31) warp_sums[wrp] = incl;
+    __syncthreads();
+    int before = incl - items, total = 0;
+    for (int w = 0; w < T / 32; w++) { const int v = warp_sums[w]; if (w < wrp) before += v; total += v; }
+    for (int p = c0; p < c1; p++) { pstart[p] = before; before += (int)((J.n_kf + pcs[p] - 1) / pcs[p]); }
+    if (tid == 0) {
+        pstart[np] = total;
+        h.np = np;
+        *reinterpret_cast<FrameBlockHdr*>(dst) = h;
+        J.ctr[0] = 0; J.ctr[1] = total; J.ctr[2] = 0;
+    }
+}
+
+int launch_bowdb(const BowDbArgs& A, const BowDbJob& one, int max_smem_frame, long long max_items, int total_kf, int max_nn, int csa, int n_sm, cudaStream_t s) {
+    int K = 32;
+    while (K < max_nn) K <<= 1;
+    allow_max_smem((const void*)bowdb_pack_kernel);
+    bowdb_pack_kernel<<<A.n_jobs, PACK_THREADS, (size_t)K * 8, s>>>(A.jobs);
+    const bool fsm = max_smem_frame > 0;
+    const int warps = bowdb_warps(max_smem_frame, fsm);
+    const size_t smem = (fsm ? (((size_t)max_smem_frame + 127) & ~size_t(127)) : 0) + (size_t)warps * BDB_WARP_BYTES;
+    long long ctas = (max_items + warps - 1) / warps;
     if (ctas > n_sm * BDB_CTAS) ctas = n_sm * BDB_CTAS;
     if (ctas < 1) ctas = 1;
-    void (*kern)(BowDbArgs) = nullptr;
-    switch (csa) {
-        case 0: kern = fsm ? bowdb_match_kernel<0, true> : bowdb_match_kernel<0, false>; break;
-        case 1: kern = fsm ? bowdb_match_kernel<1, true> : bowdb_match_kernel<1, false>; break;
-        default: kern = fsm ? bowdb_match_kernel<2, true> : bowdb_match_kernel<2, false>; break;
+    // one job: passed as a parameter; its block decides the frame's memory
+    const int kind = A.n_jobs > 1 ? TABLE : (one.frame_in_smem ? ONE_SMEM : ONE_GLOBAL);
+    void (*kern)(BowDbArgs, int, BowDbJob) = nullptr;
+    switch (csa * 3 + kind) {
+        case 0: kern = bowdb_match_kernel<0, ONE_SMEM>; break;
+        case 1: kern = bowdb_match_kernel<0, ONE_GLOBAL>; break;
+        case 2: kern = bowdb_match_kernel<0, TABLE>; break;
+        case 3: kern = bowdb_match_kernel<1, ONE_SMEM>; break;
+        case 4: kern = bowdb_match_kernel<1, ONE_GLOBAL>; break;
+        case 5: kern = bowdb_match_kernel<1, TABLE>; break;
+        case 6: kern = bowdb_match_kernel<2, ONE_SMEM>; break;
+        case 7: kern = bowdb_match_kernel<2, ONE_GLOBAL>; break;
+        default: kern = bowdb_match_kernel<2, TABLE>; break;
     }
     allow_max_smem((const void*)kern);
-    kern<<<ctas, 32 * warps, smem, s>>>(A);
-    bowdb_finalize_kernel<<<F.n_kf, FIN_THREADS, 0, s>>>(F);
-    return 2;
+    kern<<<(int)ctas, 32 * warps, smem, s>>>(A, fsm ? max_smem_frame : 0, one);
+    bowdb_finalize_kernel<<<total_kf, FIN_THREADS, 0, s>>>(A);
+    return 3;
 }
 
 }  // namespace borb

@@ -399,21 +399,26 @@ __global__ void __launch_bounds__(128) distinctive_kernel(const uint8_t* __restr
 // DBoW2::L1Scoring::score (ScoringObject.cpp:23-71).  A warp per keyframe: lanes take 32 consecutive keyframe words,
 // binary-search them in the query, and the matching terms are added in ascending word order (double, the order of the
 // reference's merge loop) so that the score is bit-identical.
-__global__ void __launch_bounds__(256) kfdb_score_kernel(const BowDev* __restrict__ table, int n_slots, const uint32_t* __restrict__ qword_g,
-                                                         const double* __restrict__ qvalue_g, int nq, int in_smem, int32_t* __restrict__ common,
-                                                         float* __restrict__ score, uint32_t* __restrict__ first_word) {
+__global__ void __launch_bounds__(256) kfdb_score_kernel(const KfdbQueryJob* __restrict__ jobs, int in_smem) {
     extern __shared__ __align__(16) uint8_t kq_sm[];
+    const KfdbQueryJob& J = jobs[blockIdx.y];                         // grid.y = job
+    const int n_slots = J.n_slots, nq = J.nq;
+    if ((int)blockIdx.x * (int)(blockDim.x >> 5) >= n_slots) return;  // the grid is sized for the largest database
     const int lane = threadIdx.x & 31;
     // the query BowVector is probed ~10 x per keyframe word: keep it in shared memory (values first: 8-byte aligned)
-    const uint32_t* qword = qword_g;
-    const double* qvalue = qvalue_g;
+    const uint32_t* qword = J.qword;
+    const double* qvalue = J.qvalue;
     if (in_smem) {
         double* sv = reinterpret_cast<double*>(kq_sm);
         uint32_t* sw = reinterpret_cast<uint32_t*>(sv + nq);
-        for (int i = threadIdx.x; i < nq; i += blockDim.x) { sv[i] = qvalue_g[i]; sw[i] = qword_g[i]; }
+        for (int i = threadIdx.x; i < nq; i += blockDim.x) { sv[i] = J.qvalue[i]; sw[i] = J.qword[i]; }
         __syncthreads();
         qword = sw; qvalue = sv;
     }
+    const BowDev* __restrict__ table = J.table;
+    int32_t* __restrict__ common = J.common;
+    float* __restrict__ score = J.score;
+    uint32_t* __restrict__ first_word = J.first_word;
     const int warps_total = gridDim.x * (blockDim.x >> 5);
     const int steps = nq > 0 ? 32 - __clz(nq) : 0;                    // iterations that finish any lower_bound over nq entries
     constexpr int U = 8;                                              // keyframe words per lane in flight: the loads and the U searches overlap
@@ -768,20 +773,6 @@ __global__ void __launch_bounds__(256) bow_transform_batch_kernel(VocDev V, cons
 }
 
 namespace {
-// ascending bitonic sort of K (a power of two) 64-bit keys in shared memory by the whole CTA; ends with a barrier
-__device__ void bitonic_sort_u64(uint64_t* k, int K) {
-    const int half = K >> 1;
-    for (int kk = 2; kk <= K; kk <<= 1)
-        for (int j = kk >> 1; j > 0; j >>= 1) {
-            for (int p = threadIdx.x; p < half; p += blockDim.x) {
-                const int i = ((p & ~(j - 1)) << 1) | (p & (j - 1));          // lower element of the p-th compare pair
-                const uint64_t a = k[i], b = k[i + j];
-                if ((a > b) == ((i & kk) == 0)) { k[i] = b; k[i + j] = a; }
-            }
-            __syncthreads();
-        }
-}
-
 // Exclusive prefix count of the run heads among sorted keys [0, m): a head is the first key of a run of equal high words.
 // Each thread owns the contiguous chunk [c0, c1); returns the number of heads before c0, and the total in *total.
 __device__ int count_heads_before(const uint64_t* k, int m, int c0, int c1, int* warp_sums, int* total) {
@@ -885,6 +876,7 @@ __global__ void __launch_bounds__(1024) bow_build_kernel(const BowFrameJob* __re
         if (J.copy.word) J.copy.start[nn] = m;
         J.counts[0] = nb;
         J.counts[1] = nn;
+        J.counts[2] = m;
     }
 }
 
@@ -917,15 +909,15 @@ int launch_initialization(const ProjArgs& A, const borb_keypoint* keys1, int n1,
     init_resolve_kernel<<<1, 32, smem, s>>>(A, keys1, n1, match12, ev_idx, ev_bin, prev, n_matches);
     return 2;
 }
-int launch_kfdb_score(const BowDev* table, int n_slots, const uint32_t* qword, const double* qvalue, int nq, int32_t* common, float* score,
-                      uint32_t* first_word, int n_sm, cudaStream_t s) {
-    if (n_slots > 0) {
-        const size_t smem = (size_t)nq * 12 + 16;
+int launch_kfdb_score(const KfdbQueryJob* d_jobs, int n_jobs, int max_slots, int max_nq, int n_sm, cudaStream_t s) {
+    if (n_jobs > 0 && max_slots > 0) {
+        const size_t smem = (size_t)max_nq * 12 + 16;
         const int in_smem = smem <= 160 * 1024;
         if (in_smem) allow_max_smem((const void*)kfdb_score_kernel);
-        int ctas = (n_slots + 3) / 4;                                 // 4 keyframes (warps) per CTA: 2000 keyframes spread over all SMs
-        if (ctas > n_sm * 8) ctas = n_sm * 8;                         // persistent: the query is staged once per CTA
-        kfdb_score_kernel<<<ctas, 128, in_smem ? smem : 0, s>>>(table, n_slots, qword, qvalue, nq, in_smem, common, score, first_word);
+        int ctas = (max_slots + 3) / 4;                               // 4 keyframes (warps) per CTA: 2000 keyframes spread over all SMs
+        const int cap = std::max(1, n_sm * 8 / n_jobs);               // persistent: the query is staged once per CTA
+        if (ctas > cap) ctas = cap;
+        kfdb_score_kernel<<<dim3(ctas, n_jobs), 128, in_smem ? smem : 0, s>>>(d_jobs, in_smem);
     }
     return 1;
 }

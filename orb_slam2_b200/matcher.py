@@ -53,6 +53,16 @@ class _BowJobC(C.Structure):                       # borb_bow_job
     _fields_ = [("frame", C.c_void_p), ("kf", _KeyFrameViewC), ("kf_frame", C.c_void_p), ("match", C.c_void_p)]
 
 
+class _KfdbQueryJobC(C.Structure):                  # borb_kfdb_query_job
+    _fields_ = [("db", C.c_void_p), ("frame", C.c_void_p), ("common_words", C.c_void_p), ("score", C.c_void_p), ("first_word", C.c_void_p),
+                ("cap", C.c_int32), ("n_slots", C.c_void_p)]
+
+
+class _BowDbJobC(C.Structure):                      # borb_bow_db_job
+    _fields_ = [("db", C.c_void_p), ("frame", C.c_void_p), ("slots", C.c_void_p), ("n_kf", C.c_int32), ("n_matches", C.c_void_p),
+                ("pair_offset", C.c_void_p), ("pairs", C.c_void_p), ("pairs_cap", C.c_int32), ("n_pairs_total", C.c_void_p)]
+
+
 class _LocalPointsJobC(C.Structure):               # borb_local_points_job
     _fields_ = [("frame", _FrameViewC), ("pts", _WorldPointsViewC), ("has_obs", C.c_void_p), ("Tcw", C.c_float * 12), ("Ow", C.c_float * 3)] + \
                [(n, C.c_float) for n in ("fx", "fy", "cx", "cy", "mbf", "log_scale_factor", "th")] + \
@@ -628,6 +638,67 @@ class ORBmatcher:
         nm = np.zeros(max(n, 1), np.int32)
         check(self._lib.borb_search_by_bow_batch(self._h, jobs, n, self.mfNNratio, int(self.mbCheckOrientation), _p(nm)), "borb_search_by_bow_batch")
         return [(int(nm[j]), match[:nF]) for j, (nF, match) in enumerate(outs)]
+
+    @staticmethod
+    def _db_jobs(dbs, n):
+        """One database per job: a sequence, or one KeyFrameDatabase shared by every job."""
+        dbs = [dbs] * n if isinstance(dbs, KeyFrameDatabase) else list(dbs)
+        assert len(dbs) == n
+        return dbs
+
+    def KfdbQueryBatch(self, dbs, frames: Sequence[FrameView]):
+        """borb_kfdb_query_batch: the KeyFrameDatabase query (KeyFrameDatabase.query) of many resident frames whose BoW ComputeBoWBatch
+        computed, in one launch.  dbs[j] is job j's database (or one database for every job).  Returns [(common_words, score,
+        first_word)] per job, equal to dbs[j].query() with the frame's BowVector.
+
+        DetectRelocalizationCandidates of these queries is relocalization_candidates(cw, sc, fw, db._seq, covisibility,
+        db._reloc_score) applied to the jobs IN JOB ORDER, each with its database's persistent mRelocScore dict: a query reads the
+        mRelocScore that earlier queries left on keyframes below its own threshold, so the job order stands for the order of the
+        sequential calls it replaces."""
+        n = len(frames)
+        dbs = self._db_jobs(dbs, n)
+        jobs = (_KfdbQueryJobC * max(n, 1))()
+        outs = []
+        for j, (db, F) in enumerate(zip(dbs, frames)):
+            ns = db.size()[0] if db is not None else 0
+            cw = np.zeros(max(ns, 1), np.int32); sc = np.zeros(max(ns, 1), np.float32); fw = np.zeros(max(ns, 1), np.uint32)
+            nsl = np.zeros(1, np.int32)
+            J = jobs[j]
+            J.db = db._h.value if db is not None else None
+            J.frame = F.resident._h.value if (F is not None and F.resident is not None) else None
+            J.common_words, J.score, J.first_word, J.cap, J.n_slots = _p(cw), _p(sc), _p(fw), len(cw), _p(nsl)
+            outs.append((cw, sc, fw, nsl))
+        check(self._lib.borb_kfdb_query_batch(self._h, jobs, n), "borb_kfdb_query_batch")
+        return [(cw[:int(nsl[0])], sc[:int(nsl[0])], fw[:int(nsl[0])]) for cw, sc, fw, nsl in outs]
+
+    def SearchByBoWDbBatch(self, dbs, slots_list, frames: Sequence[FrameView], pairs_cap=None):
+        """borb_search_by_bow_db_batch: SearchByBoW(KeyFrame*, Frame&) (src/ORBmatcher.cc:159-288) of many resident frames with BoW
+        against candidate keyframes of their databases, in one launch sequence.  slots_list[j] = slot list of job j (None: every
+        slot); pairs_cap = None (room for every pair), one int for every job, or one per job.  Returns [(nmatches, pair_offset,
+        pairs)] per job as KeyFrameDatabase.SearchByBoWPairs returns them."""
+        n = len(frames)
+        dbs = self._db_jobs(dbs, n)
+        caps = pairs_cap if isinstance(pairs_cap, (list, tuple)) else [pairs_cap] * n
+        jobs = (_BowDbJobC * max(n, 1))()
+        outs = []
+        for j, (db, sl, F, cap) in enumerate(zip(dbs, slots_list, frames, caps)):
+            if sl is None:
+                n_kf, sla = (db.size()[0] if db is not None else 0), None
+            else:
+                sla = np.ascontiguousarray(sl, np.int32); n_kf = len(sla)
+            nF = F.resident.n if (F is not None and F.resident is not None) else 0
+            cap = int(cap) if cap is not None else max(n_kf * nF, 1)
+            nm = np.zeros(max(n_kf, 1), np.int32); off = np.zeros(max(n_kf, 1), np.int32)
+            pairs = np.zeros(max(cap, 1), np.uint32); tot = np.zeros(1, np.int32)
+            J = jobs[j]
+            J.db = db._h.value if db is not None else None
+            J.frame = F.resident._h.value if (F is not None and F.resident is not None) else None
+            J.slots, J.n_kf = _p(sla), n_kf
+            J.n_matches, J.pair_offset, J.pairs, J.pairs_cap, J.n_pairs_total = _p(nm), _p(off), _p(pairs), cap, _p(tot)
+            outs.append((sla, n_kf, nm, off, pairs, tot))
+        check(self._lib.borb_search_by_bow_db_batch(self._h, jobs, n, self.mfNNratio, int(self.mbCheckOrientation)),
+              "borb_search_by_bow_db_batch")
+        return [(nm[:n_kf], off[:n_kf], pairs[:int(tot[0])]) for _, n_kf, nm, off, pairs, tot in outs]
 
     def SearchForTriangulation(self, pKF1: KeyFrameView, pKF2: KeyFrameView, F12: np.ndarray, epipole: Tuple[float, float],
                                bOnlyStereo: bool = False) -> np.ndarray:

@@ -98,3 +98,17 @@ qb, qf = voc6.ComputeBoW(outs[0][1], 2)
 Fq = M.KeyFrameView(mvKeysUn=outs[0][0], mDescriptors=outs[0][1], mFeatVec=qf)
 nm, off, pairs = db2.SearchByBoWPairs(None, Fq)
 print("bowdb pairs", int(nm.sum()), "query", db2.query(qb)[0][:4], "dense", db2.SearchByBoW(np.arange(12, dtype=np.int32), Fq)[0][:4])
+
+# relocalisation batch: two databases, one call mixing a frame block in shared memory and one in global memory (6000 features)
+from orb_slam2_b200._lib import KP_DTYPE
+kb = np.zeros(6000, KP_DTYPE)
+kb["x"] = rng.uniform(20, 600, 6000); kb["y"] = rng.uniform(20, 440, 6000); kb["angle"] = rng.uniform(0, 360, 6000); kb["size"] = 31.0; kb["class_id"] = -1
+db3 = M.KeyFrameDatabase(mt)
+for j in range(3):
+    bow_, fv_ = voc6.ComputeBoW(outs[1][1], 2)
+    db3.add(M.KeyFrameView(mvKeysUn=outs[1][0], mDescriptors=outs[1][1], mFeatVec=fv_, has_mp=np.ones(len(outs[1][0]), np.uint8)), bow_)
+FR0 = M.FrameView(outs[0][0], outs[0][1], X.GetScaleFactors(), (0.0, 0.0, 640.0, 480.0)).make_resident(mt)
+FB = M.FrameView(kb, rng.integers(0, 256, (6000, 32), dtype=np.uint8), X.GetScaleFactors(), (0.0, 0.0, 640.0, 480.0)).make_resident(mt)
+mt.ComputeBoWBatch(voc6, [FR0, FB], 2, want_host=False)
+print("kfdb query batch", [q[0][:3] for q in mt.KfdbQueryBatch([db2, db3], [FR0, FB])])
+print("bowdb batch", [int(r[0].sum()) for r in mt.SearchByBoWDbBatch([db2, db3, db2], [None, None, [0, 5, 5]], [FR0, FB, FB])])
