@@ -344,6 +344,30 @@ BORB_API borb_status borb_fuse(borb_matcher* m, const borb_frame_view* kf, const
                                float cy, float bf, float log_scale_factor, float th, int scw_variant, int32_t* best_idx,
                                int32_t* n_found);
 
+/* The search part of one Fuse call, either overload: the arguments of borb_fuse. */
+typedef struct borb_fuse_job {
+    borb_frame_view kf;            /* kf.resident must be set; kf.occupied is ignored */
+    const float* inv_level_sigma2; /* mvInvLevelSigma2; required when scw_variant == 0 */
+    borb_worldpoints_view pts;     /* valid[i] as for borb_fuse */
+    float Tcw[12];
+    float Ow[3];
+    float fx, fy, cx, cy, bf, log_scale_factor, th;
+    int32_t scw_variant;           /* 0: Fuse(pKF, vpMapPoints, th)  1: Fuse(pKF, Scw, vpPoints, th, vpReplacePoint) */
+    int32_t* best_idx;             /* output, pts.n entries */
+} borb_fuse_job;
+/* borb_fuse for n_jobs jobs in two launches (projection, then a warp per point that walks its window's grid cells and keeps the
+ * first minimum: no candidate lists, so the scratch is the projections only) and one synchronisation.  Every job's best_idx and
+ * n_found[j] are bit-identical to what borb_fuse returns for the same inputs; both overloads may be mixed, and a keyframe may appear
+ * in several jobs.  Keyframes must be device-resident.  A host view, a frame on another device, more than BORB_MATCH_MAX_FEATURES
+ * points, log_scale_factor <= 0, an incomplete points view and scw_variant == 0 without inv_level_sigma2 are refused with
+ * BORB_ERR_INVALID_ARG before anything is launched, the error text starting with "job j:".  A job with no points or a keyframe with
+ * 0 features gives best_idx -1 and n_found 0.
+ * The Fuse calls of LocalMapping::SearchInNeighbors (src/LocalMapping.cc:483-511) for ONE keyframe are NOT independent:
+ * MapPoint::Replace recomputes the surviving point's descriptor and moves observations, and later targets see that.  Batch them
+ * ACROSS camera streams instead: one call per target index with one job per stream, then one call for the
+ * Fuse(mpCurrentKeyFrame, vpFuseCandidates) of every stream.  The same holds for LoopClosing::SearchAndFuse (scw_variant 1). */
+BORB_API borb_status borb_fuse_batch(borb_matcher* m, const borb_fuse_job* jobs, int n_jobs, int32_t* n_found);
+
 /* ORBmatcher::SearchBySim3(pKF1, pKF2, vpMatches12, s12, R12, t12, th) — src/ORBmatcher.cc:1102-1326
  * (LoopClosing::ComputeSim3, src/LoopClosing.cc:375-378).  pts1 / pts2 = GetMapPointMatches() of the two keyframes
  * (one slot per feature: pts->n == kf->n) with valid[i] = pMP && !vbAlreadyMatched[i] && !isBad() (:1130-1141,:1151-1155).
@@ -485,6 +509,35 @@ BORB_API borb_status borb_search_by_bow_batch(borb_matcher* m, const borb_bow_jo
 BORB_API borb_status borb_search_for_triangulation(borb_matcher* m, const borb_keyframe_view* kf1, const borb_keyframe_view* kf2,
                                                    const float* F12, float ex, float ey, int only_stereo, int check_orientation,
                                                    int32_t* pairs, int cap, int32_t* n_pairs);
+
+/* One SearchForTriangulation(pKF1, pKF2, F12, vMatchedPairs, bOnlyStereo) (src/ORBmatcher.cc:657-823). */
+typedef struct borb_triangulation_job {
+    borb_keyframe_view kf1;        /* has_mp = GetMapPoint(i) != NULL (:697-703) is always read from here */
+    const borb_frame* kf1_frame;   /* NULL, or the resident frame kf1 was made from, BoW computed: then n, keys_un, desc, u_right, fv,
+                                      scale_factors come from it (exactly borb_bow_job::kf_frame) */
+    borb_keyframe_view kf2;        /* has_mp and level_sigma2 (mvLevelSigma2) always read from here */
+    const borb_frame* kf2_frame;
+    float F12[9];                  /* row-major, LocalMapping::ComputeF12 */
+    float ex, ey;                  /* epipole of kf1 in kf2 (:663-670) */
+    int32_t only_stereo;
+    int32_t* pairs;                /* output: 2*cap ints (idx1, idx2), ascending idx1 */
+    int32_t cap;
+    int32_t* n_pairs;
+} borb_triangulation_job;
+/* borb_search_for_triangulation for n_jobs jobs in ONE launch (a CTA per job) and one synchronisation; every job's pairs and n_pairs
+ * are bit-identical to the single call's.  A keyframe may appear in several jobs (one keyframe against all its neighbours is the
+ * main use).  A NULL/foreign-device/BoW-less kf*_frame, more than BORB_MATCH_MAX_FEATURES features, an incomplete view and a kf2
+ * without level_sigma2 are refused with BORB_ERR_INVALID_ARG before anything is launched, the error text starting with "job j:".
+ * Pairs beyond a job's cap give BORB_ERR_CAPACITY after the run (every n_pairs stays valid; the error names the first such job).
+ * A job with 0 features or an empty FeatureVector on either side gives 0 pairs and no work.
+ * LocalMapping::CreateNewMapPoints (src/LocalMapping.cc:207-268) from one call: submit every neighbour that passes the baseline
+ * test, with kf1's has_mp as it is on entry and check_orientation = 0 (the reference's ORBmatcher matcher(0.6,false)), then
+ * triangulate the neighbours IN ORDER, dropping from neighbour i's pairs every idx1 that an earlier neighbour gave a MapPoint.
+ * Without the orientation check each row's result depends only on its own idx1 and on has_mp, so this replays the sequential calls
+ * exactly (the CheckNewKeyFrames() early return is the caller stopping the replay).  With check_orientation = 1 the rotation
+ * histogram couples the rows and the replay is NOT exact. */
+BORB_API borb_status borb_search_for_triangulation_batch(borb_matcher* m, const borb_triangulation_job* jobs, int n_jobs,
+                                                         int check_orientation);
 
 /* ---- device-resident keyframe database -------------------------------------------------------------------------
  * KeyFrameDatabase (include/KeyFrameDatabase.h, src/KeyFrameDatabase.cc) re-designed for the GPU: instead of an inverted

@@ -11,6 +11,8 @@
 //              borb_search_by_bow_batch      reference-keyframe search of the N streams   (TrackReferenceKeyFrame x N)
 //              (pose optimisation on the host)
 //              borb_search_local_points_batch    isInFrustum + local-map search of the N streams   (SearchLocalPoints x N)
+//   LocalMapping, per new keyframe:
+//              borb_fuse_batch               the search part of Fuse(pKF, vpMapPoints) of the N streams (SearchInNeighbors x N)
 //
 // The program self-checks: the "local map" of every stream is made of that stream's own keypoints (projected where they were
 // seen, with their own descriptors, predicted at their own octave), so SearchByProjection must give (almost) every point back to
@@ -19,6 +21,7 @@
 // their own features, and as world points (normal = viewing ray, distances that predict the keypoint's octave) as well.  For the
 // reference-keyframe search every stream's frame is its own reference keyframe, every feature with a MapPoint: a feature can only
 // match itself (a duplicate descriptor fails the ratio test), so every match[j] is j or -1.  The vocabulary is a small seeded tree.
+// Each frame is also a keyframe into which the same back-projected points are fused: they must land on their own features.
 // Build:  g++ -std=c++14 -Iinclude integration/example_multistream_host.cc orb_slam2_b200/libborb.so -Wl,-rpath,$PWD/orb_slam2_b200
 // Exit code 0 = ran and checked, 3 = the library reported an error (e.g. no CUDA device: there is no CPU fallback).
 #include <cmath>
@@ -101,8 +104,10 @@ int main(int argc, char** argv) {
     std::vector<borb_frame*> frames(N, nullptr);
     const borb_camera cam = {517.3f, 516.5f, 318.6f, 255.3f, 0.f, 0.f, 0.f, 0.f, 0.f, 40.f};      // k1 = 0: mvKeysUn = mvKeys
     float bounds[4];
-    long total_points = 0, total_matches = 0, last_self = 0, local_self = 0, ref_self = 0, ref_other = 0;
+    long total_points = 0, total_matches = 0, last_self = 0, local_self = 0, ref_self = 0, ref_other = 0, fuse_self = 0;
     const float log_scale = std::log(cfg.scale_factor);     // Frame::mfLogScaleFactor
+    std::vector<float> inv_sigma2(cfg.n_levels);            // KeyFrame::mvInvLevelSigma2
+    for (int l = 0; l < cfg.n_levels; l++) inv_sigma2[l] = 1.0f / (scale[l] * scale[l]);
 
     for (int t = 0; t < ticks; t++) {
         for (int i = 0; i < N; i++) { make_image(imgs[i], W, H, i + 100 * t); img_ptr[i] = imgs[i].data(); image_idx[i] = i; }
@@ -194,16 +199,34 @@ int main(int argc, char** argv) {
         }
         CHECK(borb_search_by_bow_batch(mat, bjobs.data(), N, 0.7f, 1, n_ref.data()));
         CHECK(borb_search_local_points_batch(mat, pjobs.data(), N, 0.5f, 0.8f, n_local.data()));
+        // ---- LocalMapping::SearchInNeighbors: the frame as a keyframe, its back-projected keypoints as the MapPoints to fuse.  The
+        //      Fuse calls of one keyframe's targets depend on each other (MapPoint::Replace); those of different streams do not
+        std::vector<borb_fuse_job> fjobs(N);
+        std::vector<std::vector<int32_t> > fbest(N);
+        std::vector<int32_t> n_fused(N);
+        for (int i = 0; i < N; i++) {
+            fbest[i].assign(n_out[i] > 0 ? n_out[i] : 1, -1);
+            borb_fuse_job& Fj = fjobs[i];
+            Fj = borb_fuse_job();
+            Fj.kf.resident = frames[i];
+            Fj.inv_level_sigma2 = inv_sigma2.data();
+            Fj.pts = pjobs[i].pts;
+            for (int c = 0; c < 12; c++) Fj.Tcw[c] = pjobs[i].Tcw[c];
+            Fj.fx = cam.fx; Fj.fy = cam.fy; Fj.cx = cam.cx; Fj.cy = cam.cy; Fj.bf = cam.bf; Fj.log_scale_factor = log_scale; Fj.th = 3.0f;
+            Fj.best_idx = fbest[i].data();
+        }
+        CHECK(borb_fuse_batch(mat, fjobs.data(), N, n_fused.data()));
         for (int i = 0; i < N; i++) {
             total_points += n_out[i]; total_matches += n_matches[i];
-            int self = 0, sl = 0, sp = 0, sr = 0;
+            int self = 0, sl = 0, sp = 0, sr = 0, sf = 0;
             for (int j = 0; j < n_out[i]; j++) {
-                self += match[i][j] == j; sl += state[i][j] == j; sp += lmatch[i][j] == j; sr += bmatch[i][j] == j;
+                self += match[i][j] == j; sl += state[i][j] == j; sp += lmatch[i][j] == j; sr += bmatch[i][j] == j; sf += fbest[i][j] == j;
                 ref_other += bmatch[i][j] != j && bmatch[i][j] != -1;
             }
-            last_self += sl; local_self += sp; ref_self += sr;
+            last_self += sl; local_self += sp; ref_self += sr; fuse_self += sf;
             std::printf("tick %d stream %d: %d keypoints, %d matches (%d to themselves); motion model %d (%d); reference keyframe %d (%d); "
-                        "local map %d (%d)\n", t, i, n_out[i], n_matches[i], self, n_last[i], sl, n_ref[i], sr, n_local[i], sp);
+                        "local map %d (%d); fuse %d (%d)\n", t, i, n_out[i], n_matches[i], self, n_last[i], sl, n_ref[i], sr, n_local[i], sp,
+                        n_fused[i], sf);
             CHECK(borb_frame_destroy(frames[i]));
             frames[i] = nullptr;
         }
@@ -215,8 +238,9 @@ int main(int argc, char** argv) {
     std::printf("motion-model search: %ld of %ld features matched to their own last-frame point\n", last_self, total_points);
     std::printf("reference-keyframe search: %ld of %ld features matched to themselves, %ld elsewhere\n", ref_self, total_points, ref_other);
     std::printf("local-map search: %ld of %ld points matched to their own feature\n", local_self, total_points);
+    std::printf("fuse: %ld of %ld points fused onto their own feature\n", fuse_self, total_points);
     if (total_points < 100L * N * ticks || total_matches < total_points * 8 / 10 || last_self < total_points * 8 / 10 ||
-        ref_self < total_points * 8 / 10 || ref_other != 0 || local_self < total_points * 8 / 10) {
+        ref_self < total_points * 8 / 10 || ref_other != 0 || local_self < total_points * 8 / 10 || fuse_self < total_points * 8 / 10) {
         std::printf("self-check failed\n");
         return 1;
     }

@@ -111,6 +111,8 @@ _SIGNATURES = {
     "borb_search_by_bow_batch": (C.c_int, [vp, vp, C.c_int, C.c_float, C.c_int, vp]),
     "borb_frames_compute_bow": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp]),
     "borb_search_for_triangulation": (C.c_int, [vp, vp, vp, vp, C.c_float, C.c_float, C.c_int, C.c_int, vp, C.c_int, i32p]),
+    "borb_search_for_triangulation_batch": (C.c_int, [vp, vp, C.c_int, C.c_int]),
+    "borb_fuse_batch": (C.c_int, [vp, vp, C.c_int, vp]),
     "borb_voc_create": (C.c_int, [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(vp)]),
     "borb_voc_load_text": (C.c_int, [C.c_char_p, C.c_int, C.POINTER(vp)]),
     "borb_voc_destroy": (C.c_int, [vp]),

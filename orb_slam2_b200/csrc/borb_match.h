@@ -72,12 +72,17 @@ struct ProjArgs {                 // device pointers
     int check_ori;
     const float* q_angle;         // mode 1: mvKeysUn[i].angle of the query
     int th_dist;                  // mode 1: accept bestDist <= th_dist (TH_HIGH / ORBdist / TH_LOW)
-    int chi2;                     // 1: Fuse(pKF, vpMapPoints, th) reprojection gates per candidate (:907-931)
-    const float* inv_sigma2;      // chi2: mvInvLevelSigma2
     // where the resolve / argmin kernels write the results
     int32_t* out_match;           // n_mp entries (mode 1 resolve: the per-feature state, n entries), then the match count
     int32_t* ev_idx;              // mode 1: match events of the rotation histogram, n_mp entries
     uint8_t* ev_bin;
+};
+
+struct FuseJob {                  // one job of fuse_batch_kernel (k_proj.cu)
+    ProjArgs A;                   // the keyframe (u_right null for the Scw overload) and the windows project_points wrote (mode 1
+                                  // fields); th_dist = TH_LOW; out_match = best_idx, n_mp entries
+    const float* inv_sigma2;      // mvInvLevelSigma2: the reprojection gates of Fuse(pKF, vpMapPoints, th); null for the Scw overload
+    int* n_found;
 };
 
 struct LastArgs {                 // inputs of project_points_kernel
@@ -238,7 +243,17 @@ struct FrameJob {                 // one frame of borb_frames_from_extractor (k_
     float min_x, min_y, inv_w, inv_h;
 };
 
-struct TriArgs { float F[9]; float ex, ey; int only_stereo, check_ori; };
+struct TriJob {                   // one SearchForTriangulation of triangulation_kernel (k_match.cu), a CTA per job
+    KfDev q, t;                   // kf1, kf2
+    float F[9];
+    float ex, ey;
+    int only_stereo;
+    int32_t* vmatch;              // scratch, q.n entries
+    uint8_t* bins;                // scratch, q.n entries
+    int32_t* pairs;               // 2 * cap ints
+    int cap;
+    int32_t* n_pairs;
+};
 
 struct BowTables {                // a BowVector (word order) and a FeatureVector (CSR); word == null: not written
     uint32_t* word;
@@ -297,8 +312,11 @@ int launch_frame_build(const FrameJob* d_jobs, int n_jobs, int max_n, const borb
 // total_kf = sum of their n_kf
 int launch_bowdb(const BowDbArgs& A, const BowDbJob& one, int max_smem_frame, long long max_items, int total_kf, int max_nn, int csa, int n_sm, cudaStream_t s);
 bool bowdb_frame_fits_smem(int frame_bytes);
-int launch_triangulation(const KfDev& q, const KfDev& t, const TriArgs& T, int32_t* vmatch, uint8_t* bins, int32_t* pairs, int cap,
-                         int32_t* n_pairs, cudaStream_t s);
+// n_jobs searches (a job table in device memory) in one launch
+int launch_triangulation(const TriJob* d_jobs, int n_jobs, int check_ori, cudaStream_t s);
+// project_points over a LastArgs table (variant 2), then fuse_batch_kernel over a FuseJob table: 2 launches; max_nq = most points of a job
+int launch_fuse_batch(const LastArgs* d_last, const FuseJob* d_jobs, int n_jobs, int max_nq, cudaStream_t s);
+void launch_fuse_search(const FuseJob* d_jobs, int n_jobs, int max_nq, cudaStream_t s);
 int launch_bow_transform(const VocDev& V, const uint8_t* desc, int n, int levelsup, int32_t* word, double* weight, int32_t* node,
                          cudaStream_t s);
 // descent + bookkeeping for n_frames frames (a job table in device memory): 2 launches

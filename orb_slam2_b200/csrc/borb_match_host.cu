@@ -155,15 +155,13 @@ void bind_resident(const borb_frame* rf, ProjArgs& A) {
     A.keys = rf->keys; A.desc = rf->desc; A.u_right = rf->u_right; A.scale_factors = rf->sf;
     A.cell_start = rf->cell_start; A.cell_idx = rf->cell_idx;
 }
-// fills the frame fields of A after commit(); builds the grid for a host view, waits for the resident frame otherwise
-borb_status bind_frame(borb_matcher* m, const FrameInfo& I, const FrameStage& fs, ProjArgs& A) {
+// the frame fields of A: the resident frame's, or (a host view, never zero-copy) those staged at fs in the arena b
+void bind_frame_fields(const FrameInfo& I, const FrameStage& fs, uint8_t* b, ProjArgs& A) {
     if (I.rf) {
         bind_resident(I.rf, A);
         if (!fs.ur_p) A.u_right = nullptr;
-        BORB_CUDA(cudaStreamWaitEvent(m->stream, I.rf->ready, 0));
-        return BORB_OK;
+        return;
     }
-    uint8_t* b = m->arena;             // (a host view is never zero-copy: in_base == arena)
     A.n = I.n;
     A.minX = I.min_x; A.minY = I.min_y;
     A.invW = (float)GRID_COLS / (float)(I.max_x - I.min_x);
@@ -172,9 +170,21 @@ borb_status bind_frame(borb_matcher* m, const FrameInfo& I, const FrameStage& fs
     A.u_right = fs.ur_p ? (const float*)(b + fs.ur) : nullptr;
     A.scale_factors = (const float*)(b + fs.sf);
     A.cell_start = (const int*)(b + fs.cs); A.cell_idx = (const int*)(b + fs.ci);
-    if (I.n > 0) m->launches += launch_grid_sort(A.keys, A.n, A.minX, A.minY, A.invW, A.invH, (int*)(b + fs.cs), (int*)(b + fs.ci), m->stream);
-    else BORB_CUDA(cudaMemsetAsync(b + fs.cs, 0, (size_t)(GRID_CELLS + 1) * 4, m->stream));
+}
+// after commit(): builds the grid of a host view bound by bind_frame_fields, waits for the resident frame otherwise
+borb_status prepare_frame(borb_matcher* m, const FrameInfo& I, const ProjArgs& A) {
+    if (I.rf) {
+        BORB_CUDA(cudaStreamWaitEvent(m->stream, I.rf->ready, 0));
+        return BORB_OK;
+    }
+    if (I.n > 0) m->launches += launch_grid_sort(A.keys, A.n, A.minX, A.minY, A.invW, A.invH, (int*)A.cell_start, (int*)A.cell_idx, m->stream);
+    else BORB_CUDA(cudaMemsetAsync((void*)A.cell_start, 0, (size_t)(GRID_CELLS + 1) * 4, m->stream));
     return BORB_OK;
+}
+// fills the frame fields of A after commit(); builds the grid for a host view, waits for the resident frame otherwise
+borb_status bind_frame(borb_matcher* m, const FrameInfo& I, const FrameStage& fs, ProjArgs& A) {
+    bind_frame_fields(I, fs, m->arena, A);
+    return prepare_frame(m, I, A);
 }
 borb_status check_frame(const borb_frame_view* F, const FrameInfo& I, const borb_matcher* m) {
     if (I.n < 0 || I.n > MATCH_MAX_FEATURES) { set_error("frame has %d features (limit %d)", I.n, MATCH_MAX_FEATURES); return BORB_ERR_INVALID_ARG; }
@@ -191,6 +201,8 @@ borb_status job_error(int j, borb_status s) {      // prefixes the error text a 
     set_error("job %d: %s", j, e.c_str());
     return s;
 }
+// error text of a check shared by the single calls and the batches: the batches name the job
+borb_status job_fail(bool batch, int j, borb_status s) { return batch ? job_error(j, s) : s; }
 // the candidate search reads its queries from what project_points_kernel wrote
 void wire_projection(const LastArgs& L, ProjArgs& A) {
     A.n_mp = L.n_last;
@@ -708,12 +720,17 @@ QueryOff stage_query(Stager& st, const borb_frame_view* F, const FrameInfo& I, c
     o.is2 = Q.chi2 ? st.add(Q.inv_sigma2, (size_t)I.n_levels * 4) : 0;
     return o;
 }
-// device-only scratch, laid out after every input
-void reserve_query(Stager& st, const FrameInfo& I, const PointQuery& Q, QueryOff& o) {
+// device-only scratch of project_points (and the grid of a host view), laid out after every input
+void reserve_projection(Stager& st, const FrameInfo& I, const PointQuery& Q, QueryOff& o) {
     const size_t nq = (size_t)Q.n;
     reserve_grid(st, I, o.fs);
     o.px = st.reserve(nq * 4); o.py = st.reserve(nq * 4); o.pxr = st.reserve(nq * 4); o.rad = st.reserve(nq * 4);
     o.ang = st.reserve(nq * 4); o.minl = st.reserve(nq * 4); o.maxl = st.reserve(nq * 4); o.val = st.reserve(nq);
+}
+// the same plus the candidate lists and the match events of the resolve / argmin kernels
+void reserve_query(Stager& st, const FrameInfo& I, const PointQuery& Q, QueryOff& o) {
+    const size_t nq = (size_t)Q.n;
+    reserve_projection(st, I, Q, o);
     o.cand = st.reserve(nq * I.n * 4); o.cc = st.reserve(nq * 4);
     o.evi = st.reserve(nq * 4); o.evb = st.reserve(nq);
 }
@@ -745,7 +762,6 @@ void bind_query(const QueryOff& o, const PointQuery& Q, const FrameInfo& I, cons
     A.th = Q.th; A.nnratio = 0.f;
     A.cand = (uint32_t*)(b + o.cand); A.cand_cnt = (int*)(b + o.cc);
     A.mode = 1; A.check_ori = Q.check_ori; A.th_dist = Q.th_dist;
-    A.chi2 = Q.chi2; A.inv_sigma2 = Q.chi2 ? (const float*)(in + o.is2) : nullptr;
     A.out_match = out; A.ev_idx = (int32_t*)(b + o.evi); A.ev_bin = b + o.evb;
 }
 // SearchByProjection(CurrentFrame, LastFrame) of one camera stream
@@ -838,23 +854,107 @@ borb_status borb_search_by_projection_sim3(borb_matcher* m, const borb_frame_vie
     return run_point_projection(m, kf, Q, state_kf, n_matches);
 }
 
+// ---- the search part of Fuse: borb_fuse is the one-job case of borb_fuse_batch (project_points + fuse_batch_kernel, one
+// synchronisation).  The scratch of a job is its projections: fuse_batch_kernel takes the first minimum without candidate lists.
+namespace {
+borb_status fuse_jobs(borb_matcher* m, const borb_fuse_job* jobs, int n_jobs, bool batch, int32_t* n_found) {
+    struct Job { borb_frame_view kf; PointQuery Q; FrameInfo I; bool live; QueryOff o; size_t res; };
+    std::vector<Job> J(n_jobs);
+    int max_nq = 0;
+    for (int j = 0; j < n_jobs; j++) {
+        const borb_fuse_job& B = jobs[j];
+        n_found[j] = 0;
+        if (!B.scw_variant && !B.inv_level_sigma2) { set_error("Fuse(pKF, vpMapPoints, th) needs mvInvLevelSigma2"); return job_fail(batch, j, BORB_ERR_INVALID_ARG); }
+        PointQuery& Q = J[j].Q;
+        Q.variant = 2; Q.n = B.pts.n; Q.world_pos = B.pts.world_pos; Q.desc = B.pts.desc; Q.valid = B.pts.valid;
+        Q.max_distance = B.pts.max_distance; Q.min_distance = B.pts.min_distance; Q.normal = B.pts.normal;
+        Q.Tcw = B.Tcw; Q.Ow = B.Ow; Q.fx = B.fx; Q.fy = B.fy; Q.cx = B.cx; Q.cy = B.cy; Q.bf = B.bf; Q.th = B.th; Q.log_scale = B.log_scale_factor;
+        Q.th_dist = TH_LOW;                                                // (:944, :1075)
+        Q.use_normal = 1; Q.argmin = 1;
+        Q.invz_double = B.scw_variant ? 1 : 0;                             // 1.0/z (:1014) vs 1/z (:861)
+        Q.chi2 = B.scw_variant ? 0 : 1; Q.inv_sigma2 = B.inv_level_sigma2;
+        // occupancy plays no role in either Fuse (the MapPoint already in the slot is handled by the caller, :947-960)
+        J[j].kf = B.kf;
+        J[j].kf.occupied = nullptr;
+        const FrameInfo I = J[j].I = frame_info(&J[j].kf);
+        const borb_status s = check_query(&J[j].kf, I, Q, m);
+        if (s != BORB_OK) return job_fail(batch, j, s);
+        std::fill_n(B.best_idx, Q.n, -1);
+        J[j].live = I.n > 0 && Q.n > 0;
+        if (J[j].live) max_nq = std::max(max_nq, Q.n);
+    }
+    if (max_nq == 0) return BORB_OK;
+    BORB_CUDA(cudaSetDevice(m->device));
+    Stager st(m);
+    for (int j = 0; j < n_jobs; j++)
+        if (J[j].live) J[j].o = stage_query(st, &J[j].kf, J[j].I, J[j].Q);
+    const size_t o_last = st.add(nullptr, (size_t)n_jobs * sizeof(LastArgs)), o_jobs = st.add(nullptr, (size_t)n_jobs * sizeof(FuseJob));
+    const size_t input_end = st.off;
+    const size_t cnt_bytes = ((size_t)n_jobs * 4 + 15) & ~size_t(15);
+    size_t res_bytes = cnt_bytes;                // n_found of every job, then every job's best_idx: one D2H
+    for (int j = 0; j < n_jobs; j++) {
+        if (!J[j].live) continue;
+        reserve_projection(st, J[j].I, J[j].Q, J[j].o);
+        J[j].res = res_bytes; res_bytes += ((size_t)J[j].Q.n * 4 + 15) & ~size_t(15);
+    }
+    const size_t o_res = st.reserve(res_bytes);
+    const size_t total = st.off;
+    st.off = input_end;
+    borb_status s;
+    if ((s = ensure_host(m, input_end)) != BORB_OK) return s;
+    if ((s = ensure_arena(m, total)) != BORB_OK) return s;
+    if ((s = ensure_out(m, res_bytes)) != BORB_OK) return s;
+    BORB_CUDA(cudaStreamSynchronize(m->stream));
+    uint8_t* b = m->arena;
+    LastArgs* hl = reinterpret_cast<LastArgs*>(m->h_stage + o_last);
+    FuseJob* hj = reinterpret_cast<FuseJob*>(m->h_stage + o_jobs);
+    for (int j = 0; j < n_jobs; j++) {
+        LastArgs L{};
+        FuseJob F{};
+        if (J[j].live) {
+            bind_frame_fields(J[j].I, J[j].o.fs, b, F.A);
+            bind_query(J[j].o, J[j].Q, J[j].I, b, b, (int32_t*)(b + o_res + J[j].res), L, F.A);
+            F.inv_sigma2 = J[j].Q.chi2 ? (const float*)(b + J[j].o.is2) : nullptr;
+            F.n_found = (int*)(b + o_res) + j;
+        }                                            // a job without work keeps n_last = n_mp = 0: both kernels skip it
+        hl[j] = L;
+        hj[j] = F;
+    }
+    if ((s = commit(st, total)) != BORB_OK) return s;
+    BORB_CUDA(cudaMemsetAsync(b + o_res, 0, cnt_bytes, m->stream));
+    for (int j = 0; j < n_jobs; j++)
+        if (J[j].live && (s = prepare_frame(m, J[j].I, hj[j].A)) != BORB_OK) return s;
+    m->launches += launch_fuse_batch((const LastArgs*)(b + o_last), (const FuseJob*)(b + o_jobs), n_jobs, max_nq, m->stream);
+    BORB_CUDA(cudaGetLastError());
+    BORB_CUDA(cudaMemcpyAsync(m->h_out, b + o_res, res_bytes, cudaMemcpyDeviceToHost, m->stream));
+    BORB_CUDA(cudaStreamSynchronize(m->stream));
+    for (int j = 0; j < n_jobs; j++) {
+        std::memcpy(&n_found[j], m->h_out + (size_t)j * 4, 4);
+        if (J[j].live) std::memcpy(jobs[j].best_idx, m->h_out + J[j].res, (size_t)J[j].Q.n * 4);
+    }
+    return BORB_OK;
+}
+}  // namespace
+
 borb_status borb_fuse(borb_matcher* m, const borb_frame_view* kf, const float* inv_level_sigma2, const borb_worldpoints_view* pts,
                       const float* Tcw, const float* Ow, float fx, float fy, float cx, float cy, float bf, float log_scale_factor,
                       float th, int scw_variant, int32_t* best_idx, int32_t* n_found) {
     if (!m || !kf || !pts || !Tcw || !Ow || !best_idx || !n_found) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
-    if (!scw_variant && !inv_level_sigma2) { set_error("Fuse(pKF, vpMapPoints, th) needs mvInvLevelSigma2"); return BORB_ERR_INVALID_ARG; }
-    PointQuery Q{};
-    Q.variant = 2; Q.n = pts->n; Q.world_pos = pts->world_pos; Q.desc = pts->desc; Q.valid = pts->valid;
-    Q.max_distance = pts->max_distance; Q.min_distance = pts->min_distance; Q.normal = pts->normal;
-    Q.Tcw = Tcw; Q.Ow = Ow; Q.fx = fx; Q.fy = fy; Q.cx = cx; Q.cy = cy; Q.bf = bf; Q.th = th; Q.log_scale = log_scale_factor;
-    Q.th_dist = 50;                                                        // TH_LOW (:944, :1075)
-    Q.use_normal = 1; Q.argmin = 1;
-    Q.invz_double = scw_variant ? 1 : 0;                                   // 1.0/z (:1014) vs 1/z (:861)
-    Q.chi2 = scw_variant ? 0 : 1; Q.inv_sigma2 = inv_level_sigma2;
-    // occupancy plays no role in either Fuse (the MapPoint already in the slot is handled by the caller, :947-960)
-    borb_frame_view F = *kf;
-    F.occupied = nullptr;
-    return run_point_projection(m, &F, Q, best_idx, n_found);
+    borb_fuse_job B{};
+    B.kf = *kf; B.inv_level_sigma2 = inv_level_sigma2; B.pts = *pts;
+    std::memcpy(B.Tcw, Tcw, sizeof(B.Tcw)); std::memcpy(B.Ow, Ow, sizeof(B.Ow));
+    B.fx = fx; B.fy = fy; B.cx = cx; B.cy = cy; B.bf = bf; B.log_scale_factor = log_scale_factor; B.th = th;
+    B.scw_variant = scw_variant; B.best_idx = best_idx;
+    return fuse_jobs(m, &B, 1, false, n_found);
+}
+
+borb_status borb_fuse_batch(borb_matcher* m, const borb_fuse_job* jobs, int n_jobs, int32_t* n_found) {
+    if (!m || n_jobs < 0 || (n_jobs > 0 && (!jobs || !n_found))) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+    for (int j = 0; j < n_jobs; j++) {
+        if (!jobs[j].kf.resident) { set_error("job %d: borb_fuse_batch needs device-resident keyframes (borb_frame_view::resident)", j); return BORB_ERR_INVALID_ARG; }
+        if (!jobs[j].best_idx) { set_error("job %d: null output", j); return BORB_ERR_INVALID_ARG; }
+    }
+    return fuse_jobs(m, jobs, n_jobs, true, n_found);
 }
 
 borb_status borb_search_by_sim3(borb_matcher* m, const borb_frame_view* kf1, const borb_frame_view* kf2, const borb_worldpoints_view* pts1,
@@ -1652,9 +1752,6 @@ struct DbLocks {
     }
 };
 
-// error text of a check shared by the single calls and the batches: the batches name the job
-borb_status job_fail(bool batch, int j, borb_status s) { return batch ? job_error(j, s) : s; }
-
 // One query of the database score: the BowVector comes from the host (word / value) or from a resident frame.
 struct QueryJob {
     borb_kfdb* db;
@@ -1964,36 +2061,124 @@ borb_status borb_search_by_bow_db_batch(borb_matcher* m, const borb_bow_db_job* 
     return bowdb_jobs(m, S.data(), n_jobs, nnratio, check_orientation, true);
 }
 
+// ---- SearchForTriangulation: borb_search_for_triangulation is the one-job case of borb_search_for_triangulation_batch (one launch
+// of triangulation_kernel, a CTA per job, and one synchronisation).  Each side is a host view or a resident frame with its BoW.
+namespace {
+borb_status triangulation_jobs(borb_matcher* m, const borb_triangulation_job* jobs, int n_jobs, int check_ori, bool batch) {
+    struct Side { int n, nn; KfOffsets o; size_t o_hm, o_sig; };
+    struct Job { Side s1, s2; bool live; int cap; size_t vm, bins, res; };
+    std::vector<Job> J(n_jobs);
+    for (int j = 0; j < n_jobs; j++) {
+        const borb_triangulation_job& B = jobs[j];
+        if (!B.pairs || !B.n_pairs || B.cap < 0) { set_error("job %d: null output or negative capacity", j); return BORB_ERR_INVALID_ARG; }
+        *B.n_pairs = 0;
+        borb_status s = BORB_OK;
+        if (B.kf1_frame) s = check_resident_bow(B.kf1_frame, m, j, "kf1_frame");
+        else if ((s = check_kf(&B.kf1, batch ? "kf1" : "borb_search_for_triangulation(kf1)")) != BORB_OK) return job_fail(batch, j, s);
+        if (s != BORB_OK) return s;
+        if (B.kf2_frame) s = check_resident_bow(B.kf2_frame, m, j, "kf2_frame");
+        else if ((s = check_kf(&B.kf2, batch ? "kf2" : "borb_search_for_triangulation(kf2)")) != BORB_OK) return job_fail(batch, j, s);
+        if (s != BORB_OK) return s;
+        if (!B.kf2.level_sigma2 || (!B.kf2_frame && !B.kf2.scale_factors)) {
+            set_error("kf2 needs scale_factors and level_sigma2");
+            return job_fail(batch, j, BORB_ERR_INVALID_ARG);
+        }
+        Job& Q = J[j];
+        Q.s1.n = B.kf1_frame ? B.kf1_frame->n : B.kf1.n; Q.s1.nn = B.kf1_frame ? B.kf1_frame->n_nodes : B.kf1.fv.n_nodes;
+        Q.s2.n = B.kf2_frame ? B.kf2_frame->n : B.kf2.n; Q.s2.nn = B.kf2_frame ? B.kf2_frame->n_nodes : B.kf2.fv.n_nodes;
+        Q.live = Q.s1.n > 0 && Q.s1.nn > 0 && Q.s2.n > 0 && Q.s2.nn > 0;
+        Q.cap = std::min(B.cap, Q.s1.n);             // a job has at most one pair per kf1 feature
+    }
+    std::vector<int> live;
+    for (int j = 0; j < n_jobs; j++) if (J[j].live) live.push_back(j);
+    const int nl = (int)live.size();
+    if (nl == 0) return BORB_OK;
+    BORB_CUDA(cudaSetDevice(m->device));
+    Stager st(m);
+    for (int j : live) {
+        const borb_triangulation_job& B = jobs[j];
+        Job& Q = J[j];
+        if (!B.kf1_frame) Q.s1.o = stage_kf(st, &B.kf1);
+        else if (B.kf1.has_mp) Q.s1.o_hm = st.add(B.kf1.has_mp, (size_t)Q.s1.n);
+        if (!B.kf2_frame) Q.s2.o = stage_kf(st, &B.kf2);
+        else {
+            if (B.kf2.has_mp) Q.s2.o_hm = st.add(B.kf2.has_mp, (size_t)Q.s2.n);
+            Q.s2.o_sig = st.add(B.kf2.level_sigma2, (size_t)B.kf2_frame->n_levels * 4);
+        }
+    }
+    const size_t o_jobs = st.add(nullptr, (size_t)nl * sizeof(TriJob));          // filled in place
+    const size_t input_end = st.off;
+    const size_t cnt_bytes = ((size_t)nl * 4 + 15) & ~size_t(15);
+    size_t res_bytes = cnt_bytes;                  // n_pairs of every live job, then every job's pairs: one D2H
+    for (int j : live) {
+        Job& Q = J[j];
+        Q.vm = st.reserve((size_t)Q.s1.n * 4); Q.bins = st.reserve((size_t)Q.s1.n);
+        Q.res = res_bytes; res_bytes += ((size_t)Q.cap * 8 + 15) & ~size_t(15);
+    }
+    const size_t o_res = st.reserve(res_bytes);
+    const size_t total = st.off;
+    st.off = input_end;
+    borb_status s;
+    if ((s = ensure_host(m, input_end)) != BORB_OK) return s;
+    if ((s = ensure_arena(m, total)) != BORB_OK) return s;
+    if ((s = ensure_out(m, res_bytes)) != BORB_OK) return s;
+    BORB_CUDA(cudaStreamSynchronize(m->stream));
+    uint8_t* b = m->arena;
+    TriJob* hj = reinterpret_cast<TriJob*>(m->h_stage + o_jobs);
+    for (int k = 0; k < nl; k++) {
+        const borb_triangulation_job& B = jobs[live[k]];
+        const Job& Q = J[live[k]];
+        TriJob T{};
+        T.q = B.kf1_frame ? resident_kf_dev(B.kf1_frame, B.kf1.has_mp ? b + Q.s1.o_hm : nullptr) : kf_dev(m, &B.kf1, Q.s1.o);
+        if (B.kf2_frame) {
+            T.t = resident_kf_dev(B.kf2_frame, B.kf2.has_mp ? b + Q.s2.o_hm : nullptr);
+            T.t.level_sigma2 = (const float*)(b + Q.s2.o_sig);
+        } else T.t = kf_dev(m, &B.kf2, Q.s2.o);
+        for (int i = 0; i < 9; i++) T.F[i] = B.F12[i];
+        T.ex = B.ex; T.ey = B.ey; T.only_stereo = B.only_stereo;
+        T.vmatch = (int32_t*)(b + Q.vm); T.bins = b + Q.bins;
+        T.pairs = (int32_t*)(b + o_res + Q.res); T.cap = Q.cap; T.n_pairs = (int32_t*)(b + o_res) + k;
+        hj[k] = T;
+    }
+    if ((s = commit(st, total)) != BORB_OK) return s;
+    for (int j : live) {
+        if (jobs[j].kf1_frame) BORB_CUDA(cudaStreamWaitEvent(m->stream, jobs[j].kf1_frame->ready, 0));
+        if (jobs[j].kf2_frame) BORB_CUDA(cudaStreamWaitEvent(m->stream, jobs[j].kf2_frame->ready, 0));
+    }
+    m->launches += launch_triangulation((const TriJob*)(b + o_jobs), nl, check_ori, m->stream);
+    BORB_CUDA(cudaGetLastError());
+    BORB_CUDA(cudaMemcpyAsync(m->h_out, b + o_res, res_bytes, cudaMemcpyDeviceToHost, m->stream));
+    BORB_CUDA(cudaStreamSynchronize(m->stream));
+    int overflow = -1;
+    for (int k = 0; k < nl; k++) {
+        const borb_triangulation_job& B = jobs[live[k]];
+        std::memcpy(B.n_pairs, m->h_out + (size_t)k * 4, 4);
+        const int np = std::min(*B.n_pairs, B.cap);
+        if (np > 0) std::memcpy(B.pairs, m->h_out + J[live[k]].res, (size_t)np * 8);
+        if (*B.n_pairs > B.cap && overflow < 0) overflow = live[k];
+    }
+    if (overflow >= 0) {
+        set_error("%d pairs, capacity %d", *jobs[overflow].n_pairs, jobs[overflow].cap);
+        return job_fail(batch, overflow, BORB_ERR_CAPACITY);
+    }
+    return BORB_OK;
+}
+}  // namespace
+
 borb_status borb_search_for_triangulation(borb_matcher* m, const borb_keyframe_view* kf1, const borb_keyframe_view* kf2, const float* F12,
                                           float ex, float ey, int only_stereo, int check_orientation, int32_t* pairs, int cap,
                                           int32_t* n_pairs) {
     if (!m || !kf1 || !kf2 || !F12 || !pairs || !n_pairs || cap < 0) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
-    borb_status s = check_kf(kf1, "borb_search_for_triangulation(kf1)");
-    if (s == BORB_OK) s = check_kf(kf2, "borb_search_for_triangulation(kf2)");
-    if (s != BORB_OK) return s;
-    if (!kf2->scale_factors || !kf2->level_sigma2) { set_error("kf2 needs scale_factors and level_sigma2"); return BORB_ERR_INVALID_ARG; }
-    BORB_CUDA(cudaSetDevice(m->device));
-    Stager st(m);
-    const KfOffsets o1 = stage_kf(st, kf1), o2 = stage_kf(st, kf2);
-    const size_t input_end = st.off;
-    const int n1 = kf1->n > 0 ? kf1->n : 1;
-    const size_t o_vm = st.reserve((size_t)n1 * 4), o_bins = st.reserve((size_t)n1), o_pairs = st.reserve((size_t)n1 * 8), o_np = st.reserve(16);
-    const size_t total = st.off;
-    st.off = input_end;
-    if ((s = commit(st, total)) != BORB_OK) return s;
-    uint8_t* b = m->arena;
-    TriArgs T;
-    for (int i = 0; i < 9; i++) T.F[i] = F12[i];
-    T.ex = ex; T.ey = ey; T.only_stereo = only_stereo; T.check_ori = check_orientation;
-    m->launches += launch_triangulation(kf_dev(m, kf1, o1), kf_dev(m, kf2, o2), T, (int32_t*)(b + o_vm), b + o_bins, (int32_t*)(b + o_pairs), n1,
-                                        (int32_t*)(b + o_np), m->stream);
-    BORB_CUDA(cudaGetLastError());
-    BORB_CUDA(cudaMemcpyAsync(n_pairs, b + o_np, 4, cudaMemcpyDeviceToHost, m->stream));
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
-    const int np = *n_pairs < cap ? *n_pairs : cap;
-    if (np > 0) BORB_CUDA(cudaMemcpy(pairs, b + o_pairs, (size_t)np * 8, cudaMemcpyDeviceToHost));
-    if (*n_pairs > cap) { set_error("%d pairs, capacity %d", *n_pairs, cap); return BORB_ERR_CAPACITY; }
-    return BORB_OK;
+    borb_triangulation_job B{};
+    B.kf1 = *kf1; B.kf2 = *kf2;
+    std::memcpy(B.F12, F12, sizeof(B.F12));
+    B.ex = ex; B.ey = ey; B.only_stereo = only_stereo; B.pairs = pairs; B.cap = cap; B.n_pairs = n_pairs;
+    return triangulation_jobs(m, &B, 1, check_orientation, false);
+}
+
+borb_status borb_search_for_triangulation_batch(borb_matcher* m, const borb_triangulation_job* jobs, int n_jobs, int check_orientation) {
+    if (!m || n_jobs < 0 || (n_jobs > 0 && !jobs)) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+    return triangulation_jobs(m, jobs, n_jobs, check_orientation, true);
 }
 
 // ------------------------------------------------------------------------------------------------ vocabulary

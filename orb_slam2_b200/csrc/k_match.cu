@@ -8,8 +8,9 @@
 //       exactly one node, so the greedy "already claimed" skip, :209/:576, never crosses nodes); per node the distance matrix is
 //       computed with all lanes busy, then the rows are replayed in order; rotation-histogram cull (:267-285) at the end.
 //       (The database-resident search of one frame against thousands of keyframes is k_bowdb.cu.)
-//   triangulation_kernel  SearchForTriangulation (:657-823): no sequential dependence (vbMatched2 is never set in
-//       the reference), "dist<=bestDist, later wins" == min over (distance, -position); epipolar tests as :140-157.
+//   triangulation_kernel  SearchForTriangulation (:657-823) over a table of jobs, a CTA per job: no sequential dependence
+//       (vbMatched2 is never set in the reference), "dist<=bestDist, later wins" == min over (distance, -position); epipolar
+//       tests as :140-157.
 //   bow_transform_kernel  TemplatedVocabulary::transform (Thirdparty/DBoW2/DBoW2/TemplatedVocabulary.h:1218-1259):
 //       a warp per descriptor descends the tree, lanes = children, first-wins argmin (bow_transform_batch_kernel: the same
 //       descent for many resident frames, grid.y = frame).
@@ -638,12 +639,19 @@ __global__ void __launch_bounds__(32 * BOW_WARPS) bow_match_kernel(const KfDev* 
 }
 
 // ------------------------------------------------------------------------------------------------ triangulation
-__global__ void __launch_bounds__(256) triangulation_kernel(KfDev q, KfDev t, TriArgs T, int32_t* __restrict__ vmatch,
-                                                            uint8_t* __restrict__ bins, int32_t* __restrict__ pairs, int cap,
-                                                            int32_t* __restrict__ n_pairs) {
+// A CTA per job (borb_search_for_triangulation is the one-job case); the rows of a job are independent, so warps take kf1's
+// FeatureVector nodes round robin, and the job's pairs are compacted in idx1 order into its own region.
+__global__ void __launch_bounds__(256) triangulation_kernel(const TriJob* __restrict__ jobs, int check_ori) {
     __shared__ int hist[32];
     __shared__ int top[3];
     __shared__ int wsum[9];
+    const TriJob& T = jobs[blockIdx.x];
+    const KfDev& q = T.q;
+    const KfDev& t = T.t;
+    int32_t* __restrict__ vmatch = T.vmatch;
+    uint8_t* __restrict__ bins = T.bins;
+    int32_t* __restrict__ pairs = T.pairs;
+    const int cap = T.cap;
     const int tid = threadIdx.x, lane = tid & 31, wrp = tid >> 5;
     for (int i = tid; i < q.n; i += 256) vmatch[i] = -1;
     if (tid < 32) hist[tid] = 0;
@@ -690,7 +698,7 @@ __global__ void __launch_bounds__(256) triangulation_kernel(KfDev q, KfDev t, Tr
             if (bestKey != 0xFFFFFFFFu && lane == 0) {
                 const int j = (int)t.idx[ts0 + (0xFFFF - (int)(bestKey & 0xFFFFu))];
                 vmatch[i] = j;
-                if (T.check_ori) {
+                if (check_ori) {
                     const int b = rot_bin(kp1.angle, t.keys[j].angle);
                     bins[i] = (uint8_t)b;
                     atomicAdd(&hist[b], 1);
@@ -699,7 +707,7 @@ __global__ void __launch_bounds__(256) triangulation_kernel(KfDev q, KfDev t, Tr
         }
     }
     __syncthreads();
-    if (T.check_ori) {
+    if (check_ori) {
         if (tid == 0) { int a, b, c; three_maxima(hist, a, b, c); top[0] = a; top[1] = b; top[2] = c; }
         __syncthreads();
         for (int i = tid; i < q.n; i += 256)
@@ -725,7 +733,7 @@ __global__ void __launch_bounds__(256) triangulation_kernel(KfDev q, KfDev t, Tr
         running += tot;
         __syncthreads();
     }
-    if (tid == 0) *n_pairs = running;
+    if (tid == 0) *T.n_pairs = running;
 }
 
 // ------------------------------------------------------------------------------------------------ vocabulary
@@ -958,10 +966,16 @@ int launch_bow_match(const KfDev* qs, const KfDev* ts, int n_pairs, int mode, fl
                                                          max_t);
     return 1;
 }
-int launch_triangulation(const KfDev& q, const KfDev& t, const TriArgs& T, int32_t* vmatch, uint8_t* bins, int32_t* pairs, int cap,
-                         int32_t* n_pairs, cudaStream_t s) {
-    triangulation_kernel<<<1, 256, 0, s>>>(q, t, T, vmatch, bins, pairs, cap, n_pairs);
+int launch_triangulation(const TriJob* d_jobs, int n_jobs, int check_ori, cudaStream_t s) {
+    if (n_jobs <= 0) return 0;
+    triangulation_kernel<<<n_jobs, 256, 0, s>>>(d_jobs, check_ori);
     return 1;
+}
+int launch_fuse_batch(const LastArgs* d_last, const FuseJob* d_jobs, int n_jobs, int max_nq, cudaStream_t s) {
+    if (n_jobs <= 0 || max_nq <= 0) return 0;
+    project_points_batch_kernel<<<dim3((max_nq + 255) / 256, n_jobs), 256, 0, s>>>(d_last);
+    launch_fuse_search(d_jobs, n_jobs, max_nq, s);
+    return 2;
 }
 int launch_bow_transform(const VocDev& V, const uint8_t* desc, int n, int levelsup, int32_t* word, double* weight, int32_t* node,
                          cudaStream_t s) {

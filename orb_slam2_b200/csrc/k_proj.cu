@@ -1,6 +1,6 @@
 // Windowed projection search shared by every ORBmatcher::SearchByProjection overload, Fuse and SearchBySim3
 // (reference src/ORBmatcher.cc:45-129, 290-403, 825-1100, 1102-1326, 1328-1599) — candidate enumeration and the
-// order-dependent claim resolution.
+// order-dependent claim resolution; fuse_batch_kernel (below) is the list-free search of both Fuse overloads.
 //
 //   proj_candidates_kernel   Frame::GetFeaturesInArea (src/Frame.cc:327-380) + the per-candidate gates + DescriptorDistance,
 //       a warp per query.  Lanes take different GRID CELLS of the query window (a cell holds ~0.3 features, so a lane per
@@ -58,6 +58,38 @@ __device__ void three_maxima(const int* cnt, int& ind1, int& ind2, int& ind3) { 
     else if ((float)max3 < 0.1f * (float)max1) { ind3 = -1; }
 }
 
+__device__ __forceinline__ unsigned warp_min(unsigned v) { return __reduce_min_sync(0xFFFFFFFFu, v); }
+
+// The cell window of GetFeaturesInArea(x, y, rs) (Frame.cc:327-380) on A's grid: columns c0x..c1x, rows c0y..c1y; false when
+// it is empty
+__device__ __forceinline__ bool area_window(const ProjArgs& A, float x, float y, float rs, int& c0x, int& c1x, int& c0y, int& c1y) {
+    c0x = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(x, A.minX), rs), A.invW)));
+    c1x = min(GRID_COLS - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(x, A.minX), rs), A.invW)));
+    c0y = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(y, A.minY), rs), A.invH)));
+    c1y = min(GRID_ROWS - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(y, A.minY), rs), A.invH)));
+    return !(c0x >= GRID_COLS || c1x < 0 || c0y >= GRID_ROWS || c1y < 0);
+}
+
+// The per-candidate gates of the windowed searches: GetFeaturesInArea's level range and square, then the stereo consistency
+// of SearchByProjection (:91-96) where u_right is given (Fuse passes none: its stereo test is the reprojection gate)
+__device__ __forceinline__ bool area_passes(const borb_keypoint& kp, const float* __restrict__ u_right, int idx, float x, float y, float xr,
+                                            float rs, int minLevel, int maxLevel) {
+    if ((minLevel > 0) || (maxLevel >= 0)) {                 // bCheckLevels
+        if (kp.octave < minLevel) return false;
+        if (maxLevel >= 0 && kp.octave > maxLevel) return false;
+    }
+    const float dx = __fsub_rn(kp.x, x), dy = __fsub_rn(kp.y, y);
+    if (!(fabsf(dx) < rs && fabsf(dy) < rs)) return false;
+    if (u_right != nullptr) {
+        const float ur = u_right[idx];
+        if (ur > 0) {
+            const float er = fabsf(__fsub_rn(xr, ur));
+            if (er > rs) return false;
+        }
+    }
+    return true;
+}
+
 }  // namespace
 
 // cand entry: idx | dist << 16 | octave << 25;   cand_cnt = count | CAND_UNSORTED
@@ -90,42 +122,9 @@ __device__ __forceinline__ void candidates_body(const ProjArgs& A) {
             rs = A.q_radius[iMP]; minLevel = A.q_minl[iMP]; maxLevel = A.q_maxl[iMP];
         }
         // GetFeaturesInArea(x, y, rs, minLevel, maxLevel)  (Frame.cc:327-380)
-        const int c0x = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(x, A.minX), rs), A.invW)));
-        const int c1x = min(GRID_COLS - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(x, A.minX), rs), A.invW)));
-        const int c0y = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(y, A.minY), rs), A.invH)));
-        const int c1y = min(GRID_ROWS - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(y, A.minY), rs), A.invH)));
-        if (!(c0x >= GRID_COLS || c1x < 0 || c0y >= GRID_ROWS || c1y < 0)) {
-            const bool bCheckLevels = (minLevel > 0) || (maxLevel >= 0);
-            auto passes = [&](int idx) -> bool {
-                const borb_keypoint kp = A.keys[idx];
-                if (bCheckLevels) {
-                    if (kp.octave < minLevel) return false;
-                    if (maxLevel >= 0 && kp.octave > maxLevel) return false;
-                }
-                const float dx = __fsub_rn(kp.x, x), dy = __fsub_rn(kp.y, y);
-                if (!(fabsf(dx) < rs && fabsf(dy) < rs)) return false;
-                if (A.u_right != nullptr && !A.chi2) {              // stereo consistency (:91-96)
-                    const float ur = A.u_right[idx];
-                    if (ur > 0) {
-                        const float er = fabsf(__fsub_rn(xr, ur));
-                        if (er > rs) return false;
-                    }
-                }
-                if (A.chi2) {                                        // Fuse reprojection gates (:907-931)
-                    const float ex = __fsub_rn(x, kp.x), ey = __fsub_rn(y, kp.y);
-                    const float kr = A.u_right != nullptr ? A.u_right[idx] : -1.0f;
-                    const float inv = A.inv_sigma2[kp.octave];
-                    if (kr >= 0) {
-                        const float er = __fsub_rn(xr, kr);
-                        const float e2 = __fadd_rn(__fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey)), __fmul_rn(er, er));
-                        if ((double)__fmul_rn(e2, inv) > 7.8) return false;
-                    } else {
-                        const float e2 = __fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey));
-                        if ((double)__fmul_rn(e2, inv) > 5.99) return false;
-                    }
-                }
-                return true;
-            };
+        int c0x, c1x, c0y, c1y;
+        if (area_window(A, x, y, rs, c0x, c1x, c0y, c1y)) {
+            auto passes = [&](int idx) -> bool { return area_passes(A.keys[idx], A.u_right, idx, x, y, xr, rs, minLevel, maxLevel); };
             // ---- 1. a lane per grid cell, cells in (ix outer, iy inner) order
             const int ncy = c1y - c0y + 1, C = (c1x - c0x + 1) * ncy;
             for (int cb = 0; cb < C; cb += 32) {
@@ -189,6 +188,63 @@ __device__ __forceinline__ void candidates_body(const ProjArgs& A) {
 __global__ void __launch_bounds__(256) proj_candidates_kernel(ProjArgs A) { candidates_body(A); }
 // one launch for many independent (frame, MapPoint list) jobs: grid.y = job, the job's arguments come from device memory
 __global__ void __launch_bounds__(256) proj_candidates_batch_kernel(const ProjArgs* __restrict__ jobs) { candidates_body(jobs[blockIdx.y]); }
+
+// The search part of both Fuse overloads (:825-970, :972-1100) for a table of jobs, a warp per (job, query point) on grid
+// (points / 8, jobs), after project_points (variant 2) wrote the windows.  The candidate enumeration and the first-minimum
+// search are one pass, with no candidate list: the grid is sorted by cell = ix * GRID_ROWS + iy, so for each column ix of the
+// window the window's cells are ONE contiguous range of cell_idx.  Lanes stride over that range (coalesced), apply the area
+// gates and the reprojection gates (:907-931), and keep min((dist << 16) | e) with e the position in cell_idx: ascending e is
+// the (ix, iy, insertion) order of GetFeaturesInArea, so the warp minimum is the reference's `dist < bestDist` first minimum.
+__global__ void __launch_bounds__(256) fuse_batch_kernel(const FuseJob* __restrict__ jobs) {
+    const FuseJob& J = jobs[blockIdx.y];
+    const ProjArgs& A = J.A;
+    const int lane = threadIdx.x & 31;
+    const int iq = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (iq >= A.n_mp) return;
+    unsigned best = 0xFFFFFFFFu;
+    if (A.mp_valid[iq]) {
+        const float x = A.proj_x[iq], y = A.proj_y[iq], xr = A.proj_xr[iq], rs = A.q_radius[iq];
+        const int minLevel = A.q_minl[iq], maxLevel = A.q_maxl[iq];
+        int c0x, c1x, c0y, c1y;
+        if (area_window(A, x, y, rs, c0x, c1x, c0y, c1y)) {
+            const uint4 dm0 = reinterpret_cast<const uint4*>(A.mp_desc)[(size_t)iq * 2], dm1 = reinterpret_cast<const uint4*>(A.mp_desc)[(size_t)iq * 2 + 1];
+            const uint32_t dm[8] = {dm0.x, dm0.y, dm0.z, dm0.w, dm1.x, dm1.y, dm1.z, dm1.w};
+            for (int ix = c0x; ix <= c1x; ix++) {
+                const int e1 = A.cell_start[ix * GRID_ROWS + c1y + 1];
+                for (int e = A.cell_start[ix * GRID_ROWS + c0y] + lane; e < e1; e += 32) {
+                    const int idx = A.cell_idx[e];
+                    const borb_keypoint kp = A.keys[idx];
+                    if (!area_passes(kp, nullptr, idx, x, y, xr, rs, minLevel, maxLevel)) continue;
+                    if (J.inv_sigma2 != nullptr) {                      // Fuse(pKF, vpMapPoints, th) reprojection gates (:907-931)
+                        const float ex = __fsub_rn(x, kp.x), ey = __fsub_rn(y, kp.y);
+                        const float kr = A.u_right != nullptr ? A.u_right[idx] : -1.0f;
+                        const float inv = J.inv_sigma2[kp.octave];
+                        if (kr >= 0) {
+                            const float er = __fsub_rn(xr, kr);
+                            const float e2 = __fadd_rn(__fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey)), __fmul_rn(er, er));
+                            if ((double)__fmul_rn(e2, inv) > 7.8) continue;
+                        } else {
+                            const float e2 = __fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey));
+                            if ((double)__fmul_rn(e2, inv) > 5.99) continue;
+                        }
+                    }
+                    const int dist = ham_words(dm, reinterpret_cast<const uint32_t*>(A.desc + (size_t)idx * 32));
+                    best = min(best, ((unsigned)dist << 16) | (unsigned)e);
+                }
+            }
+        }
+    }
+    best = warp_min(best);
+    if (lane == 0) {
+        int out = -1;
+        if (best != 0xFFFFFFFFu && (int)(best >> 16) <= A.th_dist) { out = A.cell_idx[best & 0xFFFFu]; atomicAdd(J.n_found, 1); }
+        A.out_match[iq] = out;
+    }
+}
+
+void launch_fuse_search(const FuseJob* d_jobs, int n_jobs, int max_nq, cudaStream_t s) {
+    fuse_batch_kernel<<<dim3((max_nq + 7) / 8, n_jobs), 256, 0, s>>>(d_jobs);
+}
 
 size_t resolve_smem_bytes(int n, int n_mp) {
     return ((size_t)(n + 31) / 32 + (size_t)n + (size_t)n_mp * RES_K + (size_t)n_mp) * 4 + (size_t)n_mp + 64;

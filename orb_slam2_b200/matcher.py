@@ -53,6 +53,17 @@ class _BowJobC(C.Structure):                       # borb_bow_job
     _fields_ = [("frame", C.c_void_p), ("kf", _KeyFrameViewC), ("kf_frame", C.c_void_p), ("match", C.c_void_p)]
 
 
+class _TriangulationJobC(C.Structure):             # borb_triangulation_job
+    _fields_ = [("kf1", _KeyFrameViewC), ("kf1_frame", C.c_void_p), ("kf2", _KeyFrameViewC), ("kf2_frame", C.c_void_p), ("F12", C.c_float * 9),
+                ("ex", C.c_float), ("ey", C.c_float), ("only_stereo", C.c_int32), ("pairs", C.c_void_p), ("cap", C.c_int32), ("n_pairs", C.c_void_p)]
+
+
+class _FuseJobC(C.Structure):                      # borb_fuse_job
+    _fields_ = [("kf", _FrameViewC), ("inv_level_sigma2", C.c_void_p), ("pts", _WorldPointsViewC), ("Tcw", C.c_float * 12), ("Ow", C.c_float * 3)] + \
+               [(n, C.c_float) for n in ("fx", "fy", "cx", "cy", "bf", "log_scale_factor", "th")] + \
+               [("scw_variant", C.c_int32), ("best_idx", C.c_void_p)]
+
+
 class _KfdbQueryJobC(C.Structure):                  # borb_kfdb_query_job
     _fields_ = [("db", C.c_void_p), ("frame", C.c_void_p), ("common_words", C.c_void_p), ("score", C.c_void_p), ("first_word", C.c_void_p),
                 ("cap", C.c_int32), ("n_slots", C.c_void_p)]
@@ -712,6 +723,70 @@ class ORBmatcher:
                                                       int(bOnlyStereo), int(self.mbCheckOrientation), _p(pairs), cap, C.byref(n)),
               "borb_search_for_triangulation")
         return pairs[:n.value]
+
+    @staticmethod
+    def _tri_side(kf, keep):
+        """(borb_keyframe_view, resident frame handle, feature count) of one side of a triangulation job: a KeyFrameView, or a
+        device-resident FrameView with BoW and has_mp (then mvLevelSigma2 = mvScaleFactors^2 in float, ORBextractor's definition)."""
+        if isinstance(kf, KeyFrameView):
+            c = kf._c()
+            keep.append(list(kf._keep))                  # the same view may serve several jobs: _c() replaces kf._keep
+            return c, None, len(kf.mvKeysUn)
+        if isinstance(kf, FrameView) and kf.resident is not None:
+            hm = np.ascontiguousarray(kf.has_mp, np.uint8) if kf.has_mp is not None else None
+            sf = np.asarray(kf.mvScaleFactors, np.float32)
+            sg = np.ascontiguousarray(sf * sf, np.float32)
+            keep.append((hm, sg))
+            return _KeyFrameViewC(0, None, None, _p(hm), n_levels=len(sg), level_sigma2=_p(sg)), kf.resident._h.value, kf.resident.n
+        raise ValueError("a KeyFrameView or a device-resident FrameView")
+
+    def SearchForTriangulationBatch(self, kf1s, kf2s, F12s, epipoles, bOnlyStereo=False, caps=None):
+        """borb_search_for_triangulation_batch: SearchForTriangulation (src/ORBmatcher.cc:657-823) of many keyframe pairs in one launch.
+        kf1s[j] / kf2s[j] = KeyFrameView or device-resident FrameView (BoW from ComputeBoWBatch, has_mp set); bOnlyStereo and caps
+        (None: one pair per kf1 feature) are one value for every job or one per job.  Returns vMatchedPairs per job, equal to what
+        SearchForTriangulation returns on host views of the same data."""
+        n = len(kf1s)
+        assert n == len(kf2s) == len(F12s) == len(epipoles)
+        ost, cps = _per_job(bOnlyStereo, n), _per_job(caps, n)
+        jobs = (_TriangulationJobC * max(n, 1))()
+        keep, outs = [], []
+        for j in range(n):
+            J = jobs[j]
+            J.kf1, J.kf1_frame, n1 = self._tri_side(kf1s[j], keep)
+            J.kf2, J.kf2_frame, _ = self._tri_side(kf2s[j], keep)
+            J.F12 = (C.c_float * 9)(*np.asarray(F12s[j], np.float32).reshape(9).tolist())
+            J.ex, J.ey, J.only_stereo = float(epipoles[j][0]), float(epipoles[j][1]), int(ost[j])
+            cap = n1 if cps[j] is None else int(cps[j])
+            pairs, npairs = np.zeros((max(cap, 1), 2), np.int32), np.zeros(1, np.int32)
+            J.pairs, J.cap, J.n_pairs = _p(pairs), cap, _p(npairs)
+            outs.append((pairs, npairs))
+        check(self._lib.borb_search_for_triangulation_batch(self._h, jobs, n, int(self.mbCheckOrientation)), "borb_search_for_triangulation_batch")
+        return [pairs[:int(npairs[0])] for pairs, npairs in outs]
+
+    def FuseBatch(self, kfs: Sequence[FrameView], points: Sequence[WorldPointsView], poses, K, bf, th=3.0, Scw=False):
+        """borb_fuse_batch: the search part of Fuse (src/ORBmatcher.cc:825-970, or with Scw=True :972-1100) of many jobs in two launches.
+        kfs[j] = device-resident FrameView (mvInvLevelSigma2 set unless Scw); poses[j] = (Tcw, Ow); K, bf, th and Scw are one value for
+        every job or one per job.  Returns [(n_found, best_idx)] per job, equal to what Fuse returns."""
+        n = len(kfs)
+        assert n == len(points) == len(poses)
+        Ks, bfs, ths, scws = _per_job(K, n, 1), _per_job(bf, n), _per_job(th, n), _per_job(Scw, n)
+        jobs = (_FuseJobC * max(n, 1))()
+        keep, outs = [], []
+        for j in range(n):
+            fv, pv, logs, _, k = self._points_call(kfs[j], points[j], with_stereo=not scws[j])
+            inv = np.ascontiguousarray(kfs[j].mvInvLevelSigma2, np.float32) if kfs[j].mvInvLevelSigma2 is not None else None
+            nq = len(points[j].world_pos)
+            best = np.full(max(nq, 1), -1, np.int32)
+            Tcw, Ow = poses[j]
+            J = jobs[j]
+            J.kf, J.inv_level_sigma2, J.pts, J.Tcw = fv, _p(inv), pv, _pose12(Tcw)
+            J.Ow = (C.c_float * 3)(*np.asarray(Ow, np.float32).reshape(3).tolist())
+            J.fx, J.fy, J.cx, J.cy = [float(x) for x in Ks[j]]
+            J.bf, J.log_scale_factor, J.th, J.scw_variant, J.best_idx = float(bfs[j]), logs, float(ths[j]), int(scws[j]), _p(best)
+            keep.append((k, inv)); outs.append((nq, best))
+        nf = np.zeros(max(n, 1), np.int32)
+        check(self._lib.borb_fuse_batch(self._h, jobs, n, _p(nf)), "borb_fuse_batch")
+        return [(int(nf[j]), best[:nq]) for j, (nq, best) in enumerate(outs)]
 
 
 def _sharing_order(cw, fw, seq, skip=()):
