@@ -286,19 +286,18 @@ struct VocDev {                   // views into the packed blob
 int launch_grid_sort(const borb_keypoint* keys, int n, float minX, float minY, float invW, float invH, int* cell_start, int* cell_idx,
                      cudaStream_t s);
 void launch_candidates(const ProjArgs& A, cudaStream_t s);
-int launch_projection_batch(const ProjArgs* d_jobs, int n_jobs, int max_n, int max_n_mp, cudaStream_t s, bool last = false);
-// project_points over a LastArgs table, then the batched candidates and resolve (last: resolve<true>) over a ProjArgs table
-int launch_point_projection_batch(const LastArgs* d_last, const ProjArgs* d_jobs, int n_jobs, int max_nq, int max_n, int max_n_mp, bool last,
-                                  cudaStream_t s);
+// candidates and resolve (last: resolve<true>) of n_jobs jobs: one job runs the by-value kernels on `one` (the host copy of job 0),
+// more run the *_batch_kernels over the ProjArgs table d_jobs (unused for one job)
+int launch_projection_batch(const ProjArgs* d_jobs, const ProjArgs& one, int n_jobs, int max_n, int max_n_mp, cudaStream_t s, bool last = false);
+// project_points, then launch_projection_batch; one job by value (one_last, one), more over the LastArgs / ProjArgs tables
+int launch_point_projection_batch(const LastArgs* d_last, const ProjArgs* d_jobs, const LastArgs& one_last, const ProjArgs& one, int n_jobs,
+                                  int max_nq, int max_n, int max_n_mp, bool last, cudaStream_t s);
 void launch_resolve(const ProjArgs& A, bool last, cudaStream_t s);
-int launch_projection(const ProjArgs& A, cudaStream_t s);
-int launch_projection_last(const LastArgs& L, const ProjArgs& A, cudaStream_t s);
 int launch_initialization(const ProjArgs& A, const borb_keypoint* keys1, int n1, int32_t* match12, int32_t* ev_idx, uint8_t* ev_bin,
                           float* prev, int* n_matches, cudaStream_t s);
 // n_jobs queries (a job table in device memory) in one launch; max_slots / max_nq: the largest n_slots / nq of the jobs
 int launch_kfdb_score(const KfdbQueryJob* d_jobs, int n_jobs, int max_slots, int max_nq, int n_sm, cudaStream_t s);
 int launch_distinctive(const uint8_t* desc, const int32_t* offsets, int n_points, int32_t* best_idx, cudaStream_t s);
-int launch_frustum_projection(const LastArgs& L, const ProjArgs& A, cudaStream_t s);
 int launch_projection_argmin(const LastArgs& L, const ProjArgs& A, cudaStream_t s);
 int launch_sim3_agree(const int32_t* match1, const int32_t* match2, int n1, int n2, int32_t* match12, int* n_found, cudaStream_t s);
 // out_off: null (every pair against ts[0], output p at match + p * out_stride) or, mode 0, one target and output offset per pair

@@ -2,6 +2,7 @@
 // arrays, are staged into one device arena per call, and every result is produced by the CUDA kernels in k_match.cu.
 #include <algorithm>
 #include <atomic>
+#include <cassert>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -19,9 +20,6 @@ struct borb_matcher {
     size_t arena_bytes = 0, arena_off = 0;
     uint8_t* h_stage = nullptr;     // pinned staging mirror of the arena's input part
     size_t h_bytes = 0;
-    const uint8_t* in_base = nullptr;   // where the kernels of the current call read the staged inputs: the arena, or (small calls
-                                        // on a resident frame) h_stage itself - pinned host memory is device-addressable (UVA), which
-                                        // saves the H2D copy and its DMA latency
     uint64_t launches = 0;
     int32_t* aux = nullptr;         // small device buffer that survives an arena re-layout (SearchBySim3: first direction's matches)
     size_t aux_count = 0;
@@ -47,69 +45,106 @@ struct borb_voc {
 
 namespace {
 
-struct Stager {
-    // Lays host arrays out in one pinned buffer, then moves them with a single H2D copy; returns device addresses.
-    borb_matcher* m;
-    size_t off = 0;
-    std::vector<std::pair<const void*, std::pair<size_t, size_t>>> items;   // (src, (offset, bytes))
-    explicit Stager(borb_matcher* mm) : m(mm) {}
-    size_t reserve(size_t bytes) { off = (off + 255) & ~size_t(255); size_t o = off; off += bytes; return o; }
-    size_t add(const void* src, size_t bytes) {
-        const size_t o = reserve(bytes);
-        items.push_back({src, {o, bytes}});
+constexpr size_t ZERO_COPY_MAX = 96 * 1024;       // inputs up to this size may be read in place by the kernels (each byte is read once)
+
+// One matcher call on m->stream.  Its layout comes first, as offsets: staged inputs, then device-only scratch, then result slots.
+// begin() grows the buffers, after which addresses exist; commit() moves the inputs with one H2D copy and finish() brings the result
+// region back with one D2H copy and synchronises.  Kernels read the inputs from the arena or, for a small in-place call, from the
+// pinned staging buffer itself (device-addressable, UVA: no H2D copy and no DMA latency).  They write results to the arena, or
+// straight into the pinned landing buffer.
+class Call {
+public:
+    explicit Call(borb_matcher* m) : m_(m) {}
+    // a staged input; src == nullptr: filled through host<T>() after begin()
+    size_t in(const void* src, size_t bytes) {
+        assert(!begun_ && in_end_ == off_);              // every input comes before any scratch
+        const size_t o = put(bytes);
+        items_.push_back({src, o, bytes});
+        in_end_ = off_;
         return o;
     }
+    size_t scratch(size_t bytes) { assert(!begun_); return put(bytes); }
+    // a slot of the result region, 16-byte aligned
+    size_t result(size_t bytes) {
+        assert(!begun_);
+        const size_t o = (res_bytes_ + 15) & ~size_t(15);
+        res_bytes_ = o + bytes;
+        return o;
+    }
+    // in_place: the kernels read the inputs from the staging buffer if they fit ZERO_COPY_MAX
+    borb_status begin(bool in_place = false) {
+        assert(!begun_);
+        in_place_ = in_place && in_end_ <= ZERO_COPY_MAX;
+        res_off_ = put(res_bytes_);
+        BORB_CUDA(cudaSetDevice(m_->device));
+        borb_status s;
+        if ((s = grow_device(m_->arena, m_->arena_bytes, off_)) != BORB_OK) return s;
+        if ((s = grow_pinned(m_->h_stage, m_->h_bytes, in_end_)) != BORB_OK) return s;
+        if (res_bytes_ && (s = grow_pinned(m_->h_out, m_->h_out_bytes, res_bytes_ + 4096)) != BORB_OK) return s;
+        BORB_CUDA(cudaStreamSynchronize(m_->stream));   // the staging buffer may still feed an earlier copy
+        for (const Item& it : items_)
+            if (it.src) std::memcpy(m_->h_stage + it.off, it.src, it.bytes);
+        begun_ = true;
+        return BORB_OK;
+    }
+    bool in_place() const { return in_place_; }
+    // the staging copy of an input
+    template <class T> T* host(size_t off) const { assert(begun_ && off < in_end_); return reinterpret_cast<T*>(m_->h_stage + off); }
+    // where kernels read an input or use scratch
+    uint8_t* dev(size_t off) const { assert(begun_); return (in_place_ && off < in_end_ ? m_->h_stage : m_->arena) + off; }
+    // where kernels write a result: the arena (brought back by finish()), or direct: the landing buffer
+    uint8_t* res(size_t off, bool direct) {
+        assert(begun_);
+        download_ |= !direct;
+        return (direct ? m_->h_out : m_->arena + res_off_) + off;
+    }
+    borb_status commit() {
+        assert(begun_);
+        if (in_end_ && !in_place_) BORB_CUDA(cudaMemcpyAsync(m_->arena, m_->h_stage, in_end_, cudaMemcpyHostToDevice, m_->stream));
+        return BORB_OK;
+    }
+    borb_status wait(const borb_frame* f) const {
+        BORB_CUDA(cudaStreamWaitEvent(m_->stream, f->ready, 0));
+        return BORB_OK;
+    }
+    borb_status finish() {
+        BORB_CUDA(cudaGetLastError());
+        if (download_ && res_bytes_) BORB_CUDA(cudaMemcpyAsync(m_->h_out, m_->arena + res_off_, res_bytes_, cudaMemcpyDeviceToHost, m_->stream));
+        BORB_CUDA(cudaStreamSynchronize(m_->stream));
+        return BORB_OK;
+    }
+    // the landing buffer, after finish()
+    const uint8_t* out(size_t off) const { return m_->h_out + off; }
+
+private:
+    struct Item { const void* src; size_t off, bytes; };
+    size_t put(size_t bytes) { off_ = (off_ + 255) & ~size_t(255); const size_t o = off_; off_ += bytes; return o; }
+    // grow-only buffers; the stream is synchronised first because queued work may still use the old one
+    borb_status grow_device(uint8_t*& p, size_t& have, size_t bytes) {
+        if (have >= bytes) return BORB_OK;
+        BORB_CUDA(cudaStreamSynchronize(m_->stream));
+        cudaFree(p);
+        p = nullptr; have = 0;
+        const size_t want = bytes + bytes / 2 + (1 << 20);
+        BORB_CUDA(cudaMalloc(&p, want));
+        have = want;
+        return BORB_OK;
+    }
+    borb_status grow_pinned(uint8_t*& p, size_t& have, size_t bytes) {
+        if (have >= bytes) return BORB_OK;
+        BORB_CUDA(cudaStreamSynchronize(m_->stream));
+        if (p) cudaFreeHost(p);
+        p = nullptr; have = 0;
+        const size_t want = bytes + bytes / 2 + (1 << 16);
+        BORB_CUDA(cudaMallocHost(&p, want));
+        have = want;
+        return BORB_OK;
+    }
+    borb_matcher* m_;
+    std::vector<Item> items_;
+    size_t off_ = 0, in_end_ = 0, res_bytes_ = 0, res_off_ = 0;
+    bool begun_ = false, in_place_ = false, download_ = false;
 };
-
-borb_status ensure_arena(borb_matcher* m, size_t bytes) {
-    if (m->arena_bytes >= bytes) return BORB_OK;
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
-    cudaFree(m->arena);
-    m->arena = nullptr; m->arena_bytes = 0;
-    const size_t want = bytes + bytes / 2 + (1 << 20);
-    BORB_CUDA(cudaMalloc(&m->arena, want));
-    m->arena_bytes = want;
-    return BORB_OK;
-}
-borb_status ensure_host(borb_matcher* m, size_t bytes) {
-    if (m->h_bytes >= bytes) return BORB_OK;
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
-    if (m->h_stage) cudaFreeHost(m->h_stage);
-    m->h_stage = nullptr; m->h_bytes = 0;
-    const size_t want = bytes + bytes / 2 + (1 << 16);
-    BORB_CUDA(cudaMallocHost(&m->h_stage, want));
-    m->h_bytes = want;
-    return BORB_OK;
-}
-
-borb_status ensure_out(borb_matcher* m, size_t bytes) {
-    bytes += 4096;
-    if (m->h_out_bytes >= bytes) return BORB_OK;
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
-    if (m->h_out) cudaFreeHost(m->h_out);
-    m->h_out = nullptr; m->h_out_bytes = 0;
-    const size_t want = bytes + bytes / 2 + (1 << 16);
-    BORB_CUDA(cudaMallocHost(&m->h_out, want));
-    m->h_out_bytes = want;
-    return BORB_OK;
-}
-
-// copies the staged inputs; `extra` = device-only scratch bytes requested after the inputs
-constexpr size_t ZERO_COPY_MAX = 96 * 1024;       // inputs up to this size are read in place by the kernels (each byte is read once)
-
-borb_status commit(Stager& st, size_t total_with_scratch, bool zero_copy = false) {
-    borb_matcher* m = st.m;
-    borb_status s = ensure_host(m, st.off);
-    if (s != BORB_OK) return s;
-    if ((s = ensure_arena(m, total_with_scratch)) != BORB_OK) return s;
-    BORB_CUDA(cudaStreamSynchronize(m->stream));     // the staging buffer may still feed an earlier copy
-    for (auto& it : st.items)
-        if (it.first) std::memcpy(m->h_stage + it.second.first, it.first, it.second.second);
-    zero_copy = zero_copy && st.off <= ZERO_COPY_MAX;
-    if (st.off && !zero_copy) BORB_CUDA(cudaMemcpyAsync(m->arena, m->h_stage, st.off, cudaMemcpyHostToDevice, m->stream));
-    m->in_base = zero_copy ? m->h_stage : m->arena;
-    return BORB_OK;
-}
 
 // ---- frame side of the windowed searches: staged from the host view per call, or taken from a device-resident borb_frame
 struct FrameInfo { int n, n_levels; float min_x, min_y, max_x, max_y; bool has_ur; const borb_frame* rf; };
@@ -128,23 +163,23 @@ FrameInfo frame_info(const borb_frame_view* F) {
     return I;
 }
 // the per-call inputs of the frame (everything for a host view; only `occupied` for a resident frame)
-FrameStage stage_frame(Stager& st, const borb_frame_view* F, const FrameInfo& I, bool want_ur) {
+FrameStage stage_frame(Call& c, const borb_frame_view* F, const FrameInfo& I, bool want_ur) {
     FrameStage fs;
     if (!I.rf) {
-        fs.keys = st.add(F->keys_un, (size_t)I.n * sizeof(borb_keypoint));
-        fs.desc = st.add(F->desc, (size_t)I.n * 32);
+        fs.keys = c.in(F->keys_un, (size_t)I.n * sizeof(borb_keypoint));
+        fs.desc = c.in(F->desc, (size_t)I.n * 32);
         fs.ur_p = want_ur && F->u_right != nullptr;
-        if (fs.ur_p) fs.ur = st.add(F->u_right, (size_t)I.n * 4);
-        fs.sf = st.add(F->scale_factors, (size_t)(F->scale_factors ? I.n_levels : 0) * 4);
+        if (fs.ur_p) fs.ur = c.in(F->u_right, (size_t)I.n * 4);
+        fs.sf = c.in(F->scale_factors, (size_t)(F->scale_factors ? I.n_levels : 0) * 4);
     } else fs.ur_p = want_ur && I.has_ur;
     fs.occ_p = F->occupied != nullptr;
-    if (fs.occ_p) fs.occ = st.add(F->occupied, (size_t)I.n);
+    if (fs.occ_p) fs.occ = c.in(F->occupied, (size_t)I.n);
     return fs;
 }
-void reserve_grid(Stager& st, const FrameInfo& I, FrameStage& fs) {
+void reserve_grid(Call& c, const FrameInfo& I, FrameStage& fs) {
     if (I.rf) return;
-    fs.cs = st.reserve((size_t)(GRID_CELLS + 1) * 4);
-    fs.ci = st.reserve((size_t)MATCH_MAX_FEATURES * 4 + 16);
+    fs.cs = c.scratch((size_t)(GRID_CELLS + 1) * 4);
+    fs.ci = c.scratch((size_t)MATCH_MAX_FEATURES * 4 + 16);
 }
 // the frame fields of A that a device-resident frame provides
 void bind_resident(const borb_frame* rf, ProjArgs& A) {
@@ -155,8 +190,8 @@ void bind_resident(const borb_frame* rf, ProjArgs& A) {
     A.keys = rf->keys; A.desc = rf->desc; A.u_right = rf->u_right; A.scale_factors = rf->sf;
     A.cell_start = rf->cell_start; A.cell_idx = rf->cell_idx;
 }
-// the frame fields of A: the resident frame's, or (a host view, never zero-copy) those staged at fs in the arena b
-void bind_frame_fields(const FrameInfo& I, const FrameStage& fs, uint8_t* b, ProjArgs& A) {
+// the frame fields of A: the resident frame's, or those of a host view staged at fs
+void bind_frame_fields(const FrameInfo& I, const FrameStage& fs, const Call& c, ProjArgs& A) {
     if (I.rf) {
         bind_resident(I.rf, A);
         if (!fs.ur_p) A.u_right = nullptr;
@@ -166,26 +201,28 @@ void bind_frame_fields(const FrameInfo& I, const FrameStage& fs, uint8_t* b, Pro
     A.minX = I.min_x; A.minY = I.min_y;
     A.invW = (float)GRID_COLS / (float)(I.max_x - I.min_x);
     A.invH = (float)GRID_ROWS / (float)(I.max_y - I.min_y);
-    A.keys = (const borb_keypoint*)(b + fs.keys); A.desc = b + fs.desc;
-    A.u_right = fs.ur_p ? (const float*)(b + fs.ur) : nullptr;
-    A.scale_factors = (const float*)(b + fs.sf);
-    A.cell_start = (const int*)(b + fs.cs); A.cell_idx = (const int*)(b + fs.ci);
+    A.keys = (const borb_keypoint*)c.dev(fs.keys); A.desc = c.dev(fs.desc);
+    A.u_right = fs.ur_p ? (const float*)c.dev(fs.ur) : nullptr;
+    A.scale_factors = (const float*)c.dev(fs.sf);
+    A.cell_start = (const int*)c.dev(fs.cs); A.cell_idx = (const int*)c.dev(fs.ci);
 }
 // after commit(): builds the grid of a host view bound by bind_frame_fields, waits for the resident frame otherwise
-borb_status prepare_frame(borb_matcher* m, const FrameInfo& I, const ProjArgs& A) {
-    if (I.rf) {
-        BORB_CUDA(cudaStreamWaitEvent(m->stream, I.rf->ready, 0));
-        return BORB_OK;
-    }
+borb_status prepare_frame(borb_matcher* m, const Call& c, const FrameInfo& I, const ProjArgs& A) {
+    if (I.rf) return c.wait(I.rf);
     if (I.n > 0) m->launches += launch_grid_sort(A.keys, A.n, A.minX, A.minY, A.invW, A.invH, (int*)A.cell_start, (int*)A.cell_idx, m->stream);
     else BORB_CUDA(cudaMemsetAsync((void*)A.cell_start, 0, (size_t)(GRID_CELLS + 1) * 4, m->stream));
     return BORB_OK;
 }
-// fills the frame fields of A after commit(); builds the grid for a host view, waits for the resident frame otherwise
-borb_status bind_frame(borb_matcher* m, const FrameInfo& I, const FrameStage& fs, ProjArgs& A) {
-    bind_frame_fields(I, fs, m->arena, A);
-    return prepare_frame(m, I, A);
-}
+// The per-job kernel arguments of a Tracking-thread search.  One job is launched by value (the single calls: no table crosses PCIe);
+// more go to a staged table that the *_batch_kernels read.
+template <class T> struct JobTable {
+    int n;
+    size_t off = 0;
+    T one{};
+    JobTable(Call& c, int n_jobs) : n(n_jobs) { if (n > 1) off = c.in(nullptr, (size_t)n * sizeof(T)); }
+    T* host(const Call& c) { return n > 1 ? c.host<T>(off) : &one; }               // after begin()
+    const T* dev(const Call& c) const { return n > 1 ? (const T*)c.dev(off) : nullptr; }
+};
 borb_status check_frame(const borb_frame_view* F, const FrameInfo& I, const borb_matcher* m) {
     if (I.n < 0 || I.n > MATCH_MAX_FEATURES) { set_error("frame has %d features (limit %d)", I.n, MATCH_MAX_FEATURES); return BORB_ERR_INVALID_ARG; }
     if (I.rf) {
@@ -196,13 +233,13 @@ borb_status check_frame(const borb_frame_view* F, const FrameInfo& I, const borb
     if (I.n_levels < 1 || !F->scale_factors || !(I.max_x > I.min_x) || !(I.max_y > I.min_y)) { set_error("incomplete frame view"); return BORB_ERR_INVALID_ARG; }
     return BORB_OK;
 }
-borb_status job_error(int j, borb_status s) {      // prefixes the error text a shared check left with the job index
+// error text of a check shared by the single calls and the batches: the batches prefix it with the job index
+borb_status job_fail(bool batch, int j, borb_status s) {
+    if (!batch) return s;
     const std::string e = borb_last_error();
     set_error("job %d: %s", j, e.c_str());
     return s;
 }
-// error text of a check shared by the single calls and the batches: the batches name the job
-borb_status job_fail(bool batch, int j, borb_status s) { return batch ? job_error(j, s) : s; }
 // the candidate search reads its queries from what project_points_kernel wrote
 void wire_projection(const LastArgs& L, ProjArgs& A) {
     A.n_mp = L.n_last;
@@ -230,36 +267,35 @@ borb_status check_kf(const borb_keyframe_view* v, const char* what) {
     return BORB_OK;
 }
 
-KfOffsets stage_kf(Stager& st, const borb_keyframe_view* v) {
+KfOffsets stage_kf(Call& c, const borb_keyframe_view* v) {
     KfOffsets o{};
-    o.keys = st.add(v->keys_un, (size_t)v->n * sizeof(borb_keypoint));
-    o.desc = st.add(v->desc, (size_t)v->n * 32);
+    o.keys = c.in(v->keys_un, (size_t)v->n * sizeof(borb_keypoint));
+    o.desc = c.in(v->desc, (size_t)v->n * 32);
     o.has_mp_p = v->has_mp != nullptr;
-    o.has_mp = o.has_mp_p ? st.add(v->has_mp, (size_t)v->n) : 0;
+    o.has_mp = o.has_mp_p ? c.in(v->has_mp, (size_t)v->n) : 0;
     o.ur_p = v->u_right != nullptr;
-    o.u_right = o.ur_p ? st.add(v->u_right, (size_t)v->n * 4) : 0;
-    o.node = st.add(v->fv.node_id, (size_t)v->fv.n_nodes * 4);
-    o.start = st.add(v->fv.start, (size_t)(v->fv.n_nodes + 1) * 4);
+    o.u_right = o.ur_p ? c.in(v->u_right, (size_t)v->n * 4) : 0;
+    o.node = c.in(v->fv.node_id, (size_t)v->fv.n_nodes * 4);
+    o.start = c.in(v->fv.start, (size_t)(v->fv.n_nodes + 1) * 4);
     const int total = v->fv.n_nodes > 0 ? v->fv.start[v->fv.n_nodes] : 0;
-    o.idx = st.add(v->fv.feat_idx, (size_t)total * 4);
-    o.sf = st.add(v->scale_factors, (size_t)(v->scale_factors ? v->n_levels : 0) * 4);
-    o.sig = st.add(v->level_sigma2, (size_t)(v->level_sigma2 ? v->n_levels : 0) * 4);
+    o.idx = c.in(v->fv.feat_idx, (size_t)total * 4);
+    o.sf = c.in(v->scale_factors, (size_t)(v->scale_factors ? v->n_levels : 0) * 4);
+    o.sig = c.in(v->level_sigma2, (size_t)(v->level_sigma2 ? v->n_levels : 0) * 4);
     return o;
 }
 
-KfDev kf_dev(const borb_matcher* m, const borb_keyframe_view* v, const KfOffsets& o) {
+KfDev kf_dev(const Call& c, const borb_keyframe_view* v, const KfOffsets& o) {
     KfDev d;
-    uint8_t* b = m->arena;
     d.n = v->n; d.nn = v->fv.n_nodes;
-    d.keys = reinterpret_cast<const borb_keypoint*>(b + o.keys);
-    d.desc = b + o.desc;
-    d.has_mp = o.has_mp_p ? b + o.has_mp : nullptr;
-    d.u_right = o.ur_p ? reinterpret_cast<const float*>(b + o.u_right) : nullptr;
-    d.node = reinterpret_cast<const uint32_t*>(b + o.node);
-    d.start = reinterpret_cast<const int32_t*>(b + o.start);
-    d.idx = reinterpret_cast<const uint32_t*>(b + o.idx);
-    d.scale_factors = reinterpret_cast<const float*>(b + o.sf);
-    d.level_sigma2 = reinterpret_cast<const float*>(b + o.sig);
+    d.keys = reinterpret_cast<const borb_keypoint*>(c.dev(o.keys));
+    d.desc = c.dev(o.desc);
+    d.has_mp = o.has_mp_p ? c.dev(o.has_mp) : nullptr;
+    d.u_right = o.ur_p ? reinterpret_cast<const float*>(c.dev(o.u_right)) : nullptr;
+    d.node = reinterpret_cast<const uint32_t*>(c.dev(o.node));
+    d.start = reinterpret_cast<const int32_t*>(c.dev(o.start));
+    d.idx = reinterpret_cast<const uint32_t*>(c.dev(o.idx));
+    d.scale_factors = reinterpret_cast<const float*>(c.dev(o.sf));
+    d.level_sigma2 = reinterpret_cast<const float*>(c.dev(o.sig));
     return d;
 }
 
@@ -367,25 +403,23 @@ borb_status borb_frame_create(borb_matcher* m, const borb_frame_view* v, borb_fr
     borb_frame* f = nullptr;
     if ((s = frame_alloc(m->device, I.n, I.n_levels, v->u_right != nullptr, &f)) != BORB_OK) return s;
     f->min_x = I.min_x; f->min_y = I.min_y; f->max_x = I.max_x; f->max_y = I.max_y;
-    Stager st(m);
-    const size_t o_k = st.add(v->keys_un, (size_t)I.n * sizeof(borb_keypoint)), o_d = st.add(v->desc, (size_t)I.n * 32);
-    const size_t o_u = v->u_right ? st.add(v->u_right, (size_t)I.n * 4) : 0;
-    const size_t o_s = st.add(v->scale_factors, (size_t)I.n_levels * 4);
-    if ((s = commit(st, st.off)) != BORB_OK) { borb_frame_destroy(f); return s; }
-    uint8_t* b = m->arena;
+    Call c(m);
+    const size_t o_k = c.in(v->keys_un, (size_t)I.n * sizeof(borb_keypoint)), o_d = c.in(v->desc, (size_t)I.n * 32);
+    const size_t o_u = v->u_right ? c.in(v->u_right, (size_t)I.n * 4) : 0;
+    const size_t o_s = c.in(v->scale_factors, (size_t)I.n_levels * 4);
+    if ((s = c.begin()) != BORB_OK || (s = c.commit()) != BORB_OK) { borb_frame_destroy(f); return s; }
     cudaStream_t q = m->stream;
     if (I.n > 0) {
-        BORB_CUDA(cudaMemcpyAsync(f->keys, b + o_k, (size_t)I.n * sizeof(borb_keypoint), cudaMemcpyDeviceToDevice, q));
-        BORB_CUDA(cudaMemcpyAsync(f->desc, b + o_d, (size_t)I.n * 32, cudaMemcpyDeviceToDevice, q));
-        if (v->u_right) BORB_CUDA(cudaMemcpyAsync(f->u_right, b + o_u, (size_t)I.n * 4, cudaMemcpyDeviceToDevice, q));
+        BORB_CUDA(cudaMemcpyAsync(f->keys, c.dev(o_k), (size_t)I.n * sizeof(borb_keypoint), cudaMemcpyDeviceToDevice, q));
+        BORB_CUDA(cudaMemcpyAsync(f->desc, c.dev(o_d), (size_t)I.n * 32, cudaMemcpyDeviceToDevice, q));
+        if (v->u_right) BORB_CUDA(cudaMemcpyAsync(f->u_right, c.dev(o_u), (size_t)I.n * 4, cudaMemcpyDeviceToDevice, q));
     }
-    BORB_CUDA(cudaMemcpyAsync(f->sf, b + o_s, (size_t)I.n_levels * 4, cudaMemcpyDeviceToDevice, q));
+    BORB_CUDA(cudaMemcpyAsync(f->sf, c.dev(o_s), (size_t)I.n_levels * 4, cudaMemcpyDeviceToDevice, q));
     const float invW = (float)GRID_COLS / (float)(I.max_x - I.min_x), invH = (float)GRID_ROWS / (float)(I.max_y - I.min_y);
     if (I.n > 0) m->launches += launch_grid_sort(f->keys, I.n, I.min_x, I.min_y, invW, invH, f->cell_start, f->cell_idx, q);
     else BORB_CUDA(cudaMemsetAsync(f->cell_start, 0, (size_t)(GRID_CELLS + 1) * 4, q));
-    BORB_CUDA(cudaGetLastError());
     BORB_CUDA(cudaEventRecord(f->ready, q));
-    BORB_CUDA(cudaStreamSynchronize(q));              // the staging arena is reused by the next call on this matcher
+    if ((s = c.finish()) != BORB_OK) return s;       // the staging arena is reused by the next call on this matcher
     *out = f;
     return BORB_OK;
 }
@@ -440,21 +474,15 @@ borb_status borb_frames_from_extractor(borb_matcher* m, borb_extractor* e, const
     const size_t depth_img_bytes = (mode == 2 && !depth_on_device) ? (size_t)w * h * px : 0;
     if (mode == 2 && !depth_on_device && depth_stride_bytes < (int)(w * px)) { set_error("depth stride %d smaller than a row", depth_stride_bytes); return fail(BORB_ERR_INVALID_ARG); }
     const int ocap = (keys_un || u_right || depth_out) ? cap : 0;
-    Stager st(m);
-    const size_t o_jobs = st.reserve((size_t)n_frames * sizeof(FrameJob));
-    const size_t o_sf = st.add(e->scale.data(), (size_t)nl * 4);
-    const size_t input_end = st.off;
-    const size_t o_depth = st.reserve(depth_img_bytes * n_frames + 16);
-    const size_t o_ko = st.reserve((size_t)n_frames * ocap * sizeof(borb_keypoint) + 16);
-    const size_t o_uo = st.reserve((size_t)n_frames * ocap * 4 + 16), o_do = st.reserve((size_t)n_frames * ocap * 4 + 16);
-    const size_t total = st.off;
-    st.off = input_end;
-    if ((s = ensure_host(m, input_end)) != BORB_OK) return fail(s);
-    if ((s = ensure_arena(m, total)) != BORB_OK) return fail(s);
-    if ((s = ensure_out(m, (size_t)n_frames * ocap * (sizeof(borb_keypoint) + 8))) != BORB_OK) return fail(s);
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
-    uint8_t* b = m->arena;
-    FrameJob* hj = reinterpret_cast<FrameJob*>(m->h_stage + o_jobs);
+    Call c(m);
+    const size_t o_jobs = c.in(nullptr, (size_t)n_frames * sizeof(FrameJob));     // filled in place
+    const size_t o_sf = c.in(e->scale.data(), (size_t)nl * 4);
+    const size_t o_depth = c.scratch(depth_img_bytes * n_frames + 16);
+    // the requested outputs; the kernel writes depth_out wherever it writes u_right
+    const size_t kb = keys_un ? (size_t)n_frames * ocap * sizeof(borb_keypoint) : 0, fb = (u_right || depth_out) ? (size_t)n_frames * ocap * 4 : 0;
+    const size_t r_k = c.result(kb), r_u = c.result(fb), r_d = c.result(fb);
+    if ((s = c.begin()) != BORB_OK) return fail(s);
+    FrameJob* hj = c.host<FrameJob>(o_jobs);
     const float invW = (float)GRID_COLS / (float)(b4[2] - b4[0]), invH = (float)GRID_ROWS / (float)(b4[3] - b4[1]);
     for (int i = 0; i < n_frames; i++) {
         FrameJob& J = hj[i];
@@ -464,12 +492,12 @@ borb_status borb_frames_from_extractor(borb_matcher* m, borb_extractor* e, const
         J.src_desc = e->ws.desc + (size_t)img * g.sel_image_stride * 32;
         J.src_ur = mode == 1 ? e->ws.u_right + (size_t)(img / 2) * g.sel_image_stride : nullptr;
         J.src_depth = mode == 1 ? e->ws.depth + (size_t)(img / 2) * g.sel_image_stride : nullptr;
-        J.depth_img = mode == 2 ? (depth_on_device ? depth[i] : (const void*)(b + o_depth + (size_t)i * depth_img_bytes)) : nullptr;
+        J.depth_img = mode == 2 ? (depth_on_device ? depth[i] : (const void*)(c.dev(o_depth) + (size_t)i * depth_img_bytes)) : nullptr;
         J.keys = f->keys; J.desc = f->desc; J.u_right = f->ur_store; J.depth = f->depth_store;
         J.cell_start = f->cell_start; J.cell_idx = f->cell_idx;
         J.n = n_keys[i]; J.min_x = b4[0]; J.min_y = b4[1]; J.inv_w = invW; J.inv_h = invH;
     }
-    if ((s = commit(st, total)) != BORB_OK) return fail(s);
+    if ((s = c.commit()) != BORB_OK) return fail(s);
     cudaStream_t q = m->stream;
     // the extractor's results must be complete, and its next batch must not overwrite them while they are being read
     if (!m->ev_a) { BORB_CUDA(cudaEventCreateWithFlags(&m->ev_a, cudaEventDisableTiming)); BORB_CUDA(cudaEventCreateWithFlags(&m->ev_b, cudaEventDisableTiming)); }
@@ -477,28 +505,20 @@ borb_status borb_frames_from_extractor(borb_matcher* m, borb_extractor* e, const
     BORB_CUDA(cudaStreamWaitEvent(q, m->ev_a, 0));
     if (mode == 2 && !depth_on_device)
         for (int i = 0; i < n_frames; i++)
-            BORB_CUDA(cudaMemcpy2DAsync(b + o_depth + (size_t)i * depth_img_bytes, (size_t)w * px, depth[i], (size_t)depth_stride_bytes, (size_t)w * px, h,
+            BORB_CUDA(cudaMemcpy2DAsync(c.dev(o_depth) + (size_t)i * depth_img_bytes, (size_t)w * px, depth[i], (size_t)depth_stride_bytes, (size_t)w * px, h,
                                         cudaMemcpyHostToDevice, q));
-    for (int i = 0; i < n_frames; i++) BORB_CUDA(cudaMemcpyAsync(frames[i]->sf, b + o_sf, (size_t)nl * 4, cudaMemcpyDeviceToDevice, q));
-    m->launches += launch_frame_build((const FrameJob*)(b + o_jobs), n_frames, max_n, *cam, mode, depth_type, depth_factor, w, h, ocap,
-                                      keys_un ? (borb_keypoint*)(b + o_ko) : nullptr, (u_right || depth_out) ? (float*)(b + o_uo) : nullptr,
-                                      (float*)(b + o_do), q);
-    BORB_CUDA(cudaGetLastError());
+    for (int i = 0; i < n_frames; i++) BORB_CUDA(cudaMemcpyAsync(frames[i]->sf, c.dev(o_sf), (size_t)nl * 4, cudaMemcpyDeviceToDevice, q));
+    m->launches += launch_frame_build((const FrameJob*)c.dev(o_jobs), n_frames, max_n, *cam, mode, depth_type, depth_factor, w, h, ocap,
+                                      keys_un ? (borb_keypoint*)c.res(r_k, false) : nullptr, fb ? (float*)c.res(r_u, false) : nullptr,
+                                      (float*)c.res(r_d, false), q);
     for (int i = 0; i < n_frames; i++) BORB_CUDA(cudaEventRecord(frames[i]->ready, q));
     BORB_CUDA(cudaEventRecord(m->ev_b, q));
     BORB_CUDA(cudaStreamWaitEvent(e->stream, m->ev_b, 0));
-    uint8_t* ho = m->h_out;
-    const size_t kb = (size_t)n_frames * ocap * sizeof(borb_keypoint), fb = (size_t)n_frames * ocap * 4;
+    if ((s = c.finish()) != BORB_OK) return s;
     if (ocap > 0) {
-        if (keys_un) BORB_CUDA(cudaMemcpyAsync(ho, b + o_ko, kb, cudaMemcpyDeviceToHost, q));
-        if (u_right) BORB_CUDA(cudaMemcpyAsync(ho + kb, b + o_uo, fb, cudaMemcpyDeviceToHost, q));
-        if (depth_out) BORB_CUDA(cudaMemcpyAsync(ho + kb + fb, b + o_do, fb, cudaMemcpyDeviceToHost, q));
-    }
-    BORB_CUDA(cudaStreamSynchronize(q));
-    if (ocap > 0) {
-        if (keys_un) std::memcpy(keys_un, ho, kb);
-        if (u_right) std::memcpy(u_right, ho + kb, fb);
-        if (depth_out) std::memcpy(depth_out, ho + kb + fb, fb);
+        if (keys_un) std::memcpy(keys_un, c.out(r_k), kb);
+        if (u_right) std::memcpy(u_right, c.out(r_u), fb);
+        if (depth_out) std::memcpy(depth_out, c.out(r_d), fb);
     }
     return BORB_OK;
 }
@@ -528,129 +548,97 @@ borb_status check_mappoints(const borb_frame_view* F, const FrameInfo& I, const 
 
 struct MapPointsOff { FrameStage fs; size_t px, py, pxr, lvl, vc, md, val, obs, cand, cc; };
 
-MapPointsOff stage_mappoints(Stager& st, const borb_frame_view* F, const FrameInfo& I, const borb_mappoint_view* P) {
+MapPointsOff stage_mappoints(Call& c, const borb_frame_view* F, const FrameInfo& I, const borb_mappoint_view* P) {
     MapPointsOff o{};
     const size_t n = (size_t)P->n;
-    o.fs = stage_frame(st, F, I, true);
-    o.px = st.add(P->proj_x, n * 4); o.py = st.add(P->proj_y, n * 4); o.pxr = st.add(P->proj_xr, n * 4);
-    o.lvl = st.add(P->level, n * 4); o.vc = st.add(P->view_cos, n * 4); o.md = st.add(P->desc, n * 32);
-    o.val = P->valid ? st.add(P->valid, n) : 0;
-    o.obs = P->has_obs ? st.add(P->has_obs, n) : 0;
+    o.fs = stage_frame(c, F, I, true);
+    o.px = c.in(P->proj_x, n * 4); o.py = c.in(P->proj_y, n * 4); o.pxr = c.in(P->proj_xr, n * 4);
+    o.lvl = c.in(P->level, n * 4); o.vc = c.in(P->view_cos, n * 4); o.md = c.in(P->desc, n * 32);
+    o.val = P->valid ? c.in(P->valid, n) : 0;
+    o.obs = P->has_obs ? c.in(P->has_obs, n) : 0;
     return o;
 }
 // device-only scratch, laid out after every input
-void reserve_mappoints(Stager& st, const FrameInfo& I, const borb_mappoint_view* P, MapPointsOff& o) {
-    reserve_grid(st, I, o.fs);
-    o.cand = st.reserve((size_t)P->n * I.n * 4); o.cc = st.reserve((size_t)P->n * 4);
+void reserve_mappoints(Call& c, const FrameInfo& I, const borb_mappoint_view* P, MapPointsOff& o) {
+    reserve_grid(c, I, o.fs);
+    o.cand = c.scratch((size_t)P->n * I.n * 4); o.cc = c.scratch((size_t)P->n * 4);
 }
-// the map point side of A (the frame side comes from bind_frame / bind_resident).  in: where the kernels read the inputs,
-// b: the arena; out: P->n matches followed by the count
-void bind_mappoints(const MapPointsOff& o, const borb_mappoint_view* P, const uint8_t* in, uint8_t* b, float th, float nnratio, int32_t* out,
-                    ProjArgs& A) {
-    A.occupied = o.fs.occ_p ? in + o.fs.occ : nullptr;
-    A.n_mp = P->n; A.proj_x = (const float*)(in + o.px); A.proj_y = (const float*)(in + o.py); A.proj_xr = (const float*)(in + o.pxr);
-    A.view_cos = (const float*)(in + o.vc); A.level = (const int32_t*)(in + o.lvl); A.mp_desc = in + o.md;
-    A.mp_valid = P->valid ? in + o.val : nullptr; A.mp_has_obs = P->has_obs ? in + o.obs : nullptr;
+// the map point side of A (the frame side comes from bind_frame_fields); out: P->n matches followed by the count
+void bind_mappoints(const MapPointsOff& o, const borb_mappoint_view* P, const Call& c, float th, float nnratio, int32_t* out, ProjArgs& A) {
+    A.occupied = o.fs.occ_p ? c.dev(o.fs.occ) : nullptr;
+    A.n_mp = P->n; A.proj_x = (const float*)c.dev(o.px); A.proj_y = (const float*)c.dev(o.py); A.proj_xr = (const float*)c.dev(o.pxr);
+    A.view_cos = (const float*)c.dev(o.vc); A.level = (const int32_t*)c.dev(o.lvl); A.mp_desc = c.dev(o.md);
+    A.mp_valid = P->valid ? c.dev(o.val) : nullptr; A.mp_has_obs = P->has_obs ? c.dev(o.obs) : nullptr;
     A.th = th; A.nnratio = nnratio; A.th_dist = TH_HIGH;
-    A.cand = (uint32_t*)(b + o.cand); A.cand_cnt = (int*)(b + o.cc);
+    A.cand = (uint32_t*)c.dev(o.cand); A.cand_cnt = (int*)c.dev(o.cc);
     A.mode = 0;
     A.out_match = out;
+}
+
+// Shared body of borb_search_by_projection (one job, a host view or a resident frame) and borb_search_by_projection_batch (resident
+// frames).  The per-frame call is a few microseconds of kernel work behind ~20 us of launch + synchronisation, so independent camera
+// streams are batched the same way the extractor batches their images: one launch pair and one synchronisation for every job.
+borb_status projection_jobs(borb_matcher* m, const borb_frame_view* frames, const borb_mappoint_view* points, int n_jobs, float th,
+                            float nnratio, int32_t* const* match_feat, int32_t* n_matches, bool batch) {
+    struct Job { FrameInfo I; bool live; MapPointsOff o; size_t res; };
+    std::vector<Job> J(n_jobs);
+    int max_n = 1, max_n_mp = 0;
+    for (int j = 0; j < n_jobs; j++) {
+        const borb_mappoint_view* P = &points[j];
+        n_matches[j] = 0;
+        if (batch && !frames[j].resident) { set_error("job %d: borb_search_by_projection_batch needs device-resident frames (borb_frame_view::resident)", j); return BORB_ERR_INVALID_ARG; }
+        if (batch && !match_feat[j]) { set_error("job %d: null output", j); return BORB_ERR_INVALID_ARG; }
+        const FrameInfo I = J[j].I = frame_info(&frames[j]);
+        borb_status s = check_mappoints(&frames[j], I, P, m);
+        if (s != BORB_OK) return job_fail(batch, j, s);
+        J[j].live = P->n > 0 && I.n > 0;
+        if (!J[j].live) { std::fill_n(match_feat[j], P->n, -1); continue; }
+        max_n = std::max(max_n, I.n); max_n_mp = std::max(max_n_mp, P->n);
+    }
+    if (max_n_mp == 0) return BORB_OK;
+    Call c(m);
+    for (int j = 0; j < n_jobs; j++)
+        if (J[j].live) J[j].o = stage_mappoints(c, &frames[j], J[j].I, &points[j]);
+    JobTable<ProjArgs> jt(c, n_jobs);
+    for (int j = 0; j < n_jobs; j++) {
+        if (!J[j].live) continue;
+        reserve_mappoints(c, J[j].I, &points[j], J[j].o);
+        J[j].res = c.result((size_t)points[j].n * 4 + 4);
+    }
+    borb_status s;
+    if ((s = c.begin(n_jobs == 1 && J[0].I.rf)) != BORB_OK) return s;
+    const bool direct = c.in_place() || n_jobs > 1;      // results land in the pinned landing buffer (UVA): no D2H copy
+    ProjArgs* hj = jt.host(c);
+    for (int j = 0; j < n_jobs; j++) {
+        ProjArgs A{};
+        if (J[j].live) {
+            bind_frame_fields(J[j].I, J[j].o.fs, c, A);
+            bind_mappoints(J[j].o, &points[j], c, th, nnratio, (int32_t*)c.res(J[j].res, direct), A);
+        }                                                // a dead job keeps n_mp = 0: both kernels skip it
+        hj[j] = A;
+    }
+    if ((s = c.commit()) != BORB_OK) return s;
+    for (int j = 0; j < n_jobs; j++)
+        if (J[j].live && (s = prepare_frame(m, c, J[j].I, hj[j])) != BORB_OK) return s;
+    m->launches += launch_projection_batch(jt.dev(c), hj[0], n_jobs, max_n, max_n_mp, m->stream);
+    if ((s = c.finish()) != BORB_OK) return s;
+    for (int j = 0; j < n_jobs; j++)
+        if (J[j].live) read_counted(c.out(J[j].res), points[j].n, match_feat[j], &n_matches[j]);
+    return BORB_OK;
 }
 }  // namespace
 
 borb_status borb_search_by_projection(borb_matcher* m, const borb_frame_view* F, const borb_mappoint_view* P, float th, float nnratio,
                                       int32_t* match_feat, int32_t* n_matches) {
     if (!m || !F || !P || !match_feat || !n_matches) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
-    *n_matches = 0;
-    const FrameInfo I = frame_info(F);
-    borb_status s = check_mappoints(F, I, P, m);
-    if (s != BORB_OK) return s;
-    if (P->n == 0 || I.n == 0) { std::fill_n(match_feat, P->n, -1); return BORB_OK; }
-    BORB_CUDA(cudaSetDevice(m->device));
-    Stager st(m);
-    MapPointsOff o = stage_mappoints(st, F, I, P);
-    const size_t input_end = st.off;
-    reserve_mappoints(st, I, P, o);
-    const size_t res_bytes = (size_t)P->n * 4 + 4;
-    const size_t o_res = st.reserve(res_bytes);       // results contiguous: one D2H
-    const size_t total = st.off;
-    st.off = input_end;
-    if ((s = ensure_out(m, res_bytes)) != BORB_OK) return s;
-    if ((s = commit(st, total, I.rf != nullptr)) != BORB_OK) return s;
-    uint8_t* b = m->arena;
-    const bool direct = m->in_base != b;               // small call on a resident frame: the result is written straight into h_out too
-    ProjArgs A{};
-    if ((s = bind_frame(m, I, o.fs, A)) != BORB_OK) return s;
-    bind_mappoints(o, P, m->in_base, b, th, nnratio, (int32_t*)(direct ? m->h_out : b + o_res), A);
-    m->launches += launch_projection(A, m->stream);
-    BORB_CUDA(cudaGetLastError());
-    if (!direct) BORB_CUDA(cudaMemcpyAsync(m->h_out, b + o_res, res_bytes, cudaMemcpyDeviceToHost, m->stream));    // pinned landing buffer
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
-    read_counted(m->h_out, P->n, match_feat, n_matches);
-    return BORB_OK;
+    return projection_jobs(m, F, P, 1, th, nnratio, &match_feat, n_matches, false);
 }
 
-// SearchByProjection(F, vpMapPoints, th) for MANY independent (frame, MapPoint list) jobs in one launch pair: the per-frame call
-// is a few microseconds of kernel work behind ~20 us of launch + synchronisation, so independent camera streams are batched the
-// same way the extractor batches their images.  Frames must be device-resident (borb_frames_from_extractor / borb_frame_create).
+// Frames must be device-resident (borb_frames_from_extractor / borb_frame_create).
 borb_status borb_search_by_projection_batch(borb_matcher* m, const borb_frame_view* frames, const borb_mappoint_view* points, int n_jobs,
                                             float th, float nnratio, int32_t* const* match_feat, int32_t* n_matches) {
     if (!m || n_jobs < 0 || (n_jobs > 0 && (!frames || !points || !match_feat || !n_matches))) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
-    if (n_jobs == 0) return BORB_OK;
-    struct Job { FrameInfo I; bool live; MapPointsOff o; size_t out; };
-    std::vector<Job> J(n_jobs);
-    int max_n = 1, max_n_mp = 0;
-    for (int j = 0; j < n_jobs; j++) {
-        const borb_mappoint_view* P = &points[j];
-        n_matches[j] = 0;
-        if (!frames[j].resident) { set_error("job %d: borb_search_by_projection_batch needs device-resident frames (borb_frame_view::resident)", j); return BORB_ERR_INVALID_ARG; }
-        if (!match_feat[j]) { set_error("job %d: null output", j); return BORB_ERR_INVALID_ARG; }
-        const FrameInfo I = J[j].I = frame_info(&frames[j]);
-        borb_status s = check_mappoints(&frames[j], I, P, m);
-        if (s != BORB_OK) return job_error(j, s);
-        J[j].live = P->n > 0 && I.n > 0;
-        if (!J[j].live) { std::fill_n(match_feat[j], P->n, -1); continue; }
-        max_n = std::max(max_n, I.n); max_n_mp = std::max(max_n_mp, P->n);
-    }
-    if (max_n_mp == 0) return BORB_OK;
-    BORB_CUDA(cudaSetDevice(m->device));
-    Stager st(m);
-    for (int j = 0; j < n_jobs; j++)
-        if (J[j].live) J[j].o = stage_mappoints(st, &frames[j], J[j].I, &points[j]);
-    const size_t o_jobs = st.add(nullptr, (size_t)n_jobs * sizeof(ProjArgs));        // filled in place below
-    const size_t input_end = st.off;
-    size_t out_bytes = 0;
-    for (int j = 0; j < n_jobs; j++) {
-        if (!J[j].live) continue;
-        reserve_mappoints(st, J[j].I, &points[j], J[j].o);
-        J[j].out = out_bytes; out_bytes += ((size_t)points[j].n * 4 + 4 + 15) & ~size_t(15);
-    }
-    const size_t total = st.off;
-    st.off = input_end;
-    borb_status s;
-    if ((s = ensure_host(m, input_end)) != BORB_OK) return s;
-    if ((s = ensure_arena(m, total)) != BORB_OK) return s;
-    if ((s = ensure_out(m, out_bytes)) != BORB_OK) return s;
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
-    uint8_t* b = m->arena;
-    ProjArgs* hj = reinterpret_cast<ProjArgs*>(m->h_stage + o_jobs);
-    for (int j = 0; j < n_jobs; j++) {
-        ProjArgs A{};
-        if (J[j].live) {                                 // results land in pinned host memory directly (UVA)
-            bind_resident(frames[j].resident, A);
-            bind_mappoints(J[j].o, &points[j], b, b, th, nnratio, (int32_t*)(m->h_out + J[j].out), A);
-        }                                                // a dead job keeps n_mp = 0: both kernels skip it
-        hj[j] = A;
-    }
-    if ((s = commit(st, total)) != BORB_OK) return s;
-    for (int j = 0; j < n_jobs; j++)
-        if (J[j].live) BORB_CUDA(cudaStreamWaitEvent(m->stream, frames[j].resident->ready, 0));
-    m->launches += launch_projection_batch((const ProjArgs*)(b + o_jobs), n_jobs, max_n, max_n_mp, m->stream);
-    BORB_CUDA(cudaGetLastError());
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
-    for (int j = 0; j < n_jobs; j++)
-        if (J[j].live) read_counted(m->h_out + J[j].out, points[j].n, match_feat[j], &n_matches[j]);
-    return BORB_OK;
+    return projection_jobs(m, frames, points, n_jobs, th, nnratio, match_feat, n_matches, true);
 }
 
 // Shared body of the three SearchByProjection overloads that project world points with a pose:
@@ -704,65 +692,64 @@ borb_status check_query(const borb_frame_view* F, const FrameInfo& I, const Poin
 
 struct QueryOff { FrameStage fs; size_t lk, wp, md, vin, obs, mx, mn, nr, qa, is2, px, py, pxr, rad, ang, minl, maxl, val, cand, cc, evi, evb; };
 
-QueryOff stage_query(Stager& st, const borb_frame_view* F, const FrameInfo& I, const PointQuery& Q) {
+QueryOff stage_query(Call& c, const borb_frame_view* F, const FrameInfo& I, const PointQuery& Q) {
     QueryOff o{};
     const size_t nq = (size_t)Q.n;
-    o.fs = stage_frame(st, F, I, Q.variant == 0 || Q.chi2);
-    o.lk = Q.keys ? st.add(Q.keys, nq * sizeof(borb_keypoint)) : 0;
-    o.wp = st.add(Q.world_pos, nq * 12);
-    o.md = st.add(Q.desc, nq * 32);
-    o.vin = Q.valid ? st.add(Q.valid, nq) : 0;
-    o.obs = Q.has_obs ? st.add(Q.has_obs, nq) : 0;
-    o.mx = Q.max_distance ? st.add(Q.max_distance, nq * 4) : 0;
-    o.mn = Q.min_distance ? st.add(Q.min_distance, nq * 4) : 0;
-    o.nr = Q.normal ? st.add(Q.normal, nq * 12) : 0;
-    o.qa = Q.angle ? st.add(Q.angle, nq * 4) : 0;
-    o.is2 = Q.chi2 ? st.add(Q.inv_sigma2, (size_t)I.n_levels * 4) : 0;
+    o.fs = stage_frame(c, F, I, Q.variant == 0 || Q.chi2);
+    o.lk = Q.keys ? c.in(Q.keys, nq * sizeof(borb_keypoint)) : 0;
+    o.wp = c.in(Q.world_pos, nq * 12);
+    o.md = c.in(Q.desc, nq * 32);
+    o.vin = Q.valid ? c.in(Q.valid, nq) : 0;
+    o.obs = Q.has_obs ? c.in(Q.has_obs, nq) : 0;
+    o.mx = Q.max_distance ? c.in(Q.max_distance, nq * 4) : 0;
+    o.mn = Q.min_distance ? c.in(Q.min_distance, nq * 4) : 0;
+    o.nr = Q.normal ? c.in(Q.normal, nq * 12) : 0;
+    o.qa = Q.angle ? c.in(Q.angle, nq * 4) : 0;
+    o.is2 = Q.chi2 ? c.in(Q.inv_sigma2, (size_t)I.n_levels * 4) : 0;
     return o;
 }
 // device-only scratch of project_points (and the grid of a host view), laid out after every input
-void reserve_projection(Stager& st, const FrameInfo& I, const PointQuery& Q, QueryOff& o) {
+void reserve_projection(Call& c, const FrameInfo& I, const PointQuery& Q, QueryOff& o) {
     const size_t nq = (size_t)Q.n;
-    reserve_grid(st, I, o.fs);
-    o.px = st.reserve(nq * 4); o.py = st.reserve(nq * 4); o.pxr = st.reserve(nq * 4); o.rad = st.reserve(nq * 4);
-    o.ang = st.reserve(nq * 4); o.minl = st.reserve(nq * 4); o.maxl = st.reserve(nq * 4); o.val = st.reserve(nq);
+    reserve_grid(c, I, o.fs);
+    o.px = c.scratch(nq * 4); o.py = c.scratch(nq * 4); o.pxr = c.scratch(nq * 4); o.rad = c.scratch(nq * 4);
+    o.ang = c.scratch(nq * 4); o.minl = c.scratch(nq * 4); o.maxl = c.scratch(nq * 4); o.val = c.scratch(nq);
 }
 // the same plus the candidate lists and the match events of the resolve / argmin kernels
-void reserve_query(Stager& st, const FrameInfo& I, const PointQuery& Q, QueryOff& o) {
+void reserve_query(Call& c, const FrameInfo& I, const PointQuery& Q, QueryOff& o) {
     const size_t nq = (size_t)Q.n;
-    reserve_projection(st, I, Q, o);
-    o.cand = st.reserve(nq * I.n * 4); o.cc = st.reserve(nq * 4);
-    o.evi = st.reserve(nq * 4); o.evb = st.reserve(nq);
+    reserve_projection(c, I, Q, o);
+    o.cand = c.scratch(nq * I.n * 4); o.cc = c.scratch(nq * 4);
+    o.evi = c.scratch(nq * 4); o.evb = c.scratch(nq);
 }
-// L and the query side of A (the frame side comes from bind_frame / bind_resident).  in: where the kernels read the inputs,
-// b: the arena; out: the state (argmin: Q.n entries, otherwise I.n) followed by the match count
-void bind_query(const QueryOff& o, const PointQuery& Q, const FrameInfo& I, const uint8_t* in, uint8_t* b, int32_t* out, LastArgs& L,
-                ProjArgs& A) {
+// L and the query side of A (the frame side comes from bind_frame_fields); out: the state (argmin: Q.n entries, otherwise I.n)
+// followed by the match count
+void bind_query(const QueryOff& o, const PointQuery& Q, const FrameInfo& I, const Call& c, int32_t* out, LastArgs& L, ProjArgs& A) {
     L.variant = Q.variant;
-    L.n_last = Q.n; L.last_keys = Q.keys ? (const borb_keypoint*)(in + o.lk) : nullptr; L.world_pos = (const float*)(in + o.wp);
-    L.q_angle_in = Q.angle ? (const float*)(in + o.qa) : nullptr;
-    L.max_distance = Q.max_distance ? (const float*)(in + o.mx) : nullptr;
-    L.min_distance = Q.min_distance ? (const float*)(in + o.mn) : nullptr;
-    L.normal = Q.normal ? (const float*)(in + o.nr) : nullptr;
+    L.n_last = Q.n; L.last_keys = Q.keys ? (const borb_keypoint*)c.dev(o.lk) : nullptr; L.world_pos = (const float*)c.dev(o.wp);
+    L.q_angle_in = Q.angle ? (const float*)c.dev(o.qa) : nullptr;
+    L.max_distance = Q.max_distance ? (const float*)c.dev(o.mx) : nullptr;
+    L.min_distance = Q.min_distance ? (const float*)c.dev(o.mn) : nullptr;
+    L.normal = Q.normal ? (const float*)c.dev(o.nr) : nullptr;
     for (int i = 0; i < 3; i++) L.Ow[i] = Q.Ow ? Q.Ow[i] : 0.f;
     L.log_scale = Q.log_scale; L.n_levels = I.n_levels;
     L.invz_double = Q.invz_double; L.use_normal = Q.use_normal; L.chain = Q.chain;
     for (int i = 0; i < 12; i++) L.T2[i] = Q.chain ? Q.T2[i] : 0.f;
-    L.valid_in = Q.valid ? in + o.vin : nullptr;
+    L.valid_in = Q.valid ? c.dev(o.vin) : nullptr;
     for (int i = 0; i < 12; i++) L.T[i] = Q.Tcw[i];
     L.fx = Q.fx; L.fy = Q.fy; L.cx = Q.cx; L.cy = Q.cy; L.bf = Q.bf; L.th = Q.th;
     L.minX = I.min_x; L.minY = I.min_y; L.maxX = I.max_x; L.maxY = I.max_y;
     L.scale_factors = A.scale_factors;
     L.forward = Q.forward; L.backward = Q.backward;
-    L.proj_x = (float*)(b + o.px); L.proj_y = (float*)(b + o.py); L.proj_xr = (float*)(b + o.pxr); L.radius = (float*)(b + o.rad);
-    L.angle = (float*)(b + o.ang); L.minl = (int32_t*)(b + o.minl); L.maxl = (int32_t*)(b + o.maxl); L.valid_out = b + o.val;
-    A.occupied = o.fs.occ_p ? in + o.fs.occ : nullptr;
+    L.proj_x = (float*)c.dev(o.px); L.proj_y = (float*)c.dev(o.py); L.proj_xr = (float*)c.dev(o.pxr); L.radius = (float*)c.dev(o.rad);
+    L.angle = (float*)c.dev(o.ang); L.minl = (int32_t*)c.dev(o.minl); L.maxl = (int32_t*)c.dev(o.maxl); L.valid_out = c.dev(o.val);
+    A.occupied = o.fs.occ_p ? c.dev(o.fs.occ) : nullptr;
     wire_projection(L, A);
-    A.mp_desc = in + o.md; A.mp_has_obs = Q.has_obs ? in + o.obs : nullptr;
+    A.mp_desc = c.dev(o.md); A.mp_has_obs = Q.has_obs ? c.dev(o.obs) : nullptr;
     A.th = Q.th; A.nnratio = 0.f;
-    A.cand = (uint32_t*)(b + o.cand); A.cand_cnt = (int*)(b + o.cc);
+    A.cand = (uint32_t*)c.dev(o.cand); A.cand_cnt = (int*)c.dev(o.cc);
     A.mode = 1; A.check_ori = Q.check_ori; A.th_dist = Q.th_dist;
-    A.out_match = out; A.ev_idx = (int32_t*)(b + o.evi); A.ev_bin = b + o.evb;
+    A.out_match = out; A.ev_idx = (int32_t*)c.dev(o.evi); A.ev_bin = c.dev(o.evb);
 }
 // SearchByProjection(CurrentFrame, LastFrame) of one camera stream
 PointQuery last_frame_query(const borb_last_frame_job& B, int check_orientation) {
@@ -773,50 +760,76 @@ PointQuery last_frame_query(const borb_last_frame_job& B, int check_orientation)
     Q.check_ori = check_orientation; Q.th_dist = TH_HIGH;                  // (:1426)
     return Q;
 }
-}  // namespace
 
-static borb_status run_point_projection(borb_matcher* m, const borb_frame_view* F, const PointQuery& Q, int32_t* state, int32_t* n_matches) {
-    *n_matches = 0;
-    const FrameInfo I = frame_info(F);
-    borb_status s = check_query(F, I, Q, m);
-    if (s != BORB_OK) return s;
-    const int n_out = Q.argmin ? Q.n : I.n;
-    if (state) std::fill_n(state, n_out, -1);
-    if (Q.to_aux) {                 // caller sized m->aux; "no match" everywhere until the kernels say otherwise
-        BORB_CUDA(cudaSetDevice(m->device));
-        if (Q.n > 0) BORB_CUDA(cudaMemsetAsync(m->aux + Q.aux_off, 0xFF, (size_t)Q.n * 4, m->stream));
+// one (frame, query) pair of point_query_jobs; state: the job's output (argmin: Q.n entries, otherwise the frame's n), or null (to_aux)
+struct PointJob { const borb_frame_view* F; PointQuery Q; int32_t* state; };
+
+// Shared body of borb_search_by_projection_last / _kf / _sim3, of the two directions of borb_search_by_sim3 (argmin, to_aux: one job
+// only) and of borb_search_by_projection_last_batch (resident frames): project_points, candidates and resolve<true> (or argmin),
+// one synchronisation.  The state stays in the arena, not in mapped host memory: resolve<true> writes it with atomicMax.
+borb_status point_query_jobs(borb_matcher* m, const PointJob* jobs, int n_jobs, int32_t* n_matches, bool batch) {
+    struct Job { FrameInfo I; bool live; QueryOff o; size_t res; };
+    std::vector<Job> J(n_jobs);
+    int max_n = 1, max_nq = 0;
+    for (int j = 0; j < n_jobs; j++) {
+        const PointQuery& Q = jobs[j].Q;
+        assert(n_jobs == 1 || (!Q.argmin && !Q.to_aux));
+        n_matches[j] = 0;
+        if (batch && !jobs[j].F->resident) { set_error("job %d: borb_search_by_projection_last_batch needs device-resident frames (borb_frame_view::resident)", j); return BORB_ERR_INVALID_ARG; }
+        if (batch && !jobs[j].state) { set_error("job %d: null output", j); return BORB_ERR_INVALID_ARG; }
+        const FrameInfo I = J[j].I = frame_info(jobs[j].F);
+        borb_status s = check_query(jobs[j].F, I, Q, m);
+        if (s != BORB_OK) return job_fail(batch, j, s);
+        if (jobs[j].state) std::fill_n(jobs[j].state, Q.argmin ? Q.n : I.n, -1);
+        if (Q.to_aux && Q.n > 0) {      // caller sized m->aux; "no match" everywhere until the kernels say otherwise
+            BORB_CUDA(cudaSetDevice(m->device));
+            BORB_CUDA(cudaMemsetAsync(m->aux + Q.aux_off, 0xFF, (size_t)Q.n * 4, m->stream));
+        }
+        J[j].live = I.n > 0 && Q.n > 0;
+        if (J[j].live) { max_n = std::max(max_n, I.n); max_nq = std::max(max_nq, Q.n); }
     }
-    if (I.n == 0 || Q.n == 0) return BORB_OK;
-    BORB_CUDA(cudaSetDevice(m->device));
-    Stager st(m);
-    QueryOff o = stage_query(st, F, I, Q);
-    const size_t input_end = st.off;
-    reserve_query(st, I, Q, o);
-    const size_t res_bytes = (size_t)n_out * 4 + 4;
-    const size_t o_res = st.reserve(res_bytes);       // results contiguous: one D2H
-    const size_t total = st.off;
-    st.off = input_end;
-    if ((s = ensure_out(m, res_bytes)) != BORB_OK) return s;
-    if ((s = commit(st, total, I.rf != nullptr)) != BORB_OK) return s;
-    uint8_t* b = m->arena;
-    ProjArgs A{};
-    LastArgs L{};
-    if ((s = bind_frame(m, I, o.fs, A)) != BORB_OK) return s;
-    bind_query(o, Q, I, m->in_base, b, (int32_t*)(b + o_res), L, A);
-    m->launches += Q.argmin ? launch_projection_argmin(L, A, m->stream) : launch_projection_last(L, A, m->stream);
-    BORB_CUDA(cudaGetLastError());
-    if (Q.to_aux) {
-        BORB_CUDA(cudaMemcpyAsync(m->aux + Q.aux_off, b + o_res, (size_t)n_out * 4, cudaMemcpyDeviceToDevice, m->stream));
-        BORB_CUDA(cudaMemcpyAsync(m->h_out, b + o_res + (size_t)n_out * 4, 4, cudaMemcpyDeviceToHost, m->stream));
-        BORB_CUDA(cudaStreamSynchronize(m->stream));
-        std::memcpy(n_matches, m->h_out, 4);
-        return BORB_OK;
+    if (max_nq == 0) return BORB_OK;
+    Call c(m);
+    for (int j = 0; j < n_jobs; j++)
+        if (J[j].live) J[j].o = stage_query(c, jobs[j].F, J[j].I, jobs[j].Q);
+    JobTable<LastArgs> lt(c, n_jobs);
+    JobTable<ProjArgs> jt(c, n_jobs);
+    for (int j = 0; j < n_jobs; j++) {
+        if (!J[j].live) continue;
+        const PointQuery& Q = jobs[j].Q;
+        reserve_query(c, J[j].I, Q, J[j].o);
+        const size_t bytes = (size_t)(Q.argmin ? Q.n : J[j].I.n) * 4 + 4;
+        J[j].res = Q.to_aux ? c.scratch(bytes) : c.result(bytes);
     }
-    BORB_CUDA(cudaMemcpyAsync(m->h_out, b + o_res, res_bytes, cudaMemcpyDeviceToHost, m->stream));
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
-    read_counted(m->h_out, n_out, state, n_matches);
+    borb_status s;
+    if ((s = c.begin(n_jobs == 1 && J[0].I.rf)) != BORB_OK) return s;
+    LastArgs* hl = lt.host(c);
+    ProjArgs* hj = jt.host(c);
+    for (int j = 0; j < n_jobs; j++) {
+        LastArgs L{};
+        ProjArgs A{};
+        if (J[j].live) {
+            const PointQuery& Q = jobs[j].Q;
+            bind_frame_fields(J[j].I, J[j].o.fs, c, A);
+            bind_query(J[j].o, Q, J[j].I, c, (int32_t*)(Q.to_aux ? c.dev(J[j].res) : c.res(J[j].res, false)), L, A);
+        }                                            // a job without work keeps n_last = n_mp = 0: every kernel skips it
+        hl[j] = L;
+        hj[j] = A;
+    }
+    if ((s = c.commit()) != BORB_OK) return s;
+    for (int j = 0; j < n_jobs; j++)
+        if (J[j].live && (s = prepare_frame(m, c, J[j].I, hj[j])) != BORB_OK) return s;
+    const PointQuery& Q0 = jobs[0].Q;
+    if (Q0.argmin) m->launches += launch_projection_argmin(hl[0], hj[0], m->stream);
+    else m->launches += launch_point_projection_batch(lt.dev(c), jt.dev(c), hl[0], hj[0], n_jobs, max_nq, max_n, max_nq, true, m->stream);
+    if (Q0.to_aux) BORB_CUDA(cudaMemcpyAsync(m->aux + Q0.aux_off, c.dev(J[0].res), (size_t)Q0.n * 4, cudaMemcpyDeviceToDevice, m->stream));
+    if ((s = c.finish()) != BORB_OK) return s;
+    for (int j = 0; j < n_jobs; j++)
+        if (J[j].live && !jobs[j].Q.to_aux)
+            read_counted(c.out(J[j].res), jobs[j].Q.argmin ? jobs[j].Q.n : J[j].I.n, jobs[j].state, &n_matches[j]);
     return BORB_OK;
 }
+}  // namespace
 
 borb_status borb_search_by_projection_last(borb_matcher* m, const borb_frame_view* F, const borb_lastframe_view* Lf, const float* Tcw,
                                            float fx, float fy, float cx, float cy, float bf, float th, int forward, int backward,
@@ -826,7 +839,8 @@ borb_status borb_search_by_projection_last(borb_matcher* m, const borb_frame_vie
     B.last = *Lf;
     std::memcpy(B.Tcw, Tcw, sizeof(B.Tcw));
     B.fx = fx; B.fy = fy; B.cx = cx; B.cy = cy; B.bf = bf; B.th = th; B.forward = forward; B.backward = backward;
-    return run_point_projection(m, F, last_frame_query(B, check_orientation), state_cur, n_matches);
+    const PointJob P{F, last_frame_query(B, check_orientation), state_cur};
+    return point_query_jobs(m, &P, 1, n_matches, false);
 }
 
 borb_status borb_search_by_projection_kf(borb_matcher* m, const borb_frame_view* cur, const borb_worldpoints_view* pts, const float* Tcw,
@@ -838,7 +852,8 @@ borb_status borb_search_by_projection_kf(borb_matcher* m, const borb_frame_view*
     Q.max_distance = pts->max_distance; Q.min_distance = pts->min_distance; Q.angle = pts->angle;
     Q.Tcw = Tcw; Q.Ow = Ow; Q.fx = fx; Q.fy = fy; Q.cx = cx; Q.cy = cy; Q.th = th; Q.log_scale = log_scale_factor;
     Q.check_ori = check_orientation; Q.th_dist = orb_dist;
-    return run_point_projection(m, cur, Q, state_cur, n_matches);
+    const PointJob P{cur, Q, state_cur};
+    return point_query_jobs(m, &P, 1, n_matches, false);
 }
 
 borb_status borb_search_by_projection_sim3(borb_matcher* m, const borb_frame_view* kf, const borb_worldpoints_view* pts, const float* Tcw,
@@ -851,7 +866,16 @@ borb_status borb_search_by_projection_sim3(borb_matcher* m, const borb_frame_vie
     Q.Tcw = Tcw; Q.Ow = Ow; Q.fx = fx; Q.fy = fy; Q.cx = cx; Q.cy = cy; Q.th = (float)th; Q.log_scale = log_scale_factor;
     Q.check_ori = 0; Q.th_dist = 50;                                       // TH_LOW (:394)
     Q.use_normal = 1;
-    return run_point_projection(m, kf, Q, state_kf, n_matches);
+    const PointJob P{kf, Q, state_kf};
+    return point_query_jobs(m, &P, 1, n_matches, false);
+}
+
+borb_status borb_search_by_projection_last_batch(borb_matcher* m, const borb_last_frame_job* jobs, int n_jobs, int check_orientation,
+                                                 int32_t* n_matches) {
+    if (!m || n_jobs < 0 || (n_jobs > 0 && (!jobs || !n_matches))) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+    std::vector<PointJob> P(n_jobs);
+    for (int j = 0; j < n_jobs; j++) P[j] = PointJob{&jobs[j].cur, last_frame_query(jobs[j], check_orientation), jobs[j].state_cur};
+    return point_query_jobs(m, P.data(), n_jobs, n_matches, true);
 }
 
 // ---- the search part of Fuse: borb_fuse is the one-job case of borb_fuse_batch (project_points + fuse_batch_kernel, one
@@ -884,53 +908,41 @@ borb_status fuse_jobs(borb_matcher* m, const borb_fuse_job* jobs, int n_jobs, bo
         if (J[j].live) max_nq = std::max(max_nq, Q.n);
     }
     if (max_nq == 0) return BORB_OK;
-    BORB_CUDA(cudaSetDevice(m->device));
-    Stager st(m);
+    Call c(m);
     for (int j = 0; j < n_jobs; j++)
-        if (J[j].live) J[j].o = stage_query(st, &J[j].kf, J[j].I, J[j].Q);
-    const size_t o_last = st.add(nullptr, (size_t)n_jobs * sizeof(LastArgs)), o_jobs = st.add(nullptr, (size_t)n_jobs * sizeof(FuseJob));
-    const size_t input_end = st.off;
-    const size_t cnt_bytes = ((size_t)n_jobs * 4 + 15) & ~size_t(15);
-    size_t res_bytes = cnt_bytes;                // n_found of every job, then every job's best_idx: one D2H
+        if (J[j].live) J[j].o = stage_query(c, &J[j].kf, J[j].I, J[j].Q);
+    const size_t o_last = c.in(nullptr, (size_t)n_jobs * sizeof(LastArgs)), o_jobs = c.in(nullptr, (size_t)n_jobs * sizeof(FuseJob));
+    const size_t r_cnt = c.result((size_t)n_jobs * 4);     // n_found of every job, then every job's best_idx
     for (int j = 0; j < n_jobs; j++) {
         if (!J[j].live) continue;
-        reserve_projection(st, J[j].I, J[j].Q, J[j].o);
-        J[j].res = res_bytes; res_bytes += ((size_t)J[j].Q.n * 4 + 15) & ~size_t(15);
+        reserve_projection(c, J[j].I, J[j].Q, J[j].o);
+        J[j].res = c.result((size_t)J[j].Q.n * 4);
     }
-    const size_t o_res = st.reserve(res_bytes);
-    const size_t total = st.off;
-    st.off = input_end;
     borb_status s;
-    if ((s = ensure_host(m, input_end)) != BORB_OK) return s;
-    if ((s = ensure_arena(m, total)) != BORB_OK) return s;
-    if ((s = ensure_out(m, res_bytes)) != BORB_OK) return s;
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
-    uint8_t* b = m->arena;
-    LastArgs* hl = reinterpret_cast<LastArgs*>(m->h_stage + o_last);
-    FuseJob* hj = reinterpret_cast<FuseJob*>(m->h_stage + o_jobs);
+    if ((s = c.begin()) != BORB_OK) return s;
+    LastArgs* hl = c.host<LastArgs>(o_last);
+    FuseJob* hj = c.host<FuseJob>(o_jobs);
     for (int j = 0; j < n_jobs; j++) {
         LastArgs L{};
         FuseJob F{};
         if (J[j].live) {
-            bind_frame_fields(J[j].I, J[j].o.fs, b, F.A);
-            bind_query(J[j].o, J[j].Q, J[j].I, b, b, (int32_t*)(b + o_res + J[j].res), L, F.A);
-            F.inv_sigma2 = J[j].Q.chi2 ? (const float*)(b + J[j].o.is2) : nullptr;
-            F.n_found = (int*)(b + o_res) + j;
+            bind_frame_fields(J[j].I, J[j].o.fs, c, F.A);
+            bind_query(J[j].o, J[j].Q, J[j].I, c, (int32_t*)c.res(J[j].res, false), L, F.A);
+            F.inv_sigma2 = J[j].Q.chi2 ? (const float*)c.dev(J[j].o.is2) : nullptr;
+            F.n_found = (int*)c.res(r_cnt, false) + j;
         }                                            // a job without work keeps n_last = n_mp = 0: both kernels skip it
         hl[j] = L;
         hj[j] = F;
     }
-    if ((s = commit(st, total)) != BORB_OK) return s;
-    BORB_CUDA(cudaMemsetAsync(b + o_res, 0, cnt_bytes, m->stream));
+    if ((s = c.commit()) != BORB_OK) return s;
+    BORB_CUDA(cudaMemsetAsync(c.res(r_cnt, false), 0, (size_t)n_jobs * 4, m->stream));
     for (int j = 0; j < n_jobs; j++)
-        if (J[j].live && (s = prepare_frame(m, J[j].I, hj[j].A)) != BORB_OK) return s;
-    m->launches += launch_fuse_batch((const LastArgs*)(b + o_last), (const FuseJob*)(b + o_jobs), n_jobs, max_nq, m->stream);
-    BORB_CUDA(cudaGetLastError());
-    BORB_CUDA(cudaMemcpyAsync(m->h_out, b + o_res, res_bytes, cudaMemcpyDeviceToHost, m->stream));
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
+        if (J[j].live && (s = prepare_frame(m, c, J[j].I, hj[j].A)) != BORB_OK) return s;
+    m->launches += launch_fuse_batch((const LastArgs*)c.dev(o_last), (const FuseJob*)c.dev(o_jobs), n_jobs, max_nq, m->stream);
+    if ((s = c.finish()) != BORB_OK) return s;
     for (int j = 0; j < n_jobs; j++) {
-        std::memcpy(&n_found[j], m->h_out + (size_t)j * 4, 4);
-        if (J[j].live) std::memcpy(jobs[j].best_idx, m->h_out + J[j].res, (size_t)J[j].Q.n * 4);
+        std::memcpy(&n_found[j], c.out(r_cnt) + (size_t)j * 4, 4);
+        if (J[j].live) std::memcpy(jobs[j].best_idx, c.out(J[j].res), (size_t)J[j].Q.n * 4);
     }
     return BORB_OK;
 }
@@ -983,27 +995,25 @@ borb_status borb_search_by_sim3(borb_matcher* m, const borb_frame_view* kf1, con
     Q.max_distance = pts1->max_distance; Q.min_distance = pts1->min_distance;
     Q.Tcw = T1w; Q.chain = 1; Q.T2 = S21; Q.fx = fx; Q.fy = fy; Q.cx = cx; Q.cy = cy; Q.th = th; Q.log_scale = log_scale_factor2;
     Q.th_dist = 100; Q.argmin = 1; Q.invz_double = 1; Q.to_aux = 1; Q.aux_off = 0;        // TH_HIGH (:1218)
-    borb_status s = run_point_projection(m, &F2, Q, nullptr, &nm);
+    const PointJob P{&F2, Q, nullptr};
+    borb_status s = point_query_jobs(m, &P, 1, &nm, false);
     if (s != BORB_OK) return s;
     PointQuery R{};
     R.variant = 2; R.n = pts2->n; R.world_pos = pts2->world_pos; R.desc = pts2->desc; R.valid = pts2->valid;
     R.max_distance = pts2->max_distance; R.min_distance = pts2->min_distance;
     R.Tcw = T2w; R.chain = 1; R.T2 = S12; R.fx = fx; R.fy = fy; R.cx = cx; R.cy = cy; R.th = th; R.log_scale = log_scale_factor1;
     R.th_dist = 100; R.argmin = 1; R.invz_double = 1; R.to_aux = 1; R.aux_off = (size_t)n1;
-    s = run_point_projection(m, &F1, R, nullptr, &nm);
+    const PointJob PR{&F1, R, nullptr};
+    s = point_query_jobs(m, &PR, 1, &nm, false);
     if (s != BORB_OK) return s;
     // agreement test (:1302-1323) on the device
-    Stager st(m);
-    const size_t o_out = st.reserve((size_t)n1 * 4), o_nf = st.reserve(16);
-    const size_t total = st.off;
-    st.off = 0;
-    if ((s = commit(st, total)) != BORB_OK) return s;
-    uint8_t* b = m->arena;
-    m->launches += launch_sim3_agree(m->aux, m->aux + n1, n1, n2, (int32_t*)(b + o_out), (int*)(b + o_nf), m->stream);
-    BORB_CUDA(cudaGetLastError());
-    BORB_CUDA(cudaMemcpyAsync(match12, b + o_out, (size_t)n1 * 4, cudaMemcpyDeviceToHost, m->stream));
-    BORB_CUDA(cudaMemcpyAsync(n_found, b + o_nf, 4, cudaMemcpyDeviceToHost, m->stream));
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
+    Call c(m);
+    const size_t r_out = c.result((size_t)n1 * 4), r_nf = c.result(4);
+    if ((s = c.begin()) != BORB_OK) return s;
+    m->launches += launch_sim3_agree(m->aux, m->aux + n1, n1, n2, (int32_t*)c.res(r_out, false), (int*)c.res(r_nf, false), m->stream);
+    if ((s = c.finish()) != BORB_OK) return s;
+    std::memcpy(match12, c.out(r_out), (size_t)n1 * 4);
+    std::memcpy(n_found, c.out(r_nf), 4);
     return BORB_OK;
 }
 
@@ -1046,23 +1056,24 @@ borb_status select_local(const borb_local_points_job& B, std::vector<int32_t>& s
     return BORB_OK;
 }
 // gathered inputs are written straight into the pinned staging buffer once the layout is known (src = nullptr): gather_local
-void stage_local(Stager& st, const borb_local_points_job& B, const FrameInfo& I, LocalOff& o) {
+void stage_local(Call& c, const borb_local_points_job& B, const FrameInfo& I, LocalOff& o) {
     const borb_worldpoints_view& P = B.pts;
     const size_t nq = (size_t)o.nq;
     const bool g = o.gather;
-    o.fs = stage_frame(st, &B.frame, I, true);
-    o.wp = st.add(g ? nullptr : P.world_pos, nq * 12); o.md = st.add(g ? nullptr : P.desc, nq * 32);
-    o.obs = B.has_obs ? st.add(g ? nullptr : B.has_obs, nq) : 0;
-    o.mx = st.add(g ? nullptr : P.max_distance, nq * 4); o.mn = st.add(g ? nullptr : P.min_distance, nq * 4);
-    o.nr = st.add(g ? nullptr : P.normal, nq * 12);
+    o.fs = stage_frame(c, &B.frame, I, true);
+    o.wp = c.in(g ? nullptr : P.world_pos, nq * 12); o.md = c.in(g ? nullptr : P.desc, nq * 32);
+    o.obs = B.has_obs ? c.in(g ? nullptr : B.has_obs, nq) : 0;
+    o.mx = c.in(g ? nullptr : P.max_distance, nq * 4); o.mn = c.in(g ? nullptr : P.min_distance, nq * 4);
+    o.nr = c.in(g ? nullptr : P.normal, nq * 12);
 }
 // device-only scratch, laid out after every input
-void reserve_local(Stager& st, const FrameInfo& I, LocalOff& o) {
+void reserve_local(Call& c, const FrameInfo& I, LocalOff& o) {
     const size_t nq = (size_t)o.nq;
-    reserve_grid(st, I, o.fs);
-    o.rad = st.reserve(nq * 4); o.ang = st.reserve(nq * 4); o.minl = st.reserve(nq * 4); o.maxl = st.reserve(nq * 4);
-    o.cand = st.reserve(nq * std::max(I.n, 1) * 4); o.cc = st.reserve(nq * 4);
+    reserve_grid(c, I, o.fs);
+    o.rad = c.scratch(nq * 4); o.ang = c.scratch(nq * 4); o.minl = c.scratch(nq * 4); o.maxl = c.scratch(nq * 4);
+    o.cand = c.scratch(nq * std::max(I.n, 1) * 4); o.cc = c.scratch(nq * 4);
 }
+// h: the staging buffer
 void gather_local(uint8_t* h, const LocalOff& o, const borb_local_points_job& B, const std::vector<int32_t>& sel) {
     const borb_worldpoints_view& P = B.pts;
     for (int k = 0; k < o.nq; k++) {
@@ -1077,13 +1088,13 @@ void gather_local(uint8_t* h, const LocalOff& o, const borb_local_points_job& B,
 }
 // the results of a job, contiguous so that ONE device-to-host copy brings them back: px | py | pxr | level | viewcos | match | nm | valid
 size_t local_res_bytes(int nq) { return (size_t)nq * 25 + 16; }
-// L and the point side of A (the frame side comes from bind_frame / bind_resident).  in: where the kernels read the inputs,
-// b: the arena, r: the job's result block (zeroed: level | viewcos of points outside the frustum read as 0)
-void bind_local(const LocalOff& o, const borb_local_points_job& B, const FrameInfo& I, float viewing_cos_limit, float nnratio, const uint8_t* in,
-                uint8_t* b, uint8_t* r, LastArgs& L, ProjArgs& A) {
+// L and the point side of A (the frame side comes from bind_frame_fields).  r: the job's result block (zeroed: level | viewcos of
+// points outside the frustum read as 0)
+void bind_local(const LocalOff& o, const borb_local_points_job& B, const FrameInfo& I, float viewing_cos_limit, float nnratio, const Call& c,
+                uint8_t* r, LastArgs& L, ProjArgs& A) {
     const int nq = o.nq;
-    L.variant = 3; L.n_last = nq; L.world_pos = (const float*)(in + o.wp);
-    L.max_distance = (const float*)(in + o.mx); L.min_distance = (const float*)(in + o.mn); L.normal = (const float*)(in + o.nr);
+    L.variant = 3; L.n_last = nq; L.world_pos = (const float*)c.dev(o.wp);
+    L.max_distance = (const float*)c.dev(o.mx); L.min_distance = (const float*)c.dev(o.mn); L.normal = (const float*)c.dev(o.nr);
     for (int i = 0; i < 3; i++) L.Ow[i] = B.Ow[i];
     L.log_scale = B.log_scale_factor; L.n_levels = I.n_levels; L.view_cos_limit = viewing_cos_limit;
     L.valid_in = nullptr;
@@ -1094,12 +1105,12 @@ void bind_local(const LocalOff& o, const borb_local_points_job& B, const FrameIn
     L.proj_x = (float*)r; L.proj_y = L.proj_x + nq; L.proj_xr = L.proj_y + nq;
     L.level_out = (int32_t*)(L.proj_xr + nq); L.viewcos_out = (float*)(L.level_out + nq);
     L.valid_out = r + (size_t)nq * 24 + 16;
-    L.radius = (float*)(b + o.rad); L.angle = (float*)(b + o.ang); L.minl = (int32_t*)(b + o.minl); L.maxl = (int32_t*)(b + o.maxl);
-    A.occupied = o.fs.occ_p ? in + o.fs.occ : nullptr;
+    L.radius = (float*)c.dev(o.rad); L.angle = (float*)c.dev(o.ang); L.minl = (int32_t*)c.dev(o.minl); L.maxl = (int32_t*)c.dev(o.maxl);
+    A.occupied = o.fs.occ_p ? c.dev(o.fs.occ) : nullptr;
     wire_projection(L, A);
-    A.mp_desc = in + o.md; A.mp_has_obs = B.has_obs ? in + o.obs : nullptr;
+    A.mp_desc = c.dev(o.md); A.mp_has_obs = B.has_obs ? c.dev(o.obs) : nullptr;
     A.th = B.th; A.nnratio = nnratio; A.th_dist = TH_HIGH;
-    A.cand = (uint32_t*)(b + o.cand); A.cand_cnt = (int*)(b + o.cc);
+    A.cand = (uint32_t*)c.dev(o.cand); A.cand_cnt = (int*)c.dev(o.cc);
     A.mode = 0;
     A.out_match = (int32_t*)(L.viewcos_out + nq);
 }
@@ -1123,64 +1134,12 @@ void scatter_local(const uint8_t* r, const LocalOff& o, const borb_local_points_
         if (B.view_cos) B.view_cos[i] = rvc[k];
     }
 }
-}  // namespace
 
-borb_status borb_search_local_points(borb_matcher* m, const borb_frame_view* F, const borb_worldpoints_view* pts, const uint8_t* has_obs,
-                                     const float* Tcw, const float* Ow, float fx, float fy, float cx, float cy, float mbf,
-                                     float viewing_cos_limit, float log_scale_factor, float th, float nnratio, uint8_t* in_view,
-                                     float* proj_x, float* proj_y, float* proj_xr, int32_t* level, float* view_cos,
-                                     int32_t* match_feat, int32_t* n_matches) {
-    if (!m || !F || !pts || !Tcw || !Ow || !in_view || !match_feat || !n_matches) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
-    *n_matches = 0;
-    borb_local_points_job B{};
-    B.frame = *F; B.pts = *pts; B.has_obs = has_obs;
-    std::memcpy(B.Tcw, Tcw, sizeof(B.Tcw)); std::memcpy(B.Ow, Ow, sizeof(B.Ow));
-    B.fx = fx; B.fy = fy; B.cx = cx; B.cy = cy; B.mbf = mbf; B.log_scale_factor = log_scale_factor; B.th = th;
-    B.in_view = in_view; B.proj_x = proj_x; B.proj_y = proj_y; B.proj_xr = proj_xr; B.level = level; B.view_cos = view_cos; B.match_feat = match_feat;
-    const FrameInfo I = frame_info(F);
-    LocalOff o{};
-    m->sel.clear();
-    borb_status s = check_local(B, I, m);
-    if (s == BORB_OK) s = select_local(B, m->sel, o);
-    if (s != BORB_OK || o.nq == 0) return s;
-    BORB_CUDA(cudaSetDevice(m->device));
-    Stager st(m);
-    stage_local(st, B, I, o);
-    const size_t input_end = st.off;
-    reserve_local(st, I, o);
-    const size_t res_bytes = local_res_bytes(o.nq);
-    const size_t o_res = st.reserve(res_bytes);
-    const size_t total = st.off;
-    st.off = input_end;
-    if ((s = ensure_host(m, input_end)) != BORB_OK) return s;
-    if ((s = ensure_out(m, res_bytes)) != BORB_OK) return s;
-    if (o.gather) {
-        BORB_CUDA(cudaStreamSynchronize(m->stream));
-        gather_local(m->h_stage, o, B, m->sel);
-    }
-    if ((s = commit(st, total, I.rf != nullptr)) != BORB_OK) return s;
-    uint8_t* b = m->arena;
-    BORB_CUDA(cudaMemsetAsync(b + o_res, 0, res_bytes, m->stream));
-    ProjArgs A{};
-    LastArgs L{};
-    if ((s = bind_frame(m, I, o.fs, A)) != BORB_OK) return s;
-    bind_local(o, B, I, viewing_cos_limit, nnratio, m->in_base, b, b + o_res, L, A);
-    m->launches += launch_frustum_projection(L, A, m->stream);
-    BORB_CUDA(cudaGetLastError());
-    BORB_CUDA(cudaMemcpyAsync(m->h_out, b + o_res, res_bytes, cudaMemcpyDeviceToHost, m->stream));
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
-    scatter_local(m->h_out, o, B, m->sel, I.n > 0, n_matches);
-    return BORB_OK;
-}
-
-// ---- the two per-frame searches of the Tracking thread for many camera streams at once.  The per-job arguments go to device
-// tables (LastArgs for the projection, ProjArgs for candidates and resolve), every job's results to one region of the arena that
-// comes back with ONE device-to-host copy.  The last-frame state stays in the arena (not in mapped host memory): resolve<true>
-// writes it with atomicMax.
-borb_status borb_search_local_points_batch(borb_matcher* m, const borb_local_points_job* jobs, int n_jobs, float viewing_cos_limit,
-                                           float nnratio, int32_t* n_matches) {
-    if (!m || n_jobs < 0 || (n_jobs > 0 && (!jobs || !n_matches))) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
-    if (n_jobs == 0) return BORB_OK;
+// Shared body of borb_search_local_points (one job, a host view or a resident frame) and borb_search_local_points_batch (resident
+// frames): project_points, candidates and resolve, one synchronisation.  Every job's results go to one region of the arena, zeroed
+// first, that comes back with ONE device-to-host copy.
+borb_status local_points_jobs(borb_matcher* m, const borb_local_points_job* jobs, int n_jobs, float viewing_cos_limit, float nnratio,
+                              int32_t* n_matches, bool batch) {
     // search: valid points on a frame with features (otherwise only isInFrustum runs)
     struct Job { FrameInfo I; bool search; LocalOff o; size_t res; };
     std::vector<Job> J(n_jobs);
@@ -1190,132 +1149,77 @@ borb_status borb_search_local_points_batch(borb_matcher* m, const borb_local_poi
     for (int j = 0; j < n_jobs; j++) {
         const borb_local_points_job& B = jobs[j];
         n_matches[j] = 0;
-        if (!B.frame.resident) { set_error("job %d: borb_search_local_points_batch needs device-resident frames (borb_frame_view::resident)", j); return BORB_ERR_INVALID_ARG; }
-        if (!B.in_view || !B.match_feat) { set_error("job %d: null output", j); return BORB_ERR_INVALID_ARG; }
+        if (batch && !B.frame.resident) { set_error("job %d: borb_search_local_points_batch needs device-resident frames (borb_frame_view::resident)", j); return BORB_ERR_INVALID_ARG; }
+        if (batch && (!B.in_view || !B.match_feat)) { set_error("job %d: null output", j); return BORB_ERR_INVALID_ARG; }
         const FrameInfo I = J[j].I = frame_info(&B.frame);
         borb_status s = check_local(B, I, m);
         if (s == BORB_OK) s = select_local(B, sel, J[j].o);
-        if (s != BORB_OK) return job_error(j, s);
+        if (s != BORB_OK) return job_fail(batch, j, s);
         const int nq = J[j].o.nq;
         J[j].search = nq > 0 && I.n > 0;
         max_nq = std::max(max_nq, nq);
         if (J[j].search) { max_n = std::max(max_n, I.n); max_n_mp = std::max(max_n_mp, nq); }
     }
     if (max_nq == 0) return BORB_OK;
-    BORB_CUDA(cudaSetDevice(m->device));
-    Stager st(m);
+    Call c(m);
     for (int j = 0; j < n_jobs; j++)
-        if (J[j].o.nq > 0) stage_local(st, jobs[j], J[j].I, J[j].o);
-    const size_t o_last = st.add(nullptr, (size_t)n_jobs * sizeof(LastArgs)), o_jobs = st.add(nullptr, (size_t)n_jobs * sizeof(ProjArgs));
-    const size_t input_end = st.off;
-    size_t res_bytes = 0;                        // every job's result block, in one region
+        if (J[j].o.nq > 0) stage_local(c, jobs[j], J[j].I, J[j].o);
+    JobTable<LastArgs> lt(c, n_jobs);
+    JobTable<ProjArgs> jt(c, n_jobs);
+    size_t res_end = 0;
     for (int j = 0; j < n_jobs; j++) {
         if (J[j].o.nq == 0) continue;
-        reserve_local(st, J[j].I, J[j].o);
-        J[j].res = res_bytes; res_bytes += (local_res_bytes(J[j].o.nq) + 15) & ~size_t(15);
+        reserve_local(c, J[j].I, J[j].o);
+        J[j].res = c.result(local_res_bytes(J[j].o.nq));
+        res_end = J[j].res + local_res_bytes(J[j].o.nq);
     }
-    const size_t o_res = st.reserve(res_bytes);
-    const size_t total = st.off;
-    st.off = input_end;
     borb_status s;
-    if ((s = ensure_host(m, input_end)) != BORB_OK) return s;
-    if ((s = ensure_arena(m, total)) != BORB_OK) return s;
-    if ((s = ensure_out(m, res_bytes)) != BORB_OK) return s;
-    BORB_CUDA(cudaStreamSynchronize(m->stream));       // the staging buffer may still feed an earlier copy
-    uint8_t* b = m->arena;
-    uint8_t* h = m->h_stage;
-    LastArgs* hl = reinterpret_cast<LastArgs*>(h + o_last);
-    ProjArgs* hj = reinterpret_cast<ProjArgs*>(h + o_jobs);
+    if ((s = c.begin(n_jobs == 1 && J[0].I.rf)) != BORB_OK) return s;
+    LastArgs* hl = lt.host(c);
+    ProjArgs* hj = jt.host(c);
     for (int j = 0; j < n_jobs; j++) {
         const LocalOff& o = J[j].o;
         LastArgs L{};
         ProjArgs A{};
         if (o.nq > 0) {
-            if (o.gather) gather_local(h, o, jobs[j], sel);
-            bind_resident(jobs[j].frame.resident, A);
-            bind_local(o, jobs[j], J[j].I, viewing_cos_limit, nnratio, b, b, b + o_res + J[j].res, L, A);
-            if (!J[j].search) A = ProjArgs{};          // a frame without features keeps n_mp = 0: candidates and resolve skip it
+            if (o.gather) gather_local(c.host<uint8_t>(0), o, jobs[j], sel);
+            bind_frame_fields(J[j].I, o.fs, c, A);
+            bind_local(o, jobs[j], J[j].I, viewing_cos_limit, nnratio, c, c.res(J[j].res, false), L, A);
+            if (!J[j].search) A.n_mp = 0;              // a frame without features: candidates and resolve skip the job
         }                                            // a job without valid points keeps n_last = 0 as well
         hl[j] = L;
         hj[j] = A;
     }
-    if ((s = commit(st, total)) != BORB_OK) return s;
-    BORB_CUDA(cudaMemsetAsync(b + o_res, 0, res_bytes, m->stream));
-    for (int j = 0; j < n_jobs; j++) BORB_CUDA(cudaStreamWaitEvent(m->stream, jobs[j].frame.resident->ready, 0));
-    m->launches += launch_point_projection_batch((const LastArgs*)(b + o_last), (const ProjArgs*)(b + o_jobs), n_jobs, max_nq, max_n, max_n_mp,
-                                                 false, m->stream);
-    BORB_CUDA(cudaGetLastError());
-    BORB_CUDA(cudaMemcpyAsync(m->h_out, b + o_res, res_bytes, cudaMemcpyDeviceToHost, m->stream));
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
+    if ((s = c.commit()) != BORB_OK) return s;
+    BORB_CUDA(cudaMemsetAsync(c.res(0, false), 0, res_end, m->stream));
     for (int j = 0; j < n_jobs; j++)
-        if (J[j].o.nq > 0) scatter_local(m->h_out + J[j].res, J[j].o, jobs[j], sel, J[j].search, &n_matches[j]);
+        if (J[j].o.nq > 0 && (s = prepare_frame(m, c, J[j].I, hj[j])) != BORB_OK) return s;
+    m->launches += launch_point_projection_batch(lt.dev(c), jt.dev(c), hl[0], hj[0], n_jobs, max_nq, max_n, max_n_mp, false, m->stream);
+    if ((s = c.finish()) != BORB_OK) return s;
+    for (int j = 0; j < n_jobs; j++)
+        if (J[j].o.nq > 0) scatter_local(c.out(J[j].res), J[j].o, jobs[j], sel, J[j].search, &n_matches[j]);
     return BORB_OK;
 }
+}  // namespace
 
-borb_status borb_search_by_projection_last_batch(borb_matcher* m, const borb_last_frame_job* jobs, int n_jobs, int check_orientation,
-                                                 int32_t* n_matches) {
+borb_status borb_search_local_points(borb_matcher* m, const borb_frame_view* F, const borb_worldpoints_view* pts, const uint8_t* has_obs,
+                                     const float* Tcw, const float* Ow, float fx, float fy, float cx, float cy, float mbf,
+                                     float viewing_cos_limit, float log_scale_factor, float th, float nnratio, uint8_t* in_view,
+                                     float* proj_x, float* proj_y, float* proj_xr, int32_t* level, float* view_cos,
+                                     int32_t* match_feat, int32_t* n_matches) {
+    if (!m || !F || !pts || !Tcw || !Ow || !in_view || !match_feat || !n_matches) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+    borb_local_points_job B{};
+    B.frame = *F; B.pts = *pts; B.has_obs = has_obs;
+    std::memcpy(B.Tcw, Tcw, sizeof(B.Tcw)); std::memcpy(B.Ow, Ow, sizeof(B.Ow));
+    B.fx = fx; B.fy = fy; B.cx = cx; B.cy = cy; B.mbf = mbf; B.log_scale_factor = log_scale_factor; B.th = th;
+    B.in_view = in_view; B.proj_x = proj_x; B.proj_y = proj_y; B.proj_xr = proj_xr; B.level = level; B.view_cos = view_cos; B.match_feat = match_feat;
+    return local_points_jobs(m, &B, 1, viewing_cos_limit, nnratio, n_matches, false);
+}
+
+borb_status borb_search_local_points_batch(borb_matcher* m, const borb_local_points_job* jobs, int n_jobs, float viewing_cos_limit,
+                                           float nnratio, int32_t* n_matches) {
     if (!m || n_jobs < 0 || (n_jobs > 0 && (!jobs || !n_matches))) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
-    if (n_jobs == 0) return BORB_OK;
-    struct Job { PointQuery Q; FrameInfo I; bool live; QueryOff o; size_t res; };
-    std::vector<Job> J(n_jobs);
-    int max_n = 1, max_nq = 0;
-    for (int j = 0; j < n_jobs; j++) {
-        const borb_last_frame_job& B = jobs[j];
-        n_matches[j] = 0;
-        if (!B.cur.resident) { set_error("job %d: borb_search_by_projection_last_batch needs device-resident frames (borb_frame_view::resident)", j); return BORB_ERR_INVALID_ARG; }
-        if (!B.state_cur) { set_error("job %d: null output", j); return BORB_ERR_INVALID_ARG; }
-        const PointQuery& Q = J[j].Q = last_frame_query(B, check_orientation);
-        const FrameInfo I = J[j].I = frame_info(&B.cur);
-        borb_status s = check_query(&B.cur, I, Q, m);
-        if (s != BORB_OK) return job_error(j, s);
-        std::fill_n(B.state_cur, I.n, -1);
-        J[j].live = I.n > 0 && Q.n > 0;
-        if (J[j].live) { max_n = std::max(max_n, I.n); max_nq = std::max(max_nq, Q.n); }
-    }
-    if (max_nq == 0) return BORB_OK;
-    BORB_CUDA(cudaSetDevice(m->device));
-    Stager st(m);
-    for (int j = 0; j < n_jobs; j++)
-        if (J[j].live) J[j].o = stage_query(st, &jobs[j].cur, J[j].I, J[j].Q);
-    const size_t o_last = st.add(nullptr, (size_t)n_jobs * sizeof(LastArgs)), o_jobs = st.add(nullptr, (size_t)n_jobs * sizeof(ProjArgs));
-    const size_t input_end = st.off;
-    size_t res_bytes = 0;                        // every job's state (cur n entries) and match count, in one region
-    for (int j = 0; j < n_jobs; j++) {
-        if (!J[j].live) continue;
-        reserve_query(st, J[j].I, J[j].Q, J[j].o);
-        J[j].res = res_bytes; res_bytes += ((size_t)J[j].I.n * 4 + 4 + 15) & ~size_t(15);
-    }
-    const size_t o_res = st.reserve(res_bytes);
-    const size_t total = st.off;
-    st.off = input_end;
-    borb_status s;
-    if ((s = ensure_host(m, input_end)) != BORB_OK) return s;
-    if ((s = ensure_arena(m, total)) != BORB_OK) return s;
-    if ((s = ensure_out(m, res_bytes)) != BORB_OK) return s;
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
-    uint8_t* b = m->arena;
-    LastArgs* hl = reinterpret_cast<LastArgs*>(m->h_stage + o_last);
-    ProjArgs* hj = reinterpret_cast<ProjArgs*>(m->h_stage + o_jobs);
-    for (int j = 0; j < n_jobs; j++) {
-        LastArgs L{};
-        ProjArgs A{};
-        if (J[j].live) {
-            bind_resident(jobs[j].cur.resident, A);
-            bind_query(J[j].o, J[j].Q, J[j].I, b, b, (int32_t*)(b + o_res + J[j].res), L, A);
-        }                                            // a job without work keeps n_last = n_mp = 0: every kernel skips it
-        hl[j] = L;
-        hj[j] = A;
-    }
-    if ((s = commit(st, total)) != BORB_OK) return s;
-    for (int j = 0; j < n_jobs; j++) BORB_CUDA(cudaStreamWaitEvent(m->stream, jobs[j].cur.resident->ready, 0));
-    m->launches += launch_point_projection_batch((const LastArgs*)(b + o_last), (const ProjArgs*)(b + o_jobs), n_jobs, max_nq, max_n, max_nq,
-                                                 true, m->stream);
-    BORB_CUDA(cudaGetLastError());
-    BORB_CUDA(cudaMemcpyAsync(m->h_out, b + o_res, res_bytes, cudaMemcpyDeviceToHost, m->stream));
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
-    for (int j = 0; j < n_jobs; j++)
-        if (J[j].live) read_counted(m->h_out + J[j].res, J[j].I.n, jobs[j].state_cur, &n_matches[j]);
-    return BORB_OK;
+    return local_points_jobs(m, jobs, n_jobs, viewing_cos_limit, nnratio, n_matches, true);
 }
 
 borb_status borb_search_for_initialization(borb_matcher* m, const borb_frame_view* f1, const borb_frame_view* f2, float* prev_matched,
@@ -1328,53 +1232,47 @@ borb_status borb_search_for_initialization(borb_matcher* m, const borb_frame_vie
     if (!f1->keys_un || !f1->desc || !f2->keys_un || !f2->desc || !(f2->max_x > f2->min_x) || !(f2->max_y > f2->min_y)) {
         set_error("incomplete frame view"); return BORB_ERR_INVALID_ARG;
     }
-    BORB_CUDA(cudaSetDevice(m->device));
     const int n1 = f1->n;
     // the query windows are data the caller already has: vbPrevMatched as centre, windowSize as radius, level 0 only (:421-427)
     std::vector<float> px(n1), py(n1), rad(n1, (float)window_size);
     std::vector<int32_t> zero(n1, 0);
     std::vector<uint8_t> valid(n1);
     for (int i = 0; i < n1; i++) { px[i] = prev_matched[2 * i]; py[i] = prev_matched[2 * i + 1]; valid[i] = f1->keys_un[i].octave > 0 ? 0 : 1; }
-    Stager st(m);
-    const size_t o_k2 = st.add(f2->keys_un, (size_t)f2->n * sizeof(borb_keypoint));
-    const size_t o_d2 = st.add(f2->desc, (size_t)f2->n * 32);
-    const size_t o_k1 = st.add(f1->keys_un, (size_t)n1 * sizeof(borb_keypoint));
-    const size_t o_d1 = st.add(f1->desc, (size_t)n1 * 32);
-    const size_t o_px = st.add(px.data(), (size_t)n1 * 4), o_py = st.add(py.data(), (size_t)n1 * 4), o_rad = st.add(rad.data(), (size_t)n1 * 4);
-    const size_t o_lv = st.add(zero.data(), (size_t)n1 * 4), o_val = st.add(valid.data(), (size_t)n1);
-    const size_t o_prev = st.add(prev_matched, (size_t)n1 * 8);
-    const size_t input_end = st.off;
-    const size_t o_cs = st.reserve((size_t)(GRID_CELLS + 1) * 4), o_ci = st.reserve((size_t)MATCH_MAX_FEATURES * 4 + 16);
-    const size_t o_cand = st.reserve((size_t)n1 * f2->n * 4), o_cc = st.reserve((size_t)n1 * 4);
-    const size_t o_m12 = st.reserve((size_t)n1 * 4), o_evi = st.reserve((size_t)n1 * 4), o_evb = st.reserve((size_t)n1), o_nm = st.reserve(16);
-    const size_t total = st.off;
-    st.off = input_end;
-    borb_status s = commit(st, total);
-    if (s != BORB_OK) return s;
-    uint8_t* b = m->arena;
+    Call c(m);
+    const size_t o_k2 = c.in(f2->keys_un, (size_t)f2->n * sizeof(borb_keypoint));
+    const size_t o_d2 = c.in(f2->desc, (size_t)f2->n * 32);
+    const size_t o_k1 = c.in(f1->keys_un, (size_t)n1 * sizeof(borb_keypoint));
+    const size_t o_d1 = c.in(f1->desc, (size_t)n1 * 32);
+    const size_t o_px = c.in(px.data(), (size_t)n1 * 4), o_py = c.in(py.data(), (size_t)n1 * 4), o_rad = c.in(rad.data(), (size_t)n1 * 4);
+    const size_t o_lv = c.in(zero.data(), (size_t)n1 * 4), o_val = c.in(valid.data(), (size_t)n1);
+    const size_t o_prev = c.in(prev_matched, (size_t)n1 * 8);
+    const size_t o_cs = c.scratch((size_t)(GRID_CELLS + 1) * 4), o_ci = c.scratch((size_t)MATCH_MAX_FEATURES * 4 + 16);
+    const size_t o_cand = c.scratch((size_t)n1 * f2->n * 4), o_cc = c.scratch((size_t)n1 * 4);
+    const size_t o_m12 = c.scratch((size_t)n1 * 4), o_evi = c.scratch((size_t)n1 * 4), o_evb = c.scratch((size_t)n1), o_nm = c.scratch(16);
+    borb_status s;
+    if ((s = c.begin()) != BORB_OK || (s = c.commit()) != BORB_OK) return s;
     ProjArgs A{};
-    A.n = f2->n; A.keys = (const borb_keypoint*)(b + o_k2); A.desc = b + o_d2;
+    A.n = f2->n; A.keys = (const borb_keypoint*)c.dev(o_k2); A.desc = c.dev(o_d2);
     A.u_right = nullptr; A.occupied = nullptr;
     A.minX = f2->min_x; A.minY = f2->min_y;
     A.invW = (float)GRID_COLS / (float)(f2->max_x - f2->min_x);
     A.invH = (float)GRID_ROWS / (float)(f2->max_y - f2->min_y);
     A.scale_factors = nullptr;
-    A.cell_start = (const int*)(b + o_cs); A.cell_idx = (const int*)(b + o_ci);
-    A.n_mp = n1; A.proj_x = (const float*)(b + o_px); A.proj_y = (const float*)(b + o_py); A.proj_xr = (const float*)(b + o_px);
-    A.mp_desc = b + o_d1; A.mp_valid = b + o_val; A.mp_has_obs = nullptr;
+    A.cell_start = (const int*)c.dev(o_cs); A.cell_idx = (const int*)c.dev(o_ci);
+    A.n_mp = n1; A.proj_x = (const float*)c.dev(o_px); A.proj_y = (const float*)c.dev(o_py); A.proj_xr = (const float*)c.dev(o_px);
+    A.mp_desc = c.dev(o_d1); A.mp_valid = c.dev(o_val); A.mp_has_obs = nullptr;
     A.th = 1.f; A.nnratio = nnratio;
-    A.cand = (uint32_t*)(b + o_cand); A.cand_cnt = (int*)(b + o_cc);
-    A.q_radius = (const float*)(b + o_rad); A.q_minl = (const int32_t*)(b + o_lv); A.q_maxl = (const int32_t*)(b + o_lv);
+    A.cand = (uint32_t*)c.dev(o_cand); A.cand_cnt = (int*)c.dev(o_cc);
+    A.q_radius = (const float*)c.dev(o_rad); A.q_minl = (const int32_t*)c.dev(o_lv); A.q_maxl = (const int32_t*)c.dev(o_lv);
     A.mode = 1; A.check_ori = check_orientation; A.th_dist = 50;
-    m->launches += launch_grid_sort(A.keys, A.n, A.minX, A.minY, A.invW, A.invH, (int*)(b + o_cs), (int*)(b + o_ci), m->stream);
-    m->launches += launch_initialization(A, (const borb_keypoint*)(b + o_k1), n1, (int32_t*)(b + o_m12), (int32_t*)(b + o_evi), b + o_evb,
-                                         (float*)(b + o_prev), (int*)(b + o_nm), m->stream);
-    BORB_CUDA(cudaGetLastError());
-    BORB_CUDA(cudaMemcpyAsync(matches12, b + o_m12, (size_t)n1 * 4, cudaMemcpyDeviceToHost, m->stream));
-    BORB_CUDA(cudaMemcpyAsync(prev_matched, b + o_prev, (size_t)n1 * 8, cudaMemcpyDeviceToHost, m->stream));
-    BORB_CUDA(cudaMemcpyAsync(n_matches, b + o_nm, 4, cudaMemcpyDeviceToHost, m->stream));
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
-    return BORB_OK;
+    m->launches += launch_grid_sort(A.keys, A.n, A.minX, A.minY, A.invW, A.invH, (int*)c.dev(o_cs), (int*)c.dev(o_ci), m->stream);
+    m->launches += launch_initialization(A, (const borb_keypoint*)c.dev(o_k1), n1, (int32_t*)c.dev(o_m12), (int32_t*)c.dev(o_evi), c.dev(o_evb),
+                                         (float*)c.dev(o_prev), (int*)c.dev(o_nm), m->stream);
+    // vbPrevMatched is updated on its staged copy: the three results go straight to the caller's arrays
+    BORB_CUDA(cudaMemcpyAsync(matches12, c.dev(o_m12), (size_t)n1 * 4, cudaMemcpyDeviceToHost, m->stream));
+    BORB_CUDA(cudaMemcpyAsync(prev_matched, c.dev(o_prev), (size_t)n1 * 8, cudaMemcpyDeviceToHost, m->stream));
+    BORB_CUDA(cudaMemcpyAsync(n_matches, c.dev(o_nm), 4, cudaMemcpyDeviceToHost, m->stream));
+    return c.finish();
 }
 
 borb_status borb_distinctive_descriptors(borb_matcher* m, const uint8_t* desc, const int32_t* offsets, int n_points, int32_t* best_idx) {
@@ -1384,56 +1282,40 @@ borb_status borb_distinctive_descriptors(borb_matcher* m, const uint8_t* desc, c
     for (int i = 0; i < n_points; i++)
         if (offsets[i + 1] < offsets[i] || offsets[i] < 0 || offsets[i + 1] - offsets[i] >= (1 << 16)) { set_error("offsets must ascend; at most 65535 observations per MapPoint"); return BORB_ERR_INVALID_ARG; }
     if (total_desc > 0 && !desc) { set_error("null descriptors"); return BORB_ERR_INVALID_ARG; }
-    BORB_CUDA(cudaSetDevice(m->device));
-    Stager st(m);
-    const size_t o_d = st.add(desc, (size_t)total_desc * 32);
-    const size_t o_o = st.add(offsets, (size_t)(n_points + 1) * 4);
-    const size_t input_end = st.off;
-    const size_t o_b = st.reserve((size_t)n_points * 4);
-    const size_t total = st.off;
-    st.off = input_end;
-    borb_status s = commit(st, total);
-    if (s != BORB_OK) return s;
-    uint8_t* b = m->arena;
-    m->launches += launch_distinctive(b + o_d, (const int32_t*)(b + o_o), n_points, (int32_t*)(b + o_b), m->stream);
-    BORB_CUDA(cudaGetLastError());
-    BORB_CUDA(cudaMemcpyAsync(best_idx, b + o_b, (size_t)n_points * 4, cudaMemcpyDeviceToHost, m->stream));
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
+    Call c(m);
+    const size_t o_d = c.in(desc, (size_t)total_desc * 32);
+    const size_t o_o = c.in(offsets, (size_t)(n_points + 1) * 4);
+    const size_t r_b = c.result((size_t)n_points * 4);
+    borb_status s;
+    if ((s = c.begin()) != BORB_OK || (s = c.commit()) != BORB_OK) return s;
+    m->launches += launch_distinctive(c.dev(o_d), (const int32_t*)c.dev(o_o), n_points, (int32_t*)c.res(r_b, false), m->stream);
+    if ((s = c.finish()) != BORB_OK) return s;
+    std::memcpy(best_idx, c.out(r_b), (size_t)n_points * 4);
     return BORB_OK;
 }
 
 static borb_status bow_common(borb_matcher* m, const borb_keyframe_view* qs, int n_q, const borb_keyframe_view* t, int mode, float nnratio,
                               int check_ori, int32_t* match, int32_t* n_matches) {
     // mode 0: qs[0..n_q) keyframes vs ONE frame t, out stride t->n.   mode 1: n_q == 1, q = kf1, t = kf2, out stride q->n.
-    BORB_CUDA(cudaSetDevice(m->device));
-    Stager st(m);
+    Call c(m);
     std::vector<KfOffsets> qo(n_q);
-    for (int i = 0; i < n_q; i++) qo[i] = stage_kf(st, &qs[i]);
-    const KfOffsets to = stage_kf(st, t);
-    const size_t o_qd = st.reserve((size_t)n_q * sizeof(KfDev)), o_td = st.reserve(sizeof(KfDev));
-    const size_t input_end = st.off;
+    for (int i = 0; i < n_q; i++) qo[i] = stage_kf(c, &qs[i]);
+    const KfOffsets to = stage_kf(c, t);
+    const size_t o_qd = c.in(nullptr, (size_t)n_q * sizeof(KfDev)), o_td = c.in(nullptr, sizeof(KfDev));     // filled in place
     const int out_stride = mode == 0 ? t->n : qs[0].n;
-    const size_t o_match = st.reserve((size_t)n_q * (out_stride > 0 ? out_stride : 1) * 4);
-    const size_t o_bins = st.reserve((size_t)n_q * (out_stride > 0 ? out_stride : 1));
-    const size_t o_nm = st.reserve((size_t)n_q * 4);
-    const size_t total = st.off;
-    st.off = input_end;
-    // the KfDev tables are part of the staged input: fill them in the staging buffer after the layout is known
-    borb_status s = ensure_arena(m, total);
-    if (s != BORB_OK) return s;
-    std::vector<KfDev> qd(n_q);
-    for (int i = 0; i < n_q; i++) qd[i] = kf_dev(m, &qs[i], qo[i]);
-    const KfDev td = kf_dev(m, t, to);
-    st.items.push_back({qd.data(), {o_qd, (size_t)n_q * sizeof(KfDev)}});
-    st.items.push_back({&td, {o_td, sizeof(KfDev)}});
-    if ((s = commit(st, total)) != BORB_OK) return s;
-    uint8_t* b = m->arena;
-    m->launches += launch_bow_match((const KfDev*)(b + o_qd), (const KfDev*)(b + o_td), n_q, mode, nnratio, check_ori, (int32_t*)(b + o_match),
-                                    out_stride, nullptr, b + o_bins, (int32_t*)(b + o_nm), t->n, m->stream);
-    BORB_CUDA(cudaGetLastError());
-    if (out_stride > 0) BORB_CUDA(cudaMemcpyAsync(match, b + o_match, (size_t)n_q * out_stride * 4, cudaMemcpyDeviceToHost, m->stream));
-    BORB_CUDA(cudaMemcpyAsync(n_matches, b + o_nm, (size_t)n_q * 4, cudaMemcpyDeviceToHost, m->stream));
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
+    const size_t o_bins = c.scratch((size_t)n_q * (out_stride > 0 ? out_stride : 1));
+    const size_t r_match = c.result((size_t)n_q * (out_stride > 0 ? out_stride : 1) * 4), r_nm = c.result((size_t)n_q * 4);
+    borb_status s;
+    if ((s = c.begin()) != BORB_OK) return s;
+    KfDev* hq = c.host<KfDev>(o_qd);
+    for (int i = 0; i < n_q; i++) hq[i] = kf_dev(c, &qs[i], qo[i]);
+    *c.host<KfDev>(o_td) = kf_dev(c, t, to);
+    if ((s = c.commit()) != BORB_OK) return s;
+    m->launches += launch_bow_match((const KfDev*)c.dev(o_qd), (const KfDev*)c.dev(o_td), n_q, mode, nnratio, check_ori, (int32_t*)c.res(r_match, false),
+                                    out_stride, nullptr, c.dev(o_bins), (int32_t*)c.res(r_nm, false), t->n, m->stream);
+    if ((s = c.finish()) != BORB_OK) return s;
+    if (out_stride > 0) std::memcpy(match, c.out(r_match), (size_t)n_q * out_stride * 4);
+    std::memcpy(n_matches, c.out(r_nm), (size_t)n_q * 4);
     return BORB_OK;
 }
 
@@ -1492,56 +1374,45 @@ borb_status borb_search_by_bow_batch(borb_matcher* m, const borb_bow_job* jobs, 
         if (!B.match) { set_error("job %d: null output", j); return BORB_ERR_INVALID_ARG; }
         if (B.kf_frame) {
             if ((s = check_resident_bow(B.kf_frame, m, j, "kf_frame")) != BORB_OK) return s;
-        } else if ((s = check_kf(&B.kf, "keyframe")) != BORB_OK) return job_error(j, s);
+        } else if ((s = check_kf(&B.kf, "keyframe")) != BORB_OK) return job_fail(true, j, s);
         max_t = std::max(max_t, B.frame->n);
         off[j] = total_n; total_n += (size_t)B.frame->n;
     }
-    BORB_CUDA(cudaSetDevice(m->device));
-    Stager st(m);
+    Call c(m);
     std::vector<KfOffsets> ko(n_jobs);
     std::vector<size_t> o_hm(n_jobs, 0);
     for (int j = 0; j < n_jobs; j++) {
         const borb_bow_job& B = jobs[j];
-        if (!B.kf_frame) ko[j] = stage_kf(st, &B.kf);
-        else if (B.kf.has_mp) o_hm[j] = st.add(B.kf.has_mp, (size_t)B.kf_frame->n);
+        if (!B.kf_frame) ko[j] = stage_kf(c, &B.kf);
+        else if (B.kf.has_mp) o_hm[j] = c.in(B.kf.has_mp, (size_t)B.kf_frame->n);
     }
-    const size_t o_q = st.add(nullptr, (size_t)n_jobs * sizeof(KfDev)), o_t = st.add(nullptr, (size_t)n_jobs * sizeof(KfDev));   // filled in place
-    const size_t o_off = st.add(nullptr, (size_t)n_jobs * sizeof(size_t));
-    const size_t input_end = st.off;
-    const size_t cnt_bytes = ((size_t)n_jobs * 4 + 15) & ~size_t(15);
-    const size_t res_bytes = cnt_bytes + total_n * 4;                  // n_matches of every job, then every job's matches: one D2H
-    const size_t o_res = st.reserve(res_bytes), o_bins = st.reserve(total_n + 16);
-    const size_t total = st.off;
-    st.off = input_end;
+    const size_t o_q = c.in(nullptr, (size_t)n_jobs * sizeof(KfDev)), o_t = c.in(nullptr, (size_t)n_jobs * sizeof(KfDev));   // filled in place
+    const size_t o_off = c.in(nullptr, (size_t)n_jobs * sizeof(size_t));
+    const size_t o_bins = c.scratch(total_n + 16);
+    const size_t r_cnt = c.result((size_t)n_jobs * 4), r_match = c.result(total_n * 4);     // n_matches of every job, then every job's matches
     borb_status s;
-    if ((s = ensure_host(m, input_end)) != BORB_OK) return s;
-    if ((s = ensure_arena(m, total)) != BORB_OK) return s;
-    if ((s = ensure_out(m, res_bytes)) != BORB_OK) return s;
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
-    uint8_t* b = m->arena;
-    KfDev* hq = reinterpret_cast<KfDev*>(m->h_stage + o_q);
-    KfDev* ht = reinterpret_cast<KfDev*>(m->h_stage + o_t);
-    size_t* hoff = reinterpret_cast<size_t*>(m->h_stage + o_off);
+    if ((s = c.begin()) != BORB_OK) return s;
+    KfDev* hq = c.host<KfDev>(o_q);
+    KfDev* ht = c.host<KfDev>(o_t);
+    size_t* hoff = c.host<size_t>(o_off);
     for (int j = 0; j < n_jobs; j++) {
         const borb_bow_job& B = jobs[j];
-        hq[j] = B.kf_frame ? resident_kf_dev(B.kf_frame, B.kf.has_mp ? b + o_hm[j] : nullptr) : kf_dev(m, &B.kf, ko[j]);
+        hq[j] = B.kf_frame ? resident_kf_dev(B.kf_frame, B.kf.has_mp ? c.dev(o_hm[j]) : nullptr) : kf_dev(c, &B.kf, ko[j]);
         ht[j] = resident_kf_dev(B.frame, nullptr);
         hoff[j] = off[j];
     }
-    if ((s = commit(st, total)) != BORB_OK) return s;
+    if ((s = c.commit()) != BORB_OK) return s;
     for (int j = 0; j < n_jobs; j++) {
-        BORB_CUDA(cudaStreamWaitEvent(m->stream, jobs[j].frame->ready, 0));
-        if (jobs[j].kf_frame) BORB_CUDA(cudaStreamWaitEvent(m->stream, jobs[j].kf_frame->ready, 0));
+        if ((s = c.wait(jobs[j].frame)) != BORB_OK) return s;
+        if (jobs[j].kf_frame && (s = c.wait(jobs[j].kf_frame)) != BORB_OK) return s;
     }
-    m->launches += launch_bow_match((const KfDev*)(b + o_q), (const KfDev*)(b + o_t), n_jobs, 0, nnratio, check_orientation,
-                                    (int32_t*)(b + o_res + cnt_bytes), 0, (const size_t*)(b + o_off), b + o_bins, (int32_t*)(b + o_res), max_t,
-                                    m->stream);
-    BORB_CUDA(cudaGetLastError());
-    BORB_CUDA(cudaMemcpyAsync(m->h_out, b + o_res, res_bytes, cudaMemcpyDeviceToHost, m->stream));
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
+    m->launches += launch_bow_match((const KfDev*)c.dev(o_q), (const KfDev*)c.dev(o_t), n_jobs, 0, nnratio, check_orientation,
+                                    (int32_t*)c.res(r_match, false), 0, (const size_t*)c.dev(o_off), c.dev(o_bins), (int32_t*)c.res(r_cnt, false),
+                                    max_t, m->stream);
+    if ((s = c.finish()) != BORB_OK) return s;
     for (int j = 0; j < n_jobs; j++) {
-        std::memcpy(&n_matches[j], m->h_out + (size_t)j * 4, 4);
-        std::memcpy(jobs[j].match, m->h_out + cnt_bytes + off[j] * 4, (size_t)jobs[j].frame->n * 4);
+        std::memcpy(&n_matches[j], c.out(r_cnt) + (size_t)j * 4, 4);
+        std::memcpy(jobs[j].match, c.out(r_match) + off[j] * 4, (size_t)jobs[j].frame->n * 4);
     }
     return BORB_OK;
 }
@@ -1702,7 +1573,7 @@ borb_status borb_kfdb_size(const borb_kfdb* db, int32_t* n_slots, uint64_t* devi
 }
 
 // caller holds db->mu
-static borb_status kfdb_sync_table(borb_kfdb* db, cudaStream_t stream) {
+static borb_status kfdb_sync_table(borb_kfdb* db) {
     if (!db->dirty) return BORB_OK;
     const size_t n = db->entries.size();
     if (n > db->table_cap) {
@@ -1713,7 +1584,6 @@ static borb_status kfdb_sync_table(borb_kfdb* db, cudaStream_t stream) {
         BORB_CUDA(cudaMalloc(&db->d_table, db->table_cap * sizeof(BowDev)));
         BORB_CUDA(cudaMalloc(&db->d_stream, db->table_cap * sizeof(KfStream)));
     }
-    (void)stream;
     std::vector<BowDev> t(n);
     std::vector<KfStream> st(n);
     for (size_t i = 0; i < n; i++) {
@@ -1746,8 +1616,8 @@ struct DbLocks {
         dbs.erase(std::unique(dbs.begin(), dbs.end()), dbs.end());
         for (borb_kfdb* db : dbs) held.emplace_back(db->mu);
     }
-    borb_status sync(cudaStream_t s) {
-        for (borb_kfdb* db : dbs) { borb_status st = kfdb_sync_table(db, s); if (st != BORB_OK) return st; }
+    borb_status sync() {
+        for (borb_kfdb* db : dbs) { borb_status st = kfdb_sync_table(db); if (st != BORB_OK) return st; }
         return BORB_OK;
     }
 };
@@ -1767,11 +1637,11 @@ borb_status kfdb_query_jobs(borb_matcher* m, const QueryJob* q, int n_jobs, bool
     std::vector<int> ns(n_jobs);
     std::vector<size_t> o_w(n_jobs, 0), o_v(n_jobs, 0), ho(n_jobs, 0);
     int max_slots = 0, max_nq = 0;
+    Call c(m);
     {
         std::vector<borb_kfdb*> dbs(n_jobs);
         for (int j = 0; j < n_jobs; j++) dbs[j] = q[j].db;
         DbLocks lk(std::move(dbs));
-        size_t out_bytes = 0;
         for (int j = 0; j < n_jobs; j++) {
             ns[j] = (int)q[j].db->entries.size();
             *q[j].n_slots = ns[j];
@@ -1779,44 +1649,38 @@ borb_status kfdb_query_jobs(borb_matcher* m, const QueryJob* q, int n_jobs, bool
         for (int j = 0; j < n_jobs; j++)
             if (q[j].cap < ns[j]) { set_error("output capacity %d < %d database slots", q[j].cap, ns[j]); return job_fail(batch, j, BORB_ERR_CAPACITY); }
         for (int j = 0; j < n_jobs; j++) {
-            ho[j] = out_bytes; out_bytes += ((size_t)ns[j] * 12 + 15) & ~size_t(15);
             max_slots = std::max(max_slots, ns[j]);
             max_nq = std::max(max_nq, q[j].frame ? q[j].frame->n_bow : q[j].n_bow);
         }
         if (max_slots == 0) return BORB_OK;
         BORB_CUDA(cudaSetDevice(m->device));
-        borb_status s = lk.sync(m->stream);
+        borb_status s = lk.sync();
         if (s != BORB_OK) return s;
-        Stager st(m);
         for (int j = 0; j < n_jobs; j++)
-            if (!q[j].frame) { o_w[j] = st.add(q[j].word, (size_t)q[j].n_bow * 4); o_v[j] = st.add(q[j].value, (size_t)q[j].n_bow * 8); }
-        const size_t o_jobs = st.add(nullptr, (size_t)n_jobs * sizeof(KfdbQueryJob));     // filled in place
-        const size_t total = st.off;
-        if ((s = ensure_host(m, total)) != BORB_OK) return s;
-        if ((s = ensure_arena(m, total)) != BORB_OK) return s;
-        if ((s = ensure_out(m, out_bytes + 64)) != BORB_OK) return s;
-        BORB_CUDA(cudaStreamSynchronize(m->stream));
-        uint8_t* b = m->arena;
-        KfdbQueryJob* hj = reinterpret_cast<KfdbQueryJob*>(m->h_stage + o_jobs);
+            if (!q[j].frame) { o_w[j] = c.in(q[j].word, (size_t)q[j].n_bow * 4); o_v[j] = c.in(q[j].value, (size_t)q[j].n_bow * 8); }
+        const size_t o_jobs = c.in(nullptr, (size_t)n_jobs * sizeof(KfdbQueryJob));     // filled in place
+        for (int j = 0; j < n_jobs; j++) ho[j] = c.result((size_t)ns[j] * 12);
+        if ((s = c.begin()) != BORB_OK) return s;
+        KfdbQueryJob* hj = c.host<KfdbQueryJob>(o_jobs);
         for (int j = 0; j < n_jobs; j++) {
             // the three result arrays are written by the kernel straight into the pinned landing buffer (device-addressable, UVA)
-            uint8_t* o = m->h_out + ho[j];
+            uint8_t* o = c.res(ho[j], true);
             KfdbQueryJob J{};
             J.table = q[j].db->d_table; J.n_slots = ns[j];
             if (q[j].frame) { J.qword = q[j].frame->bow_word; J.qvalue = q[j].frame->bow_value; J.nq = q[j].frame->n_bow; }
-            else { J.qword = (const uint32_t*)(b + o_w[j]); J.qvalue = (const double*)(b + o_v[j]); J.nq = q[j].n_bow; }
+            else { J.qword = (const uint32_t*)c.dev(o_w[j]); J.qvalue = (const double*)c.dev(o_v[j]); J.nq = q[j].n_bow; }
             J.common = (int32_t*)o; J.score = (float*)(o + (size_t)ns[j] * 4); J.first_word = (uint32_t*)(o + (size_t)ns[j] * 8);
             hj[j] = J;
         }
-        if ((s = commit(st, total)) != BORB_OK) return s;
+        if ((s = c.commit()) != BORB_OK) return s;
         for (int j = 0; j < n_jobs; j++)
-            if (q[j].frame) BORB_CUDA(cudaStreamWaitEvent(m->stream, q[j].frame->ready, 0));
-        m->launches += launch_kfdb_score((const KfdbQueryJob*)(b + o_jobs), n_jobs, max_slots, max_nq, q[0].db->n_sm, m->stream);
-        BORB_CUDA(cudaGetLastError());
+            if (q[j].frame && (s = c.wait(q[j].frame)) != BORB_OK) return s;
+        m->launches += launch_kfdb_score((const KfdbQueryJob*)c.dev(o_jobs), n_jobs, max_slots, max_nq, q[0].db->n_sm, m->stream);
     }
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
+    const borb_status s = c.finish();
+    if (s != BORB_OK) return s;
     for (int j = 0; j < n_jobs; j++) {
-        const uint8_t* o = m->h_out + ho[j];
+        const uint8_t* o = c.out(ho[j]);
         std::memcpy(q[j].common, o, (size_t)ns[j] * 4);
         std::memcpy(q[j].score, o + (size_t)ns[j] * 4, (size_t)ns[j] * 4);
         std::memcpy(q[j].first_word, o + (size_t)ns[j] * 8, (size_t)ns[j] * 4);
@@ -1854,6 +1718,7 @@ borb_status bowdb_jobs(borb_matcher* m, const SearchJob* J, int n_jobs, float nn
     std::vector<int> work;
     for (int j = 0; j < n_jobs; j++) if (P[j].work) work.push_back(j);
     const int nw = (int)work.size();
+    Call c(m);
     {
         std::vector<borb_kfdb*> dbs(n_jobs);
         for (int j = 0; j < n_jobs; j++) dbs[j] = J[j].db;
@@ -1869,25 +1734,23 @@ borb_status bowdb_jobs(borb_matcher* m, const SearchJob* J, int n_jobs, float nn
         }
         if (nw == 0) return BORB_OK;
         BORB_CUDA(cudaSetDevice(m->device));
-        borb_status s = lk.sync(m->stream);
+        borb_status s = lk.sync();
         if (s != BORB_OK) return s;
-        Stager st(m);
         for (int j : work) {
             const SearchJob& S = J[j];
             Plan& p = P[j];
             if (!S.frame) {                                            // a host view: its raw arrays, packed on the device like a resident frame
                 const borb_keyframe_view* v = S.view;
-                p.o_node = st.add(v->fv.node_id, (size_t)p.nn * 4); p.o_start = st.add(v->fv.start, (size_t)(p.nn + 1) * 4);
-                p.o_idx = st.add(v->fv.feat_idx, (size_t)p.m * 4);
-                p.o_keys = st.add(v->keys_un, (size_t)p.n * sizeof(borb_keypoint)); p.o_desc = st.add(v->desc, (size_t)p.n * 32);
+                p.o_node = c.in(v->fv.node_id, (size_t)p.nn * 4); p.o_start = c.in(v->fv.start, (size_t)(p.nn + 1) * 4);
+                p.o_idx = c.in(v->fv.feat_idx, (size_t)p.m * 4);
+                p.o_keys = c.in(v->keys_un, (size_t)p.n * sizeof(borb_keypoint)); p.o_desc = c.in(v->desc, (size_t)p.n * 32);
             }
-            p.o_sl = S.slots ? st.add(S.slots, (size_t)S.n_kf * 4) : 0;
+            p.o_sl = S.slots ? c.in(S.slots, (size_t)S.n_kf * 4) : 0;
         }
-        const size_t o_jobs = st.add(nullptr, (size_t)nw * sizeof(BowDbJob));       // filled in place
-        const size_t input_end = st.off;
-        size_t hist_bytes = 0, tab_bytes = 0, out_bytes = 0;
+        const size_t o_jobs = c.in(nullptr, (size_t)nw * sizeof(BowDbJob));       // filled in place
+        size_t hist_bytes = 0, tab_bytes = 0;
         for (int j : work) { hist_bytes += (size_t)J[j].n_kf * 32 * 4; tab_bytes += (size_t)J[j].n_kf * P[j].m * 4; }
-        const size_t o_hist = st.reserve(hist_bytes), o_tab = st.reserve(tab_bytes);
+        const size_t o_hist = c.scratch(hist_bytes), o_tab = c.scratch(tab_bytes);
         size_t hist_off = o_hist, tab_off = o_tab;
         int max_smem_frame = 0, max_nn = 0, total_kf = 0;
         long long max_items = 0;
@@ -1895,25 +1758,19 @@ borb_status bowdb_jobs(borb_matcher* m, const SearchJob* J, int n_jobs, float nn
             const SearchJob& S = J[j];
             Plan& p = P[j];
             p.h = frame_block_layout(p.nn, p.m, p.n);
-            p.o_fb = st.reserve((size_t)p.h.bytes);
-            p.o_ctr = st.reserve(16);
+            p.o_fb = c.scratch((size_t)p.h.bytes);
+            p.o_ctr = c.scratch(16);
             p.o_hist = hist_off; hist_off += (size_t)S.n_kf * 32 * 4;
             p.o_tab = tab_off; tab_off += (size_t)S.n_kf * p.m * 4;
-            p.o_dense = S.dense ? st.reserve((size_t)S.n_kf * p.n * 4) : 0;
-            p.ho = out_bytes; out_bytes += ((size_t)S.n_kf * 8 + (S.pairs ? (size_t)S.pairs_cap * 4 : 0) + 15) & ~size_t(15);
+            p.o_dense = S.dense ? c.scratch((size_t)S.n_kf * p.n * 4) : 0;
+            p.ho = c.result((size_t)S.n_kf * 8 + (S.pairs ? (size_t)S.pairs_cap * 4 : 0));
             if (bowdb_frame_fits_smem(p.h.bytes)) max_smem_frame = std::max(max_smem_frame, p.h.bytes);
             max_nn = std::max(max_nn, p.nn);
             max_items += (long long)std::min(p.nn, p.m) * S.n_kf;
             total_kf += S.n_kf;
         }
-        const size_t total = st.off;
-        st.off = input_end;
-        if ((s = ensure_host(m, input_end)) != BORB_OK) return s;
-        if ((s = ensure_arena(m, total)) != BORB_OK) return s;
-        if ((s = ensure_out(m, out_bytes + 64)) != BORB_OK) return s;
-        BORB_CUDA(cudaStreamSynchronize(m->stream));
-        uint8_t* b = m->arena;
-        BowDbJob* hj = reinterpret_cast<BowDbJob*>(m->h_stage + o_jobs);
+        if ((s = c.begin()) != BORB_OK) return s;
+        BowDbJob* hj = c.host<BowDbJob>(o_jobs);
         int kf_base = 0;
         for (int w = 0; w < nw; w++) {
             const SearchJob& S = J[work[w]];
@@ -1923,47 +1780,46 @@ borb_status bowdb_jobs(borb_matcher* m, const SearchJob* J, int n_jobs, float nn
                 D.fv_node = S.frame->fv_node; D.fv_start = S.frame->fv_start; D.fv_idx = S.frame->fv_idx;
                 D.keys = S.frame->keys; D.desc = S.frame->desc;
             } else {
-                D.fv_node = (const uint32_t*)(b + p.o_node); D.fv_start = (const int32_t*)(b + p.o_start); D.fv_idx = (const uint32_t*)(b + p.o_idx);
-                D.keys = (const borb_keypoint*)(b + p.o_keys); D.desc = b + p.o_desc;
+                D.fv_node = (const uint32_t*)c.dev(p.o_node); D.fv_start = (const int32_t*)c.dev(p.o_start); D.fv_idx = (const uint32_t*)c.dev(p.o_idx);
+                D.keys = (const borb_keypoint*)c.dev(p.o_keys); D.desc = c.dev(p.o_desc);
             }
             D.nn = p.nn; D.m = p.m; D.n = p.n; D.item_target = g_bow_item_target.load();
-            D.frame_block = b + p.o_fb; D.frame_bytes = p.h.bytes; D.frame_in_smem = bowdb_frame_fits_smem(p.h.bytes) ? 1 : 0;
-            D.table = S.db->d_stream; D.slots = S.slots ? (const int32_t*)(b + p.o_sl) : nullptr;
+            D.frame_block = c.dev(p.o_fb); D.frame_bytes = p.h.bytes; D.frame_in_smem = bowdb_frame_fits_smem(p.h.bytes) ? 1 : 0;
+            D.table = S.db->d_stream; D.slots = S.slots ? (const int32_t*)c.dev(p.o_sl) : nullptr;
             D.n_kf = S.n_kf; D.kf_base = kf_base; kf_base += S.n_kf;
-            D.ctr = (int*)(b + p.o_ctr);
-            D.table_out = (uint32_t*)(b + p.o_tab); D.hist_out = (int*)(b + p.o_hist);
+            D.ctr = (int*)c.dev(p.o_ctr);
+            D.table_out = (uint32_t*)c.dev(p.o_tab); D.hist_out = (int*)c.dev(p.o_hist);
             // counts, offsets and the compact pair list are written by the finalize kernel straight into the pinned landing buffer
             // (device-addressable, UVA) - no device-to-host copies; the dense table (MBs) still goes through one copy
-            uint8_t* o = m->h_out + p.ho;
+            uint8_t* o = c.res(p.ho, true);
             D.n_matches = (int32_t*)o; D.pair_off = (int32_t*)(o + (size_t)S.n_kf * 4);
             D.pairs = S.pairs ? (uint32_t*)(o + (size_t)S.n_kf * 8) : nullptr; D.pairs_cap = S.pairs_cap;
-            D.dense = S.dense ? (int32_t*)(b + p.o_dense) : nullptr; D.dense_stride = p.n;
+            D.dense = S.dense ? (int32_t*)c.dev(p.o_dense) : nullptr; D.dense_stride = p.n;
             hj[w] = D;
         }
-        if ((s = commit(st, total)) != BORB_OK) return s;
-        BORB_CUDA(cudaMemsetAsync(b + o_hist, 0, hist_bytes, m->stream));
-        BORB_CUDA(cudaMemsetAsync(b + o_tab, 0xFF, tab_bytes, m->stream));
+        if ((s = c.commit()) != BORB_OK) return s;
+        BORB_CUDA(cudaMemsetAsync(c.dev(o_hist), 0, hist_bytes, m->stream));
+        BORB_CUDA(cudaMemsetAsync(c.dev(o_tab), 0xFF, tab_bytes, m->stream));
         for (int j : work) {
-            if (J[j].dense) BORB_CUDA(cudaMemsetAsync(b + P[j].o_dense, 0xFF, (size_t)J[j].n_kf * P[j].n * 4, m->stream));
-            if (J[j].frame) BORB_CUDA(cudaStreamWaitEvent(m->stream, J[j].frame->ready, 0));
+            if (J[j].dense) BORB_CUDA(cudaMemsetAsync(c.dev(P[j].o_dense), 0xFF, (size_t)J[j].n_kf * P[j].n * 4, m->stream));
+            if (J[j].frame && (s = c.wait(J[j].frame)) != BORB_OK) return s;
         }
         BowDbArgs A{};
-        A.jobs = (const BowDbJob*)(b + o_jobs); A.n_jobs = nw; A.static_sched = g_bow_static.load();
+        A.jobs = (const BowDbJob*)c.dev(o_jobs); A.n_jobs = nw; A.static_sched = g_bow_static.load();
         A.nnratio = nnratio; A.check_ori = check_ori;
         if (m->timing) BORB_CUDA(cudaEventRecord(m->t0, m->stream));
         m->launches += launch_bowdb(A, hj[0], max_smem_frame, max_items, total_kf, max_nn, g_bow_csa.load(), J[work[0]].db->n_sm, m->stream);
         if (m->timing) BORB_CUDA(cudaEventRecord(m->t1, m->stream));
-        BORB_CUDA(cudaGetLastError());
         for (int j : work)
-            if (J[j].dense) BORB_CUDA(cudaMemcpyAsync(J[j].dense, b + P[j].o_dense, (size_t)J[j].n_kf * P[j].n * 4, cudaMemcpyDeviceToHost, m->stream));
+            if (J[j].dense) BORB_CUDA(cudaMemcpyAsync(J[j].dense, c.dev(P[j].o_dense), (size_t)J[j].n_kf * P[j].n * 4, cudaMemcpyDeviceToHost, m->stream));
     }
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
+    if (const borb_status s = c.finish(); s != BORB_OK) return s;
     if (m->timing) { float ms = 0.f; if (cudaEventElapsedTime(&ms, m->t0, m->t1) == cudaSuccess) m->last_ms = ms; else cudaGetLastError(); }
     int overflow = -1;
     long long over_total = 0;
     for (int j : work) {
         const SearchJob& S = J[j];
-        const uint8_t* o = m->h_out + P[j].ho;
+        const uint8_t* o = c.out(P[j].ho);
         std::memcpy(S.n_matches, o, (size_t)S.n_kf * 4);
         if (S.pair_offset) std::memcpy(S.pair_offset, o + (size_t)S.n_kf * 4, (size_t)S.n_kf * 4);
         if (!S.pairs) continue;
@@ -2093,68 +1949,56 @@ borb_status triangulation_jobs(borb_matcher* m, const borb_triangulation_job* jo
     for (int j = 0; j < n_jobs; j++) if (J[j].live) live.push_back(j);
     const int nl = (int)live.size();
     if (nl == 0) return BORB_OK;
-    BORB_CUDA(cudaSetDevice(m->device));
-    Stager st(m);
+    Call c(m);
     for (int j : live) {
         const borb_triangulation_job& B = jobs[j];
         Job& Q = J[j];
-        if (!B.kf1_frame) Q.s1.o = stage_kf(st, &B.kf1);
-        else if (B.kf1.has_mp) Q.s1.o_hm = st.add(B.kf1.has_mp, (size_t)Q.s1.n);
-        if (!B.kf2_frame) Q.s2.o = stage_kf(st, &B.kf2);
+        if (!B.kf1_frame) Q.s1.o = stage_kf(c, &B.kf1);
+        else if (B.kf1.has_mp) Q.s1.o_hm = c.in(B.kf1.has_mp, (size_t)Q.s1.n);
+        if (!B.kf2_frame) Q.s2.o = stage_kf(c, &B.kf2);
         else {
-            if (B.kf2.has_mp) Q.s2.o_hm = st.add(B.kf2.has_mp, (size_t)Q.s2.n);
-            Q.s2.o_sig = st.add(B.kf2.level_sigma2, (size_t)B.kf2_frame->n_levels * 4);
+            if (B.kf2.has_mp) Q.s2.o_hm = c.in(B.kf2.has_mp, (size_t)Q.s2.n);
+            Q.s2.o_sig = c.in(B.kf2.level_sigma2, (size_t)B.kf2_frame->n_levels * 4);
         }
     }
-    const size_t o_jobs = st.add(nullptr, (size_t)nl * sizeof(TriJob));          // filled in place
-    const size_t input_end = st.off;
-    const size_t cnt_bytes = ((size_t)nl * 4 + 15) & ~size_t(15);
-    size_t res_bytes = cnt_bytes;                  // n_pairs of every live job, then every job's pairs: one D2H
+    const size_t o_jobs = c.in(nullptr, (size_t)nl * sizeof(TriJob));          // filled in place
+    const size_t r_cnt = c.result((size_t)nl * 4);       // n_pairs of every live job, then every job's pairs
     for (int j : live) {
         Job& Q = J[j];
-        Q.vm = st.reserve((size_t)Q.s1.n * 4); Q.bins = st.reserve((size_t)Q.s1.n);
-        Q.res = res_bytes; res_bytes += ((size_t)Q.cap * 8 + 15) & ~size_t(15);
+        Q.vm = c.scratch((size_t)Q.s1.n * 4); Q.bins = c.scratch((size_t)Q.s1.n);
+        Q.res = c.result((size_t)Q.cap * 8);
     }
-    const size_t o_res = st.reserve(res_bytes);
-    const size_t total = st.off;
-    st.off = input_end;
     borb_status s;
-    if ((s = ensure_host(m, input_end)) != BORB_OK) return s;
-    if ((s = ensure_arena(m, total)) != BORB_OK) return s;
-    if ((s = ensure_out(m, res_bytes)) != BORB_OK) return s;
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
-    uint8_t* b = m->arena;
-    TriJob* hj = reinterpret_cast<TriJob*>(m->h_stage + o_jobs);
+    if ((s = c.begin()) != BORB_OK) return s;
+    TriJob* hj = c.host<TriJob>(o_jobs);
     for (int k = 0; k < nl; k++) {
         const borb_triangulation_job& B = jobs[live[k]];
         const Job& Q = J[live[k]];
         TriJob T{};
-        T.q = B.kf1_frame ? resident_kf_dev(B.kf1_frame, B.kf1.has_mp ? b + Q.s1.o_hm : nullptr) : kf_dev(m, &B.kf1, Q.s1.o);
+        T.q = B.kf1_frame ? resident_kf_dev(B.kf1_frame, B.kf1.has_mp ? c.dev(Q.s1.o_hm) : nullptr) : kf_dev(c, &B.kf1, Q.s1.o);
         if (B.kf2_frame) {
-            T.t = resident_kf_dev(B.kf2_frame, B.kf2.has_mp ? b + Q.s2.o_hm : nullptr);
-            T.t.level_sigma2 = (const float*)(b + Q.s2.o_sig);
-        } else T.t = kf_dev(m, &B.kf2, Q.s2.o);
+            T.t = resident_kf_dev(B.kf2_frame, B.kf2.has_mp ? c.dev(Q.s2.o_hm) : nullptr);
+            T.t.level_sigma2 = (const float*)c.dev(Q.s2.o_sig);
+        } else T.t = kf_dev(c, &B.kf2, Q.s2.o);
         for (int i = 0; i < 9; i++) T.F[i] = B.F12[i];
         T.ex = B.ex; T.ey = B.ey; T.only_stereo = B.only_stereo;
-        T.vmatch = (int32_t*)(b + Q.vm); T.bins = b + Q.bins;
-        T.pairs = (int32_t*)(b + o_res + Q.res); T.cap = Q.cap; T.n_pairs = (int32_t*)(b + o_res) + k;
+        T.vmatch = (int32_t*)c.dev(Q.vm); T.bins = c.dev(Q.bins);
+        T.pairs = (int32_t*)c.res(Q.res, false); T.cap = Q.cap; T.n_pairs = (int32_t*)c.res(r_cnt, false) + k;
         hj[k] = T;
     }
-    if ((s = commit(st, total)) != BORB_OK) return s;
+    if ((s = c.commit()) != BORB_OK) return s;
     for (int j : live) {
-        if (jobs[j].kf1_frame) BORB_CUDA(cudaStreamWaitEvent(m->stream, jobs[j].kf1_frame->ready, 0));
-        if (jobs[j].kf2_frame) BORB_CUDA(cudaStreamWaitEvent(m->stream, jobs[j].kf2_frame->ready, 0));
+        if (jobs[j].kf1_frame && (s = c.wait(jobs[j].kf1_frame)) != BORB_OK) return s;
+        if (jobs[j].kf2_frame && (s = c.wait(jobs[j].kf2_frame)) != BORB_OK) return s;
     }
-    m->launches += launch_triangulation((const TriJob*)(b + o_jobs), nl, check_ori, m->stream);
-    BORB_CUDA(cudaGetLastError());
-    BORB_CUDA(cudaMemcpyAsync(m->h_out, b + o_res, res_bytes, cudaMemcpyDeviceToHost, m->stream));
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
+    m->launches += launch_triangulation((const TriJob*)c.dev(o_jobs), nl, check_ori, m->stream);
+    if ((s = c.finish()) != BORB_OK) return s;
     int overflow = -1;
     for (int k = 0; k < nl; k++) {
         const borb_triangulation_job& B = jobs[live[k]];
-        std::memcpy(B.n_pairs, m->h_out + (size_t)k * 4, 4);
+        std::memcpy(B.n_pairs, c.out(r_cnt) + (size_t)k * 4, 4);
         const int np = std::min(*B.n_pairs, B.cap);
-        if (np > 0) std::memcpy(B.pairs, m->h_out + J[live[k]].res, (size_t)np * 8);
+        if (np > 0) std::memcpy(B.pairs, c.out(J[live[k]].res), (size_t)np * 8);
         if (*B.n_pairs > B.cap && overflow < 0) overflow = live[k];
     }
     if (overflow >= 0) {
@@ -2383,66 +2227,55 @@ borb_status borb_frames_compute_bow(borb_matcher* m, borb_voc* v, borb_frame* co
     auto wants = [&](int i) {
         return (bow_word && bow_word[i]) || (bow_value && bow_value[i]) || (fv_node && fv_node[i]) || (fv_start && fv_start[i]) || (fv_idx && fv_idx[i]);
     };
-    BORB_CUDA(cudaSetDevice(m->device));
-    Stager st(m);
-    const size_t o_jobs = st.add(nullptr, (size_t)n_frames * sizeof(BowFrameJob));     // filled in place
-    const size_t input_end = st.off;
+    Call c(m);
+    const size_t o_jobs = c.in(nullptr, (size_t)n_frames * sizeof(BowFrameJob));     // filled in place
     std::vector<size_t> o_scr(n_frames), o_copy(n_frames, 0);
-    const size_t cnt_bytes = ((size_t)n_frames * 12 + 15) & ~size_t(15);
-    size_t res_bytes = cnt_bytes;                       // (n_bow, n_nodes, fv_start[n_nodes]) of every frame, then the host copies: one D2H
+    const size_t r_cnt = c.result((size_t)n_frames * 12);     // (n_bow, n_nodes, fv_start[n_nodes]) of every frame, then the host copies
     for (int i = 0; i < n_frames; i++) {
         const size_t n = (size_t)frames[i]->n;
-        o_scr[i] = st.reserve(n * 16);                  // weight f64 | word i32 | node i32
-        if (wants(i)) { o_copy[i] = res_bytes; res_bytes += (n * 24 + 4 + 15) & ~size_t(15); }   // value | word | node | start | idx
+        o_scr[i] = c.scratch(n * 16);                   // weight f64 | word i32 | node i32
+        if (wants(i)) o_copy[i] = c.result(n * 24 + 4);   // value | word | node | start | idx
     }
-    const size_t o_res = st.reserve(res_bytes);
-    const size_t total = st.off;
-    st.off = input_end;
     borb_status s;
-    if ((s = ensure_host(m, input_end)) != BORB_OK) return s;
-    if ((s = ensure_arena(m, total)) != BORB_OK) return s;
-    if ((s = ensure_out(m, res_bytes)) != BORB_OK) return s;
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
-    uint8_t* b = m->arena;
-    BowFrameJob* hj = reinterpret_cast<BowFrameJob*>(m->h_stage + o_jobs);
+    if ((s = c.begin()) != BORB_OK) return s;
+    BowFrameJob* hj = c.host<BowFrameJob>(o_jobs);
     for (int i = 0; i < n_frames; i++) {
         borb_frame* f = frames[i];
         const size_t n = (size_t)f->n;
         BowFrameJob J{};
         J.desc = f->desc; J.n = f->n;
-        J.weight = (double*)(b + o_scr[i]); J.word = (int32_t*)(b + o_scr[i] + n * 8); J.node = (int32_t*)(b + o_scr[i] + n * 12);
+        uint8_t* w = c.dev(o_scr[i]);
+        J.weight = (double*)w; J.word = (int32_t*)(w + n * 8); J.node = (int32_t*)(w + n * 12);
         J.dst = BowTables{f->bow_word, f->bow_value, f->fv_node, f->fv_start, f->fv_idx};
         if (wants(i)) {
-            uint8_t* c = b + o_res + o_copy[i];
-            J.copy = BowTables{(uint32_t*)(c + n * 8), (double*)c, (uint32_t*)(c + n * 12), (int32_t*)(c + n * 16), (uint32_t*)(c + n * 20 + 4)};
+            uint8_t* cp = c.res(o_copy[i], false);
+            J.copy = BowTables{(uint32_t*)(cp + n * 8), (double*)cp, (uint32_t*)(cp + n * 12), (int32_t*)(cp + n * 16), (uint32_t*)(cp + n * 20 + 4)};
         }
-        J.counts = (int32_t*)(b + o_res) + 3 * i;
+        J.counts = (int32_t*)c.res(r_cnt, false) + 3 * i;
         hj[i] = J;
         f->has_bow = false;                             // the storage is rewritten from here on
     }
-    if ((s = commit(st, total)) != BORB_OK) return s;
-    for (int i = 0; i < n_frames; i++) BORB_CUDA(cudaStreamWaitEvent(m->stream, frames[i]->ready, 0));
-    m->launches += launch_bow_frames(v->dev, (const BowFrameJob*)(b + o_jobs), n_frames, max_n, levelsup, m->stream);
-    BORB_CUDA(cudaGetLastError());
+    if ((s = c.commit()) != BORB_OK) return s;
+    for (int i = 0; i < n_frames; i++)
+        if ((s = c.wait(frames[i])) != BORB_OK) return s;
+    m->launches += launch_bow_frames(v->dev, (const BowFrameJob*)c.dev(o_jobs), n_frames, max_n, levelsup, m->stream);
     for (int i = 0; i < n_frames; i++) BORB_CUDA(cudaEventRecord(frames[i]->ready, m->stream));
-    BORB_CUDA(cudaMemcpyAsync(m->h_out, b + o_res, res_bytes, cudaMemcpyDeviceToHost, m->stream));
-    BORB_CUDA(cudaStreamSynchronize(m->stream));
-    const uint8_t* h = m->h_out;
+    if ((s = c.finish()) != BORB_OK) return s;
     for (int i = 0; i < n_frames; i++) {
         borb_frame* f = frames[i];
         int32_t cnt[3];
-        std::memcpy(cnt, h + (size_t)i * 12, 12);
+        std::memcpy(cnt, c.out(r_cnt) + (size_t)i * 12, 12);
         f->n_bow = cnt[0]; f->n_nodes = cnt[1]; f->n_fv = cnt[2]; f->has_bow = true;
         if (n_bow) n_bow[i] = cnt[0];
         if (n_nodes) n_nodes[i] = cnt[1];
         if (!wants(i)) continue;
         const size_t n = (size_t)f->n;
-        const uint8_t* c = h + o_copy[i];
-        if (bow_value && bow_value[i]) std::memcpy(bow_value[i], c, (size_t)cnt[0] * 8);
-        if (bow_word && bow_word[i]) std::memcpy(bow_word[i], c + n * 8, (size_t)cnt[0] * 4);
-        if (fv_node && fv_node[i]) std::memcpy(fv_node[i], c + n * 12, (size_t)cnt[1] * 4);
-        if (fv_start && fv_start[i]) std::memcpy(fv_start[i], c + n * 16, (size_t)(cnt[1] + 1) * 4);
-        if (fv_idx && fv_idx[i]) std::memcpy(fv_idx[i], c + n * 20 + 4, (size_t)cnt[2] * 4);
+        const uint8_t* cp = c.out(o_copy[i]);
+        if (bow_value && bow_value[i]) std::memcpy(bow_value[i], cp, (size_t)cnt[0] * 8);
+        if (bow_word && bow_word[i]) std::memcpy(bow_word[i], cp + n * 8, (size_t)cnt[0] * 4);
+        if (fv_node && fv_node[i]) std::memcpy(fv_node[i], cp + n * 12, (size_t)cnt[1] * 4);
+        if (fv_start && fv_start[i]) std::memcpy(fv_start[i], cp + n * 16, (size_t)(cnt[1] + 1) * 4);
+        if (fv_idx && fv_idx[i]) std::memcpy(fv_idx[i], cp + n * 20 + 4, (size_t)cnt[2] * 4);
     }
     return BORB_OK;
 }

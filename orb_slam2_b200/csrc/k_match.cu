@@ -897,19 +897,6 @@ int launch_grid_sort(const borb_keypoint* keys, int n, float minX, float minY, f
     grid_sort_kernel<<<1, 1024, K * 4, s>>>(keys, n, minX, minY, invW, invH, K, cell_start, cell_idx);
     return 1;
 }
-int launch_projection(const ProjArgs& A, cudaStream_t s) {
-    launch_candidates(A, s);
-    launch_resolve(A, false, s);
-    return 2;
-}
-int launch_projection_last(const LastArgs& L, const ProjArgs& A, cudaStream_t s) {
-    if (L.n_last > 0) {
-        project_points_kernel<<<(L.n_last + 255) / 256, 256, 0, s>>>(L);
-        launch_candidates(A, s);
-    }
-    launch_resolve(A, true, s);
-    return 3;
-}
 int launch_initialization(const ProjArgs& A, const borb_keypoint* keys1, int n1, int32_t* match12, int32_t* ev_idx, uint8_t* ev_bin,
                           float* prev, int* n_matches, cudaStream_t s) {
     launch_candidates(A, s);
@@ -933,15 +920,12 @@ int launch_distinctive(const uint8_t* desc, const int32_t* offsets, int n_points
     if (n_points > 0) distinctive_kernel<<<(n_points + 3) / 4, 128, 0, s>>>(desc, offsets, n_points, best_idx);
     return 1;
 }
-int launch_frustum_projection(const LastArgs& L, const ProjArgs& A, cudaStream_t s) {
-    if (L.n_last > 0) project_points_kernel<<<(L.n_last + 255) / 256, 256, 0, s>>>(L);
-    return 1 + launch_projection(A, s);
-}
-int launch_point_projection_batch(const LastArgs* d_last, const ProjArgs* d_jobs, int n_jobs, int max_nq, int max_n, int max_n_mp, bool last,
-                                  cudaStream_t s) {
+int launch_point_projection_batch(const LastArgs* d_last, const ProjArgs* d_jobs, const LastArgs& one_last, const ProjArgs& one, int n_jobs,
+                                  int max_nq, int max_n, int max_n_mp, bool last, cudaStream_t s) {
     if (n_jobs <= 0 || max_nq <= 0) return 0;
-    project_points_batch_kernel<<<dim3((max_nq + 255) / 256, n_jobs), 256, 0, s>>>(d_last);
-    return 1 + launch_projection_batch(d_jobs, n_jobs, max_n, max_n_mp, s, last);
+    if (n_jobs == 1) project_points_kernel<<<(one_last.n_last + 255) / 256, 256, 0, s>>>(one_last);
+    else project_points_batch_kernel<<<dim3((max_nq + 255) / 256, n_jobs), 256, 0, s>>>(d_last);
+    return 1 + launch_projection_batch(d_jobs, one, n_jobs, max_n, max_n_mp, s, last);
 }
 int launch_projection_argmin(const LastArgs& L, const ProjArgs& A, cudaStream_t s) {
     cudaMemsetAsync(A.out_match + A.n_mp, 0, sizeof(int), s);

@@ -101,7 +101,7 @@ __device__ __forceinline__ void candidates_body(const ProjArgs& A) {
     int count = 0;
     bool unsorted = false;
     // Every per-query input is fetched up front, independent loads back to back: in the small-call path they live in pinned
-    // HOST memory (borb_match_host.cu: in_base) and a dependent chain of PCIe round trips would dominate the kernel.
+    // HOST memory (borb_match_host.cu: Call::dev) and a dependent chain of PCIe round trips would dominate the kernel.
     const uint8_t valid_q = A.mp_valid != nullptr ? A.mp_valid[iMP] : (uint8_t)1;
     const int lvl_q = (A.mode == 0) ? A.level[iMP] : 0;
     const float vc_q = (A.mode == 0) ? A.view_cos[iMP] : 0.f;
@@ -402,8 +402,13 @@ void launch_candidates(const ProjArgs& A, cudaStream_t s) {
     if (A.n_mp > 0) proj_candidates_kernel<<<(A.n_mp + 7) / 8, 256, 0, s>>>(A);
 }
 
-int launch_projection_batch(const ProjArgs* d_jobs, int n_jobs, int max_n, int max_n_mp, cudaStream_t s, bool last) {
+int launch_projection_batch(const ProjArgs* d_jobs, const ProjArgs& one, int n_jobs, int max_n, int max_n_mp, cudaStream_t s, bool last) {
     if (n_jobs <= 0 || max_n_mp <= 0) return 0;
+    if (n_jobs == 1) {
+        launch_candidates(one, s);
+        launch_resolve(one, last, s);
+        return 2;
+    }
     proj_candidates_batch_kernel<<<dim3((max_n_mp + 7) / 8, n_jobs), 256, 0, s>>>(d_jobs);
     const size_t smem = resolve_smem_bytes(max_n, max_n_mp);
     const int threads = max_n_mp > 512 ? 1024 : (max_n_mp > 256 ? 512 : 256);

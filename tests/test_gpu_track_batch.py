@@ -192,6 +192,8 @@ def test_one_launch_sequence_whatever_the_job_count(M, oracle, views):
     FR = F.make_resident(mt)
     Cur, Last, T, K2 = last_job(M, views[8], 28, 0.1)
     CR = Cur.make_resident(mt)
+    PF, mps = mf.projection_case(views[7], 100, n_mp=50)
+    PR = PF.make_resident(mt)
     deltas = []
     for n in (1, 8):
         c0 = launches(mt)
@@ -199,8 +201,21 @@ def test_one_launch_sequence_whatever_the_job_count(M, oracle, views):
         c1 = launches(mt)
         mt.SearchByProjectionLastBatch([CR] * n, [Last] * n, [T] * n, K2, BF, 15.0)
         c2 = launches(mt)
-        deltas.append((c1 - c0, c2 - c1))
-    assert deltas[0] == deltas[1] == (3, 3), deltas
+        mt.SearchByProjectionBatch([PR] * n, [mps] * n, 3.0)
+        c3 = launches(mt)
+        deltas.append((c1 - c0, c2 - c1, c3 - c2))
+    assert deltas[0] == deltas[1] == (3, 3, 2), deltas
+
+    # the single calls: the same sequence on a resident frame, one grid sort more on a host view
+    def count(call):
+        c0 = launches(mt)
+        call()
+        return launches(mt) - c0
+
+    for frame, local_frame, cur, grid in ((PR, FR, CR, 0), (PF, F, Cur, 1)):
+        assert count(lambda: mt.SearchByProjection(frame, mps, 3.0)) == 2 + grid
+        assert count(lambda: mt.SearchLocalPoints(local_frame, P, pose[0], pose[1], K, BF, 3.0, has_obs=ho)) == 3 + grid
+        assert count(lambda: mt.SearchByProjectionLast(cur, Last, T, K2, BF, 15.0)) == 3 + grid
 
 
 def test_argument_errors_name_the_job_and_launch_nothing(M, oracle, views):
