@@ -256,7 +256,8 @@ borb_status ensure(borb_extractor* e, int w, int h, int n_images) {
     BORB_CUDA(cudaMalloc(&ws.sad, n * g.sel_image_stride * sizeof(int)));
     BORB_CUDA(cudaMalloc(&ws.pair_idx, n * 2 * sizeof(int)));
     BORB_CUDA(cudaMalloc(&ws.st_bins, n * stereo_bins_bytes_per_pair()));
-    BORB_CUDA(cudaMalloc(&ws.st_recs, n * (size_t)stereo_rec_stride(g) * stereo_rec_bytes()));
+    ws.st_recs_bytes = n * (size_t)stereo_rec_stride(g) * stereo_rec_bytes();
+    BORB_CUDA(cudaMalloc(&ws.st_recs, ws.st_recs_bytes));
     BORB_CUDA(cudaMalloc(&ws.tabs, (tabs.size() + 4) * sizeof(int16_t)));
     BORB_CUDA(cudaMemcpy(ws.tabs, tabs.data(), tabs.size() * sizeof(int16_t), cudaMemcpyHostToDevice));
     const std::vector<uint32_t>& slots = brief_slot_table();
@@ -474,10 +475,22 @@ borb_status enqueue_stereo(borb_extractor* eL, borb_extractor* eR, int n_pairs, 
         BORB_CUDA(cudaMemcpyAsync(e->ws.pair_idx, e->h_counts, idx.size() * sizeof(int), cudaMemcpyHostToDevice, e->stream));
         e->pair_cache = idx;
     }
+    // the records are the RIGHT images' keypoints: with two handles the right one may hold more than the left (nfeatures)
+    const int rec_stride = stereo_rec_stride(eR->geom);
+    const size_t rec_bytes = (size_t)n_pairs * rec_stride * stereo_rec_bytes();
+    if (rec_bytes > e->ws.st_recs_bytes) {
+        BORB_CUDA(cudaStreamSynchronize(e->stream));      // earlier stereo launches may still read the old buffer
+        cudaFree(e->ws.st_recs);
+        e->ws.st_recs = nullptr;
+        e->ws.st_recs_bytes = 0;
+        BORB_CUDA(cudaMalloc(&e->ws.st_recs, rec_bytes));
+        e->ws.st_recs_bytes = rec_bytes;
+    }
     StereoView L{eL->ws.pyr, eL->ws.kps, eL->ws.desc, eL->ws.nkp, eL->geom.pyr_image_stride, eL->geom.sel_image_stride};
     StereoView R{eR->ws.pyr, eR->ws.kps, eR->ws.desc, eR->ws.nkp, eR->geom.pyr_image_stride, eR->geom.sel_image_stride};
     mark(e, 6);
-    e->launches += launch_stereo(g, L, R, e->ws.pair_idx, n_pairs, bf, b, e->ws.u_right, e->ws.depth, e->ws.sad, g.sel_image_stride, e->ws.st_bins, e->ws.st_recs, e->stream);
+    e->launches += launch_stereo(g, L, R, e->ws.pair_idx, n_pairs, bf, b, e->ws.u_right, e->ws.depth, e->ws.sad, g.sel_image_stride,
+                                 e->ws.st_bins, e->ws.st_recs, rec_stride, e->stream);
     mark(e, 7);
     BORB_CUDA(cudaGetLastError());
     // borb_stereo_frames_results reads pairs in the default layout (left 2p, right 2p+1 of this handle's batch) only
@@ -868,6 +881,13 @@ borb_status borb_stereo_match2(borb_extractor* left, borb_extractor* right, floa
         set_error("left/right extractors differ in device or geometry");
         return BORB_ERR_INVALID_ARG;
     }
+    // the match kernel reads both pyramids and both keypoint sets with one scale table (level offsets, pitches, row bands)
+    for (int l = 0; l < left->geom.nlevels; l++)
+        if (left->geom.lv[l].scale != right->geom.lv[l].scale) {
+            set_error("left/right extractors differ in scale factor at level %d (%g vs %g)", l, (double)left->geom.lv[l].scale,
+                      (double)right->geom.lv[l].scale);
+            return BORB_ERR_INVALID_ARG;
+        }
     BORB_CUDA(cudaSetDevice(left->device));
     BORB_CUDA(cudaStreamSynchronize(right->stream));   // right results must be complete before left's stream reads them
     begin_step(left);

@@ -100,7 +100,8 @@ struct Workspace {
     uint32_t* brief_slots = nullptr;   // rBRIEF tap order, brief_slot_table()
     int* pair_idx = nullptr;       // 2 * max_pairs (left,right image indices)
     int* st_bins = nullptr;        // stereo row-bin offsets, per pair
-    void* st_recs = nullptr;       // stereo binned right-keypoint records, per pair
+    void* st_recs = nullptr;       // stereo binned right-keypoint records, per pair (sized by the right images' geometry)
+    size_t st_recs_bytes = 0;
     uint8_t* stage = nullptr;      // tightly packed H2D landing buffer (grow-only)
     size_t stage_bytes = 0;
     void* fast_tmaps = nullptr;    // HOST: per-level CUtensorMap set for fast_kernel (passed by value at launch)
@@ -154,8 +155,8 @@ struct StereoView {          // device pointers of one side of a stereo pair set
 };
 int launch_stereo(const Geometry& g, const StereoView& L, const StereoView& R, const int* d_pair_idx, int n_pairs,
                   float bf, float b, float* d_u_right, float* d_depth, int* d_sad, int out_stride, int* d_bins, void* d_recs,
-                  cudaStream_t s);
-int stereo_rec_stride(const Geometry& g);
+                  int rec_stride, cudaStream_t s);
+int stereo_rec_stride(const Geometry& g);   // records per pair for right images of geometry g
 size_t stereo_bins_bytes_per_pair();
 size_t stereo_rec_bytes();
 size_t quadtree_smem_bytes(int node_cap);

@@ -287,7 +287,7 @@ __global__ void __launch_bounds__(256) stereo_median_kernel(StereoView Lv, const
     }
 }
 
-// Worst-case records per pair: a band spans 2*ceil(2*scale_max)+2 rows, i.e. at most (that >> 3) + 2 bins.
+// Worst-case records per pair of right images of geometry g (their keypoint capacity): a band spans 2*ceil(2*scale_max)+2 rows, i.e. at most (that >> 3) + 2 bins.
 int stereo_rec_stride(const Geometry& g) {
     const int band = 2 * (int)ceilf(2.0f * g.lv[g.nlevels - 1].scale) + 3;
     return g.sel_image_stride * ((band >> SBIN_SHIFT) + 2);
@@ -297,8 +297,7 @@ size_t stereo_rec_bytes() { return sizeof(RightRec); }
 
 int launch_stereo(const Geometry& g, const StereoView& L, const StereoView& R, const int* d_pair_idx, int n_pairs,
                   float bf, float b, float* d_u_right, float* d_depth, int* d_sad, int out_stride, int* d_bins, void* d_recs,
-                  cudaStream_t s) {
-    const int rec_stride = stereo_rec_stride(g);
+                  int rec_stride, cudaStream_t s) {
     stereo_bin_kernel<<<n_pairs, 256, 0, s>>>(g, R, d_pair_idx, d_bins, reinterpret_cast<RightRec*>(d_recs), rec_stride);
     dim3 grid((g.sel_image_stride + 7) / 8, n_pairs);
     stereo_match_kernel<<<grid, 256, 0, s>>>(g, L, R, d_pair_idx, bf, b, d_u_right, d_depth, d_sad, out_stride, d_bins,
