@@ -113,7 +113,9 @@ BORB_API borb_status borb_sync(borb_extractor* e);
 
 /* Device-resident input variant: d_gray points to n_images images already in HBM on the handle's
  * device (image i at d_gray + i*image_stride, rows `pitch` bytes apart).  No host copies unless the
- * output pointers are non-NULL.  Used for the HBM-resident throughput measurement. */
+ * output pointers are non-NULL.  Used for the HBM-resident throughput measurement.  With rectification maps installed
+ * (borb_extractor_set_rectify_maps) the images are RAW width x height frames, rectified while they are read; the input
+ * format of borb_extractor_set_input_format does not apply: device images are always CV_8UC1. */
 BORB_API borb_status borb_extract_batch_device(borb_extractor* e, const uint8_t* d_gray, int n_images, int width, int height,
                                       size_t pitch, size_t image_stride, borb_keypoint* kps, uint8_t* desc, int cap,
                                       int* n_out);
@@ -249,6 +251,13 @@ BORB_API borb_status borb_frames_from_extractor(borb_matcher* m, borb_extractor*
                                                 int depth_type, float depth_factor, int depth_stride_bytes, borb_keypoint* keys_un,
                                                 float* u_right, float* depth_out, int cap, float* bounds4, borb_frame** frames);
 BORB_API borb_status borb_frame_info(const borb_frame* f, int32_t* n, int32_t* n_levels, int32_t* has_u_right);
+/* Read-only introspection of a resident frame (tests, debugging): waits for the frame to be complete and copies mvKeysUn (n),
+ * mDescriptors (n x 32), mvuRight / mvDepth (n; BORB_ERR_INVALID_ARG on a monocular frame) and the feature grid of
+ * Frame::AssignFeaturesToGrid flattened: cell_start[64*48 + 1], cell c = x*48 + y holding cell_idx[cell_start[c] ..
+ * cell_start[c+1]) in insertion order; cell_idx needs room for n entries (cell_start[64*48] are written: features whose
+ * PosInGrid fails are in no cell).  Any pointer may be NULL. */
+BORB_API borb_status borb_debug_frame_read(const borb_frame* f, borb_keypoint* keys, uint8_t* desc, float* u_right, float* depth,
+                                           int32_t* cell_start, int32_t* cell_idx);
 
 /* Local map points that passed Frame::isInFrustum (src/Frame.cc:269-325), in vpMapPoints order. */
 typedef struct borb_mappoint_view {

@@ -84,6 +84,25 @@ int frameref_features_in_area(const orbport_kp* k, int n, float minX, float minY
     return (int)v.size();
 }
 
+// AssignFeaturesToGrid, with Frame::mGrid flattened the way the device keeps it: cell c = x*FRAME_GRID_ROWS + y holds
+// cell_idx[cell_start[c] .. cell_start[c+1]) in insertion order (cell_start: FRAME_GRID_COLS*FRAME_GRID_ROWS + 1 entries,
+// cell_idx: n).  Returns the number of features in the grid.
+int frameref_assign_grid(const orbport_kp* k, int n, float minX, float minY, float maxX, float maxY, int32_t* cell_start, int32_t* cell_idx) {
+    set_bounds(minX, minY, maxX, maxY);
+    Frame F;
+    F.N = n;
+    F.mvKeysUn = make_keys(k, n);
+    F.AssignFeaturesToGrid();
+    int r = 0;
+    for (int x = 0; x < FRAME_GRID_COLS; x++)
+        for (int y = 0; y < FRAME_GRID_ROWS; y++) {
+            cell_start[x * FRAME_GRID_ROWS + y] = r;
+            for (size_t i : F.mGrid[x][y]) cell_idx[r++] = (int32_t)i;
+        }
+    cell_start[FRAME_GRID_COLS * FRAME_GRID_ROWS] = r;
+    return r;
+}
+
 // Frame::isInFrustum for n MapPoints (same outputs as orbport_is_in_frustum); the pose goes through SetPose / UpdatePoseMatrices
 int frameref_is_in_frustum(const float* world_pos, const float* normal, const float* max_distance, const float* min_distance,
                            const uint8_t* valid, int n, const float* Tcw, float fx, float fy, float cx, float cy, float mbf, float minX,

@@ -217,6 +217,20 @@ def _ptr(x):
     return None if x is None else C.c_void_p(x.ctypes.data)
 
 
+def port_remap(img, map_x, map_y):
+    """cv::remap(img, dst, map_x, map_y, INTER_LINEAR) restated (oracle/orb_prims.h remap_linear_u8, pinned to cv2)."""
+    lib = _plib()
+    img = _a(img, np.uint8); mx = _a(map_x, np.float32); my = _a(map_y, np.float32)
+    assert mx.shape == my.shape and mx.ndim == 2
+    out = np.zeros(mx.shape, np.uint8)
+    lib.orbport_remap_linear.restype = None
+    lib.orbport_remap_linear.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                         C.c_int]
+    lib.orbport_remap_linear(_ptr(img), img.shape[1], img.shape[0], img.strides[0], _ptr(mx), _ptr(my), _ptr(out), mx.shape[1],
+                             mx.shape[0], out.strides[0])
+    return out
+
+
 def port_features_in_area(keys, bounds, x, y, r, min_level, max_level):
     lib = _plib()
     keys = _a(keys, KP_DTYPE)
@@ -856,6 +870,29 @@ def ref_features_in_area(keys, bounds, x, y, r, min_level, max_level):
     n = lib.frameref_features_in_area(_ptr(keys), len(keys), *[float(b) for b in bounds], float(x), float(y), float(r), min_level,
                                       max_level, _ptr(out), len(out))
     return out[:n]
+
+
+GRID_CELLS = 64 * 48
+
+
+def _assign_grid(fn, keys, bounds):
+    keys = _a(keys, KP_DTYPE)
+    cs = np.zeros(GRID_CELLS + 1, np.int32)
+    ci = np.zeros(max(len(keys), 1), np.int32)
+    fn.restype = C.c_int
+    fn.argtypes = [C.c_void_p, C.c_int] + [C.c_float] * 4 + [C.c_void_p, C.c_void_p]
+    n = fn(_ptr(keys), len(keys), *[float(b) for b in bounds], _ptr(cs), _ptr(ci))
+    return cs, ci[:n]
+
+
+def ref_assign_grid(keys, bounds):
+    """Frame::AssignFeaturesToGrid of the reference source: (cell_start[64*48+1], cell_idx), cell = x*48 + y, insertion order."""
+    return _assign_grid(C.CDLL(FRAMEREF_SO).frameref_assign_grid, keys, bounds)
+
+
+def port_assign_grid(keys, bounds):
+    """The restatement's feature grid (oracle/orb_port_match.cpp build_grid), flattened as ref_assign_grid."""
+    return _assign_grid(_plib().orbport_assign_grid, keys, bounds)
 
 
 def ref_is_in_frustum(F, P, Tcw, K, mbf, viewing_cos_limit=0.5):

@@ -110,6 +110,19 @@ int orbport_features_in_area(const orbport_kp* k, int n, float minX, float minY,
     return (int)v.size();
 }
 
+// build_grid flattened the way the device keeps it: cell c = x*GRID_ROWS + y holds cell_idx[cell_start[c] .. cell_start[c+1])
+// in insertion order (cell_start: GRID_COLS*GRID_ROWS + 1 entries, cell_idx: n).  Returns the number of features in the grid.
+int orbport_assign_grid(const orbport_kp* k, int n, float minX, float minY, float maxX, float maxY, int32_t* cell_start, int32_t* cell_idx) {
+    const Grid g = build_grid(k, n, minX, minY, maxX, maxY);
+    int r = 0;
+    for (int c = 0; c < GRID_COLS * GRID_ROWS; c++) {
+        cell_start[c] = r;
+        for (int i : g.cell[c]) cell_idx[r++] = i;
+    }
+    cell_start[GRID_COLS * GRID_ROWS] = r;
+    return r;
+}
+
 // match_feat[iMP] = frame feature index claimed by map point iMP, or -1.  occupied may be NULL.
 int orbport_search_by_projection(const orbport_kp* keys_un, const uint8_t* desc, const float* u_right, const uint8_t* occupied, int N,
                                  float minX, float minY, float maxX, float maxY, const float* scale_factors, int n_mp,

@@ -26,9 +26,16 @@
 
 namespace orbprims {
 
-// cvRound: round-half-to-even (SSE cvtsd2si / cvtss2si under the default rounding mode).
-static inline int cv_round(double v) { return (int)std::lrint(v); }
-static inline int cv_round(float v) { return (int)std::lrintf(v); }
+// cvRound: round-half-to-even (SSE cvtsd2si / cvtss2si under the default rounding mode).  The 32-bit conversion saturates:
+// NaN and results outside int range give INT_MIN (the "integer indefinite" value), never a wrapped 64-bit result.
+static inline int cv_round(double v) {
+    const long r = std::lrint(v);
+    return (v != v || r < INT32_MIN || r > INT32_MAX) ? INT32_MIN : (int)r;
+}
+static inline int cv_round(float v) {
+    const long r = std::lrintf(v);
+    return (v != v || r < INT32_MIN || r > INT32_MAX) ? INT32_MIN : (int)r;
+}
 static inline int cv_floor(double v) { int i = (int)v; return i - (i > v); }
 static inline int cv_ceil(double v) { int i = (int)v; return i + (i < v); }
 

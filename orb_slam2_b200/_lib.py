@@ -77,6 +77,7 @@ _SIGNATURES = {
     "borb_frame_destroy": (C.c_int, [vp]),
     "borb_frames_from_extractor": (C.c_int, [vp, vp, vp, C.c_int, vp, vp, C.c_int, vp, C.c_int, C.c_float, C.c_int, vp, vp, vp, C.c_int, vp, vp]),
     "borb_frame_info": (C.c_int, [vp, i32p, i32p, i32p]),
+    "borb_debug_frame_read": (C.c_int, [vp, vp, vp, vp, vp, vp, vp]),
     "borb_search_by_projection": (C.c_int, [vp, vp, vp, C.c_float, C.c_float, vp, i32p]),
     "borb_search_by_projection_batch": (C.c_int, [vp, vp, vp, C.c_int, C.c_float, C.c_float, vp, vp]),
     "borb_search_by_projection_last": (C.c_int, [vp, vp, vp, vp, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float,

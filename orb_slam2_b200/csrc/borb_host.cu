@@ -411,8 +411,18 @@ borb_status upload_slots(borb_extractor* e, const uint8_t* const* slots, int n, 
     return BORB_OK;
 }
 
-borb_status upload_device(borb_extractor* e, const uint8_t* d_gray, int n, int w, int h, size_t pitch, size_t image_stride) {
+// Device images -> level 0.  With rectification maps installed the images are RAW frames (w, h the raw size) and the remap
+// reads them in place; stereo_pairs applies set 1 (when installed) to the odd images, as upload_slots does.  The input
+// format of host images does not apply: device images are always CV_8UC1.
+borb_status upload_device(borb_extractor* e, const uint8_t* d_gray, int n, int w, int h, size_t pitch, size_t image_stride,
+                          bool stereo_pairs = false) {
     const Geometry& g = e->geom;
+    if (e->d_map[0][0]) {
+        if (pitch > (size_t)INT_MAX) { set_error("pitch %zu too large", pitch); return BORB_ERR_INVALID_ARG; }
+        e->launches += launch_repack_remap(g, e->ws, d_gray, (int)pitch, image_stride, w, h, e->d_map[0][0], e->d_map[0][1],
+                                           stereo_pairs ? e->d_map[1][0] : nullptr, stereo_pairs ? e->d_map[1][1] : nullptr, n, e->stream);
+        return BORB_OK;
+    }
     cudaMemcpy3DParms p = {};
     p.srcPtr = make_cudaPitchedPtr((void*)d_gray, pitch, w, image_stride / pitch);
     p.dstPtr = make_cudaPitchedPtr(e->ws.pyr + g.lv[0].pyr_off, g.lv[0].pitch, w, g.pyr_image_stride / g.lv[0].pitch);
@@ -706,7 +716,9 @@ borb_status borb_extract_batch_device(borb_extractor* e, const uint8_t* d_gray, 
     if (st != BORB_OK) return st;
     if (n == 0) return BORB_OK;
     if (!d_gray || pitch < (size_t)w) { set_error("bad arguments"); return BORB_ERR_INVALID_ARG; }
-    if ((st = ensure(e, w, h, n)) != BORB_OK) return st;
+    int gw = w, gh = h;
+    if ((st = rectified_size(e, w, h, &gw, &gh)) != BORB_OK) return st;
+    if ((st = ensure(e, gw, gh, n)) != BORB_OK) return st;
     begin_step(e);
     mark(e, 0);
     if ((st = upload_device(e, d_gray, n, w, h, pitch, image_stride)) != BORB_OK) return st;
@@ -944,10 +956,12 @@ borb_status borb_stereo_frames_device_enqueue(borb_extractor* e, const uint8_t* 
     if (st != BORB_OK) return st;
     if (n_pairs == 0) return BORB_OK;
     if (!d_gray || pitch < (size_t)w || !(b > 0.f)) { set_error("bad arguments"); return BORB_ERR_INVALID_ARG; }
-    if ((st = ensure(e, w, h, 2 * n_pairs)) != BORB_OK) return st;
+    int gw = w, gh = h;
+    if ((st = rectified_size(e, w, h, &gw, &gh)) != BORB_OK) return st;
+    if ((st = ensure(e, gw, gh, 2 * n_pairs)) != BORB_OK) return st;
     begin_step(e);
     mark(e, 0);
-    if ((st = upload_device(e, d_gray, 2 * n_pairs, w, h, pitch, image_stride)) != BORB_OK) return st;
+    if ((st = upload_device(e, d_gray, 2 * n_pairs, w, h, pitch, image_stride, true)) != BORB_OK) return st;
     if ((st = enqueue_extract(e, 2 * n_pairs)) != BORB_OK) return st;
     if ((st = enqueue_stereo(e, e, n_pairs, nullptr, nullptr, bf, b)) != BORB_OK) return st;
     if ((st = download_kps(e, 0, n_pairs, 2, nullptr, nullptr, cap, n_left)) != BORB_OK) return st;

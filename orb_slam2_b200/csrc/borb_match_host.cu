@@ -531,6 +531,28 @@ borb_status borb_frame_info(const borb_frame* f, int32_t* n, int32_t* n_levels, 
     return BORB_OK;
 }
 
+borb_status borb_debug_frame_read(const borb_frame* f, borb_keypoint* keys, uint8_t* desc, float* u_right, float* depth, int32_t* cell_start,
+                                  int32_t* cell_idx) {
+    if (!f) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+    if ((u_right || depth) && !f->u_right) { set_error("a monocular frame has no mvuRight / mvDepth"); return BORB_ERR_INVALID_ARG; }
+    BORB_CUDA(cudaSetDevice(f->device));
+    BORB_CUDA(cudaEventSynchronize(f->ready));
+    const size_t n = (size_t)f->n;
+    if (n > 0) {
+        if (keys) BORB_CUDA(cudaMemcpy(keys, f->keys, n * sizeof(borb_keypoint), cudaMemcpyDeviceToHost));
+        if (desc) BORB_CUDA(cudaMemcpy(desc, f->desc, n * 32, cudaMemcpyDeviceToHost));
+        if (u_right) BORB_CUDA(cudaMemcpy(u_right, f->u_right, n * 4, cudaMemcpyDeviceToHost));
+        if (depth) BORB_CUDA(cudaMemcpy(depth, f->depth, n * 4, cudaMemcpyDeviceToHost));
+    }
+    std::vector<int32_t> cs(GRID_CELLS + 1);
+    BORB_CUDA(cudaMemcpy(cs.data(), f->cell_start, cs.size() * 4, cudaMemcpyDeviceToHost));
+    if (cell_start) std::memcpy(cell_start, cs.data(), cs.size() * 4);
+    const int in_grid = cs[GRID_CELLS];
+    if (in_grid < 0 || (size_t)in_grid > n) { set_error("grid of %d entries for %d features", in_grid, f->n); return BORB_ERR_STATE; }
+    if (cell_idx && in_grid > 0) BORB_CUDA(cudaMemcpy(cell_idx, f->cell_idx, (size_t)in_grid * 4, cudaMemcpyDeviceToHost));
+    return BORB_OK;
+}
+
 // ---- SearchByProjection(F, vpMapPoints, th): one (frame, map point list) pair of borb_search_by_projection or of
 // borb_search_by_projection_batch
 namespace {

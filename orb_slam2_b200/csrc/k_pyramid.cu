@@ -151,7 +151,10 @@ __global__ void __launch_bounds__(256) repack_remap_kernel(const uint8_t* __rest
     for (int i = 0; i < 4; i++)
         if (x0 + i < l0.w) {
             const size_t o = (size_t)y * l0.w + x0 + i;
-            const int sx = __float2int_rn(__fmul_rn(MX[o], 32.f)), sy = __float2int_rn(__fmul_rn(MY[o], 32.f));
+            // cvRound gives INT_MIN for NaN (the pixel reads the border); __float2int_rn(NaN) would be 0, i.e. pixel (0, 0).
+            // Out-of-range values saturate either way and land outside any source image.
+            const float mx = __fmul_rn(MX[o], 32.f), my = __fmul_rn(MY[o], 32.f);
+            const int sx = mx == mx ? __float2int_rn(mx) : INT_MIN, sy = my == my ? __float2int_rn(my) : INT_MIN;
             const int ix = max(-32768, min(32767, sx >> 5)), iy = max(-32768, min(32767, sy >> 5));     // saturate_cast<short>
             const int fx = sx & 31, fy = sy & 31;
             auto tap = [&](int yy, int xx) -> int {

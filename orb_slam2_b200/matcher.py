@@ -204,16 +204,30 @@ class ResidentFrame:
         except Exception:
             pass
 
+    def read(self, stereo: bool = True) -> dict:
+        """borb_debug_frame_read: what the device holds for this frame — keys_un, desc, u_right / depth (stereo / RGB-D frames) and
+        the feature grid flattened as cell_start[64*48 + 1], cell_idx (cell = x*48 + y, insertion order)."""
+        n = self.n
+        k = np.zeros(max(n, 1), KP_DTYPE); d = np.zeros((max(n, 1), 32), np.uint8)
+        ur = np.zeros(max(n, 1), np.float32) if stereo else None
+        dp = np.zeros(max(n, 1), np.float32) if stereo else None
+        cs = np.zeros(64 * 48 + 1, np.int32); ci = np.zeros(max(n, 1), np.int32)
+        check(self._lib.borb_debug_frame_read(self._h, _p(k), _p(d), _p(ur), _p(dp), _p(cs), _p(ci)), "borb_debug_frame_read")
+        return dict(keys_un=k[:n], desc=d[:n], u_right=ur[:n] if stereo else None, depth=dp[:n] if stereo else None, cell_start=cs,
+                    cell_idx=ci[:cs[-1]])
+
 
 class _CameraC(C.Structure):
     _fields_ = [(n, C.c_float) for n in ("fx", "fy", "cx", "cy", "k1", "k2", "p1", "p2", "k3", "bf")]
 
 
 def frames_from_extractor(matcher: "ORBmatcher", extractor, images, n_keys, K, dist=(0, 0, 0, 0, 0), bf: float = 0.0, mode: int = 0,
-                          depth=None, depth_factor: float = 1.0, want_host: bool = True):
+                          depth=None, depth_factor: float = 1.0, want_host: bool = True, depth_on_device: bool = False):
     """borb_frames_from_extractor: the Frame constructor tail (UndistortKeyPoints, ComputeStereoFromRGBD, AssignFeaturesToGrid,
     src/Frame.cc:404-434,643-664,230-245) on the device for images of the extractor's last batch.  K = (fx, fy, cx, cy),
     dist = (k1, k2, p1, p2, k3); mode 0 mono / 1 stereo / 2 RGB-D with depth = list of (h,w) float32 (metres) or uint16 (raw) maps.
+    Host maps whose rows are contiguous keep their row stride (one padded stride shared by the batch); with depth_on_device the
+    maps are tightly packed CUDA tensors (float32, or int16 / uint16 holding the raw values) and are read in place.
     Returns (frames, host) where frames[i] is a FrameView bound to the resident frame and host = dict(keys_un, u_right, depth, bounds)."""
     lib = _lib.load()
     images = np.ascontiguousarray(images, np.int32); nk = np.ascontiguousarray(n_keys, np.int32)
@@ -225,10 +239,17 @@ def frames_from_extractor(matcher: "ORBmatcher", extractor, images, n_keys, K, d
     b4 = np.zeros(4, np.float32)
     handles = (C.c_void_p * max(nf, 1))()
     dptr, dtype_flag, stride, keep = None, 0, 0, []
-    if mode == 2:
-        keep = [np.ascontiguousarray(d) for d in depth]
-        dtype_flag = 1 if keep[0].dtype == np.uint16 else 0
-        keep = [np.ascontiguousarray(d, np.uint16 if dtype_flag else np.float32) for d in keep]
+    if mode == 2 and depth_on_device:
+        keep = list(depth)
+        assert all(d.is_cuda and d.is_contiguous() and d.element_size() == keep[0].element_size() for d in keep)
+        dtype_flag = (1 if keep[0].element_size() == 2 else 0) | 4
+        dptr = (C.c_void_p * nf)(*[d.data_ptr() for d in keep])
+    elif mode == 2:
+        dtype_flag = 1 if np.asarray(depth[0]).dtype == np.uint16 else 0
+        dt = np.uint16 if dtype_flag else np.float32
+        keep = [np.asarray(d) for d in depth]
+        if not all(d.dtype == dt and d.strides[1] == d.itemsize and d.strides[0] == keep[0].strides[0] for d in keep):
+            keep = [np.ascontiguousarray(d, dt) for d in keep]
         stride = keep[0].strides[0]
         dptr = (C.c_void_p * nf)(*[d.ctypes.data for d in keep])
     check(lib.borb_frames_from_extractor(matcher._h, extractor._h, _p(images), nf, _p(nk), C.byref(cam), int(mode), dptr, dtype_flag,

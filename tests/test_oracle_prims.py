@@ -11,6 +11,7 @@ import pytest
 
 cv2 = pytest.importorskip("cv2")
 from orb_slam2_b200 import synth
+from tests.frame_input_cases import adversarial_remap_maps
 
 u8p = C.POINTER(C.c_uint8)
 i32p = C.POINTER(C.c_int32)
@@ -152,6 +153,39 @@ def test_remap_linear_matches_cv2(lib):
         lib.orbport_remap_linear(im.ctypes.data_as(u8p), im.shape[1], im.shape[0], im.strides[0], m1c.ctypes.data_as(f32p),
                                  m2c.ctypes.data_as(f32p), got.ctypes.data_as(u8p), m1.shape[1], m1.shape[0], got.strides[0])
         assert np.array_equal(got, want), int((got != want).sum())
+
+
+def _port_remap(lib, im, m1, m2):
+    got = np.zeros(m1.shape, np.uint8)
+    m1c, m2c = np.ascontiguousarray(m1, np.float32), np.ascontiguousarray(m2, np.float32)
+    lib.orbport_remap_linear(im.ctypes.data_as(u8p), im.shape[1], im.shape[0], im.strides[0], m1c.ctypes.data_as(f32p),
+                             m2c.ctypes.data_as(f32p), got.ctypes.data_as(u8p), m1.shape[1], m1.shape[0], got.strides[0])
+    return got
+
+
+@pytest.mark.parametrize("src,dst", [((64, 48), (61, 45)), ((64, 48), (130, 97)), ((37, 29), (23, 17)), ((160, 120), (159, 121))])
+def test_remap_linear_adversarial_maps_match_cv2(lib, src, dst):
+    """Map values where the 1/32-px rounding goes wrong: NaN, +-inf, finite values whose *32 leaves int range (cvRound saturates to
+    INT_MIN: the pixel reads the border), k/32 +- 1/64 ties (round half to even), taps at ix = -1 and ix = src_w - 1, destinations
+    larger and smaller than the source with dst_w % 4 in {1, 2, 3}."""
+    for mx, my in adversarial_remap_maps(src, dst, seed=sum(src) + sum(dst)):
+        im = np.random.default_rng(dst[0]).integers(1, 256, (src[1], src[0]), dtype=np.uint8)     # no zero pixel: border reads show
+        want = cv2.remap(im, mx, my, cv2.INTER_LINEAR)
+        got = _port_remap(lib, im, mx, my)
+        bad = np.argwhere(got != want)
+        assert len(bad) == 0, (len(bad), [(float(mx[tuple(b)]), float(my[tuple(b)])) for b in bad[:5]])
+
+
+def test_remap_linear_out_of_range_values_read_the_border(lib):
+    """The cases that separate a saturating cvRound from a wrapping one, pixel by pixel."""
+    im = np.full((40, 50), 200, np.uint8)
+    for v in (134217744.0, 2.0 ** 31, 2.0 ** 26, -(2.0 ** 26) - 64, np.inf, -np.inf, np.nan, 3.0e38):
+        mx = np.full((3, 5), 10.0, np.float32); my = np.full((3, 5), 10.0, np.float32)
+        mx[1, 2] = v
+        my[2, 3] = v
+        want = cv2.remap(im, mx, my, cv2.INTER_LINEAR)
+        assert want[1, 2] == 0 and want[2, 3] == 0 and want[0, 0] == 200, v
+        assert np.array_equal(_port_remap(lib, im, mx, my), want), v
 
 
 def test_small_float_gemm_order_matches_cv2():
