@@ -2061,6 +2061,8 @@ borb_status borb_voc_create(const int32_t* parent, const uint8_t* is_leaf, const
     // children in order of appearance; word ids in order of leaf appearance (loadFromTextFile :1378-1420)
     std::vector<int32_t> cstart(n_nodes + 1, 0), cids(n_nodes > 1 ? n_nodes - 1 : 0), word(n_nodes, -1);
     for (int i = 1; i < n_nodes; i++) cstart[parent[i] + 1]++;
+    for (int i = 0; i < n_nodes; i++)                  // the descent packs a child's rank into 23 bits (bow_descend, k_match.cu)
+        if (cstart[i + 1] >= (1 << 23)) { set_error("node %d: %d children, limit %d", i, cstart[i + 1], (1 << 23) - 1); return BORB_ERR_INVALID_ARG; }
     for (int i = 0; i < n_nodes; i++) cstart[i + 1] += cstart[i];
     std::vector<int32_t> fill(cstart.begin(), cstart.end() - 1);
     for (int i = 1; i < n_nodes; i++) cids[fill[parent[i]]++] = i;

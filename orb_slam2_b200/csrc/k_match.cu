@@ -754,10 +754,11 @@ __device__ __forceinline__ void bow_descend(const VocDev& V, const uint8_t* __re
         for (int c = c0 + lane; c < c1; c += 32) {
             const int id = V.child_ids[c];
             const int d = ham_words(feat, reinterpret_cast<const uint32_t*>(V.desc + (size_t)id * 32));
-            best = min(best, ((unsigned)d << 16) | (unsigned)(c - c0));     // strict '<': first child wins ties (:1244)
+            // distance <= 256 in the top 9 bits, the child's rank in the low 23 (borb_voc_create refuses wider nodes)
+            best = min(best, ((unsigned)d << 23) | (unsigned)(c - c0));     // strict '<': first child wins ties (:1244)
         }
         best = warp_min(best);
-        final_id = V.child_ids[c0 + (int)(best & 0xFFFFu)];
+        final_id = V.child_ids[c0 + (int)(best & 0x7FFFFFu)];
         if (level == nid_level) nid = final_id;
     }
     if (lane == 0) {

@@ -112,3 +112,18 @@ FB = M.FrameView(kb, rng.integers(0, 256, (6000, 32), dtype=np.uint8), X.GetScal
 mt.ComputeBoWBatch(voc6, [FR0, FB], 2, want_host=False)
 print("kfdb query batch", [q[0][:3] for q in mt.KfdbQueryBatch([db2, db3], [FR0, FB])])
 print("bowdb batch", [int(r[0].sum()) for r in mt.SearchByBoWDbBatch([db2, db3, db2], [None, None, [0, 5, 5]], [FR0, FB, FB])])
+
+# place-recognition envelope (tests/bow_envelope.py): the flat 70,000-word vocabulary, the 8192 x 8192 one-node database search,
+# and a job table of 2 * n_SM + 1 small shared-memory jobs (some CTA loads three or more frame blocks)
+from tests import bow_envelope as BE
+af = BE.vocabulary("flat70000")
+vf = M.ORBVocabulary.from_arrays(af["parent"], af["is_leaf"], af["desc"], af["weight"], af["k"], af["L"])
+print("flat voc", vf.transform_raw(BE.descriptors("flat70000")["high_ranks"], 0)[0][:4])
+c1 = BE.search_case("one_node_8192")
+db4 = M.KeyFrameDatabase(mt)
+for kf_ in c1["kfs"]:
+    db4.add(kf_, {0: 1.0})
+print("bowdb one node 8192", db4.SearchByBoWPairs(None, c1["F"])[0])
+import torch
+n_sm = torch.cuda.get_device_properties(0).multi_processor_count
+print("bowdb table", sum(int(r[0].sum()) for r in mt.SearchByBoWDbBatch(db2, [[j % 12] for j in range(2 * n_sm + 1)], [FR0] * (2 * n_sm + 1))))
