@@ -467,7 +467,9 @@ BORB_API borb_status borb_search_for_initialization(borb_matcher* m, const borb_
 BORB_API borb_status borb_distinctive_descriptors(borb_matcher* m, const uint8_t* desc, const int32_t* offsets, int n_points,
                                                   int32_t* best_idx);
 
-/* DBoW2::FeatureVector (ordered map NodeId -> feature indices) as CSR; node_id ascending. */
+/* DBoW2::FeatureVector (ordered map NodeId -> feature indices) as CSR: node_id strictly ascending, 0 <= start[0] <=
+ * start[1] <= ... <= start[n_nodes], and every feat_idx[r], r < start[n_nodes], below the view's n.  Every entry point that takes a
+ * borb_keyframe_view as a host view checks this and refuses a violator with BORB_ERR_INVALID_ARG before anything is launched. */
 typedef struct borb_featvec_view {
     int32_t n_nodes;
     const uint32_t* node_id;

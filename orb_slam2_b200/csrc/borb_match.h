@@ -300,9 +300,10 @@ int launch_kfdb_score(const KfdbQueryJob* d_jobs, int n_jobs, int max_slots, int
 int launch_distinctive(const uint8_t* desc, const int32_t* offsets, int n_points, int32_t* best_idx, cudaStream_t s);
 int launch_projection_argmin(const LastArgs& L, const ProjArgs& A, cudaStream_t s);
 int launch_sim3_agree(const int32_t* match1, const int32_t* match2, int n1, int n2, int32_t* match12, int* n_found, cudaStream_t s);
-// out_off: null (every pair against ts[0], output p at match + p * out_stride) or, mode 0, one target and output offset per pair
+// n_pairs searches in one launch (tables in device memory): pair p matches qs[p] against ts[p] and writes its output (mode 0: ts[p].n
+// entries, mode 1: qs[p].n) at match + out_off[p], its rotation bins at bins + out_off[p]; max_t = the largest ts[p].n
 int launch_bow_match(const KfDev* qs, const KfDev* ts, int n_pairs, int mode, float nnratio, int check_ori, int32_t* match,
-                     int out_stride, const size_t* out_off, uint8_t* bins, int32_t* n_matches, int max_t, cudaStream_t s);
+                     const size_t* out_off, uint8_t* bins, int32_t* n_matches, int max_t, cudaStream_t s);
 void host_image_bounds(int w, int h, const borb_camera& c, float* b4);
 int launch_frame_build(const FrameJob* d_jobs, int n_jobs, int max_n, const borb_camera& cam, int mode, int depth_type, float depth_factor, int w,
                        int h, int out_cap, borb_keypoint* keys_out, float* ur_out, float* depth_out, cudaStream_t s);

@@ -253,51 +253,78 @@ void read_counted(const uint8_t* r, int n, int32_t* out, int32_t* count) {
     std::memcpy(count, r + (size_t)n * 4, 4);
 }
 
-struct KfOffsets { size_t keys, desc, has_mp, u_right, node, start, idx, sf, sig; bool has_mp_p, ur_p; };
-
+// The checks of a host view, FeatureVector included: the kernels index shared and global memory with its node ranges and feature
+// indices, and the staging sizes its uploads from start[n_nodes].
 borb_status check_kf(const borb_keyframe_view* v, const char* what) {
-    if (!v || v->n < 0 || v->n > MATCH_MAX_FEATURES || (v->n > 0 && (!v->keys_un || !v->desc))) {
+    if (!v || v->n < 0 || v->n > MATCH_MAX_FEATURES || (v->n > 0 && (!v->keys_un || !v->desc)) ||
+        (v->n_levels < 0 && (v->scale_factors || v->level_sigma2))) {
         set_error("%s: bad keyframe view (n=%d, limit %d)", what, v ? v->n : -1, MATCH_MAX_FEATURES);
         return BORB_ERR_INVALID_ARG;
     }
-    if (v->fv.n_nodes < 0 || (v->fv.n_nodes > 0 && (!v->fv.node_id || !v->fv.start || !v->fv.feat_idx))) {
+    const borb_featvec_view& fv = v->fv;
+    if (fv.n_nodes < 0 || (fv.n_nodes > 0 && (!fv.node_id || !fv.start || !fv.feat_idx))) {
         set_error("%s: bad feature vector", what);
         return BORB_ERR_INVALID_ARG;
     }
+    if (fv.n_nodes == 0) return BORB_OK;
+    for (int a = 0; a < fv.n_nodes; a++)
+        if (fv.start[a + 1] < fv.start[a] || (a == 0 ? fv.start[0] < 0 : fv.node_id[a] <= fv.node_id[a - 1])) {
+            set_error("%s: FeatureVector nodes must ascend", what);
+            return BORB_ERR_INVALID_ARG;
+        }
+    for (int r = 0; r < fv.start[fv.n_nodes]; r++)
+        if (fv.feat_idx[r] >= (uint32_t)v->n) {
+            set_error("%s: FeatureVector index %u outside the keyframe's %d features", what, fv.feat_idx[r], v->n);
+            return BORB_ERR_INVALID_ARG;
+        }
     return BORB_OK;
 }
 
-KfOffsets stage_kf(Call& c, const borb_keyframe_view* v) {
-    KfOffsets o{};
-    o.keys = c.in(v->keys_un, (size_t)v->n * sizeof(borb_keypoint));
-    o.desc = c.in(v->desc, (size_t)v->n * 32);
-    o.has_mp_p = v->has_mp != nullptr;
-    o.has_mp = o.has_mp_p ? c.in(v->has_mp, (size_t)v->n) : 0;
-    o.ur_p = v->u_right != nullptr;
-    o.u_right = o.ur_p ? c.in(v->u_right, (size_t)v->n * 4) : 0;
-    o.node = c.in(v->fv.node_id, (size_t)v->fv.n_nodes * 4);
-    o.start = c.in(v->fv.start, (size_t)(v->fv.n_nodes + 1) * 4);
-    const int total = v->fv.n_nodes > 0 ? v->fv.start[v->fv.n_nodes] : 0;
-    o.idx = c.in(v->fv.feat_idx, (size_t)total * 4);
-    o.sf = c.in(v->scale_factors, (size_t)(v->scale_factors ? v->n_levels : 0) * 4);
-    o.sig = c.in(v->level_sigma2, (size_t)(v->level_sigma2 ? v->n_levels : 0) * 4);
-    return o;
-}
+const borb_keyframe_view NO_VIEW{};          // the view of a resident side that takes nothing from the caller
 
-KfDev kf_dev(const Call& c, const borb_keyframe_view* v, const KfOffsets& o) {
-    KfDev d;
-    d.n = v->n; d.nn = v->fv.n_nodes;
-    d.keys = reinterpret_cast<const borb_keypoint*>(c.dev(o.keys));
-    d.desc = c.dev(o.desc);
-    d.has_mp = o.has_mp_p ? c.dev(o.has_mp) : nullptr;
-    d.u_right = o.ur_p ? reinterpret_cast<const float*>(c.dev(o.u_right)) : nullptr;
-    d.node = reinterpret_cast<const uint32_t*>(c.dev(o.node));
-    d.start = reinterpret_cast<const int32_t*>(c.dev(o.start));
-    d.idx = reinterpret_cast<const uint32_t*>(c.dev(o.idx));
-    d.scale_factors = reinterpret_cast<const float*>(c.dev(o.sf));
-    d.level_sigma2 = reinterpret_cast<const float*>(c.dev(o.sig));
-    return d;
-}
+// One side of a BoW-guided search (SearchByBoW, SearchForTriangulation, the frame of the database search): a host view v, staged per
+// call, or a resident frame rf with its BoW, of which only v's has_mp and level_sigma2, when given, cross PCIe.  stage() comes before
+// Call::begin(), bind() after it.
+struct KfSide {
+    const borb_keyframe_view* v = &NO_VIEW;
+    const borb_frame* rf = nullptr;
+    size_t keys = 0, desc = 0, has_mp = 0, u_right = 0, node = 0, start = 0, idx = 0, sf = 0, sig = 0;
+
+    int n() const { return rf ? rf->n : v->n; }
+    int nn() const { return rf ? rf->n_nodes : v->fv.n_nodes; }
+    int m() const { return rf ? rf->n_fv : (v->fv.n_nodes > 0 ? v->fv.start[v->fv.n_nodes] : 0); }   // features inside the nodes
+    void stage(Call& c) {
+        if (v->has_mp) has_mp = c.in(v->has_mp, (size_t)n());
+        if (v->level_sigma2) sig = c.in(v->level_sigma2, (size_t)(rf ? rf->n_levels : v->n_levels) * 4);
+        if (rf) return;
+        keys = c.in(v->keys_un, (size_t)v->n * sizeof(borb_keypoint));
+        desc = c.in(v->desc, (size_t)v->n * 32);
+        if (v->u_right) u_right = c.in(v->u_right, (size_t)v->n * 4);
+        node = c.in(v->fv.node_id, (size_t)nn() * 4);
+        start = c.in(v->fv.start, (size_t)(nn() > 0 ? nn() + 1 : 0) * 4);
+        idx = c.in(v->fv.feat_idx, (size_t)m() * 4);
+        if (v->scale_factors) sf = c.in(v->scale_factors, (size_t)v->n_levels * 4);
+    }
+    KfDev bind(const Call& c) const {
+        KfDev d{};
+        d.n = n(); d.nn = nn();
+        d.has_mp = v->has_mp ? c.dev(has_mp) : nullptr;
+        d.level_sigma2 = v->level_sigma2 ? reinterpret_cast<const float*>(c.dev(sig)) : nullptr;
+        if (rf) {
+            d.keys = rf->keys; d.desc = rf->desc; d.u_right = rf->u_right; d.scale_factors = rf->sf;
+            d.node = rf->fv_node; d.start = rf->fv_start; d.idx = rf->fv_idx;
+            return d;
+        }
+        d.keys = reinterpret_cast<const borb_keypoint*>(c.dev(keys));
+        d.desc = c.dev(desc);
+        d.u_right = v->u_right ? reinterpret_cast<const float*>(c.dev(u_right)) : nullptr;
+        d.scale_factors = v->scale_factors ? reinterpret_cast<const float*>(c.dev(sf)) : nullptr;
+        d.node = reinterpret_cast<const uint32_t*>(c.dev(node));
+        d.start = reinterpret_cast<const int32_t*>(c.dev(start));
+        d.idx = reinterpret_cast<const uint32_t*>(c.dev(idx));
+        return d;
+    }
+};
 
 // packed vocabulary blob: header {magic, n_nodes, k, L, offsets...} followed by 256-byte aligned sections
 struct VocHeader { uint32_t magic; int32_t n_nodes, k, L; uint64_t off_desc, off_weight, off_word, off_cstart, off_cids, bytes; };
@@ -1316,52 +1343,9 @@ borb_status borb_distinctive_descriptors(borb_matcher* m, const uint8_t* desc, c
     return BORB_OK;
 }
 
-static borb_status bow_common(borb_matcher* m, const borb_keyframe_view* qs, int n_q, const borb_keyframe_view* t, int mode, float nnratio,
-                              int check_ori, int32_t* match, int32_t* n_matches) {
-    // mode 0: qs[0..n_q) keyframes vs ONE frame t, out stride t->n.   mode 1: n_q == 1, q = kf1, t = kf2, out stride q->n.
-    Call c(m);
-    std::vector<KfOffsets> qo(n_q);
-    for (int i = 0; i < n_q; i++) qo[i] = stage_kf(c, &qs[i]);
-    const KfOffsets to = stage_kf(c, t);
-    const size_t o_qd = c.in(nullptr, (size_t)n_q * sizeof(KfDev)), o_td = c.in(nullptr, sizeof(KfDev));     // filled in place
-    const int out_stride = mode == 0 ? t->n : qs[0].n;
-    const size_t o_bins = c.scratch((size_t)n_q * (out_stride > 0 ? out_stride : 1));
-    const size_t r_match = c.result((size_t)n_q * (out_stride > 0 ? out_stride : 1) * 4), r_nm = c.result((size_t)n_q * 4);
-    borb_status s;
-    if ((s = c.begin()) != BORB_OK) return s;
-    KfDev* hq = c.host<KfDev>(o_qd);
-    for (int i = 0; i < n_q; i++) hq[i] = kf_dev(c, &qs[i], qo[i]);
-    *c.host<KfDev>(o_td) = kf_dev(c, t, to);
-    if ((s = c.commit()) != BORB_OK) return s;
-    m->launches += launch_bow_match((const KfDev*)c.dev(o_qd), (const KfDev*)c.dev(o_td), n_q, mode, nnratio, check_ori, (int32_t*)c.res(r_match, false),
-                                    out_stride, nullptr, c.dev(o_bins), (int32_t*)c.res(r_nm, false), t->n, m->stream);
-    if ((s = c.finish()) != BORB_OK) return s;
-    if (out_stride > 0) std::memcpy(match, c.out(r_match), (size_t)n_q * out_stride * 4);
-    std::memcpy(n_matches, c.out(r_nm), (size_t)n_q * 4);
-    return BORB_OK;
-}
-
-borb_status borb_search_by_bow(borb_matcher* m, const borb_keyframe_view* kfs, int n_kf, const borb_keyframe_view* frame, float nnratio,
-                               int check_orientation, int32_t* match, int32_t* n_matches) {
-    if (!m || !frame || !match || !n_matches || n_kf < 0 || (n_kf > 0 && !kfs)) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
-    borb_status s = check_kf(frame, "borb_search_by_bow(frame)");
-    for (int i = 0; i < n_kf && s == BORB_OK; i++) s = check_kf(&kfs[i], "borb_search_by_bow(keyframe)");
-    if (s != BORB_OK) return s;
-    if (n_kf == 0) return BORB_OK;
-    return bow_common(m, kfs, n_kf, frame, 0, nnratio, check_orientation, match, n_matches);
-}
-
-borb_status borb_search_by_bow_kf(borb_matcher* m, const borb_keyframe_view* kf1, const borb_keyframe_view* kf2, float nnratio,
-                                  int check_orientation, int32_t* match12, int32_t* n_matches) {
-    if (!m || !kf1 || !kf2 || !match12 || !n_matches) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
-    borb_status s = check_kf(kf1, "borb_search_by_bow_kf(kf1)");
-    if (s == BORB_OK) s = check_kf(kf2, "borb_search_by_bow_kf(kf2)");
-    if (s != BORB_OK) return s;
-    return bow_common(m, kf1, 1, kf2, 1, nnratio, check_orientation, match12, n_matches);
-}
-
-// ---- TrackReferenceKeyFrame's SearchByBoW(KeyFrame*, Frame&) for many camera streams in one launch: each job's frame is resident
-// with its BoW (borb_frames_compute_bow); its keyframe is a host view, or a resident frame of which only has_mp crosses PCIe.
+// ---- SearchByBoW: borb_search_by_bow (keyframes against one frame), borb_search_by_bow_kf (one keyframe pair) and
+// borb_search_by_bow_batch (TrackReferenceKeyFrame of many camera streams: a keyframe against its own resident frame with BoW) are
+// jobs of one launch of bow_match_kernel and one synchronisation.
 namespace {
 borb_status check_resident_bow(const borb_frame* f, const borb_matcher* m, int j, const char* what) {
     if (!f) { set_error("job %d: %s is not a device-resident frame", j, what); return BORB_ERR_INVALID_ARG; }
@@ -1370,24 +1354,81 @@ borb_status check_resident_bow(const borb_frame* f, const borb_matcher* m, int j
     if (f->n > MATCH_MAX_FEATURES) { set_error("job %d: %s has %d features (limit %d)", j, what, f->n, MATCH_MAX_FEATURES); return BORB_ERR_INVALID_ARG; }
     return BORB_OK;
 }
-// a resident frame as the SearchByBoW side of a KfDev (has_mp from the caller)
-KfDev resident_kf_dev(const borb_frame* f, const uint8_t* has_mp) {
-    KfDev d{};
-    d.n = f->n; d.nn = f->n_nodes;
-    d.keys = f->keys; d.desc = f->desc; d.has_mp = has_mp; d.u_right = f->u_right;
-    d.node = f->fv_node; d.start = f->fv_start; d.idx = f->fv_idx;
-    d.scale_factors = f->sf;
-    return d;
+
+// q: the keyframe; t: the frame (mode 0) or kf2 (mode 1); match: t.n() entries (mode 0) or q.n() (mode 1)
+struct BowJob { KfSide q, t; int32_t* match; };
+
+// The arguments are checked by the callers.  Consecutive jobs with the same target share its staging.
+borb_status bow_jobs(borb_matcher* m, std::vector<BowJob>& J, int mode, float nnratio, int check_ori, int32_t* n_matches) {
+    const int n_jobs = (int)J.size();
+    std::vector<size_t> off(n_jobs + 1, 0);           // each job's matches in the result block
+    int max_t = 0;
+    for (int j = 0; j < n_jobs; j++) {
+        off[j + 1] = off[j] + (size_t)(mode == 0 ? J[j].t.n() : J[j].q.n());
+        max_t = std::max(max_t, J[j].t.n());
+    }
+    Call c(m);
+    for (int j = 0; j < n_jobs; j++) {
+        J[j].q.stage(c);
+        if (j > 0 && J[j].t.v == J[j - 1].t.v && J[j].t.rf == J[j - 1].t.rf) J[j].t = J[j - 1].t;
+        else J[j].t.stage(c);
+    }
+    const size_t o_q = c.in(nullptr, (size_t)n_jobs * sizeof(KfDev)), o_t = c.in(nullptr, (size_t)n_jobs * sizeof(KfDev));   // filled in place
+    const size_t o_off = c.in(nullptr, (size_t)n_jobs * sizeof(size_t));
+    const size_t o_bins = c.scratch(off[n_jobs] + 16);
+    const size_t r_cnt = c.result((size_t)n_jobs * 4), r_match = c.result(off[n_jobs] * 4);     // n_matches of every job, then every job's matches
+    borb_status s;
+    if ((s = c.begin()) != BORB_OK) return s;
+    KfDev* hq = c.host<KfDev>(o_q);
+    KfDev* ht = c.host<KfDev>(o_t);
+    size_t* hoff = c.host<size_t>(o_off);
+    for (int j = 0; j < n_jobs; j++) {
+        hq[j] = J[j].q.bind(c);
+        ht[j] = J[j].t.bind(c);
+        hoff[j] = off[j];
+    }
+    if ((s = c.commit()) != BORB_OK) return s;
+    for (const BowJob& B : J) {
+        if (B.q.rf && (s = c.wait(B.q.rf)) != BORB_OK) return s;
+        if (B.t.rf && (s = c.wait(B.t.rf)) != BORB_OK) return s;
+    }
+    m->launches += launch_bow_match((const KfDev*)c.dev(o_q), (const KfDev*)c.dev(o_t), n_jobs, mode, nnratio, check_ori,
+                                    (int32_t*)c.res(r_match, false), (const size_t*)c.dev(o_off), c.dev(o_bins), (int32_t*)c.res(r_cnt, false),
+                                    max_t, m->stream);
+    if ((s = c.finish()) != BORB_OK) return s;
+    std::memcpy(n_matches, c.out(r_cnt), (size_t)n_jobs * 4);
+    for (int j = 0; j < n_jobs; j++) std::memcpy(J[j].match, c.out(r_match) + off[j] * 4, (off[j + 1] - off[j]) * 4);
+    return BORB_OK;
 }
 }  // namespace
+
+borb_status borb_search_by_bow(borb_matcher* m, const borb_keyframe_view* kfs, int n_kf, const borb_keyframe_view* frame, float nnratio,
+                               int check_orientation, int32_t* match, int32_t* n_matches) {
+    if (!m || !frame || !match || !n_matches || n_kf < 0 || (n_kf > 0 && !kfs)) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+    borb_status s = check_kf(frame, "borb_search_by_bow(frame)");
+    for (int i = 0; i < n_kf && s == BORB_OK; i++) s = check_kf(&kfs[i], "borb_search_by_bow(keyframe)");
+    if (s != BORB_OK) return s;
+    if (n_kf == 0) return BORB_OK;
+    std::vector<BowJob> J(n_kf);
+    for (int i = 0; i < n_kf; i++) J[i] = BowJob{KfSide{&kfs[i]}, KfSide{frame}, match + (size_t)i * frame->n};
+    return bow_jobs(m, J, 0, nnratio, check_orientation, n_matches);
+}
+
+borb_status borb_search_by_bow_kf(borb_matcher* m, const borb_keyframe_view* kf1, const borb_keyframe_view* kf2, float nnratio,
+                                  int check_orientation, int32_t* match12, int32_t* n_matches) {
+    if (!m || !kf1 || !kf2 || !match12 || !n_matches) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+    borb_status s = check_kf(kf1, "borb_search_by_bow_kf(kf1)");
+    if (s == BORB_OK) s = check_kf(kf2, "borb_search_by_bow_kf(kf2)");
+    if (s != BORB_OK) return s;
+    std::vector<BowJob> J{BowJob{KfSide{kf1}, KfSide{kf2}, match12}};
+    return bow_jobs(m, J, 1, nnratio, check_orientation, n_matches);
+}
 
 borb_status borb_search_by_bow_batch(borb_matcher* m, const borb_bow_job* jobs, int n_jobs, float nnratio, int check_orientation,
                                      int32_t* n_matches) {
     if (!m || n_jobs < 0 || (n_jobs > 0 && (!jobs || !n_matches))) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
     if (n_jobs == 0) return BORB_OK;
-    int max_t = 0;
-    std::vector<size_t> off(n_jobs);                  // each job's matches in the result block (frames differ in n)
-    size_t total_n = 0;
+    std::vector<BowJob> J(n_jobs);
     for (int j = 0; j < n_jobs; j++) {
         const borb_bow_job& B = jobs[j];
         n_matches[j] = 0;
@@ -1397,46 +1438,9 @@ borb_status borb_search_by_bow_batch(borb_matcher* m, const borb_bow_job* jobs, 
         if (B.kf_frame) {
             if ((s = check_resident_bow(B.kf_frame, m, j, "kf_frame")) != BORB_OK) return s;
         } else if ((s = check_kf(&B.kf, "keyframe")) != BORB_OK) return job_fail(true, j, s);
-        max_t = std::max(max_t, B.frame->n);
-        off[j] = total_n; total_n += (size_t)B.frame->n;
+        J[j] = BowJob{KfSide{&B.kf, B.kf_frame}, KfSide{&NO_VIEW, B.frame}, B.match};
     }
-    Call c(m);
-    std::vector<KfOffsets> ko(n_jobs);
-    std::vector<size_t> o_hm(n_jobs, 0);
-    for (int j = 0; j < n_jobs; j++) {
-        const borb_bow_job& B = jobs[j];
-        if (!B.kf_frame) ko[j] = stage_kf(c, &B.kf);
-        else if (B.kf.has_mp) o_hm[j] = c.in(B.kf.has_mp, (size_t)B.kf_frame->n);
-    }
-    const size_t o_q = c.in(nullptr, (size_t)n_jobs * sizeof(KfDev)), o_t = c.in(nullptr, (size_t)n_jobs * sizeof(KfDev));   // filled in place
-    const size_t o_off = c.in(nullptr, (size_t)n_jobs * sizeof(size_t));
-    const size_t o_bins = c.scratch(total_n + 16);
-    const size_t r_cnt = c.result((size_t)n_jobs * 4), r_match = c.result(total_n * 4);     // n_matches of every job, then every job's matches
-    borb_status s;
-    if ((s = c.begin()) != BORB_OK) return s;
-    KfDev* hq = c.host<KfDev>(o_q);
-    KfDev* ht = c.host<KfDev>(o_t);
-    size_t* hoff = c.host<size_t>(o_off);
-    for (int j = 0; j < n_jobs; j++) {
-        const borb_bow_job& B = jobs[j];
-        hq[j] = B.kf_frame ? resident_kf_dev(B.kf_frame, B.kf.has_mp ? c.dev(o_hm[j]) : nullptr) : kf_dev(c, &B.kf, ko[j]);
-        ht[j] = resident_kf_dev(B.frame, nullptr);
-        hoff[j] = off[j];
-    }
-    if ((s = c.commit()) != BORB_OK) return s;
-    for (int j = 0; j < n_jobs; j++) {
-        if ((s = c.wait(jobs[j].frame)) != BORB_OK) return s;
-        if (jobs[j].kf_frame && (s = c.wait(jobs[j].kf_frame)) != BORB_OK) return s;
-    }
-    m->launches += launch_bow_match((const KfDev*)c.dev(o_q), (const KfDev*)c.dev(o_t), n_jobs, 0, nnratio, check_orientation,
-                                    (int32_t*)c.res(r_match, false), 0, (const size_t*)c.dev(o_off), c.dev(o_bins), (int32_t*)c.res(r_cnt, false),
-                                    max_t, m->stream);
-    if ((s = c.finish()) != BORB_OK) return s;
-    for (int j = 0; j < n_jobs; j++) {
-        std::memcpy(&n_matches[j], c.out(r_cnt) + (size_t)j * 4, 4);
-        std::memcpy(jobs[j].match, c.out(r_match) + off[j] * 4, (size_t)jobs[j].frame->n * 4);
-    }
-    return BORB_OK;
+    return bow_jobs(m, J, 0, nnratio, check_orientation, n_matches);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1512,10 +1516,6 @@ borb_status borb_kfdb_add(borb_kfdb* db, const borb_keyframe_view* kf, const uin
         if (bow_word[i] <= bow_word[i - 1]) { set_error("BowVector words must ascend (std::map order)"); return BORB_ERR_INVALID_ARG; }
     const int nn = kf->fv.n_nodes;
     const int m = nn > 0 ? kf->fv.start[nn] : 0;
-    for (int a = 0; a < nn; a++)
-        if (kf->fv.start[a + 1] < kf->fv.start[a] || (a > 0 && kf->fv.node_id[a] <= kf->fv.node_id[a - 1])) { set_error("FeatureVector nodes must ascend"); return BORB_ERR_INVALID_ARG; }
-    for (int r = 0; r < m; r++)
-        if (kf->fv.feat_idx[r] >= (uint32_t)kf->n) { set_error("FeatureVector index %u outside the keyframe's %d features", kf->fv.feat_idx[r], kf->n); return BORB_ERR_INVALID_ARG; }
     std::lock_guard<std::mutex> lk(db->mu);
     BORB_CUDA(cudaSetDevice(db->device));
     // one device block per keyframe: [node | start | orig | angle | hasmp | desc (rows in FeatureVector order) | bow words | bow values]
@@ -1725,13 +1725,13 @@ struct SearchJob {
 // slot lists, which are checked here under the database locks (a batch checks every job with keyframes, a single call only one
 // that has work, as before).
 borb_status bowdb_jobs(borb_matcher* m, const SearchJob* J, int n_jobs, float nnratio, int check_ori, bool batch) {
-    struct Plan { int nn, m, n; bool work; FrameBlockHdr h; size_t o_node, o_start, o_idx, o_keys, o_desc, o_fb, o_sl, o_ctr, o_hist, o_tab, o_dense, ho; };
+    struct Plan { KfSide f; int nn, m, n; bool work; FrameBlockHdr h; size_t o_fb, o_sl, o_ctr, o_hist, o_tab, o_dense, ho; };
     std::vector<Plan> P(n_jobs);
     for (int j = 0; j < n_jobs; j++) {
         const SearchJob& S = J[j];
         Plan& p = P[j];
-        if (S.frame) { p.nn = S.frame->n_nodes; p.m = S.frame->n_fv; p.n = S.frame->n; }
-        else { p.nn = S.view->fv.n_nodes; p.m = p.nn > 0 ? S.view->fv.start[p.nn] : 0; p.n = S.view->n; }
+        p.f = S.frame ? KfSide{&NO_VIEW, S.frame} : KfSide{S.view};
+        p.nn = p.f.nn(); p.m = p.f.m(); p.n = p.f.n();
         p.work = S.n_kf > 0 && p.m > 0;
         if (S.n_pairs_total) *S.n_pairs_total = 0;
         if (S.dense) for (size_t i = 0; i < (size_t)S.n_kf * p.n; i++) S.dense[i] = -1;
@@ -1761,12 +1761,7 @@ borb_status bowdb_jobs(borb_matcher* m, const SearchJob* J, int n_jobs, float nn
         for (int j : work) {
             const SearchJob& S = J[j];
             Plan& p = P[j];
-            if (!S.frame) {                                            // a host view: its raw arrays, packed on the device like a resident frame
-                const borb_keyframe_view* v = S.view;
-                p.o_node = c.in(v->fv.node_id, (size_t)p.nn * 4); p.o_start = c.in(v->fv.start, (size_t)(p.nn + 1) * 4);
-                p.o_idx = c.in(v->fv.feat_idx, (size_t)p.m * 4);
-                p.o_keys = c.in(v->keys_un, (size_t)p.n * sizeof(borb_keypoint)); p.o_desc = c.in(v->desc, (size_t)p.n * 32);
-            }
+            p.f.stage(c);                                              // a host view is packed on the device like a resident frame
             p.o_sl = S.slots ? c.in(S.slots, (size_t)S.n_kf * 4) : 0;
         }
         const size_t o_jobs = c.in(nullptr, (size_t)nw * sizeof(BowDbJob));       // filled in place
@@ -1797,14 +1792,9 @@ borb_status bowdb_jobs(borb_matcher* m, const SearchJob* J, int n_jobs, float nn
         for (int w = 0; w < nw; w++) {
             const SearchJob& S = J[work[w]];
             const Plan& p = P[work[w]];
+            const KfDev f = p.f.bind(c);
             BowDbJob D{};
-            if (S.frame) {
-                D.fv_node = S.frame->fv_node; D.fv_start = S.frame->fv_start; D.fv_idx = S.frame->fv_idx;
-                D.keys = S.frame->keys; D.desc = S.frame->desc;
-            } else {
-                D.fv_node = (const uint32_t*)c.dev(p.o_node); D.fv_start = (const int32_t*)c.dev(p.o_start); D.fv_idx = (const uint32_t*)c.dev(p.o_idx);
-                D.keys = (const borb_keypoint*)c.dev(p.o_keys); D.desc = c.dev(p.o_desc);
-            }
+            D.fv_node = f.node; D.fv_start = f.start; D.fv_idx = f.idx; D.keys = f.keys; D.desc = f.desc;
             D.nn = p.nn; D.m = p.m; D.n = p.n; D.item_target = g_bow_item_target.load();
             D.frame_block = c.dev(p.o_fb); D.frame_bytes = p.h.bytes; D.frame_in_smem = bowdb_frame_fits_smem(p.h.bytes) ? 1 : 0;
             D.table = S.db->d_stream; D.slots = S.slots ? (const int32_t*)c.dev(p.o_sl) : nullptr;
@@ -1860,16 +1850,9 @@ borb_status bowdb_jobs(borb_matcher* m, const SearchJob* J, int n_jobs, float nn
 }
 
 // the checks of the single database searches on their host view
-borb_status check_db_view(borb_matcher* m, borb_kfdb* db, const borb_keyframe_view* frame, int n_kf) {
+borb_status check_db_view(borb_matcher* m, borb_kfdb* db, const borb_keyframe_view* frame) {
     if (m->device != db->device) { set_error("matcher and keyframe database live on different devices"); return BORB_ERR_INVALID_ARG; }
-    borb_status s = check_kf(frame, "SearchByBoW(database, frame)");
-    if (s != BORB_OK || n_kf == 0) return s;
-    const int nn = frame->fv.n_nodes, mf = nn > 0 ? frame->fv.start[nn] : 0;
-    for (int a = 0; a < nn; a++)
-        if (frame->fv.start[a + 1] < frame->fv.start[a] || (a > 0 && frame->fv.node_id[a] <= frame->fv.node_id[a - 1])) { set_error("FeatureVector nodes must ascend"); return BORB_ERR_INVALID_ARG; }
-    for (int r = 0; r < mf; r++)
-        if (frame->fv.feat_idx[r] >= (uint32_t)frame->n) { set_error("FeatureVector index outside the frame's features"); return BORB_ERR_INVALID_ARG; }
-    return BORB_OK;
+    return check_kf(frame, "SearchByBoW(database, frame)");
 }
 
 // the checks of a batch job's database and resident frame
@@ -1908,7 +1891,7 @@ borb_status borb_kfdb_query_batch(borb_matcher* m, const borb_kfdb_query_job* jo
 borb_status borb_search_by_bow_db(borb_matcher* m, borb_kfdb* db, const int32_t* slots, int n_kf, const borb_keyframe_view* frame,
                                   float nnratio, int check_orientation, int32_t* match, int32_t* n_matches) {
     if (!m || !db || !frame || !match || !n_matches || n_kf < 0) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
-    borb_status s = check_db_view(m, db, frame, n_kf);
+    borb_status s = check_db_view(m, db, frame);
     if (s != BORB_OK) return s;
     const SearchJob J{db, nullptr, frame, slots, n_kf, match, n_matches, nullptr, nullptr, 0, nullptr};
     return bowdb_jobs(m, &J, 1, nnratio, check_orientation, false);
@@ -1918,7 +1901,7 @@ borb_status borb_search_by_bow_db_pairs(borb_matcher* m, borb_kfdb* db, const in
                                         float nnratio, int check_orientation, int32_t* n_matches, int32_t* pair_offset, uint32_t* pairs,
                                         int pairs_cap, int32_t* n_pairs_total) {
     if (!m || !db || !frame || !n_matches || n_kf < 0 || pairs_cap < 0 || (pairs && !pair_offset)) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
-    borb_status s = check_db_view(m, db, frame, n_kf);
+    borb_status s = check_db_view(m, db, frame);
     if (s != BORB_OK) return s;
     const SearchJob J{db, nullptr, frame, slots, n_kf, nullptr, n_matches, pair_offset, pairs, pairs_cap, n_pairs_total};
     return bowdb_jobs(m, &J, 1, nnratio, check_orientation, false);
@@ -1943,8 +1926,7 @@ borb_status borb_search_by_bow_db_batch(borb_matcher* m, const borb_bow_db_job* 
 // of triangulation_kernel, a CTA per job, and one synchronisation).  Each side is a host view or a resident frame with its BoW.
 namespace {
 borb_status triangulation_jobs(borb_matcher* m, const borb_triangulation_job* jobs, int n_jobs, int check_ori, bool batch) {
-    struct Side { int n, nn; KfOffsets o; size_t o_hm, o_sig; };
-    struct Job { Side s1, s2; bool live; int cap; size_t vm, bins, res; };
+    struct Job { KfSide s1, s2; bool live; int cap; size_t vm, bins, res; };
     std::vector<Job> J(n_jobs);
     for (int j = 0; j < n_jobs; j++) {
         const borb_triangulation_job& B = jobs[j];
@@ -1962,10 +1944,10 @@ borb_status triangulation_jobs(borb_matcher* m, const borb_triangulation_job* jo
             return job_fail(batch, j, BORB_ERR_INVALID_ARG);
         }
         Job& Q = J[j];
-        Q.s1.n = B.kf1_frame ? B.kf1_frame->n : B.kf1.n; Q.s1.nn = B.kf1_frame ? B.kf1_frame->n_nodes : B.kf1.fv.n_nodes;
-        Q.s2.n = B.kf2_frame ? B.kf2_frame->n : B.kf2.n; Q.s2.nn = B.kf2_frame ? B.kf2_frame->n_nodes : B.kf2.fv.n_nodes;
-        Q.live = Q.s1.n > 0 && Q.s1.nn > 0 && Q.s2.n > 0 && Q.s2.nn > 0;
-        Q.cap = std::min(B.cap, Q.s1.n);             // a job has at most one pair per kf1 feature
+        Q.s1 = KfSide{&B.kf1, B.kf1_frame};
+        Q.s2 = KfSide{&B.kf2, B.kf2_frame};
+        Q.live = Q.s1.n() > 0 && Q.s1.nn() > 0 && Q.s2.n() > 0 && Q.s2.nn() > 0;
+        Q.cap = std::min(B.cap, Q.s1.n());           // a job has at most one pair per kf1 feature
     }
     std::vector<int> live;
     for (int j = 0; j < n_jobs; j++) if (J[j].live) live.push_back(j);
@@ -1973,21 +1955,14 @@ borb_status triangulation_jobs(borb_matcher* m, const borb_triangulation_job* jo
     if (nl == 0) return BORB_OK;
     Call c(m);
     for (int j : live) {
-        const borb_triangulation_job& B = jobs[j];
-        Job& Q = J[j];
-        if (!B.kf1_frame) Q.s1.o = stage_kf(c, &B.kf1);
-        else if (B.kf1.has_mp) Q.s1.o_hm = c.in(B.kf1.has_mp, (size_t)Q.s1.n);
-        if (!B.kf2_frame) Q.s2.o = stage_kf(c, &B.kf2);
-        else {
-            if (B.kf2.has_mp) Q.s2.o_hm = c.in(B.kf2.has_mp, (size_t)Q.s2.n);
-            Q.s2.o_sig = c.in(B.kf2.level_sigma2, (size_t)B.kf2_frame->n_levels * 4);
-        }
+        J[j].s1.stage(c);
+        J[j].s2.stage(c);
     }
     const size_t o_jobs = c.in(nullptr, (size_t)nl * sizeof(TriJob));          // filled in place
     const size_t r_cnt = c.result((size_t)nl * 4);       // n_pairs of every live job, then every job's pairs
     for (int j : live) {
         Job& Q = J[j];
-        Q.vm = c.scratch((size_t)Q.s1.n * 4); Q.bins = c.scratch((size_t)Q.s1.n);
+        Q.vm = c.scratch((size_t)Q.s1.n() * 4); Q.bins = c.scratch((size_t)Q.s1.n());
         Q.res = c.result((size_t)Q.cap * 8);
     }
     borb_status s;
@@ -1997,11 +1972,8 @@ borb_status triangulation_jobs(borb_matcher* m, const borb_triangulation_job* jo
         const borb_triangulation_job& B = jobs[live[k]];
         const Job& Q = J[live[k]];
         TriJob T{};
-        T.q = B.kf1_frame ? resident_kf_dev(B.kf1_frame, B.kf1.has_mp ? c.dev(Q.s1.o_hm) : nullptr) : kf_dev(c, &B.kf1, Q.s1.o);
-        if (B.kf2_frame) {
-            T.t = resident_kf_dev(B.kf2_frame, B.kf2.has_mp ? c.dev(Q.s2.o_hm) : nullptr);
-            T.t.level_sigma2 = (const float*)c.dev(Q.s2.o_sig);
-        } else T.t = kf_dev(c, &B.kf2, Q.s2.o);
+        T.q = Q.s1.bind(c);
+        T.t = Q.s2.bind(c);
         for (int i = 0; i < 9; i++) T.F[i] = B.F12[i];
         T.ex = B.ex; T.ey = B.ey; T.only_stereo = B.only_stereo;
         T.vmatch = (int32_t*)c.dev(Q.vm); T.bins = c.dev(Q.bins);

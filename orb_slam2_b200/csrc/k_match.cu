@@ -3,8 +3,8 @@
 //   grid_sort_kernel      Frame::AssignFeaturesToGrid (src/Frame.cc:230-245): (cell, insertion) order by a bitonic sort in shared
 //       memory.  The windowed search itself (GetFeaturesInArea + claim resolution) lives in k_proj.cu.
 //   project_points_kernel the pose projections / frustum tests that feed it (src/ORBmatcher.cc:290-403,1328-1599, src/Frame.cc:269-325).
-//   bow_match_kernel      SearchByBoW(KeyFrame*,Frame&) (:159-288) and SearchByBoW(KeyFrame*,KeyFrame*) (:522-655) for keyframes
-//       staged from the host: a CTA per (keyframe, frame) pair deals the FeatureVector nodes to 8 warps (a feature lives in
+//   bow_match_kernel      SearchByBoW(KeyFrame*,Frame&) (:159-288) and SearchByBoW(KeyFrame*,KeyFrame*) (:522-655) over a
+//       table of pairs: a CTA per (keyframe, target) pair deals the FeatureVector nodes to 8 warps (a feature lives in
 //       exactly one node, so the greedy "already claimed" skip, :209/:576, never crosses nodes); per node the distance matrix is
 //       computed with all lanes busy, then the rows are replayed in order; rotation-histogram cull (:267-285) at the end.
 //       (The database-resident search of one frame against thousands of keyframes is k_bowdb.cu.)
@@ -491,11 +491,10 @@ constexpr int BOW_JCAP = 1024;      // widest target bucket the matrix path hand
 constexpr int BOW_RCAP = 256;       // rows per chunk
 constexpr int BOW_WARP_WORDS = BOW_DCAP / 2 + BOW_JCAP / 2 + BOW_RCAP / 2;
 
-// out_off (mode 0 only, may be null): pair p searches its own frame ts[p] and writes at match + out_off[p] (borb_search_by_bow_batch);
-// null: every pair searches ts[0] and writes at match + p * out_stride.
-__global__ void __launch_bounds__(32 * BOW_WARPS) bow_match_kernel(const KfDev* __restrict__ qs, const KfDev* __restrict__ ts, int n_pairs,
-                                                                   int mode, float nnratio, int check_ori, int32_t* __restrict__ match,
-                                                                   int out_stride, const size_t* __restrict__ out_off, uint8_t* __restrict__ bins,
+// A CTA per pair: pair p searches qs[p] against ts[p] and writes its match (and rotation bins) at out_off[p].
+__global__ void __launch_bounds__(32 * BOW_WARPS) bow_match_kernel(const KfDev* __restrict__ qs, const KfDev* __restrict__ ts, int mode,
+                                                                   float nnratio, int check_ori, int32_t* __restrict__ match,
+                                                                   const size_t* __restrict__ out_off, uint8_t* __restrict__ bins,
                                                                    int32_t* __restrict__ n_matches, int max_t) {
     extern __shared__ uint32_t sm[];
     __shared__ int hist[32];
@@ -508,8 +507,8 @@ __global__ void __launch_bounds__(32 * BOW_WARPS) bow_match_kernel(const KfDev* 
     uint16_t* J = D + BOW_DCAP;                                                  // target feature per column (0xFFFF = unusable)
     uint16_t* R = J + BOW_JCAP;                                                  // query feature per row of the chunk
     const KfDev q = qs[pair];
-    const KfDev t = ts[(mode == 0 && out_off == nullptr) ? 0 : pair];
-    const size_t o0 = out_off != nullptr ? out_off[pair] : (size_t)pair * out_stride;
+    const KfDev t = ts[pair];
+    const size_t o0 = out_off[pair];
     int32_t* out = match + o0;
     uint8_t* bin = bins + o0;
     const int nout = mode == 0 ? t.n : q.n;
@@ -943,12 +942,11 @@ int launch_sim3_agree(const int32_t* match1, const int32_t* match2, int n1, int 
     return 1;
 }
 int launch_bow_match(const KfDev* qs, const KfDev* ts, int n_pairs, int mode, float nnratio, int check_ori, int32_t* match,
-                     int out_stride, const size_t* out_off, uint8_t* bins, int32_t* n_matches, int max_t, cudaStream_t s) {
+                     const size_t* out_off, uint8_t* bins, int32_t* n_matches, int max_t, cudaStream_t s) {
     const int words = (max_t + 31) / 32;
     const size_t smem = (size_t)(words + BOW_WARPS * BOW_WARP_WORDS) * 4;
     allow_max_smem((const void*)bow_match_kernel);
-    bow_match_kernel<<<n_pairs, 32 * BOW_WARPS, smem, s>>>(qs, ts, n_pairs, mode, nnratio, check_ori, match, out_stride, out_off, bins, n_matches,
-                                                         max_t);
+    bow_match_kernel<<<n_pairs, 32 * BOW_WARPS, smem, s>>>(qs, ts, mode, nnratio, check_ori, match, out_off, bins, n_matches, max_t);
     return 1;
 }
 int launch_triangulation(const TriJob* d_jobs, int n_jobs, int check_ori, cudaStream_t s) {

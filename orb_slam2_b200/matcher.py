@@ -655,16 +655,7 @@ class ORBmatcher:
             match = np.full(max(nF, 1), -1, np.int32)
             J = jobs[j]
             J.frame = F.resident._h.value if F.resident is not None else None
-            if isinstance(kf, KeyFrameView):
-                J.kf = kf._c()
-                keep.append(list(kf._keep))              # the same view may serve several jobs: _c() replaces kf._keep
-            elif isinstance(kf, FrameView) and kf.resident is not None:
-                hm = np.ascontiguousarray(kf.has_mp, np.uint8) if kf.has_mp is not None else None
-                J.kf = _KeyFrameViewC(0, None, None, _p(hm))
-                J.kf_frame = kf.resident._h.value
-                keep.append(hm)
-            else:
-                raise ValueError(f"kfs[{j}]: a KeyFrameView or a device-resident FrameView")
+            J.kf, J.kf_frame, _ = self._kf_side(kf, keep)
             J.match = _p(match)
             outs.append((nF, match))
         nm = np.zeros(max(n, 1), np.int32)
@@ -746,9 +737,10 @@ class ORBmatcher:
         return pairs[:n.value]
 
     @staticmethod
-    def _tri_side(kf, keep):
-        """(borb_keyframe_view, resident frame handle, feature count) of one side of a triangulation job: a KeyFrameView, or a
-        device-resident FrameView with BoW and has_mp (then mvLevelSigma2 = mvScaleFactors^2 in float, ORBextractor's definition)."""
+    def _kf_side(kf, keep):
+        """(borb_keyframe_view, resident frame handle, feature count) of the keyframe side of a batched BoW-guided search: a
+        KeyFrameView, or a device-resident FrameView with BoW and has_mp (then only has_mp and mvLevelSigma2 = mvScaleFactors^2 in
+        float, ORBextractor's definition, cross PCIe)."""
         if isinstance(kf, KeyFrameView):
             c = kf._c()
             keep.append(list(kf._keep))                  # the same view may serve several jobs: _c() replaces kf._keep
@@ -760,6 +752,8 @@ class ORBmatcher:
             keep.append((hm, sg))
             return _KeyFrameViewC(0, None, None, _p(hm), n_levels=len(sg), level_sigma2=_p(sg)), kf.resident._h.value, kf.resident.n
         raise ValueError("a KeyFrameView or a device-resident FrameView")
+
+    _tri_side = _kf_side        # the name callers that assemble borb_triangulation_job tables by hand already use
 
     def SearchForTriangulationBatch(self, kf1s, kf2s, F12s, epipoles, bOnlyStereo=False, caps=None):
         """borb_search_for_triangulation_batch: SearchForTriangulation (src/ORBmatcher.cc:657-823) of many keyframe pairs in one launch.
@@ -773,8 +767,8 @@ class ORBmatcher:
         keep, outs = [], []
         for j in range(n):
             J = jobs[j]
-            J.kf1, J.kf1_frame, n1 = self._tri_side(kf1s[j], keep)
-            J.kf2, J.kf2_frame, _ = self._tri_side(kf2s[j], keep)
+            J.kf1, J.kf1_frame, n1 = self._kf_side(kf1s[j], keep)
+            J.kf2, J.kf2_frame, _ = self._kf_side(kf2s[j], keep)
             J.F12 = (C.c_float * 9)(*np.asarray(F12s[j], np.float32).reshape(9).tolist())
             J.ex, J.ey, J.only_stereo = float(epipoles[j][0]), float(epipoles[j][1]), int(ost[j])
             cap = n1 if cps[j] is None else int(cps[j])
