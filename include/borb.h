@@ -571,6 +571,9 @@ BORB_API borb_status borb_kfdb_add(borb_kfdb* db, const borb_keyframe_view* kf, 
                                    int n_bow, int32_t* slot_out);
 BORB_API borb_status borb_kfdb_erase(borb_kfdb* db, int32_t slot);                     /* KeyFrameDatabase::erase :49-66 */
 BORB_API borb_status borb_kfdb_set_has_mp(borb_kfdb* db, int32_t slot, const uint8_t* has_mp);   /* MapPoints culled / added since add() */
+/* borb_kfdb_set_has_mp for n slots (repeats allowed, the last mask wins) with one device synchronisation; every slot is checked
+ * before any mask changes. */
+BORB_API borb_status borb_kfdb_set_has_mp_batch(borb_kfdb* db, int n, const int32_t* slots, const uint8_t* const* has_mp);
 BORB_API borb_status borb_kfdb_size(const borb_kfdb* db, int32_t* n_slots, uint64_t* device_bytes);
 /* One query BowVector against every keyframe.  Outputs have one entry per slot (erased slots: 0 common words):
  * common_words[s], score[s] = (float)L1 score, first_word[s] = smallest shared word id (0xFFFFFFFF if none). */
@@ -635,6 +638,32 @@ typedef struct borb_bow_db_job {
  * single calls are the one-job case of the same launches. */
 BORB_API borb_status borb_search_by_bow_db_batch(borb_matcher* m, const borb_bow_db_job* jobs, int n_jobs, float nnratio,
                                                  int check_orientation);
+
+/* Loop closure: ORBmatcher::SearchByBoW(KeyFrame* pKF1, KeyFrame* pKF2, vector<MapPoint*>&) (src/ORBmatcher.cc:522-655) of the
+ * loop-closing keyframe against its candidates (LoopClosing::ComputeSim3, src/LoopClosing.cc:251-280), both sides read from the
+ * database: nothing crosses PCIe but the slot list and the results.  Both MapPoint masks are the database's (the caller keeps them
+ * current with borb_kfdb_set_has_mp).  Job j returns for candidate k the count and, in pairs[pair_offset[k] .. + n_matches[k]),
+ * (query feature) | (candidate feature) << 16 in the query's FeatureVector order: exactly borb_search_by_bow_kf(query, candidate).
+ * A query slot that is also a candidate is searched like any other.  Locks, outputs and errors as borb_search_by_bow_db_batch; the
+ * argument errors (text "job j:") are a NULL database or one on another device, a query slot that is erased, out of range or was
+ * added without features, a candidate that is not a live slot, slots == NULL with n_kf different from the slot count, pairs without
+ * pair_offset.  3 launches whatever n_jobs, one synchronisation; the single call is the one-job case. */
+typedef struct borb_bow_kf_db_job {
+    borb_kfdb* db;
+    int32_t query_slot;            /* KF1: the loop-closing keyframe, a live slot of db added with features */
+    const int32_t* slots;          /* KF2 candidates (repeats allowed); NULL: every slot, n_kf must be the slot count */
+    int32_t n_kf;
+    int32_t* n_matches;            /* outputs as borb_search_by_bow_db_pairs, pairs = query feature | candidate feature << 16, */
+    int32_t* pair_offset;          /*   each candidate's block in the query's FeatureVector order */
+    uint32_t* pairs;
+    int32_t pairs_cap;
+    int32_t* n_pairs_total;
+} borb_bow_kf_db_job;
+BORB_API borb_status borb_search_by_bow_kf_db_batch(borb_matcher* m, const borb_bow_kf_db_job* jobs, int n_jobs, float nnratio,
+                                                    int check_orientation);
+BORB_API borb_status borb_search_by_bow_kf_db_pairs(borb_matcher* m, borb_kfdb* db, int32_t query_slot, const int32_t* slots, int n_kf,
+                                                    float nnratio, int check_orientation, int32_t* n_matches, int32_t* pair_offset,
+                                                    uint32_t* pairs, int pairs_cap, int32_t* n_pairs_total);
 
 /* ---------------------------------------------------------------- vocabulary (BoW feeder) ---- */
 /* ORBVocabulary = DBoW2::TemplatedVocabulary<FORB> (Thirdparty/DBoW2/DBoW2/TemplatedVocabulary.h).  The tree lives
@@ -704,7 +733,8 @@ BORB_API borb_status borb_debug_set_fast_mode(borb_extractor* e, int mode);
  * min(cap, 512 * *n_bins) entries go to dst (may be NULL). */
 BORB_API borb_status borb_debug_brief_slots(uint32_t* dst, int cap, int* n_bins);
 /* Distance arithmetic of the database SearchByBoW kernel: 2 (default) = three 3:2 compressors + 5 POPC per 256-bit distance,
- * 1 = full carry-save adder tree + 4 POPC, 0 = 8 POPC.  Same results; kept switchable for measurements. */
+ * 1 = full carry-save adder tree + 4 POPC, 0 = 8 POPC.  Same results; kept switchable for measurements.  Applies to the
+ * relocalisation search (borb_search_by_bow_db*); the loop-closure search (borb_search_by_bow_kf_db_*) always uses mode 2. */
 BORB_API borb_status borb_debug_set_bow_csa(int mode);
 /* Work-item size of the same kernel: keyframes per item = target / (bucket width)^2, clamped to [1, 32] (default 2560); a negative
  * target selects the static item-to-warp schedule instead of the atomic work counter. */

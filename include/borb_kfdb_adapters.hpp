@@ -16,6 +16,7 @@
 #include <list>
 #include <mutex>
 #include <set>
+#include <stdexcept>
 #include <unordered_map>
 #include <utility>
 #include <vector>
@@ -197,6 +198,61 @@ inline std::vector<KeyFrameT*> kfdb_detect_loop(KfdbState<KeyFrameT>& S, KeyFram
     for (const auto& it : acc)
         if (it.first > minScoreToRetain && !added.count(it.second)) { out.push_back(it.second); added.insert(it.second); }
     return out;
+}
+
+// ORBmatcher::SearchByBoW(KeyFrame* pKF, KeyFrame* pKFi, vpMatches12) (src/ORBmatcher.cc:522-655) of the loop-closing keyframe
+// against every keyframe of `candidates` in ONE borb_search_by_bow_kf_db_pairs call (LoopClosing::ComputeSim3, :251-280).  Every
+// keyframe must have been added with its features.  The MapPoint masks of the query and the candidates are refreshed from
+// GetMapPointMatches() first (what the reference reads at call time) in one borb_kfdb_set_has_mp_batch, then vvpMatches[i] is
+// rebuilt as SearchByBoWKF rebuilds vpMatches12.  A candidate that has left the database meanwhile (erased after it passed
+// DetectLoopCandidates) gets 0 matches, which ComputeSim3 discards.  Returns the counts.
+template <class KeyFrameT, class MapPointT>
+inline std::vector<int> kfdb_search_loop_candidates(KfdbState<KeyFrameT>& S, KeyFrameT* pKF, const std::vector<KeyFrameT*>& candidates,
+                                                    float nnratio, bool checkOri, std::vector<std::vector<MapPointT*> >& vvpMatches) {
+    const size_t nc = candidates.size();
+    vvpMatches.assign(nc, std::vector<MapPointT*>());
+    std::vector<int> counts(nc, 0);
+    const std::vector<MapPointT*> vpMapPoints1 = pKF->GetMapPointMatches();
+    for (size_t i = 0; i < nc; i++) vvpMatches[i].assign(vpMapPoints1.size(), static_cast<MapPointT*>(nullptr));
+    if (nc == 0) return counts;
+    std::lock_guard<std::mutex> lk(S.mu);
+    const auto qit = S.slot_of.find(pKF);
+    if (qit == S.slot_of.end()) throw std::runtime_error("kfdb_search_loop_candidates: the loop-closing keyframe is not in the database");
+    std::vector<size_t> live;                                        // candidates still in the database
+    std::vector<int32_t> slots, mask_slots(1, qit->second);
+    std::vector<std::vector<MapPointT*> > mps2(nc);
+    std::vector<std::vector<uint8_t> > masks(1);
+    auto good = [](const std::vector<MapPointT*>& mps) {
+        std::vector<uint8_t> hm(mps.size());
+        for (size_t i = 0; i < mps.size(); i++) hm[i] = mps[i] && !mps[i]->isBad();                // :558-562, :574-580
+        return hm;
+    };
+    masks[0] = good(vpMapPoints1);
+    for (size_t i = 0; i < nc; i++) {
+        const auto it = S.slot_of.find(candidates[i]);
+        if (it == S.slot_of.end()) continue;
+        live.push_back(i);
+        slots.push_back(it->second);
+        mps2[i] = candidates[i]->GetMapPointMatches();
+        if (candidates[i] != pKF) { mask_slots.push_back(it->second); masks.push_back(good(mps2[i])); }
+    }
+    if (live.empty()) return counts;
+    std::vector<const uint8_t*> mask_ptr(masks.size());
+    for (size_t i = 0; i < masks.size(); i++) mask_ptr[i] = masks[i].data();
+    check(borb_kfdb_set_has_mp_batch(S.db, (int)mask_slots.size(), mask_slots.data(), mask_ptr.data()), "borb_kfdb_set_has_mp_batch");
+    const int nl = (int)live.size();
+    std::vector<int32_t> nm(nl), off(nl);
+    std::vector<uint32_t> pairs(vpMapPoints1.size() * nl + 1);
+    int32_t total = 0;
+    check(borb_search_by_bow_kf_db_pairs(thread_matcher(S.device), S.db, qit->second, slots.data(), nl, nnratio, checkOri, nm.data(), off.data(),
+                                         pairs.data(), (int)pairs.size(), &total), "borb_search_by_bow_kf_db_pairs");
+    for (int k = 0; k < nl; k++) {
+        const size_t i = live[k];
+        counts[i] = nm[k];
+        for (int32_t p = off[k]; p < off[k] + nm[k]; p++)
+            vvpMatches[i][pairs[p] & 0xFFFFu] = mps2[i][pairs[p] >> 16];                            // :602
+    }
+    return counts;
 }
 
 }  // namespace adapt

@@ -62,4 +62,13 @@ std::vector<KeyFrame*> KeyFrameDatabase::DetectRelocalizationCandidates(Frame* F
     return borb::adapt::kfdb_detect_relocalization(state_of(this), F);
 }
 
+#ifndef BORB_KFDB_SCORING_ONLY
+// LoopClosing::ComputeSim3's SearchByBoW(mpCurrentKF, pKF, vvpMapPointMatches[i]) (src/LoopClosing.cc:251-280) for every candidate
+// in one call on the resident keyframes (INTEGRATION.md shows the change to ComputeSim3).  Returns nmatches per candidate.
+std::vector<int> SearchLoopCandidatesByBoW(KeyFrameDatabase* pDB, KeyFrame* pKF, const std::vector<KeyFrame*>& candidates, float nnratio,
+                                           bool checkOri, std::vector<std::vector<MapPoint*> >& vvpMatches) {
+    return borb::adapt::kfdb_search_loop_candidates<KeyFrame, MapPoint>(state_of(pDB), pKF, candidates, nnratio, checkOri, vvpMatches);
+}
+#endif
+
 }  // namespace ORB_SLAM2

@@ -94,12 +94,15 @@ _SIGNATURES = {
     "borb_kfdb_add": (C.c_int, [vp, vp, vp, vp, C.c_int, i32p]),
     "borb_kfdb_erase": (C.c_int, [vp, C.c_int32]),
     "borb_kfdb_set_has_mp": (C.c_int, [vp, C.c_int32, vp]),
+    "borb_kfdb_set_has_mp_batch": (C.c_int, [vp, C.c_int, vp, vp]),
     "borb_kfdb_size": (C.c_int, [vp, i32p, C.POINTER(C.c_uint64)]),
     "borb_kfdb_query": (C.c_int, [vp, vp, vp, vp, C.c_int, vp, vp, vp, C.c_int, i32p]),
     "borb_search_by_bow_db": (C.c_int, [vp, vp, vp, C.c_int, vp, C.c_float, C.c_int, vp, vp]),
     "borb_search_by_bow_db_pairs": (C.c_int, [vp, vp, vp, C.c_int, vp, C.c_float, C.c_int, vp, vp, vp, C.c_int, i32p]),
     "borb_kfdb_query_batch": (C.c_int, [vp, vp, C.c_int]),
     "borb_search_by_bow_db_batch": (C.c_int, [vp, vp, C.c_int, C.c_float, C.c_int]),
+    "borb_search_by_bow_kf_db_batch": (C.c_int, [vp, vp, C.c_int, C.c_float, C.c_int]),
+    "borb_search_by_bow_kf_db_pairs": (C.c_int, [vp, vp, C.c_int32, vp, C.c_int, C.c_float, C.c_int, vp, vp, vp, C.c_int, i32p]),
     "borb_search_local_points": (C.c_int, [vp, vp, vp, vp, vp, vp] + [C.c_float] * 9 + [vp] * 7 + [i32p]),
     "borb_search_local_points_batch": (C.c_int, [vp, vp, C.c_int, C.c_float, C.c_float, vp]),
     "borb_search_by_projection_last_batch": (C.c_int, [vp, vp, C.c_int, C.c_int, vp]),

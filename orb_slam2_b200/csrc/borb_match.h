@@ -174,7 +174,10 @@ struct BowDbJob {
     const uint32_t* fv_node;
     const int32_t* fv_start;      // nn + 1
     const uint32_t* fv_idx;       // m
-    const borb_keypoint* keys;
+    union {
+        const borb_keypoint* keys;
+        const uint2* q_meta;      // SearchByBoW(KeyFrame*, KeyFrame*): the query slot's KfStream rows (fv_node / fv_start / desc are
+    };                            // its stream's, desc in row order, fv_idx unused)
     const uint8_t* desc;          // n x 32, 16-byte aligned
     int nn, m, n, item_target;    // item_target: keyframes per work item = item_target / nt^2, clamped to 1..32
     uint8_t* frame_block;         // FrameBlockHdr + sections, 128-byte aligned, frame_bytes = frame_block_layout(nn, m, n).bytes
@@ -309,8 +312,9 @@ int launch_frame_build(const FrameJob* d_jobs, int n_jobs, int max_n, const borb
                        int h, int out_cap, borb_keypoint* keys_out, float* ur_out, float* depth_out, cudaStream_t s);
 // pack + match + finalize over A.jobs (3 launches): one = a host copy of job 0 (what the match kernel reads of a single job),
 // max_smem_frame = largest frame_bytes of the jobs with frame_in_smem, max_items = an upper bound of the work items of all jobs,
-// total_kf = sum of their n_kf
-int launch_bowdb(const BowDbArgs& A, const BowDbJob& one, int max_smem_frame, long long max_items, int total_kf, int max_nn, int csa, int n_sm, cudaStream_t s);
+// total_kf = sum of their n_kf; kfkf: the jobs are SearchByBoW(KeyFrame*, KeyFrame*) of a database slot against candidates
+int launch_bowdb(const BowDbArgs& A, const BowDbJob& one, int max_smem_frame, long long max_items, int total_kf, int max_nn, int csa, int n_sm,
+                 bool kfkf, cudaStream_t s);
 bool bowdb_frame_fits_smem(int frame_bytes);
 // n_jobs searches (a job table in device memory) in one launch
 int launch_triangulation(const TriJob* d_jobs, int n_jobs, int check_ori, cudaStream_t s);

@@ -1574,16 +1574,26 @@ borb_status borb_kfdb_erase(borb_kfdb* db, int32_t slot) {
     return BORB_OK;
 }
 
-borb_status borb_kfdb_set_has_mp(borb_kfdb* db, int32_t slot, const uint8_t* has_mp) {
-    if (!db || !has_mp) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+borb_status borb_kfdb_set_has_mp_batch(borb_kfdb* db, int n, const int32_t* slots, const uint8_t* const* has_mp) {
+    if (!db || n < 0 || (n > 0 && (!slots || !has_mp))) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
     std::lock_guard<std::mutex> lk(db->mu);
-    if (slot < 0 || slot >= (int)db->entries.size() || !db->entries[slot].alive) { set_error("bad keyframe slot"); return BORB_ERR_INVALID_ARG; }
+    for (int i = 0; i < n; i++) {
+        if (!has_mp[i]) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+        if (slots[i] < 0 || slots[i] >= (int)db->entries.size() || !db->entries[slots[i]].alive) { set_error("bad keyframe slot"); return BORB_ERR_INVALID_ARG; }
+    }
+    if (n == 0) return BORB_OK;
     BORB_CUDA(cudaSetDevice(db->device));
-    borb_kfdb::Entry& e = db->entries[slot];
-    for (size_t r = 0; r < e.orig.size(); r++) e.meta[2 * r] = (e.meta[2 * r] & ~0x10000u) | (has_mp[e.orig[r]] ? 0x10000u : 0u);
     BORB_CUDA(cudaDeviceSynchronize());           // a search enqueued under the mutex may still be reading the records
-    if (!e.meta.empty()) BORB_CUDA(cudaMemcpy(e.d_meta, e.meta.data(), e.meta.size() * 4, cudaMemcpyHostToDevice));
+    for (int i = 0; i < n; i++) {
+        borb_kfdb::Entry& e = db->entries[slots[i]];
+        for (size_t r = 0; r < e.orig.size(); r++) e.meta[2 * r] = (e.meta[2 * r] & ~0x10000u) | (has_mp[i][e.orig[r]] ? 0x10000u : 0u);
+        if (!e.meta.empty()) BORB_CUDA(cudaMemcpy(e.d_meta, e.meta.data(), e.meta.size() * 4, cudaMemcpyHostToDevice));
+    }
     return BORB_OK;
+}
+
+borb_status borb_kfdb_set_has_mp(borb_kfdb* db, int32_t slot, const uint8_t* has_mp) {
+    return borb_kfdb_set_has_mp_batch(db, 1, &slot, &has_mp);
 }
 
 borb_status borb_kfdb_size(const borb_kfdb* db, int32_t* n_slots, uint64_t* device_bytes) {
@@ -1718,28 +1728,29 @@ struct SearchJob {
     const int32_t* slots; int n_kf;
     int32_t* dense;                    // borb_search_by_bow_db: match[k * n + j]
     int32_t* n_matches; int32_t* pair_offset; uint32_t* pairs; int pairs_cap; int32_t* n_pairs_total;
+    int32_t query_slot;                // SearchByBoW(KeyFrame*, KeyFrame*): the query keyframe, a slot of db (frame and view unused)
 };
 
-// Shared body of borb_search_by_bow_db, _db_pairs and _db_batch: pack, match and finalize over the job table (3 launches; none when
-// no job has a keyframe and a feature inside a node) and one synchronisation.  The arguments are checked by the callers, except the
-// slot lists, which are checked here under the database locks (a batch checks every job with keyframes, a single call only one
-// that has work, as before).
-borb_status bowdb_jobs(borb_matcher* m, const SearchJob* J, int n_jobs, float nnratio, int check_ori, bool batch) {
+// Shared body of borb_search_by_bow_db, _db_pairs and _db_batch, and (kfkf) of borb_search_by_bow_kf_db_pairs and _batch: pack,
+// match and finalize over the job table (3 launches; none when no job has a keyframe and a feature inside a node) and one
+// synchronisation.  The arguments are checked by the callers, except the slot lists and the query slots, which are checked here under
+// the database locks (a batch checks every job with keyframes, a single call only one that has work, as before).
+borb_status bowdb_jobs(borb_matcher* m, const SearchJob* J, int n_jobs, float nnratio, int check_ori, bool batch, bool kfkf = false) {
     struct Plan { KfSide f; int nn, m, n; bool work; FrameBlockHdr h; size_t o_fb, o_sl, o_ctr, o_hist, o_tab, o_dense, ho; };
     std::vector<Plan> P(n_jobs);
     for (int j = 0; j < n_jobs; j++) {
         const SearchJob& S = J[j];
         Plan& p = P[j];
-        p.f = S.frame ? KfSide{&NO_VIEW, S.frame} : KfSide{S.view};
-        p.nn = p.f.nn(); p.m = p.f.m(); p.n = p.f.n();
-        p.work = S.n_kf > 0 && p.m > 0;
+        if (!kfkf) {
+            p.f = S.frame ? KfSide{&NO_VIEW, S.frame} : KfSide{S.view};
+            p.nn = p.f.nn(); p.m = p.f.m(); p.n = p.f.n();
+        }                                                              // else: read from the database under its lock
+        p.work = S.n_kf > 0 && (kfkf || p.m > 0);
         if (S.n_pairs_total) *S.n_pairs_total = 0;
         if (S.dense) for (size_t i = 0; i < (size_t)S.n_kf * p.n; i++) S.dense[i] = -1;
         for (int i = 0; i < S.n_kf; i++) { S.n_matches[i] = 0; if (S.pair_offset) S.pair_offset[i] = 0; }
     }
     std::vector<int> work;
-    for (int j = 0; j < n_jobs; j++) if (P[j].work) work.push_back(j);
-    const int nw = (int)work.size();
     Call c(m);
     {
         std::vector<borb_kfdb*> dbs(n_jobs);
@@ -1747,6 +1758,16 @@ borb_status bowdb_jobs(borb_matcher* m, const SearchJob* J, int n_jobs, float nn
         DbLocks lk(std::move(dbs));
         for (int j = 0; j < n_jobs; j++) {
             const SearchJob& S = J[j];
+            if (kfkf) {
+                const int q = S.query_slot;
+                if (q < 0 || q >= (int)S.db->entries.size() || !S.db->entries[q].alive || S.db->entries[q].n == 0) {
+                    set_error("query slot %d is not a live keyframe added with features", q);
+                    return job_fail(batch, j, BORB_ERR_INVALID_ARG);
+                }
+                const KfStream& st = S.db->entries[q].stream;
+                P[j].nn = st.nn; P[j].m = st.m; P[j].n = st.n;
+                P[j].work = S.n_kf > 0 && st.m > 0;
+            }
             if (S.n_kf == 0 || (!batch && !P[j].work)) continue;      // the single calls return zeros before looking at the slots
             const int n_slots = (int)S.db->entries.size();
             if (!S.slots && S.n_kf != n_slots) { set_error("slots == NULL searches every slot: n_kf must be %d", n_slots); return job_fail(batch, j, BORB_ERR_INVALID_ARG); }
@@ -1754,6 +1775,8 @@ borb_status bowdb_jobs(borb_matcher* m, const SearchJob* J, int n_jobs, float nn
                 for (int i = 0; i < S.n_kf; i++)
                     if (S.slots[i] < 0 || S.slots[i] >= n_slots || !S.db->entries[S.slots[i]].alive) { set_error("slot %d is not a live keyframe", S.slots[i]); return job_fail(batch, j, BORB_ERR_INVALID_ARG); }
         }
+        for (int j = 0; j < n_jobs; j++) if (P[j].work) work.push_back(j);
+        const int nw = (int)work.size();
         if (nw == 0) return BORB_OK;
         BORB_CUDA(cudaSetDevice(m->device));
         borb_status s = lk.sync();
@@ -1761,7 +1784,7 @@ borb_status bowdb_jobs(borb_matcher* m, const SearchJob* J, int n_jobs, float nn
         for (int j : work) {
             const SearchJob& S = J[j];
             Plan& p = P[j];
-            p.f.stage(c);                                              // a host view is packed on the device like a resident frame
+            if (!kfkf) p.f.stage(c);                                   // a host view is packed on the device like a resident frame
             p.o_sl = S.slots ? c.in(S.slots, (size_t)S.n_kf * 4) : 0;
         }
         const size_t o_jobs = c.in(nullptr, (size_t)nw * sizeof(BowDbJob));       // filled in place
@@ -1792,9 +1815,14 @@ borb_status bowdb_jobs(borb_matcher* m, const SearchJob* J, int n_jobs, float nn
         for (int w = 0; w < nw; w++) {
             const SearchJob& S = J[work[w]];
             const Plan& p = P[work[w]];
-            const KfDev f = p.f.bind(c);
             BowDbJob D{};
-            D.fv_node = f.node; D.fv_start = f.start; D.fv_idx = f.idx; D.keys = f.keys; D.desc = f.desc;
+            if (kfkf) {
+                const KfStream& st = S.db->entries[S.query_slot].stream;
+                D.fv_node = st.node; D.fv_start = st.start; D.q_meta = st.meta; D.desc = st.desc;
+            } else {
+                const KfDev f = p.f.bind(c);
+                D.fv_node = f.node; D.fv_start = f.start; D.fv_idx = f.idx; D.keys = f.keys; D.desc = f.desc;
+            }
             D.nn = p.nn; D.m = p.m; D.n = p.n; D.item_target = g_bow_item_target.load();
             D.frame_block = c.dev(p.o_fb); D.frame_bytes = p.h.bytes; D.frame_in_smem = bowdb_frame_fits_smem(p.h.bytes) ? 1 : 0;
             D.table = S.db->d_stream; D.slots = S.slots ? (const int32_t*)c.dev(p.o_sl) : nullptr;
@@ -1820,7 +1848,8 @@ borb_status bowdb_jobs(borb_matcher* m, const SearchJob* J, int n_jobs, float nn
         A.jobs = (const BowDbJob*)c.dev(o_jobs); A.n_jobs = nw; A.static_sched = g_bow_static.load();
         A.nnratio = nnratio; A.check_ori = check_ori;
         if (m->timing) BORB_CUDA(cudaEventRecord(m->t0, m->stream));
-        m->launches += launch_bowdb(A, hj[0], max_smem_frame, max_items, total_kf, max_nn, g_bow_csa.load(), J[work[0]].db->n_sm, m->stream);
+        m->launches += launch_bowdb(A, hj[0], max_smem_frame, max_items, total_kf, max_nn, g_bow_csa.load(), J[work[0]].db->n_sm, kfkf,
+                                   m->stream);
         if (m->timing) BORB_CUDA(cudaEventRecord(m->t1, m->stream));
         for (int j : work)
             if (J[j].dense) BORB_CUDA(cudaMemcpyAsync(J[j].dense, c.dev(P[j].o_dense), (size_t)J[j].n_kf * P[j].n * 4, cudaMemcpyDeviceToHost, m->stream));
@@ -1855,11 +1884,11 @@ borb_status check_db_view(borb_matcher* m, borb_kfdb* db, const borb_keyframe_vi
     return check_kf(frame, "SearchByBoW(database, frame)");
 }
 
-// the checks of a batch job's database and resident frame
-borb_status check_db_job(borb_matcher* m, borb_kfdb* db, const borb_frame* f, int j) {
+// the checks of a batch job's database, and of its resident frame unless it searches a database slot (f == NULL, kfkf)
+borb_status check_db_job(borb_matcher* m, borb_kfdb* db, const borb_frame* f, int j, bool kfkf = false) {
     if (!db) { set_error("job %d: null database", j); return BORB_ERR_INVALID_ARG; }
     if (db->device != m->device) { set_error("job %d: database and matcher live on different devices", j); return BORB_ERR_INVALID_ARG; }
-    return check_resident_bow(f, m, j, "frame");
+    return kfkf ? BORB_OK : check_resident_bow(f, m, j, "frame");
 }
 
 }  // namespace
@@ -1920,6 +1949,29 @@ borb_status borb_search_by_bow_db_batch(borb_matcher* m, const borb_bow_db_job* 
         S[j] = SearchJob{B.db, B.frame, nullptr, B.slots, B.n_kf, nullptr, B.n_matches, B.pair_offset, B.pairs, B.pairs_cap, B.n_pairs_total};
     }
     return bowdb_jobs(m, S.data(), n_jobs, nnratio, check_orientation, true);
+}
+
+borb_status borb_search_by_bow_kf_db_batch(borb_matcher* m, const borb_bow_kf_db_job* jobs, int n_jobs, float nnratio, int check_orientation) {
+    if (!m || n_jobs < 0 || (n_jobs > 0 && !jobs)) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+    if (n_jobs == 0) return BORB_OK;
+    std::vector<SearchJob> S(n_jobs);
+    for (int j = 0; j < n_jobs; j++) {
+        const borb_bow_kf_db_job& B = jobs[j];
+        borb_status s = check_db_job(m, B.db, nullptr, j, true);
+        if (s != BORB_OK) return s;
+        if (B.n_kf < 0 || B.pairs_cap < 0 || (B.n_kf > 0 && !B.n_matches)) { set_error("job %d: null output or negative count", j); return BORB_ERR_INVALID_ARG; }
+        if (B.pairs && !B.pair_offset) { set_error("job %d: pairs without pair_offset", j); return BORB_ERR_INVALID_ARG; }
+        S[j] = SearchJob{B.db, nullptr, nullptr, B.slots, B.n_kf, nullptr, B.n_matches, B.pair_offset, B.pairs, B.pairs_cap, B.n_pairs_total,
+                         B.query_slot};
+    }
+    return bowdb_jobs(m, S.data(), n_jobs, nnratio, check_orientation, true, true);
+}
+
+borb_status borb_search_by_bow_kf_db_pairs(borb_matcher* m, borb_kfdb* db, int32_t query_slot, const int32_t* slots, int n_kf, float nnratio,
+                                           int check_orientation, int32_t* n_matches, int32_t* pair_offset, uint32_t* pairs, int pairs_cap,
+                                           int32_t* n_pairs_total) {
+    const borb_bow_kf_db_job J{db, query_slot, slots, n_kf, n_matches, pair_offset, pairs, pairs_cap, n_pairs_total};
+    return borb_search_by_bow_kf_db_batch(m, &J, 1, nnratio, check_orientation);
 }
 
 // ---- SearchForTriangulation: borb_search_for_triangulation is the one-job case of borb_search_for_triangulation_batch (one launch

@@ -266,6 +266,140 @@ __device__ __forceinline__ void bowdb_job_items(const BowDbArgs& A, const BowDbJ
     }
 }
 
+// SearchByBoW(KeyFrame* pKF1, KeyFrame* pKF2) (src/ORBmatcher.cc:522-655) of the loop-closing keyframe (the query, a slot of the
+// database packed into the block like a frame) against many candidates: the roles of the two sides swap.  Rows are the QUERY's
+// features with a good MapPoint (:558-562), shared by every candidate; columns are the candidate's bucket features with a good
+// MapPoint (:574-580), and the claims sit on them (vbMatched2, :576, :603).  A candidate feature lies in one node, so a (candidate,
+// node) bucket is still an independent claim scope.  An item is (query node, <= 32 candidates); lane j finds candidate j's bucket,
+// then the warp takes the candidates one after the other: lane = query row (32 at a time, descriptor from the block), the column
+// loop over the candidate's bucket is warp-uniform (broadcast loads).  Best / second best are the lexicographic min / second min of
+// (distance, column) — the first minimum in the candidate's FeatureVector order wins (:586-595).  Rows with a distance below TH_LOW
+// at all are replayed in row order against the bucket's claims, a row whose best or second best was claimed meanwhile rescanned by
+// the warp, with the strict gate of :598 and the ratio test of :600.  The match goes to the (candidate x query position) table as
+// candidate feature | bin << 16, the bin of query angle - candidate angle (:607), so the relocalisation finalize culls and compacts it.
+template <bool FSM>
+__device__ __forceinline__ void bowkf_job_items(const BowDbArgs& A, const BowDbJob& J, const uint8_t* fb, uint8_t* ws) {
+    const int lane = threadIdx.x & 31, wrp = threadIdx.x >> 5;
+    const FrameBlockHdr* H = reinterpret_cast<const FrameBlockHdr*>(fb);
+    const int mf = H->m, np = H->np;
+    const uint32_t* fnode = reinterpret_cast<const uint32_t*>(fb + H->off_node);
+    const int32_t* fstart = reinterpret_cast<const int32_t*>(fb + H->off_start);
+    const float* fangle = reinterpret_cast<const float*>(fb + H->off_angle);
+    const uint4* fdesc = reinterpret_cast<const uint4*>(fb + H->off_desc);
+    const int32_t* pnode = reinterpret_cast<const int32_t*>(fb + H->off_pnode);
+    const int32_t* pcs = reinterpret_cast<const int32_t*>(fb + H->off_pcs);
+    const int32_t* pstart = reinterpret_cast<const int32_t*>(fb + H->off_pstart);
+    const uint2* qmeta = J.q_meta;                                // the query's rows, in block order: the good-MapPoint flag
+    uint32_t* claim = reinterpret_cast<uint32_t*>(ws);            // claimed columns when the bucket is wider than 32
+
+    const int items = pstart[np];
+    const int warps_total = gridDim.x * (blockDim.x >> 5);
+    int it_static = blockIdx.x + gridDim.x * wrp;
+    while (true) {
+        int it = 0;
+        if (A.static_sched) { it = it_static; it_static += warps_total; }
+        else {
+            if (lane == 0) it = atomicAdd(J.ctr, 1);
+            it = __shfl_sync(0xFFFFFFFFu, it, 0);
+        }
+        if (it >= items) break;
+        int lo = 0, hi = np;                                      // largest p with pstart[p] <= it
+        while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (pstart[mid] <= it) lo = mid; else hi = mid; }
+        const int bf = pnode[lo], cs = pcs[lo];
+        const int k0 = (it - pstart[lo]) * cs, k1 = min(J.n_kf, k0 + cs);
+        const uint32_t node = fnode[bf];
+        const int ts = fstart[bf], nt = fstart[bf + 1] - ts;
+
+        // lane j: candidate k0 + j; the bucket of `node` in its FeatureVector (ascending node ids)
+        const int k = k0 + lane;
+        int rs = 0, cnt = 0;
+        const uint2* kmeta = nullptr; const uint4* kdesc = nullptr;
+        if (k < k1) {
+            const KfStream* Kp = J.table + (J.slots ? J.slots[k] : k);
+            const int nn = Kp->nn;
+            if (nn > 0) {
+                const uint32_t* kn = Kp->node;
+                int idx = min(bf, nn - 1);
+                if (kn[idx] != node) {
+                    int l2 = 0, h2 = nn;
+                    while (l2 < h2) { const int mid = (l2 + h2) >> 1; if (kn[mid] < node) l2 = mid + 1; else h2 = mid; }
+                    idx = (l2 < nn && kn[l2] == node) ? l2 : -1;
+                }
+                if (idx >= 0) {
+                    rs = Kp->start[idx]; cnt = Kp->start[idx + 1] - rs;
+                    kmeta = Kp->meta + rs; kdesc = reinterpret_cast<const uint4*>(Kp->desc) + (size_t)rs * 2;
+                }
+            }
+        }
+        unsigned todo = __ballot_sync(0xFFFFFFFFu, cnt > 0);
+        while (todo) {
+            const int src = __ffs(todo) - 1;
+            todo &= todo - 1;
+            const int nc = __shfl_sync(0xFFFFFFFFu, cnt, src);
+            const uint2* cm = reinterpret_cast<const uint2*>(__shfl_sync(0xFFFFFFFFu, reinterpret_cast<unsigned long long>(kmeta), src));
+            const uint4* cd = reinterpret_cast<const uint4*>(__shfl_sync(0xFFFFFFFFu, reinterpret_cast<unsigned long long>(kdesc), src));
+            const bool wide = nc > 32;
+            uint32_t claimed = 0;
+            if (wide) { for (int w = lane; w < ((nc + 31) >> 5); w += 32) claim[w] = 0; __syncwarp(); }
+            auto is_claimed = [&](unsigned col) -> bool { return wide ? ((claim[col >> 5] >> (col & 31)) & 1u) != 0 : ((claimed >> col) & 1u) != 0; };
+            auto good = [&](int col) -> bool { return ((cm[col].x >> 16) & 1u) != 0; };
+            for (int r0 = 0; r0 < nt; r0 += 32) {
+                const int r = ts + r0 + lane;
+                const bool act = r0 + lane < nt && ((qmeta[r].x >> 16) & 1u) != 0;
+                uint4 q0 = make_uint4(0, 0, 0, 0), q1 = q0;
+                if (act) { q0 = fdesc[2 * r]; q1 = fdesc[2 * r + 1]; }
+                unsigned k1v = 0xFFFFFFFFu, k2v = 0xFFFFFFFFu;
+                for (int c = 0; c < nc; c++) {
+                    if (!good(c)) continue;                                        // warp-uniform
+                    const int d = ham256<2>(q0, q1, cd[2 * c], cd[2 * c + 1]);
+                    const unsigned key = ((unsigned)d << 16) | (unsigned)c;
+                    k2v = min(k2v, max(k1v, key));
+                    k1v = min(k1v, key);
+                }
+                unsigned low = __ballot_sync(0xFFFFFFFFu, act && (k1v >> 16) < (unsigned)TH_LOW);
+                while (low) {
+                    const int L = __ffs(low) - 1;
+                    low &= low - 1;
+                    unsigned kk1 = __shfl_sync(0xFFFFFFFFu, k1v, L), kk2 = __shfl_sync(0xFFFFFFFFu, k2v, L);
+                    const bool stale = is_claimed(kk1 & 0xFFFFu) || (kk2 != 0xFFFFFFFFu && is_claimed(kk2 & 0xFFFFu));
+                    if (stale) {
+                        uint4 r0v, r1v;
+                        r0v.x = __shfl_sync(0xFFFFFFFFu, q0.x, L); r0v.y = __shfl_sync(0xFFFFFFFFu, q0.y, L);
+                        r0v.z = __shfl_sync(0xFFFFFFFFu, q0.z, L); r0v.w = __shfl_sync(0xFFFFFFFFu, q0.w, L);
+                        r1v.x = __shfl_sync(0xFFFFFFFFu, q1.x, L); r1v.y = __shfl_sync(0xFFFFFFFFu, q1.y, L);
+                        r1v.z = __shfl_sync(0xFFFFFFFFu, q1.z, L); r1v.w = __shfl_sync(0xFFFFFFFFu, q1.w, L);
+                        unsigned m1 = 0xFFFFFFFFu, m2 = 0xFFFFFFFFu;
+                        for (int col = lane; col < nc; col += 32) {
+                            if (is_claimed((unsigned)col) || !good(col)) continue;
+                            const int d = ham256<2>(r0v, r1v, cd[2 * col], cd[2 * col + 1]);
+                            const unsigned key = ((unsigned)d << 16) | (unsigned)col;
+                            if (key < m1) { m2 = m1; m1 = key; } else if (key < m2) m2 = key;
+                        }
+                        kk1 = __reduce_min_sync(0xFFFFFFFFu, m1);
+                        kk2 = __reduce_min_sync(0xFFFFFFFFu, m1 == kk1 ? m2 : m1);
+                    }
+                    if (kk1 == 0xFFFFFFFFu) continue;
+                    const int bestDist1 = (int)(kk1 >> 16);
+                    if (bestDist1 >= TH_LOW) continue;                                         // :598
+                    const int bestDist2 = kk2 == 0xFFFFFFFFu ? 256 : (int)(kk2 >> 16);
+                    if (!((float)bestDist1 < __fmul_rn(A.nnratio, (float)bestDist2))) continue;   // :600
+                    const unsigned pb = kk1 & 0xFFFFu;
+                    if (wide) { if (lane == 0) claim[pb >> 5] |= 1u << (pb & 31); __syncwarp(); }
+                    else claimed |= 1u << pb;
+                    if (lane == 0) {
+                        const uint2 cv = cm[pb];
+                        const int pos = ts + r0 + L;
+                        const int bin = A.check_ori ? rot_bin(fangle[pos], __uint_as_float(cv.y)) : 0;
+                        J.table_out[(size_t)(k0 + src) * mf + pos] = (cv.x & 0xFFFFu) | ((uint32_t)bin << 16);   // vpMatches12[idx1] (:602)
+                        atomicAdd(&J.hist_out[(size_t)(k0 + src) * 32 + bin], 1);                                 // rotHist[bin] (:614)
+                    }
+                }
+            }
+            __syncwarp();                                         // the claim words are reset for the next candidate
+        }
+    }
+}
+
 // Job scheduling.  A call with one job (every single call) passes it as a kernel parameter (ONE_SMEM / ONE_GLOBAL): its fields stay
 // in the constant bank instead of registers, which keeps the item loop at the register budget of 64.  A job table (TABLE):
 // a CTA works on one job at a time: its warps take the job's items from the job's counter, and only when that
@@ -273,15 +407,21 @@ __device__ __forceinline__ void bowdb_job_items(const BowDbArgs& A, const BowDbJ
 // items.  So a CTA visits a job at most once, and fetches a shared-memory frame block (one 1-D TMA bulk copy) only for a job it
 // is about to work on.  CTAs start at jobs spread over the job table, so many small jobs are taken by different CTAs.  Blocks
 // that do not fit next to the warp scratch are read through L1 from global memory (FSM = false), in the same launch.
+// KFKF selects the items of SearchByBoW(KeyFrame*, KeyFrame*) (bowkf_job_items) instead of those of (KeyFrame*, Frame&).
 enum { ONE_SMEM = 0, ONE_GLOBAL = 1, TABLE = 2 };
-template <int CSA, int KIND>
-__global__ void __launch_bounds__(32 * BDB_WARPS, BDB_CTAS) bowdb_match_kernel(BowDbArgs A, int smem_frame, const __grid_constant__ BowDbJob J0) {
+template <int CSA, bool FSM, bool KFKF>
+__device__ __forceinline__ void job_items(const BowDbArgs& A, const BowDbJob& J, const uint8_t* fb, uint8_t* ws) {
+    if constexpr (KFKF) bowkf_job_items<FSM>(A, J, fb, ws);
+    else bowdb_job_items<CSA, FSM>(A, J, fb, ws);
+}
+template <int CSA, int KIND, bool KFKF>
+__device__ __forceinline__ void bowdb_match(const BowDbArgs& A, int smem_frame, const BowDbJob& J0) {
     extern __shared__ __align__(128) uint8_t sm[];
     __shared__ __align__(8) unsigned long long bar;
     __shared__ BowDbJob sJ;
     __shared__ int s_job, s_next, s_left, s_loads;     // the job cursor (the next job to look at, jobs not looked at) and the block loads so far
     const int tid = threadIdx.x;
-    if (KIND == ONE_GLOBAL) { bowdb_job_items<CSA, false>(A, J0, J0.frame_block, sm + (size_t)(tid >> 5) * BDB_WARP_BYTES); return; }
+    if (KIND == ONE_GLOBAL) { job_items<CSA, false, KFKF>(A, J0, J0.frame_block, sm + (size_t)(tid >> 5) * BDB_WARP_BYTES); return; }
     if (KIND == ONE_SMEM) {
         if (tid == 0) {
             asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(&bar)));
@@ -302,7 +442,7 @@ __global__ void __launch_bounds__(32 * BDB_WARPS, BDB_CTAS) bowdb_match_kernel(B
             "BOWDB_DONE1:\n"
             "}\n" ::"r"(smem_u32(&bar))
             : "memory");
-        bowdb_job_items<CSA, true>(A, J0, sm, sm + (((size_t)smem_frame + 127) & ~size_t(127)) + (size_t)(tid >> 5) * BDB_WARP_BYTES);
+        job_items<CSA, true, KFKF>(A, J0, sm, sm + (((size_t)smem_frame + 127) & ~size_t(127)) + (size_t)(tid >> 5) * BDB_WARP_BYTES);
         return;
     }
     if (tid == 0) {
@@ -342,13 +482,22 @@ __global__ void __launch_bounds__(32 * BDB_WARPS, BDB_CTAS) bowdb_match_kernel(B
                 "BOWDB_DONE:\n"
                 "}\n" ::"r"(smem_u32(&bar)), "r"((uint32_t)s_loads & 1u)
                 : "memory");
-            bowdb_job_items<CSA, true>(A, sJ, sm, ws);
+            job_items<CSA, true, KFKF>(A, sJ, sm, ws);
         } else {
-            bowdb_job_items<CSA, false>(A, sJ, sJ.frame_block, ws);
+            job_items<CSA, false, KFKF>(A, sJ, sJ.frame_block, ws);
         }
         __syncthreads();                                          // every warp is done with this job's block
         if (tid == 0 && sJ.frame_in_smem) s_loads++;
     }
+}
+template <int CSA, int KIND>
+__global__ void __launch_bounds__(32 * BDB_WARPS, BDB_CTAS) bowdb_match_kernel(BowDbArgs A, int smem_frame, const __grid_constant__ BowDbJob J0) {
+    bowdb_match<CSA, KIND, false>(A, smem_frame, J0);
+}
+// One distance arithmetic (MODE 2, the default) only: borb_debug_set_bow_csa applies to bowdb_match_kernel.
+template <int KIND>
+__global__ void __launch_bounds__(32 * BDB_WARPS, BDB_CTAS) bowkf_match_kernel(BowDbArgs A, int smem_frame, const __grid_constant__ BowDbJob J0) {
+    bowdb_match<2, KIND, true>(A, smem_frame, J0);
 }
 
 // Rotation-consistency cull and compaction, a 128-thread CTA per keyframe.  table_out row: one u32 per frame position
@@ -455,8 +604,11 @@ bool bowdb_frame_fits_smem(int frame_bytes) { return bowdb_warps(frame_bytes, tr
 // column-loop iterations whatever the bucket width (a keyframe's bucket of the node is about as full as the frame's), and the
 // item prefix pstart.  Also resets the job's work counter and pair cursor and stores its item count next to them.
 // Shared memory: 8 B per sort key (next power of two >= nn, at least 32).
+// KFKF: the query is a database slot; its stream rows are already in FeatureVector order, with the feature index and angle in
+// q_meta, so row r is copied as it is.
 constexpr int PACK_THREADS = 512;
-__global__ void __launch_bounds__(PACK_THREADS) bowdb_pack_kernel(const BowDbJob* __restrict__ jobs) {
+template <bool KFKF>
+__device__ __forceinline__ void bowdb_pack(const BowDbJob* __restrict__ jobs) {
     extern __shared__ __align__(16) uint64_t pk_sm[];
     __shared__ int warp_sums[PACK_THREADS / 32];
     __shared__ int s_np;
@@ -475,9 +627,14 @@ __global__ void __launch_bounds__(PACK_THREADS) bowdb_pack_kernel(const BowDbJob
     for (int i = tid; i <= nn; i += T) start[i] = nn > 0 ? J.fv_start[i] : 0;
     for (int t = tid; t < 2 * m; t += T) {                                // a thread per descriptor half
         const int r = t >> 1;
-        const uint32_t j = J.fv_idx[r];
-        desc[t] = src[(size_t)j * 2 + (t & 1)];
-        if ((t & 1) == 0) { orig[r] = (uint16_t)j; angle[r] = J.keys[j].angle; }
+        if constexpr (KFKF) {
+            desc[t] = src[t];
+            if ((t & 1) == 0) { const uint2 mt = J.q_meta[r]; orig[r] = (uint16_t)(mt.x & 0xFFFFu); angle[r] = __uint_as_float(mt.y); }
+        } else {
+            const uint32_t j = J.fv_idx[r];
+            desc[t] = src[(size_t)j * 2 + (t & 1)];
+            if ((t & 1) == 0) { orig[r] = (uint16_t)j; angle[r] = J.keys[j].angle; }
+        }
     }
     // work list: (widest first, then node index) as one ascending 64-bit key; empty nodes sort last
     int K = 32;
@@ -523,12 +680,16 @@ __global__ void __launch_bounds__(PACK_THREADS) bowdb_pack_kernel(const BowDbJob
         J.ctr[0] = 0; J.ctr[1] = total; J.ctr[2] = 0;
     }
 }
+__global__ void __launch_bounds__(PACK_THREADS) bowdb_pack_kernel(const BowDbJob* __restrict__ jobs) { bowdb_pack<false>(jobs); }
+__global__ void __launch_bounds__(PACK_THREADS) bowkf_pack_kernel(const BowDbJob* __restrict__ jobs) { bowdb_pack<true>(jobs); }
 
-int launch_bowdb(const BowDbArgs& A, const BowDbJob& one, int max_smem_frame, long long max_items, int total_kf, int max_nn, int csa, int n_sm, cudaStream_t s) {
+int launch_bowdb(const BowDbArgs& A, const BowDbJob& one, int max_smem_frame, long long max_items, int total_kf, int max_nn, int csa, int n_sm,
+                 bool kfkf, cudaStream_t s) {
     int K = 32;
     while (K < max_nn) K <<= 1;
-    allow_max_smem((const void*)bowdb_pack_kernel);
-    bowdb_pack_kernel<<<A.n_jobs, PACK_THREADS, (size_t)K * 8, s>>>(A.jobs);
+    void (*pack)(const BowDbJob*) = kfkf ? bowkf_pack_kernel : bowdb_pack_kernel;
+    allow_max_smem((const void*)pack);
+    pack<<<A.n_jobs, PACK_THREADS, (size_t)K * 8, s>>>(A.jobs);
     const bool fsm = max_smem_frame > 0;
     const int warps = bowdb_warps(max_smem_frame, fsm);
     const size_t smem = (fsm ? (((size_t)max_smem_frame + 127) & ~size_t(127)) : 0) + (size_t)warps * BDB_WARP_BYTES;
@@ -538,7 +699,8 @@ int launch_bowdb(const BowDbArgs& A, const BowDbJob& one, int max_smem_frame, lo
     // one job: passed as a parameter; its block decides the frame's memory
     const int kind = A.n_jobs > 1 ? TABLE : (one.frame_in_smem ? ONE_SMEM : ONE_GLOBAL);
     void (*kern)(BowDbArgs, int, BowDbJob) = nullptr;
-    switch (csa * 3 + kind) {
+    if (kfkf) kern = kind == TABLE ? bowkf_match_kernel<TABLE> : (kind == ONE_SMEM ? bowkf_match_kernel<ONE_SMEM> : bowkf_match_kernel<ONE_GLOBAL>);
+    else switch (csa * 3 + kind) {
         case 0: kern = bowdb_match_kernel<0, ONE_SMEM>; break;
         case 1: kern = bowdb_match_kernel<0, ONE_GLOBAL>; break;
         case 2: kern = bowdb_match_kernel<0, TABLE>; break;

@@ -74,6 +74,11 @@ class _BowDbJobC(C.Structure):                      # borb_bow_db_job
                 ("pair_offset", C.c_void_p), ("pairs", C.c_void_p), ("pairs_cap", C.c_int32), ("n_pairs_total", C.c_void_p)]
 
 
+class _BowKfDbJobC(C.Structure):                    # borb_bow_kf_db_job
+    _fields_ = [("db", C.c_void_p), ("query_slot", C.c_int32), ("slots", C.c_void_p), ("n_kf", C.c_int32), ("n_matches", C.c_void_p),
+                ("pair_offset", C.c_void_p), ("pairs", C.c_void_p), ("pairs_cap", C.c_int32), ("n_pairs_total", C.c_void_p)]
+
+
 class _LocalPointsJobC(C.Structure):               # borb_local_points_job
     _fields_ = [("frame", _FrameViewC), ("pts", _WorldPointsViewC), ("has_obs", C.c_void_p), ("Tcw", C.c_float * 12), ("Ow", C.c_float * 3)] + \
                [(n, C.c_float) for n in ("fx", "fy", "cx", "cy", "mbf", "log_scale_factor", "th")] + \
@@ -723,6 +728,33 @@ class ORBmatcher:
               "borb_search_by_bow_db_batch")
         return [(nm[:n_kf], off[:n_kf], pairs[:int(tot[0])]) for _, n_kf, nm, off, pairs, tot in outs]
 
+    def SearchByBoWKFDbBatch(self, dbs, query_slots, slots_list, pairs_cap=None):
+        """borb_search_by_bow_kf_db_batch: SearchByBoW(KeyFrame*, KeyFrame*) (src/ORBmatcher.cc:522-655) of many loop-closing keyframes,
+        each a slot of its database, against candidate slots of the same database, in one launch sequence.  slots_list[j] = the
+        candidates of job j (None: every slot); pairs_cap as SearchByBoWDbBatch.  Returns [(nmatches, pair_offset, pairs)] per job as
+        KeyFrameDatabase.SearchByBoWKFPairs returns them."""
+        n = len(query_slots)
+        dbs = self._db_jobs(dbs, n)
+        caps = pairs_cap if isinstance(pairs_cap, (list, tuple)) else [pairs_cap] * n
+        jobs = (_BowKfDbJobC * max(n, 1))()
+        outs = []
+        for j, (db, q, sl, cap) in enumerate(zip(dbs, query_slots, slots_list, caps)):
+            if sl is None:
+                n_kf, sla = (db.size()[0] if db is not None else 0), None
+            else:
+                sla = np.ascontiguousarray(sl, np.int32); n_kf = len(sla)
+            cap = int(cap) if cap is not None else max(n_kf * (db._n_features(q) if db is not None else 0), 1)
+            nm = np.zeros(max(n_kf, 1), np.int32); off = np.zeros(max(n_kf, 1), np.int32)
+            pairs = np.zeros(max(cap, 1), np.uint32); tot = np.zeros(1, np.int32)
+            J = jobs[j]
+            J.db = db._h.value if db is not None else None
+            J.query_slot, J.slots, J.n_kf = int(q), _p(sla), n_kf
+            J.n_matches, J.pair_offset, J.pairs, J.pairs_cap, J.n_pairs_total = _p(nm), _p(off), _p(pairs), cap, _p(tot)
+            outs.append((sla, n_kf, nm, off, pairs, tot))
+        check(self._lib.borb_search_by_bow_kf_db_batch(self._h, jobs, n, self.mfNNratio, int(self.mbCheckOrientation)),
+              "borb_search_by_bow_kf_db_batch")
+        return [(nm[:n_kf], off[:n_kf], pairs[:int(tot[0])]) for _, n_kf, nm, off, pairs, tot in outs]
+
     def SearchForTriangulation(self, pKF1: KeyFrameView, pKF2: KeyFrameView, F12: np.ndarray, epipole: Tuple[float, float],
                                bOnlyStereo: bool = False) -> np.ndarray:
         """src/ORBmatcher.cc:657-823.  Returns vMatchedPairs as an (m,2) int array (idx1, idx2), ascending idx1."""
@@ -917,6 +949,7 @@ class KeyFrameDatabase:
         self._h = h
         self._seq = []                  # insertion sequence number per slot (inverted-file list order)
         self._reloc_score = {}          # KeyFrame::mRelocScore per slot, persistent across queries as in the reference
+        self._n = []                    # features per slot (the default pair capacity of the searches from a slot)
 
     def __del__(self):
         if getattr(self, "_h", None):
@@ -935,6 +968,7 @@ class KeyFrameDatabase:
         kc = pKF._c()
         check(self._lib.borb_kfdb_add(self._h, C.byref(kc), _p(w), _p(v), len(w), C.byref(slot)), "borb_kfdb_add")
         self._seq.append(len(self._seq))
+        self._n.append(len(pKF.mvKeysUn))
         return slot.value
 
     def erase(self, slot: int) -> None:
@@ -945,6 +979,10 @@ class KeyFrameDatabase:
         check(self._lib.borb_kfdb_clear(self._h), "borb_kfdb_clear")
         self._seq = []
         self._reloc_score = {}
+        self._n = []
+
+    def _n_features(self, slot: int) -> int:
+        return self._n[slot] if 0 <= slot < len(self._n) else 0
 
     def set_has_mp(self, slot: int, has_mp: np.ndarray) -> None:
         hm = np.ascontiguousarray(has_mp, np.uint8)
@@ -1006,6 +1044,25 @@ class KeyFrameDatabase:
                                                     _p(off), _p(pairs) if want_pairs else None, cap if want_pairs else 0, C.byref(tot)),
               "borb_search_by_bow_db_pairs")
         return nm[:n_kf], off[:n_kf], pairs[:tot.value] if want_pairs else None
+
+    def SearchByBoWKFPairs(self, query_slot: int, slots, pairs_cap: Optional[int] = None):
+        """SearchByBoW(KeyFrame*, KeyFrame*) (src/ORBmatcher.cc:522-655) of the keyframe in `query_slot` against the candidate slots
+        `slots` (None = every slot), both read from the database with their current MapPoint masks: returns (nmatches[n_kf],
+        pair_offset[n_kf], pairs) where pairs[off[k]:off[k]+nm[k]] = (query feature | candidate feature << 16) in the query's
+        FeatureVector order."""
+        m = self._m
+        if slots is None:
+            n_kf, sl = self.size()[0], None
+        else:
+            sl = np.ascontiguousarray(slots, np.int32); n_kf = len(sl)
+        cap = int(pairs_cap) if pairs_cap is not None else max(n_kf * self._n_features(int(query_slot)), 1)
+        nm = np.zeros(max(n_kf, 1), np.int32); off = np.zeros(max(n_kf, 1), np.int32)
+        pairs = np.zeros(max(cap, 1), np.uint32)
+        tot = C.c_int32(0)
+        check(self._lib.borb_search_by_bow_kf_db_pairs(m._h, self._h, int(query_slot), _p(sl), n_kf, m.mfNNratio, int(m.mbCheckOrientation),
+                                                       _p(nm), _p(off), _p(pairs), cap, C.byref(tot)),
+              "borb_search_by_bow_kf_db_pairs")
+        return nm[:n_kf], off[:n_kf], pairs[:tot.value]
 
 
 class ORBVocabulary:
