@@ -397,7 +397,9 @@ BORB_API borb_status borb_search_by_sim3(borb_matcher* m, const borb_frame_view*
  * in this frame, not bad); has_obs[i] = Observations()>0 (NULL: all).  Tcw = [mRcw | mtcw], Ow = mOw, mbf, log_scale_factor =
  * Frame members; viewing_cos_limit = 0.5 at the call site.  in_view[i] = mbTrackInView (the caller runs IncreaseVisible on
  * it); proj_x/proj_y/proj_xr/level/view_cos (each may be NULL) = mTrackProjX/Y/XR, mnTrackScaleLevel, mTrackViewCos
- * (0 where not in view); match_feat / n_matches as in borb_search_by_projection. */
+ * (0 where not in view); match_feat / n_matches as in borb_search_by_projection.  As in the reference, a point at the camera
+ * centre (PcZ == 0) is in view when its min distance is 0: its projection and viewCos are NaN (the NaN payload is not
+ * specified), its level is 0, and it gets no match. */
 BORB_API borb_status borb_search_local_points(borb_matcher* m, const borb_frame_view* frame, const borb_worldpoints_view* pts,
                                               const uint8_t* has_obs, const float* Tcw, const float* Ow, float fx, float fy, float cx,
                                               float cy, float mbf, float viewing_cos_limit, float log_scale_factor, float th,

@@ -52,6 +52,9 @@ Grid build_grid(const orbport_kp* k, int n, float minX, float minY, float maxX, 
 
 std::vector<int> features_in_area(const Grid& g, const orbport_kp* k, float x, float y, float r, int minLevel, int maxLevel) {
     std::vector<int> out;
+    // a NaN centre (a point at the camera centre, orbport_is_in_frustum): the reference's (int)floor(NaN) is INT_MIN on x86,
+    // which empties the window; said here without the undefined conversion
+    if (!(x == x) || !(y == y)) return out;
     const int nMinCellX = std::max(0, (int)std::floor((x - g.minX - r) * g.invW));
     if (nMinCellX >= GRID_COLS) return out;
     const int nMaxCellX = std::min(GRID_COLS - 1, (int)std::ceil((x - g.minX + r) * g.invW));
@@ -1007,7 +1010,9 @@ extern "C" int orbport_detect_reloc_candidates(int n_kf, const int32_t* kf_start
 
 // Frame::isInFrustum — reference src/Frame.cc:269-325, for n MapPoints (Tracking::SearchLocalPoints, src/Tracking.cc:1167-1180).
 // Tcw = [mRcw | mtcw], Ow = mOw.  Outputs are the fields the reference stores on the MapPoint: mbTrackInView,
-// mTrackProjX, mTrackProjY, mTrackProjXR, mnTrackScaleLevel, mTrackViewCos (untouched where in_view = 0).
+// mTrackProjX, mTrackProjY, mTrackProjXR, mnTrackScaleLevel, mTrackViewCos (untouched where in_view = 0).  A point at the
+// camera centre (PcZ == 0) projects to NaN, and NaN passes every test that follows: with mfMinDistance == 0 the point is in
+// view with NaN track fields and level 0, as in the reference; features_in_area then finds nothing for it.
 extern "C" int orbport_is_in_frustum(const float* world_pos, const float* normal, const float* max_distance, const float* min_distance,
                                      const uint8_t* valid, int n, const float* Tcw, const float* Ow, float fx, float fy, float cx,
                                      float cy, float mbf, float minX, float minY, float maxX, float maxY, float viewingCosLimit,
@@ -1027,7 +1032,6 @@ extern "C" int orbport_is_in_frustum(const float* world_pos, const float* normal
         const float v = fy * PcY * invz + cy;
         if (u < minX || u > maxX) continue;
         if (v < minY || v > maxY) continue;
-        if (!(u == u) || !(v == v)) continue;              // NaN (PcZ == 0): the reference would go on with undefined grid cells
         const float maxDistance = 1.2f * max_distance[i];
         const float minDistance = 0.8f * min_distance[i];
         const float PO[3] = {P[0] - Ow[0], P[1] - Ow[1], P[2] - Ow[2]};

@@ -173,8 +173,9 @@ __device__ __forceinline__ void project_point(const LastArgs& L, int i) {
             const float invz = __fdiv_rn(1.0f, zc);                           // 1.0f/PcZ (:286)
             u = __fadd_rn(__fmul_rn(__fmul_rn(L.fx, xc), invz), L.cx);
             v = __fadd_rn(__fmul_rn(__fmul_rn(L.fy, yc), invz), L.cy);
+            // no NaN test: at PcZ == 0 (a point at the camera centre) u and v are NaN and pass, as in the reference; the
+            // track fields then hold NaN and the search window is empty (area_window)
             if (u < L.minX || u > L.maxX || v < L.minY || v > L.maxY) ok = false;
-            if (!(u == u) || !(v == v)) ok = false;
             ur = __fsub_rn(u, __fmul_rn(L.bf, invz));                         // mTrackProjXR (:319)
         } else if (L.variant == 2) {
             if (q2 < 0.0f) ok = false;                                        // depth must be positive (:329-330)

@@ -61,8 +61,10 @@ __device__ void three_maxima(const int* cnt, int& ind1, int& ind2, int& ind3) { 
 __device__ __forceinline__ unsigned warp_min(unsigned v) { return __reduce_min_sync(0xFFFFFFFFu, v); }
 
 // The cell window of GetFeaturesInArea(x, y, rs) (Frame.cc:327-380) on A's grid: columns c0x..c1x, rows c0y..c1y; false when
-// it is empty
+// it is empty.  A NaN centre (a point at the camera centre, Frame::isInFrustum) has an empty window: the reference's
+// (int)floor(NaN) is INT_MIN on x86, while the device conversion gives 0, which would make the window cell (0, 0).
 __device__ __forceinline__ bool area_window(const ProjArgs& A, float x, float y, float rs, int& c0x, int& c1x, int& c0y, int& c1y) {
+    if (!(x == x) || !(y == y)) return false;
     c0x = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(x, A.minX), rs), A.invW)));
     c1x = min(GRID_COLS - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(x, A.minX), rs), A.invW)));
     c0y = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(y, A.minY), rs), A.invH)));
