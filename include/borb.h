@@ -462,6 +462,28 @@ BORB_API borb_status borb_search_for_initialization(borb_matcher* m, const borb_
                                                     float* prev_matched, int window_size, float nnratio, int check_orientation,
                                                     int32_t* matches12, int32_t* n_matches);
 
+/* One camera stream's ORBmatcher::SearchForInitialization(mInitialFrame, mCurrentFrame, mvbPrevMatched, mvIniMatches, windowSize)
+ * (src/ORBmatcher.cc:405-520, src/Tracking.cc:600). */
+typedef struct borb_init_job {
+    const borb_frame* initial;     /* F1 = mInitialFrame, resident */
+    const borb_frame* current;     /* F2 = mCurrentFrame, resident (its feature grid is used as built) */
+    float* prev_matched;           /* in/out, initial->n x 2: vbPrevMatched, updated as the single call does (:513-517) */
+    int32_t window_size;           /* 100 at the call site */
+    int32_t* matches12;            /* output, initial->n entries: vnMatches12 */
+} borb_init_job;
+/* borb_search_for_initialization for n_jobs camera streams on resident frames in two launches and one synchronisation, whatever
+ * n_jobs is.  nnratio and check_orientation apply to every job.  Every job's matches12, prev_matched and n_matches[j] are
+ * bit-identical to what borb_search_for_initialization returns on host views of the same two frames.  A frame may appear in several
+ * jobs (one initial frame against several current frames), and initial == current is allowed.  A NULL frame, a frame on another
+ * device, a NULL prev_matched or matches12 for an initial frame with features, and a NULL jobs or n_matches when n_jobs > 0 are
+ * refused with BORB_ERR_INVALID_ARG before anything is launched, the error text starting with "job j:".  A job whose initial or
+ * current frame has 0 features gets matches12 -1 and 0 matches, its prev_matched untouched.
+ * Per job, only prev_matched crosses PCIe (initial->n x 8 bytes each way, plus initial->n x 4 + 4 bytes of results); the device
+ * scratch is initial->n x 36 bytes (the 8 smallest window entries and the window size of each initial-frame feature), with no
+ * initial->n x current->n candidate list. */
+BORB_API borb_status borb_search_for_initialization_batch(borb_matcher* m, const borb_init_job* jobs, int n_jobs,
+                                                          float nnratio, int check_orientation, int32_t* n_matches);
+
 /* MapPoint::ComputeDistinctiveDescriptors — src/MapPoint.cc:242-307, for n_points MapPoints in one launch.
  * desc: the observing keyframes' descriptors (pKF->mDescriptors.row(idx) of every non-bad observation, in
  * mObservations order), MapPoint p owning rows offsets[p] .. offsets[p+1]-1.  best_idx[p] = row (relative to

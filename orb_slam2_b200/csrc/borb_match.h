@@ -85,6 +85,21 @@ struct FuseJob {                  // one job of fuse_batch_kernel (k_proj.cu)
     int* n_found;
 };
 
+constexpr int INIT_K = 8;         // window entries per F1 feature kept by init_prefix_kernel
+
+struct InitJob {                  // one SearchForInitialization of borb_search_for_initialization_batch (k_proj.cu)
+    ProjArgs A;                   // F2 = the current frame: keys, descriptors, grid and bounds of the resident frame (bind_resident)
+    const borb_keypoint* keys1;   // F1 = the initial frame
+    const uint8_t* desc1;
+    int n1;                       // 0: nothing to do (the host wrote the result of a job without features)
+    float window;                 // (float)windowSize
+    const float* prev_in;         // vbPrevMatched, n1 x 2
+    uint32_t* prefix;             // scratch, n1 x INIT_K: the smallest window keys as F2 feature | dist << 16, in (dist, e) order
+    int* win_count;               // scratch, n1: the window's entries (0: skipped feature or empty window)
+    int32_t* out;                 // n1 entries of vnMatches12, then the match count
+    float* prev_out;              // n1 x 2: vbPrevMatched after the call (:513-517)
+};
+
 struct LastArgs {                 // inputs of project_points_kernel
     int variant;                  // 0: (CurrentFrame, LastFrame) :1328   1: (CurrentFrame, KeyFrame) :1472   2: (KeyFrame, Scw) :290
                                   // 3: Frame::isInFrustum (src/Frame.cc:269-325), feeding SearchByProjection(F, vpMapPoints)
@@ -298,6 +313,10 @@ int launch_point_projection_batch(const LastArgs* d_last, const ProjArgs* d_jobs
 void launch_resolve(const ProjArgs& A, bool last, cudaStream_t s);
 int launch_initialization(const ProjArgs& A, const borb_keypoint* keys1, int n1, int32_t* match12, int32_t* ev_idx, uint8_t* ev_bin,
                           float* prev, int* n_matches, cudaStream_t s);
+// SearchForInitialization of n_jobs jobs in 2 launches: one job by value (`one`), more over the InitJob table d_jobs;
+// max_n1 / max_n2 = the most features of an initial / current frame of a live job
+int launch_init_batch(const InitJob* d_jobs, const InitJob& one, int n_jobs, int max_n1, int max_n2, float nnratio, int check_ori,
+                      cudaStream_t s);
 // n_jobs queries (a job table in device memory) in one launch; max_slots / max_nq: the largest n_slots / nq of the jobs
 int launch_kfdb_score(const KfdbQueryJob* d_jobs, int n_jobs, int max_slots, int max_nq, int n_sm, cudaStream_t s);
 int launch_distinctive(const uint8_t* desc, const int32_t* offsets, int n_points, int32_t* best_idx, cudaStream_t s);

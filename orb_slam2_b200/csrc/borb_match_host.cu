@@ -1324,6 +1324,74 @@ borb_status borb_search_for_initialization(borb_matcher* m, const borb_frame_vie
     return c.finish();
 }
 
+// Tracking::MonocularInitialization of many camera streams: every job reads its two resident frames in place (keys, descriptors and
+// the current frame's grid as built), only vbPrevMatched crosses PCIe, and two launches serve every job (k_proj.cu).
+borb_status borb_search_for_initialization_batch(borb_matcher* m, const borb_init_job* jobs, int n_jobs, float nnratio, int check_orientation,
+                                                 int32_t* n_matches) {
+    if (!m || n_jobs < 0) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+    if (n_jobs > 0 && (!jobs || !n_matches)) { set_error("job 0: null job table or n_matches"); return BORB_ERR_INVALID_ARG; }
+    struct Job { int n1 = 0, n2 = 0; bool live = false; size_t prev = 0, pre = 0, cnt = 0, res = 0, rprev = 0; };
+    std::vector<Job> J(n_jobs);
+    for (int j = 0; j < n_jobs; j++) {
+        const borb_init_job& B = jobs[j];
+        if (!B.initial || !B.current) { set_error("job %d: null frame (the batch takes device-resident frames)", j); return BORB_ERR_INVALID_ARG; }
+        for (const borb_frame* f : {B.initial, B.current}) {
+            borb_frame_view v{};
+            v.resident = f;
+            const borb_status s = check_frame(&v, frame_info(&v), m);
+            if (s != BORB_OK) return job_fail(true, j, s);
+        }
+        J[j].n1 = B.initial->n; J[j].n2 = B.current->n;
+        if (J[j].n1 > 0 && (!B.prev_matched || !B.matches12)) { set_error("job %d: null prev_matched or matches12", j); return BORB_ERR_INVALID_ARG; }
+    }
+    int max_n1 = 0, max_n2 = 0;
+    for (int j = 0; j < n_jobs; j++) {                  // a job without features gets the single call's result here (prev_matched untouched)
+        n_matches[j] = 0;
+        J[j].live = J[j].n1 > 0 && J[j].n2 > 0;
+        if (!J[j].live) { std::fill_n(jobs[j].matches12, J[j].n1, -1); continue; }
+        max_n1 = std::max(max_n1, J[j].n1); max_n2 = std::max(max_n2, J[j].n2);
+    }
+    if (max_n1 == 0) return BORB_OK;
+    Call c(m);
+    for (int j = 0; j < n_jobs; j++)
+        if (J[j].live) J[j].prev = c.in(jobs[j].prev_matched, (size_t)J[j].n1 * 8);
+    JobTable<InitJob> jt(c, n_jobs);
+    for (int j = 0; j < n_jobs; j++) {
+        if (!J[j].live) continue;
+        J[j].pre = c.scratch((size_t)J[j].n1 * INIT_K * 4);
+        J[j].cnt = c.scratch((size_t)J[j].n1 * 4);
+        J[j].res = c.result((size_t)J[j].n1 * 4 + 4);
+        J[j].rprev = c.result((size_t)J[j].n1 * 8);
+    }
+    borb_status s;
+    if ((s = c.begin(n_jobs == 1)) != BORB_OK) return s;
+    InitJob* hj = jt.host(c);
+    for (int j = 0; j < n_jobs; j++) {
+        InitJob I{};
+        if (J[j].live) {                                 // a dead job keeps n1 = 0: both kernels skip it
+            const borb_init_job& B = jobs[j];
+            bind_resident(B.current, I.A);
+            I.keys1 = B.initial->keys; I.desc1 = B.initial->desc; I.n1 = J[j].n1;
+            I.window = (float)B.window_size;
+            I.prev_in = (const float*)c.dev(J[j].prev);
+            I.prefix = (uint32_t*)c.dev(J[j].pre); I.win_count = (int*)c.dev(J[j].cnt);
+            I.out = (int32_t*)c.res(J[j].res, true); I.prev_out = (float*)c.res(J[j].rprev, true);     // straight into the landing buffer
+        }
+        hj[j] = I;
+    }
+    if ((s = c.commit()) != BORB_OK) return s;
+    for (int j = 0; j < n_jobs; j++)
+        if (J[j].live && ((s = c.wait(jobs[j].initial)) != BORB_OK || (s = c.wait(jobs[j].current)) != BORB_OK)) return s;
+    m->launches += launch_init_batch(jt.dev(c), hj[0], n_jobs, max_n1, max_n2, nnratio, check_orientation, m->stream);
+    if ((s = c.finish()) != BORB_OK) return s;
+    for (int j = 0; j < n_jobs; j++) {
+        if (!J[j].live) continue;
+        read_counted(c.out(J[j].res), J[j].n1, jobs[j].matches12, &n_matches[j]);
+        std::memcpy(jobs[j].prev_matched, c.out(J[j].rprev), (size_t)J[j].n1 * 8);
+    }
+    return BORB_OK;
+}
+
 borb_status borb_distinctive_descriptors(borb_matcher* m, const uint8_t* desc, const int32_t* offsets, int n_points, int32_t* best_idx) {
     if (!m || !offsets || !best_idx || n_points < 0) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
     if (n_points == 0) return BORB_OK;

@@ -19,6 +19,7 @@
 //       number of queries, the cost.)
 //       LAST = false: best / second-best + ratio test (:98-121), out[query] = feature.
 //       LAST = true : best only, threshold th_dist, out[feature] = query, match events for the rotation histogram (:1426-1466).
+//   init_prefix_kernel / init_replay_kernel   SearchForInitialization (:405-520) of many frame pairs on resident frames (below).
 // All float tests use _rn intrinsics (no FMA contraction) so comparisons match the reference bit for bit.
 #include "borb_match.h"
 
@@ -434,6 +435,201 @@ void launch_resolve(const ProjArgs& A, bool last, cudaStream_t s) {
         allow_max_smem((const void*)proj_resolve_kernel<false>);
         proj_resolve_kernel<false><<<1, threads, smem, s>>>(A);
     }
+}
+
+// ------------------------------------------------------------------------------------------------ SearchForInitialization
+// ORBmatcher::SearchForInitialization (:405-520) of many (initial F1, current F2) pairs of resident frames, two launches for any
+// number of jobs and O(n1 x INIT_K) scratch per job instead of an n1 x n2 candidate list.
+//   init_prefix_kernel   a warp per (job, F1 feature) on grid (features / 8, jobs), independent across queries.  A feature with
+//       octave > 0 is skipped (:421-423); otherwise its level-0 window GetFeaturesInArea(prev.x, prev.y, windowSize, 0, 0) is walked
+//       on F2's resident grid, each window column as ONE contiguous cell_idx range (as fuse_batch_kernel does), keeping the window's
+//       entry count and its INIT_K smallest keys (dist << 16) | e, with e the entry's position in cell_idx.
+//   init_replay_kernel   a warp per job replays F1's features in order with vMatchedDistance / vnMatches21 in shared memory.  A
+//       query's best and second best are the first two prefix entries that are not excluded (vMatchedDistance[i2] <= dist, :441-442).
+//       Only when the prefix runs out before it yields two while the window held more than INIT_K entries is the window walked
+//       again in line, under the current exclusion set.
+// Bit identity rests on two facts:
+//   1. Ascending e is the reference's vIndices2 order.  The grid is sorted by cell = ix * GRID_ROWS + iy, then by insertion, and
+//      GetFeaturesInArea walks ix outer, iy inner (Frame.cc:352-377).  So the reference's `dist < bestDist` / `dist < bestDist2`
+//      scan ends with the smallest and the second smallest key (dist << 16) | e among the entries it does not skip.
+//   2. The prefix holds the INIT_K smallest keys of the whole window.  When it yields two entries that are not excluded, no entry
+//      outside it can come before either of them: they are the first two of the whole window under the same exclusion set.
+// A displaced match (:462-466) needs no bookkeeping beyond vnMatches21: an F1 feature takes at most one F2 feature in the whole
+// call, so its final match is that feature if it still owns it.  The rotation histogram counts every match event (rotHist keeps the
+// displaced ones, :478), then the surviving matches outside the three largest bins are dropped (:485-510).
+namespace {
+// GetFeaturesInArea(x, y, rs, 0, 0) on A's grid: f(e, feature, distance to dq) for every entry of the window, lanes striding
+// over each column's cell_idx range
+template <class F>
+__device__ __forceinline__ void init_window(const ProjArgs& A, float x, float y, float rs, const uint32_t* dq, F f) {
+    int c0x, c1x, c0y, c1y;
+    if (!area_window(A, x, y, rs, c0x, c1x, c0y, c1y)) return;
+    const int lane = threadIdx.x & 31;
+    for (int ix = c0x; ix <= c1x; ix++) {
+        const int e1 = A.cell_start[ix * GRID_ROWS + c1y + 1];
+        for (int e = A.cell_start[ix * GRID_ROWS + c0y] + lane; e < e1; e += 32) {
+            const int idx = A.cell_idx[e];
+            if (!area_passes(A.keys[idx], nullptr, idx, x, y, x, rs, 0, 0)) continue;
+            f(e, idx, ham_words(dq, reinterpret_cast<const uint32_t*>(A.desc + (size_t)idx * 32)));
+        }
+    }
+}
+
+__device__ __forceinline__ void load_desc(const uint8_t* desc, int i, uint32_t* d) {
+    const uint4 a = reinterpret_cast<const uint4*>(desc)[(size_t)i * 2], b = reinterpret_cast<const uint4*>(desc)[(size_t)i * 2 + 1];
+    d[0] = a.x; d[1] = a.y; d[2] = a.z; d[3] = a.w; d[4] = b.x; d[5] = b.y; d[6] = b.z; d[7] = b.w;
+}
+}  // namespace
+
+__device__ __forceinline__ void init_prefix_body(const InitJob& J) {
+    const ProjArgs& A = J.A;
+    const int lane = threadIdx.x & 31;
+    const int i1 = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (i1 >= J.n1) return;
+    unsigned top[INIT_K];                                    // this lane's smallest keys, ascending
+#pragma unroll
+    for (int k = 0; k < INIT_K; k++) top[k] = 0xFFFFFFFFu;
+    int cnt = 0;
+    if (J.keys1[i1].octave <= 0) {                           // the single call's level test (level1 > 0: skipped)
+        uint32_t dq[8];
+        load_desc(J.desc1, i1, dq);
+        init_window(A, J.prev_in[2 * i1], J.prev_in[2 * i1 + 1], J.window, dq, [&](int e, int, int dist) {
+            cnt++;
+            const unsigned key = ((unsigned)dist << 16) | (unsigned)e;
+            if (key < top[INIT_K - 1]) {
+                top[INIT_K - 1] = key;
+#pragma unroll
+                for (int k = INIT_K - 1; k > 0; k--)
+                    if (top[k] < top[k - 1]) { const unsigned t = top[k]; top[k] = top[k - 1]; top[k - 1] = t; }
+            }
+        });
+    }
+    cnt = __reduce_add_sync(0xFFFFFFFFu, cnt);
+    // the warp's INIT_K smallest keys, in order: keys are distinct (e is), so one lane pops each
+    uint32_t mine = 0xFFFFFFFFu;
+#pragma unroll
+    for (int k = 0; k < INIT_K; k++) {
+        const unsigned m = warp_min(top[0]);
+        if (top[0] == m) {
+#pragma unroll
+            for (int t = 0; t < INIT_K - 1; t++) top[t] = top[t + 1];
+            top[INIT_K - 1] = 0xFFFFFFFFu;
+        }
+        if (lane == k && m != 0xFFFFFFFFu) mine = (m & 0xFFFF0000u) | (uint32_t)A.cell_idx[m & 0xFFFFu];
+    }
+    if (lane < INIT_K) J.prefix[(size_t)i1 * INIT_K + lane] = mine;
+    if (lane == 0) J.win_count[i1] = cnt;
+}
+
+__device__ __forceinline__ void init_replay_body(const InitJob& J, float nnratio, int check_ori) {
+    const ProjArgs& A = J.A;
+    extern __shared__ uint32_t ism[];
+    uint16_t* matchedDist = reinterpret_cast<uint16_t*>(ism);            // vMatchedDistance, 0xFFFF = INT_MAX
+    uint16_t* owner = matchedDist + ((A.n + 1) & ~1);                     // vnMatches21, 0xFFFF = -1
+    uint16_t* took = owner + ((A.n + 1) & ~1);                            // per F1 feature: the F2 feature it took, 0xFFFF = none
+    __shared__ int hist[32];
+    __shared__ uint32_t pre[32 * INIT_K];                                 // the prefixes of the current 32 queries
+    const int lane = threadIdx.x;
+    const int n1 = J.n1;
+    for (int i = lane; i < A.n; i += 32) { matchedDist[i] = 0xFFFFu; owner[i] = 0xFFFFu; }
+    for (int i = lane; i < n1; i += 32) took[i] = 0xFFFFu;
+    hist[lane] = 0;
+    __syncwarp();
+    for (int base = 0; base < n1; base += 32) {
+        // 32 queries' prefixes at once: the replay itself then touches shared memory only
+        const int q = base + lane;
+        const int cnt_l = q < n1 ? J.win_count[q] : 0;
+        const int nq = min(32, n1 - base);
+        for (int k = lane; k < nq * INIT_K; k += 32) pre[k] = J.prefix[(size_t)base * INIT_K + k];
+        unsigned todo = __ballot_sync(0xFFFFFFFFu, cnt_l > 0);           // (also: every lane has written its part of pre)
+        while (todo) {
+            const int src = __ffs(todo) - 1;
+            todo &= todo - 1;
+            const int i1 = base + src;
+            const int cnt = __shfl_sync(0xFFFFFFFFu, cnt_l, src);
+            const uint32_t ent = lane < INIT_K ? pre[src * INIT_K + lane] : 0xFFFFFFFFu;      // lane k: prefix entry k
+            const bool open = ent != 0xFFFFFFFFu && (unsigned)matchedDist[ent & 0xFFFFu] > (ent >> 16);
+            const unsigned ok = __ballot_sync(0xFFFFFFFFu, open);
+            unsigned e1 = 0xFFFFFFFFu, e2 = 0xFFFFFFFFu;           // F2 feature | dist << 16 of best and second best
+            if (__popc(ok) >= 2 || cnt <= INIT_K) {
+                if (ok) e1 = __shfl_sync(0xFFFFFFFFu, ent, __ffs(ok) - 1);
+                const unsigned ok2 = ok & (ok - 1);
+                if (ok2) e2 = __shfl_sync(0xFFFFFFFFu, ent, __ffs(ok2) - 1);
+            } else {                                                // the prefix ran out: walk the window under the exclusion set
+                uint32_t dq[8];
+                load_desc(J.desc1, i1, dq);
+                unsigned k1 = 0xFFFFFFFFu, k2 = 0xFFFFFFFFu;
+                init_window(A, J.prev_in[2 * i1], J.prev_in[2 * i1 + 1], J.window, dq, [&](int e, int idx, int dist) {
+                    if ((unsigned)matchedDist[idx] <= (unsigned)dist) return;
+                    const unsigned key = ((unsigned)dist << 16) | (unsigned)e;
+                    if (key < k1) { k2 = k1; k1 = key; } else if (key < k2) k2 = key;
+                });
+                const unsigned best = warp_min(k1);
+                const unsigned second = warp_min(k1 == best ? k2 : k1);
+                if (best != 0xFFFFFFFFu) e1 = (best & 0xFFFF0000u) | (uint32_t)A.cell_idx[best & 0xFFFFu];
+                e2 = second;                                        // only its distance is read
+            }
+            if (e1 != 0xFFFFFFFFu) {
+                const int bestDist = (int)(e1 >> 16);
+                const float bd2 = e2 != 0xFFFFFFFFu ? (float)(int)(e2 >> 16) : 2147483648.f;      // (float)INT_MAX
+                if (bestDist <= TH_LOW && (float)bestDist < __fmul_rn(bd2, nnratio) && lane == 0) {
+                    const int i2 = (int)(e1 & 0xFFFFu);
+                    owner[i2] = (uint16_t)i1;                       // the earlier owner, if any, has lost it
+                    matchedDist[i2] = (uint16_t)bestDist;
+                    took[i1] = (uint16_t)i2;
+                }
+            }
+            __syncwarp();                                           // the next query reads what lane 0 wrote
+        }
+        __syncwarp();                                               // pre is rewritten for the next 32 queries
+    }
+    const borb_keypoint* __restrict__ keys1 = J.keys1;
+    if (check_ori) {
+        for (int i = lane; i < n1; i += 32)                         // every match event, displaced ones included
+            if (took[i] != 0xFFFFu) atomicAdd(&hist[rot_bin(keys1[i].angle, A.keys[took[i]].angle)], 1);
+        __syncwarp();
+    }
+    int b1 = -1, b2 = -1, b3 = -1;
+    if (check_ori) three_maxima(hist, b1, b2, b3);
+    int nm = 0;
+    for (int i = lane; i < n1; i += 32) {
+        const int t = took[i];
+        int m = (t != 0xFFFF && owner[t] == i) ? t : -1;
+        if (m >= 0 && check_ori) {
+            const int b = rot_bin(keys1[i].angle, A.keys[m].angle);
+            if (b != b1 && b != b2 && b != b3) m = -1;
+        }
+        float px = J.prev_in[2 * i], py = J.prev_in[2 * i + 1];
+        if (m >= 0) { px = A.keys[m].x; py = A.keys[m].y; nm++; }     // vbPrevMatched (:513-517)
+        J.out[i] = m;
+        J.prev_out[2 * i] = px; J.prev_out[2 * i + 1] = py;
+    }
+    nm = __reduce_add_sync(0xFFFFFFFFu, nm);
+    if (lane == 0) J.out[n1] = nm;
+}
+
+__global__ void __launch_bounds__(256) init_prefix_kernel(InitJob J) { init_prefix_body(J); }
+__global__ void __launch_bounds__(256) init_prefix_batch_kernel(const InitJob* __restrict__ jobs) { init_prefix_body(jobs[blockIdx.y]); }
+__global__ void __launch_bounds__(32) init_replay_kernel(InitJob J, float nnratio, int check_ori) { init_replay_body(J, nnratio, check_ori); }
+__global__ void __launch_bounds__(32) init_replay_batch_kernel(const InitJob* __restrict__ jobs, float nnratio, int check_ori) {
+    const InitJob& J = jobs[blockIdx.x];
+    if (J.n1 > 0) init_replay_body(J, nnratio, check_ori);
+}
+
+int launch_init_batch(const InitJob* d_jobs, const InitJob& one, int n_jobs, int max_n1, int max_n2, float nnratio, int check_ori,
+                      cudaStream_t s) {
+    if (n_jobs <= 0 || max_n1 <= 0) return 0;
+    const size_t smem = (size_t)(2 * ((max_n2 + 1) & ~1) + max_n1) * 2 + 16;
+    if (n_jobs == 1) {
+        init_prefix_kernel<<<(one.n1 + 7) / 8, 256, 0, s>>>(one);
+        allow_max_smem((const void*)init_replay_kernel);
+        init_replay_kernel<<<1, 32, smem, s>>>(one, nnratio, check_ori);
+    } else {
+        init_prefix_batch_kernel<<<dim3((max_n1 + 7) / 8, n_jobs), 256, 0, s>>>(d_jobs);
+        allow_max_smem((const void*)init_replay_batch_kernel);
+        init_replay_batch_kernel<<<n_jobs, 32, smem, s>>>(d_jobs, nnratio, check_ori);
+    }
+    return 2;
 }
 
 }  // namespace borb

@@ -91,6 +91,11 @@ class _LastFrameJobC(C.Structure):                 # borb_last_frame_job
                [("forward", C.c_int32), ("backward", C.c_int32), ("state_cur", C.c_void_p)]
 
 
+class _InitJobC(C.Structure):                      # borb_init_job
+    _fields_ = [("initial", C.c_void_p), ("current", C.c_void_p), ("prev_matched", C.c_void_p), ("window_size", C.c_int32),
+                ("matches12", C.c_void_p)]
+
+
 def _p(a):
     return a.ctypes.data if a is not None else None
 
@@ -556,6 +561,31 @@ class ORBmatcher:
         check(self._lib.borb_search_for_initialization(self._h, C.byref(views[0]), C.byref(views[1]), _p(prev), int(windowSize), self.mfNNratio,
                                                        int(self.mbCheckOrientation), _p(m12), C.byref(nm)), "borb_search_for_initialization")
         return nm.value, m12[:n1], prev[:n1]
+
+    def SearchForInitializationBatch(self, F1s: Sequence[FrameView], F2s: Sequence[FrameView], prevs, windowSize=100):
+        """borb_search_for_initialization_batch: SearchForInitialization of many camera streams in two launches.  F1s[j] / F2s[j] =
+        job j's initial and current frames, device-resident (FrameView.resident); prevs[j] = its vbPrevMatched (N1,2); windowSize is
+        one value or one per job.  Returns [(nmatches, vnMatches12, updated vbPrevMatched)] per job, equal to what
+        SearchForInitialization returns on host views of the same frames."""
+        n = len(F1s)
+        assert n == len(F2s) == len(prevs)
+        wins = _per_job(windowSize, n)
+        jobs = (_InitJobC * max(n, 1))()
+        outs = []
+        for j in range(n):
+            F1, F2 = F1s[j], F2s[j]
+            n1 = F1.resident.n if F1.resident is not None else len(F1.mvKeysUn)
+            prev = np.ascontiguousarray(np.asarray(prevs[j], np.float32).reshape(-1, 2)).copy()
+            if len(prev) == 0:
+                prev = np.zeros((1, 2), np.float32)
+            m12 = np.full(max(n1, 1), -1, np.int32)
+            jobs[j] = _InitJobC(F1.resident._h if F1.resident is not None else None, F2.resident._h if F2.resident is not None else None,
+                                _p(prev), int(wins[j]), _p(m12))
+            outs.append((n1, m12, prev))
+        nm = np.zeros(max(n, 1), np.int32)
+        check(self._lib.borb_search_for_initialization_batch(self._h, jobs, n, self.mfNNratio, int(self.mbCheckOrientation), _p(nm)),
+              "borb_search_for_initialization_batch")
+        return [(int(nm[j]), m12[:n1], prev[:n1]) for j, (n1, m12, prev) in enumerate(outs)]
 
     def ComputeDistinctiveDescriptors(self, groups) -> np.ndarray:
         """MapPoint::ComputeDistinctiveDescriptors (src/MapPoint.cc:242-307) for a batch of MapPoints: groups[p] = (N_p,32)

@@ -112,6 +112,7 @@ FB = M.FrameView(kb, rng.integers(0, 256, (6000, 32), dtype=np.uint8), X.GetScal
 mt.ComputeBoWBatch(voc6, [FR0, FB], 2, want_host=False)
 print("kfdb query batch", [q[0][:3] for q in mt.KfdbQueryBatch([db2, db3], [FR0, FB])])
 print("bowdb batch", [int(r[0].sum()) for r in mt.SearchByBoWDbBatch([db2, db3, db2], [None, None, [0, 5, 5]], [FR0, FB, FB])])
+print("init batch", [r[0] for r in mt.SearchForInitializationBatch([FR0, FR0, FB], [FR0, FB, FR0], [np.stack([outs[0][0]["x"], outs[0][0]["y"]], 1)] * 2 + [np.stack([kb["x"], kb["y"]], 1)], [100, 100, 30])])
 
 # place-recognition envelope (tests/bow_envelope.py): the flat 70,000-word vocabulary, the 8192 x 8192 one-node database search,
 # and a job table of 2 * n_SM + 1 small shared-memory jobs (some CTA loads three or more frame blocks)
