@@ -484,6 +484,74 @@ typedef struct borb_init_job {
 BORB_API borb_status borb_search_for_initialization_batch(borb_matcher* m, const borb_init_job* jobs, int n_jobs,
                                                           float nnratio, int check_orientation, int32_t* n_matches);
 
+/* One lost camera stream's ORBmatcher::SearchByProjection(CurrentFrame, pKF, sFound, th, ORBdist) after PnP in
+ * Tracking::Relocalization (src/Tracking.cc:1452 with th 10, ORBdist 100, and :1466 with th 3, ORBdist 64; src/ORBmatcher.cc:1472-1599):
+ * the per-frame arguments of borb_search_by_projection_kf. */
+typedef struct borb_kf_projection_job {
+    borb_frame_view cur;           /* cur.resident must be set; cur.occupied[i2] = CurrentFrame.mvpMapPoints[i2] != NULL, read per job */
+    borb_worldpoints_view pts;     /* pKF->GetMapPointMatches(), valid[i] = pMP && !isBad() && !sFound.count(pMP) */
+    float Tcw[12];                 /* CurrentFrame.mTcw rows 0..2 (the PnP pose) */
+    float Ow[3];                   /* -Rcw.t()*tcw (:1476-1478) */
+    float fx, fy, cx, cy;          /* CurrentFrame.fx, fy, cx, cy */
+    float log_scale_factor;        /* CurrentFrame.mfLogScaleFactor */
+    float th;                      /* 10 or 3 */
+    int32_t orb_dist;              /* 100 or 64 */
+    int32_t* state_cur;            /* output, cur n entries, as in borb_search_by_projection_kf */
+} borb_kf_projection_job;
+/* borb_search_by_projection_kf for n_jobs camera streams in one launch sequence (projection, candidates, resolve with a rotation
+ * histogram per job) and one synchronisation.  check_orientation applies to every job (the relocalisation matcher is
+ * ORBmatcher(0.9, true), src/Tracking.cc:1396).  Every job's state_cur and n_matches[j] are bit-identical to the single call's.
+ * Frames must be device-resident; a host view, a frame on another device, more than BORB_MATCH_MAX_FEATURES points,
+ * log_scale_factor <= 0, an incomplete points view and a NULL state_cur are refused with BORB_ERR_INVALID_ARG before anything is
+ * launched, the error text starting with "job j:".  A job with no points or a frame with 0 features gets state_cur -1 and 0 matches.
+ * The device scratch of a job includes a candidate list of pts.n x cur n x 4 bytes, as for borb_search_by_projection_last_batch. */
+BORB_API borb_status borb_search_by_projection_kf_batch(borb_matcher* m, const borb_kf_projection_job* jobs, int n_jobs,
+                                                        int check_orientation, int32_t* n_matches);
+
+/* One loop-closing stream's final ORBmatcher::SearchByProjection(mpCurrentKF, mScw, mvpLoopMapPoints, mvpCurrentMatchedPoints, 10)
+ * in LoopClosing::ComputeSim3 (src/LoopClosing.cc:375; src/ORBmatcher.cc:290-403): the arguments of borb_search_by_projection_sim3. */
+typedef struct borb_sim3_projection_job {
+    borb_frame_view kf;            /* kf.resident must be set; kf.occupied[idx] = vpMatched[idx] != NULL on entry, read per job */
+    borb_worldpoints_view pts;     /* mvpLoopMapPoints, valid[i] = !isBad() && !spAlreadyFound.count(pMP) */
+    float Tcw[12];                 /* [Rcw | tcw] with the Sim3 scale divided out (:298-303) */
+    float Ow[3];                   /* -Rcw.t()*tcw */
+    float fx, fy, cx, cy;          /* pKF->fx, fy, cx, cy */
+    float log_scale_factor;        /* pKF->mfLogScaleFactor */
+    int32_t th;                    /* 10 */
+    int32_t* state_kf;             /* output, kf n entries, as in borb_search_by_projection_sim3 */
+} borb_sim3_projection_job;
+/* borb_search_by_projection_sim3 for n_jobs streams in one launch sequence (projection, candidates, resolve) and one
+ * synchronisation.  Every job's state_kf and n_matches[j] are bit-identical to the single call's.  Keyframes must be
+ * device-resident; refusals, defaults and scratch as for borb_search_by_projection_kf_batch. */
+BORB_API borb_status borb_search_by_projection_sim3_batch(borb_matcher* m, const borb_sim3_projection_job* jobs, int n_jobs,
+                                                          int32_t* n_matches);
+
+/* One ORBmatcher::SearchBySim3(mpCurrentKF, pKF, vpMapPointMatches, s, R, t, 7.5) of LoopClosing::ComputeSim3
+ * (src/LoopClosing.cc:323; src/ORBmatcher.cc:1102-1326): the arguments of borb_search_by_sim3. */
+typedef struct borb_sim3_job {
+    borb_frame_view kf1;           /* pKF1 = mpCurrentKF, kf1.resident must be set; kf1.occupied is ignored */
+    borb_frame_view kf2;           /* pKF2 = the loop candidate, resident; kf2.occupied is ignored */
+    borb_worldpoints_view pts1;    /* kf1's GetMapPointMatches(), one slot per feature (pts1.n == kf1's n), valid as for the single call */
+    borb_worldpoints_view pts2;    /* kf2's, pts2.n == kf2's n */
+    float T1w[12];                 /* the keyframe poses (3x4) */
+    float T2w[12];
+    float S12[12];                 /* [s12*R12 | t12] and [(1/s12)*R12^T | -sR21*t12] (:1119-1122) */
+    float S21[12];
+    float fx, fy, cx, cy;          /* pKF1's intrinsics, used for both directions (:1105-1108) */
+    float log_scale_factor1, log_scale_factor2;
+    float th;                      /* 7.5 */
+    int32_t* match12;              /* output, kf1 n entries, as in borb_search_by_sim3 */
+} borb_sim3_job;
+/* borb_search_by_sim3 for n_jobs (keyframe, candidate) pairs in three launches (projection of both directions of every job, a warp
+ * per point that walks its window's grid cells and keeps the first minimum, then the agreement test) and one synchronisation,
+ * whatever n_jobs is.  Every job's match12 and n_found[j] are bit-identical to what borb_search_by_sim3 returns; kf1 == kf2 is
+ * allowed and a keyframe may appear in several jobs.  Keyframes must be device-resident; a host view, a frame on another device,
+ * more than BORB_MATCH_MAX_FEATURES points, pts1.n / pts2.n different from the keyframe's n, log_scale_factor <= 0, an incomplete
+ * points view and a NULL match12 are refused with BORB_ERR_INVALID_ARG before anything is launched, the error text starting with
+ * "job j:".  A job whose keyframes have 0 features gets match12 -1 and n_found 0.  The device scratch of a job is the projections
+ * of its pts1.n + pts2.n points and (pts1.n + pts2.n) x 4 bytes of per-direction matches, with no candidate list. */
+BORB_API borb_status borb_search_by_sim3_batch(borb_matcher* m, const borb_sim3_job* jobs, int n_jobs, int32_t* n_found);
+
 /* MapPoint::ComputeDistinctiveDescriptors — src/MapPoint.cc:242-307, for n_points MapPoints in one launch.
  * desc: the observing keyframes' descriptors (pKF->mDescriptors.row(idx) of every non-bad observation, in
  * mObservations order), MapPoint p owning rows offsets[p] .. offsets[p+1]-1.  best_idx[p] = row (relative to

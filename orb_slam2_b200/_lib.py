@@ -107,6 +107,9 @@ _SIGNATURES = {
     "borb_search_local_points": (C.c_int, [vp, vp, vp, vp, vp, vp] + [C.c_float] * 9 + [vp] * 7 + [i32p]),
     "borb_search_local_points_batch": (C.c_int, [vp, vp, C.c_int, C.c_float, C.c_float, vp]),
     "borb_search_by_projection_last_batch": (C.c_int, [vp, vp, C.c_int, C.c_int, vp]),
+    "borb_search_by_projection_kf_batch": (C.c_int, [vp, vp, C.c_int, C.c_int, vp]),
+    "borb_search_by_projection_sim3_batch": (C.c_int, [vp, vp, C.c_int, vp]),
+    "borb_search_by_sim3_batch": (C.c_int, [vp, vp, C.c_int, vp]),
     "borb_fuse": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int,
                             vp, i32p]),
     "borb_search_by_sim3": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float,

@@ -72,7 +72,7 @@ struct ProjArgs {                 // device pointers
     int check_ori;
     const float* q_angle;         // mode 1: mvKeysUn[i].angle of the query
     int th_dist;                  // mode 1: accept bestDist <= th_dist (TH_HIGH / ORBdist / TH_LOW)
-    // where the resolve / argmin kernels write the results
+    // where the resolve / fuse kernels write the results
     int32_t* out_match;           // n_mp entries (mode 1 resolve: the per-feature state, n entries), then the match count
     int32_t* ev_idx;              // mode 1: match events of the rotation histogram, n_mp entries
     uint8_t* ev_bin;
@@ -83,6 +83,14 @@ struct FuseJob {                  // one job of fuse_batch_kernel (k_proj.cu)
                                   // fields); th_dist = TH_LOW; out_match = best_idx, n_mp entries
     const float* inv_sigma2;      // mvInvLevelSigma2: the reprojection gates of Fuse(pKF, vpMapPoints, th); null for the Scw overload
     int* n_found;
+};
+
+struct Sim3AgreeJob {             // one SearchBySim3 of sim3_agree_batch_kernel (k_proj.cu)
+    const int32_t* match1;        // KF1's points searched in KF2: n1 entries, a KF2 feature or -1 (fuse_batch_kernel's best_idx)
+    const int32_t* match2;        // KF2's points searched in KF1: n2 entries
+    int n1, n2;                   // n1 = 0: nothing to do (the host wrote the result of a job without features)
+    int32_t* match12;             // n1 entries
+    int* n_found;                 // preset to 0
 };
 
 constexpr int INIT_K = 8;         // window entries per F1 feature kept by init_prefix_kernel
@@ -320,8 +328,6 @@ int launch_init_batch(const InitJob* d_jobs, const InitJob& one, int n_jobs, int
 // n_jobs queries (a job table in device memory) in one launch; max_slots / max_nq: the largest n_slots / nq of the jobs
 int launch_kfdb_score(const KfdbQueryJob* d_jobs, int n_jobs, int max_slots, int max_nq, int n_sm, cudaStream_t s);
 int launch_distinctive(const uint8_t* desc, const int32_t* offsets, int n_points, int32_t* best_idx, cudaStream_t s);
-int launch_projection_argmin(const LastArgs& L, const ProjArgs& A, cudaStream_t s);
-int launch_sim3_agree(const int32_t* match1, const int32_t* match2, int n1, int n2, int32_t* match12, int* n_found, cudaStream_t s);
 // n_pairs searches in one launch (tables in device memory): pair p matches qs[p] against ts[p] and writes its output (mode 0: ts[p].n
 // entries, mode 1: qs[p].n) at match + out_off[p], its rotation bins at bins + out_off[p]; max_t = the largest ts[p].n
 int launch_bow_match(const KfDev* qs, const KfDev* ts, int n_pairs, int mode, float nnratio, int check_ori, int32_t* match,
@@ -340,6 +346,10 @@ int launch_triangulation(const TriJob* d_jobs, int n_jobs, int check_ori, cudaSt
 // project_points over a LastArgs table (variant 2), then fuse_batch_kernel over a FuseJob table: 2 launches; max_nq = most points of a job
 int launch_fuse_batch(const LastArgs* d_last, const FuseJob* d_jobs, int n_jobs, int max_nq, cudaStream_t s);
 void launch_fuse_search(const FuseJob* d_jobs, int n_jobs, int max_nq, cudaStream_t s);
+// SearchBySim3 of n_jobs jobs in 3 launches: launch_fuse_batch over the 2 n_jobs direction entries of d_last / d_dirs (job j: 2j and
+// 2j + 1), then sim3_agree_batch_kernel over d_jobs; max_nq = most points of a direction, max_n1 = most KF1 features of a job
+int launch_sim3_batch(const LastArgs* d_last, const FuseJob* d_dirs, const Sim3AgreeJob* d_jobs, int n_jobs, int max_nq, int max_n1,
+                      cudaStream_t s);
 int launch_bow_transform(const VocDev& V, const uint8_t* desc, int n, int levelsup, int32_t* word, double* weight, int32_t* node,
                          cudaStream_t s);
 // descent + bookkeeping for n_frames frames (a job table in device memory): 2 launches

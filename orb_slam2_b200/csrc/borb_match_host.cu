@@ -21,8 +21,6 @@ struct borb_matcher {
     uint8_t* h_stage = nullptr;     // pinned staging mirror of the arena's input part
     size_t h_bytes = 0;
     uint64_t launches = 0;
-    int32_t* aux = nullptr;         // small device buffer that survives an arena re-layout (SearchBySim3: first direction's matches)
-    size_t aux_count = 0;
     uint8_t* h_out = nullptr;       // pinned landing buffer for results (one D2H per call)
     size_t h_out_bytes = 0;
     std::vector<int32_t> sel;       // indices of the valid queries of the current call
@@ -365,7 +363,6 @@ borb_status borb_matcher_destroy(borb_matcher* m) {
     cudaSetDevice(m->device);
     if (m->stream) cudaStreamSynchronize(m->stream);
     cudaFree(m->arena);
-    cudaFree(m->aux);
     if (m->h_stage) cudaFreeHost(m->h_stage);
     if (m->h_out) cudaFreeHost(m->h_out);
     if (m->ev_a) { cudaEventDestroy(m->ev_a); cudaEventDestroy(m->ev_b); }
@@ -710,11 +707,8 @@ struct PointQuery {
     // variant 2 family (order-independent overloads share the projection code)
     int invz_double, use_normal, chain;
     const float* T2;                // chain: [sR | t] applied after Tcw
-    int argmin;                     // 1: per-query first-minimum (no claim replay); `state` then has Q.n entries
     int chi2;                       // Fuse(pKF, ...) reprojection gates
     const float* inv_sigma2;        // chi2: mvInvLevelSigma2 (n_levels)
-    int to_aux;                     // 1: leave the result in m->aux + aux_off (device) instead of downloading it
-    size_t aux_off;
 };
 
 namespace {
@@ -764,15 +758,15 @@ void reserve_projection(Call& c, const FrameInfo& I, const PointQuery& Q, QueryO
     o.px = c.scratch(nq * 4); o.py = c.scratch(nq * 4); o.pxr = c.scratch(nq * 4); o.rad = c.scratch(nq * 4);
     o.ang = c.scratch(nq * 4); o.minl = c.scratch(nq * 4); o.maxl = c.scratch(nq * 4); o.val = c.scratch(nq);
 }
-// the same plus the candidate lists and the match events of the resolve / argmin kernels
+// the same plus the candidate lists and the match events of the resolve kernel
 void reserve_query(Call& c, const FrameInfo& I, const PointQuery& Q, QueryOff& o) {
     const size_t nq = (size_t)Q.n;
     reserve_projection(c, I, Q, o);
     o.cand = c.scratch(nq * I.n * 4); o.cc = c.scratch(nq * 4);
     o.evi = c.scratch(nq * 4); o.evb = c.scratch(nq);
 }
-// L and the query side of A (the frame side comes from bind_frame_fields); out: the state (argmin: Q.n entries, otherwise I.n)
-// followed by the match count
+// L and the query side of A (the frame side comes from bind_frame_fields); out: where the search kernel writes (the resolve kernel:
+// I.n entries of state followed by the match count; fuse_batch_kernel: one entry per query)
 void bind_query(const QueryOff& o, const PointQuery& Q, const FrameInfo& I, const Call& c, int32_t* out, LastArgs& L, ProjArgs& A) {
     L.variant = Q.variant;
     L.n_last = Q.n; L.last_keys = Q.keys ? (const borb_keypoint*)c.dev(o.lk) : nullptr; L.world_pos = (const float*)c.dev(o.wp);
@@ -809,31 +803,45 @@ PointQuery last_frame_query(const borb_last_frame_job& B, int check_orientation)
     Q.check_ori = check_orientation; Q.th_dist = TH_HIGH;                  // (:1426)
     return Q;
 }
+// SearchByProjection(CurrentFrame, pKF, sAlreadyFound, th, ORBdist) of one relocalising camera stream
+PointQuery kf_query(const borb_kf_projection_job& B, int check_orientation) {
+    PointQuery Q{};
+    Q.variant = 1; Q.n = B.pts.n; Q.world_pos = B.pts.world_pos; Q.desc = B.pts.desc; Q.valid = B.pts.valid;
+    Q.max_distance = B.pts.max_distance; Q.min_distance = B.pts.min_distance; Q.angle = B.pts.angle;
+    Q.Tcw = B.Tcw; Q.Ow = B.Ow; Q.fx = B.fx; Q.fy = B.fy; Q.cx = B.cx; Q.cy = B.cy; Q.th = B.th; Q.log_scale = B.log_scale_factor;
+    Q.check_ori = check_orientation; Q.th_dist = B.orb_dist;
+    return Q;
+}
+// SearchByProjection(pKF, Scw, vpPoints, vpMatched, th) of one loop-closing camera stream
+PointQuery sim3_projection_query(const borb_sim3_projection_job& B) {
+    PointQuery Q{};
+    Q.variant = 2; Q.n = B.pts.n; Q.world_pos = B.pts.world_pos; Q.desc = B.pts.desc; Q.valid = B.pts.valid;
+    Q.max_distance = B.pts.max_distance; Q.min_distance = B.pts.min_distance; Q.normal = B.pts.normal;
+    Q.Tcw = B.Tcw; Q.Ow = B.Ow; Q.fx = B.fx; Q.fy = B.fy; Q.cx = B.cx; Q.cy = B.cy; Q.th = (float)B.th; Q.log_scale = B.log_scale_factor;
+    Q.check_ori = 0; Q.th_dist = TH_LOW;                                   // (:394)
+    Q.use_normal = 1;
+    return Q;
+}
 
-// one (frame, query) pair of point_query_jobs; state: the job's output (argmin: Q.n entries, otherwise the frame's n), or null (to_aux)
+// one (frame, query) pair of point_query_jobs; state: the job's output, the frame's n entries
 struct PointJob { const borb_frame_view* F; PointQuery Q; int32_t* state; };
 
-// Shared body of borb_search_by_projection_last / _kf / _sim3, of the two directions of borb_search_by_sim3 (argmin, to_aux: one job
-// only) and of borb_search_by_projection_last_batch (resident frames): project_points, candidates and resolve<true> (or argmin),
-// one synchronisation.  The state stays in the arena, not in mapped host memory: resolve<true> writes it with atomicMax.
-borb_status point_query_jobs(borb_matcher* m, const PointJob* jobs, int n_jobs, int32_t* n_matches, bool batch) {
+// Shared body of borb_search_by_projection_last / _kf / _sim3 and of their _batch forms (resident frames): project_points,
+// candidates and resolve<true>, one synchronisation.  batch: the name of the batched entry point (its errors name the job), null for
+// a single call.  The state stays in the arena, not in mapped host memory: resolve<true> writes it with atomicMax.
+borb_status point_query_jobs(borb_matcher* m, const PointJob* jobs, int n_jobs, int32_t* n_matches, const char* batch) {
     struct Job { FrameInfo I; bool live; QueryOff o; size_t res; };
     std::vector<Job> J(n_jobs);
     int max_n = 1, max_nq = 0;
     for (int j = 0; j < n_jobs; j++) {
         const PointQuery& Q = jobs[j].Q;
-        assert(n_jobs == 1 || (!Q.argmin && !Q.to_aux));
         n_matches[j] = 0;
-        if (batch && !jobs[j].F->resident) { set_error("job %d: borb_search_by_projection_last_batch needs device-resident frames (borb_frame_view::resident)", j); return BORB_ERR_INVALID_ARG; }
+        if (batch && !jobs[j].F->resident) { set_error("job %d: %s needs device-resident frames (borb_frame_view::resident)", j, batch); return BORB_ERR_INVALID_ARG; }
         if (batch && !jobs[j].state) { set_error("job %d: null output", j); return BORB_ERR_INVALID_ARG; }
         const FrameInfo I = J[j].I = frame_info(jobs[j].F);
         borb_status s = check_query(jobs[j].F, I, Q, m);
-        if (s != BORB_OK) return job_fail(batch, j, s);
-        if (jobs[j].state) std::fill_n(jobs[j].state, Q.argmin ? Q.n : I.n, -1);
-        if (Q.to_aux && Q.n > 0) {      // caller sized m->aux; "no match" everywhere until the kernels say otherwise
-            BORB_CUDA(cudaSetDevice(m->device));
-            BORB_CUDA(cudaMemsetAsync(m->aux + Q.aux_off, 0xFF, (size_t)Q.n * 4, m->stream));
-        }
+        if (s != BORB_OK) return job_fail(batch != nullptr, j, s);
+        std::fill_n(jobs[j].state, I.n, -1);
         J[j].live = I.n > 0 && Q.n > 0;
         if (J[j].live) { max_n = std::max(max_n, I.n); max_nq = std::max(max_nq, Q.n); }
     }
@@ -845,10 +853,8 @@ borb_status point_query_jobs(borb_matcher* m, const PointJob* jobs, int n_jobs, 
     JobTable<ProjArgs> jt(c, n_jobs);
     for (int j = 0; j < n_jobs; j++) {
         if (!J[j].live) continue;
-        const PointQuery& Q = jobs[j].Q;
-        reserve_query(c, J[j].I, Q, J[j].o);
-        const size_t bytes = (size_t)(Q.argmin ? Q.n : J[j].I.n) * 4 + 4;
-        J[j].res = Q.to_aux ? c.scratch(bytes) : c.result(bytes);
+        reserve_query(c, J[j].I, jobs[j].Q, J[j].o);
+        J[j].res = c.result((size_t)J[j].I.n * 4 + 4);
     }
     borb_status s;
     if ((s = c.begin(n_jobs == 1 && J[0].I.rf)) != BORB_OK) return s;
@@ -858,9 +864,8 @@ borb_status point_query_jobs(borb_matcher* m, const PointJob* jobs, int n_jobs, 
         LastArgs L{};
         ProjArgs A{};
         if (J[j].live) {
-            const PointQuery& Q = jobs[j].Q;
             bind_frame_fields(J[j].I, J[j].o.fs, c, A);
-            bind_query(J[j].o, Q, J[j].I, c, (int32_t*)(Q.to_aux ? c.dev(J[j].res) : c.res(J[j].res, false)), L, A);
+            bind_query(J[j].o, jobs[j].Q, J[j].I, c, (int32_t*)c.res(J[j].res, false), L, A);
         }                                            // a job without work keeps n_last = n_mp = 0: every kernel skips it
         hl[j] = L;
         hj[j] = A;
@@ -868,14 +873,10 @@ borb_status point_query_jobs(borb_matcher* m, const PointJob* jobs, int n_jobs, 
     if ((s = c.commit()) != BORB_OK) return s;
     for (int j = 0; j < n_jobs; j++)
         if (J[j].live && (s = prepare_frame(m, c, J[j].I, hj[j])) != BORB_OK) return s;
-    const PointQuery& Q0 = jobs[0].Q;
-    if (Q0.argmin) m->launches += launch_projection_argmin(hl[0], hj[0], m->stream);
-    else m->launches += launch_point_projection_batch(lt.dev(c), jt.dev(c), hl[0], hj[0], n_jobs, max_nq, max_n, max_nq, true, m->stream);
-    if (Q0.to_aux) BORB_CUDA(cudaMemcpyAsync(m->aux + Q0.aux_off, c.dev(J[0].res), (size_t)Q0.n * 4, cudaMemcpyDeviceToDevice, m->stream));
+    m->launches += launch_point_projection_batch(lt.dev(c), jt.dev(c), hl[0], hj[0], n_jobs, max_nq, max_n, max_nq, true, m->stream);
     if ((s = c.finish()) != BORB_OK) return s;
     for (int j = 0; j < n_jobs; j++)
-        if (J[j].live && !jobs[j].Q.to_aux)
-            read_counted(c.out(J[j].res), jobs[j].Q.argmin ? jobs[j].Q.n : J[j].I.n, jobs[j].state, &n_matches[j]);
+        if (J[j].live) read_counted(c.out(J[j].res), J[j].I.n, jobs[j].state, &n_matches[j]);
     return BORB_OK;
 }
 }  // namespace
@@ -889,34 +890,31 @@ borb_status borb_search_by_projection_last(borb_matcher* m, const borb_frame_vie
     std::memcpy(B.Tcw, Tcw, sizeof(B.Tcw));
     B.fx = fx; B.fy = fy; B.cx = cx; B.cy = cy; B.bf = bf; B.th = th; B.forward = forward; B.backward = backward;
     const PointJob P{F, last_frame_query(B, check_orientation), state_cur};
-    return point_query_jobs(m, &P, 1, n_matches, false);
+    return point_query_jobs(m, &P, 1, n_matches, nullptr);
 }
 
 borb_status borb_search_by_projection_kf(borb_matcher* m, const borb_frame_view* cur, const borb_worldpoints_view* pts, const float* Tcw,
                                          const float* Ow, float fx, float fy, float cx, float cy, float log_scale_factor, float th,
                                          int orb_dist, int check_orientation, int32_t* state_cur, int32_t* n_matches) {
     if (!m || !cur || !pts || !Tcw || !Ow || !state_cur || !n_matches) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
-    PointQuery Q{};
-    Q.variant = 1; Q.n = pts->n; Q.world_pos = pts->world_pos; Q.desc = pts->desc; Q.valid = pts->valid;
-    Q.max_distance = pts->max_distance; Q.min_distance = pts->min_distance; Q.angle = pts->angle;
-    Q.Tcw = Tcw; Q.Ow = Ow; Q.fx = fx; Q.fy = fy; Q.cx = cx; Q.cy = cy; Q.th = th; Q.log_scale = log_scale_factor;
-    Q.check_ori = check_orientation; Q.th_dist = orb_dist;
-    const PointJob P{cur, Q, state_cur};
-    return point_query_jobs(m, &P, 1, n_matches, false);
+    borb_kf_projection_job B{};
+    B.pts = *pts;
+    std::memcpy(B.Tcw, Tcw, sizeof(B.Tcw)); std::memcpy(B.Ow, Ow, sizeof(B.Ow));
+    B.fx = fx; B.fy = fy; B.cx = cx; B.cy = cy; B.log_scale_factor = log_scale_factor; B.th = th; B.orb_dist = orb_dist;
+    const PointJob P{cur, kf_query(B, check_orientation), state_cur};
+    return point_query_jobs(m, &P, 1, n_matches, nullptr);
 }
 
 borb_status borb_search_by_projection_sim3(borb_matcher* m, const borb_frame_view* kf, const borb_worldpoints_view* pts, const float* Tcw,
                                            const float* Ow, float fx, float fy, float cx, float cy, float log_scale_factor, int th,
                                            int32_t* state_kf, int32_t* n_matches) {
     if (!m || !kf || !pts || !Tcw || !Ow || !state_kf || !n_matches) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
-    PointQuery Q{};
-    Q.variant = 2; Q.n = pts->n; Q.world_pos = pts->world_pos; Q.desc = pts->desc; Q.valid = pts->valid;
-    Q.max_distance = pts->max_distance; Q.min_distance = pts->min_distance; Q.normal = pts->normal;
-    Q.Tcw = Tcw; Q.Ow = Ow; Q.fx = fx; Q.fy = fy; Q.cx = cx; Q.cy = cy; Q.th = (float)th; Q.log_scale = log_scale_factor;
-    Q.check_ori = 0; Q.th_dist = 50;                                       // TH_LOW (:394)
-    Q.use_normal = 1;
-    const PointJob P{kf, Q, state_kf};
-    return point_query_jobs(m, &P, 1, n_matches, false);
+    borb_sim3_projection_job B{};
+    B.pts = *pts;
+    std::memcpy(B.Tcw, Tcw, sizeof(B.Tcw)); std::memcpy(B.Ow, Ow, sizeof(B.Ow));
+    B.fx = fx; B.fy = fy; B.cx = cx; B.cy = cy; B.log_scale_factor = log_scale_factor; B.th = th;
+    const PointJob P{kf, sim3_projection_query(B), state_kf};
+    return point_query_jobs(m, &P, 1, n_matches, nullptr);
 }
 
 borb_status borb_search_by_projection_last_batch(borb_matcher* m, const borb_last_frame_job* jobs, int n_jobs, int check_orientation,
@@ -924,7 +922,22 @@ borb_status borb_search_by_projection_last_batch(borb_matcher* m, const borb_las
     if (!m || n_jobs < 0 || (n_jobs > 0 && (!jobs || !n_matches))) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
     std::vector<PointJob> P(n_jobs);
     for (int j = 0; j < n_jobs; j++) P[j] = PointJob{&jobs[j].cur, last_frame_query(jobs[j], check_orientation), jobs[j].state_cur};
-    return point_query_jobs(m, P.data(), n_jobs, n_matches, true);
+    return point_query_jobs(m, P.data(), n_jobs, n_matches, "borb_search_by_projection_last_batch");
+}
+
+borb_status borb_search_by_projection_kf_batch(borb_matcher* m, const borb_kf_projection_job* jobs, int n_jobs, int check_orientation,
+                                               int32_t* n_matches) {
+    if (!m || n_jobs < 0 || (n_jobs > 0 && (!jobs || !n_matches))) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+    std::vector<PointJob> P(n_jobs);
+    for (int j = 0; j < n_jobs; j++) P[j] = PointJob{&jobs[j].cur, kf_query(jobs[j], check_orientation), jobs[j].state_cur};
+    return point_query_jobs(m, P.data(), n_jobs, n_matches, "borb_search_by_projection_kf_batch");
+}
+
+borb_status borb_search_by_projection_sim3_batch(borb_matcher* m, const borb_sim3_projection_job* jobs, int n_jobs, int32_t* n_matches) {
+    if (!m || n_jobs < 0 || (n_jobs > 0 && (!jobs || !n_matches))) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+    std::vector<PointJob> P(n_jobs);
+    for (int j = 0; j < n_jobs; j++) P[j] = PointJob{&jobs[j].kf, sim3_projection_query(jobs[j]), jobs[j].state_kf};
+    return point_query_jobs(m, P.data(), n_jobs, n_matches, "borb_search_by_projection_sim3_batch");
 }
 
 // ---- the search part of Fuse: borb_fuse is the one-job case of borb_fuse_batch (project_points + fuse_batch_kernel, one
@@ -943,7 +956,7 @@ borb_status fuse_jobs(borb_matcher* m, const borb_fuse_job* jobs, int n_jobs, bo
         Q.max_distance = B.pts.max_distance; Q.min_distance = B.pts.min_distance; Q.normal = B.pts.normal;
         Q.Tcw = B.Tcw; Q.Ow = B.Ow; Q.fx = B.fx; Q.fy = B.fy; Q.cx = B.cx; Q.cy = B.cy; Q.bf = B.bf; Q.th = B.th; Q.log_scale = B.log_scale_factor;
         Q.th_dist = TH_LOW;                                                // (:944, :1075)
-        Q.use_normal = 1; Q.argmin = 1;
+        Q.use_normal = 1;
         Q.invz_double = B.scw_variant ? 1 : 0;                             // 1.0/z (:1014) vs 1/z (:861)
         Q.chi2 = B.scw_variant ? 0 : 1; Q.inv_sigma2 = B.inv_level_sigma2;
         // occupancy plays no role in either Fuse (the MapPoint already in the slot is handled by the caller, :947-960)
@@ -1018,52 +1031,131 @@ borb_status borb_fuse_batch(borb_matcher* m, const borb_fuse_job* jobs, int n_jo
     return fuse_jobs(m, jobs, n_jobs, true, n_found);
 }
 
+// ---- SearchBySim3: borb_search_by_sim3 is the one-job case of borb_search_by_sim3_batch.  A job is two direction jobs of
+// fuse_batch_kernel, both in one launch pair, whose matches stay in the arena; sim3_agree_batch_kernel then keeps the pairs the two
+// directions agree on.  3 launches and one synchronisation whatever n_jobs is; the scratch of a direction is its projections and its
+// matches, with no candidate list.
+namespace {
+// the points P of one keyframe, seen from camera 1 or 2 (Tw: that camera's pose) and chained into the other camera by S
+PointQuery sim3_direction(const borb_sim3_job& B, const borb_worldpoints_view& P, const float* Tw, const float* S, float log_scale) {
+    PointQuery Q{};
+    Q.variant = 2; Q.n = P.n; Q.world_pos = P.world_pos; Q.desc = P.desc; Q.valid = P.valid;
+    Q.max_distance = P.max_distance; Q.min_distance = P.min_distance;
+    Q.Tcw = Tw; Q.chain = 1; Q.T2 = S; Q.fx = B.fx; Q.fy = B.fy; Q.cx = B.cx; Q.cy = B.cy; Q.th = B.th; Q.log_scale = log_scale;
+    Q.th_dist = TH_HIGH; Q.invz_double = 1;                                // (:1221, :1301); invz = 1.0/z (:1166, :1246)
+    return Q;
+}
+
+borb_status sim3_jobs(borb_matcher* m, const borb_sim3_job* jobs, int n_jobs, bool batch, int32_t* n_found) {
+    // direction 2j: KF1's points into KF2 (:1146-1222); 2j + 1: KF2's points into KF1 (:1224-1300)
+    struct Dir { borb_frame_view kf; PointQuery Q; FrameInfo I; QueryOff o; size_t out = 0; };
+    std::vector<Dir> D(2 * (size_t)n_jobs);
+    std::vector<size_t> res(n_jobs);
+    std::vector<char> live(n_jobs);
+    int max_nq = 0, max_n1 = 0;
+    for (int j = 0; j < n_jobs; j++) {
+        const borb_sim3_job& B = jobs[j];
+        n_found[j] = 0;
+        Dir& d12 = D[2 * (size_t)j];
+        Dir& d21 = D[2 * (size_t)j + 1];
+        d12.kf = B.kf2; d12.Q = sim3_direction(B, B.pts1, B.T1w, B.S21, B.log_scale_factor2);
+        d21.kf = B.kf1; d21.Q = sim3_direction(B, B.pts2, B.T2w, B.S12, B.log_scale_factor1);
+        d12.kf.occupied = d21.kf.occupied = nullptr;               // vpMatches12 enters through pts*.valid (:1130-1155)
+        d12.I = frame_info(&d12.kf);
+        d21.I = frame_info(&d21.kf);
+        const int n1 = d21.I.n, n2 = d12.I.n;
+        if (B.pts1.n != n1 || B.pts2.n != n2) {
+            set_error("SearchBySim3: one MapPoint slot per keyframe feature (GetMapPointMatches)");
+            return job_fail(batch, j, BORB_ERR_INVALID_ARG);
+        }
+        borb_status s = check_query(&d12.kf, d12.I, d12.Q, m);
+        if (s == BORB_OK) s = check_query(&d21.kf, d21.I, d21.Q, m);
+        if (s != BORB_OK) return job_fail(batch, j, s);
+        std::fill_n(B.match12, n1, -1);
+        live[j] = n1 > 0 && n2 > 0;
+        if (live[j]) { max_nq = std::max(max_nq, std::max(n1, n2)); max_n1 = std::max(max_n1, n1); }
+    }
+    if (max_nq == 0) return BORB_OK;
+    const size_t nd = D.size();
+    Call c(m);
+    for (size_t k = 0; k < nd; k++)
+        if (live[k / 2]) D[k].o = stage_query(c, &D[k].kf, D[k].I, D[k].Q);
+    const size_t o_last = c.in(nullptr, nd * sizeof(LastArgs)), o_dirs = c.in(nullptr, nd * sizeof(FuseJob));
+    const size_t o_jobs = c.in(nullptr, (size_t)n_jobs * sizeof(Sim3AgreeJob));
+    const size_t o_sink = c.scratch(nd * 4);                   // fuse_batch_kernel's per-direction counts: the agreement test counts instead
+    const size_t r_cnt = c.result((size_t)n_jobs * 4);         // n_found of every job, then every job's match12
+    for (size_t k = 0; k < nd; k++) {
+        if (!live[k / 2]) continue;
+        reserve_projection(c, D[k].I, D[k].Q, D[k].o);
+        D[k].out = c.scratch((size_t)D[k].Q.n * 4);
+    }
+    for (int j = 0; j < n_jobs; j++)
+        if (live[j]) res[j] = c.result((size_t)jobs[j].pts1.n * 4);
+    borb_status s;
+    if ((s = c.begin()) != BORB_OK) return s;
+    LastArgs* hl = c.host<LastArgs>(o_last);
+    FuseJob* hd = c.host<FuseJob>(o_dirs);
+    Sim3AgreeJob* hj = c.host<Sim3AgreeJob>(o_jobs);
+    for (size_t k = 0; k < nd; k++) {
+        LastArgs L{};
+        FuseJob F{};
+        if (live[k / 2]) {
+            bind_frame_fields(D[k].I, D[k].o.fs, c, F.A);          // no u_right: stage_frame is asked for none without chi2
+            bind_query(D[k].o, D[k].Q, D[k].I, c, (int32_t*)c.dev(D[k].out), L, F.A);
+            F.n_found = (int*)c.dev(o_sink) + k;
+        }                                            // a job without work keeps n_last = n_mp = n1 = 0: every kernel skips it
+        hl[k] = L;
+        hd[k] = F;
+    }
+    for (int j = 0; j < n_jobs; j++) {
+        Sim3AgreeJob A{};
+        if (live[j]) {
+            A.match1 = (const int32_t*)c.dev(D[2 * (size_t)j].out); A.match2 = (const int32_t*)c.dev(D[2 * (size_t)j + 1].out);
+            A.n1 = jobs[j].pts1.n; A.n2 = jobs[j].pts2.n;
+            A.match12 = (int32_t*)c.res(res[j], false);
+            A.n_found = (int*)c.res(r_cnt, false) + j;
+        }
+        hj[j] = A;
+    }
+    if ((s = c.commit()) != BORB_OK) return s;
+    BORB_CUDA(cudaMemsetAsync(c.res(r_cnt, false), 0, (size_t)n_jobs * 4, m->stream));
+    for (size_t k = 0; k < nd; k++)
+        if (live[k / 2] && (s = prepare_frame(m, c, D[k].I, hd[k].A)) != BORB_OK) return s;
+    m->launches += launch_sim3_batch((const LastArgs*)c.dev(o_last), (const FuseJob*)c.dev(o_dirs), (const Sim3AgreeJob*)c.dev(o_jobs), n_jobs,
+                                     max_nq, max_n1, m->stream);
+    if ((s = c.finish()) != BORB_OK) return s;
+    for (int j = 0; j < n_jobs; j++) {
+        std::memcpy(&n_found[j], c.out(r_cnt) + (size_t)j * 4, 4);
+        if (live[j]) std::memcpy(jobs[j].match12, c.out(res[j]), (size_t)jobs[j].pts1.n * 4);
+    }
+    return BORB_OK;
+}
+}  // namespace
+
 borb_status borb_search_by_sim3(borb_matcher* m, const borb_frame_view* kf1, const borb_frame_view* kf2, const borb_worldpoints_view* pts1,
                                 const borb_worldpoints_view* pts2, const float* T1w, const float* T2w, const float* S12, const float* S21,
                                 float fx, float fy, float cx, float cy, float log_scale_factor1, float log_scale_factor2, float th,
                                 int32_t* match12, int32_t* n_found) {
     if (!m || !kf1 || !kf2 || !pts1 || !pts2 || !T1w || !T2w || !S12 || !S21 || !match12 || !n_found) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
-    *n_found = 0;
-    const int n1 = frame_info(kf1).n, n2 = frame_info(kf2).n;
-    if (pts1->n != n1 || pts2->n != n2) { set_error("SearchBySim3: one MapPoint slot per keyframe feature (GetMapPointMatches)"); return BORB_ERR_INVALID_ARG; }
-    for (int i = 0; i < n1; i++) match12[i] = -1;
-    if (n1 == 0 || n2 == 0) return BORB_OK;
-    borb_frame_view F1 = *kf1, F2 = *kf2;
-    F1.occupied = nullptr; F2.occupied = nullptr;
-    BORB_CUDA(cudaSetDevice(m->device));
-    const size_t need = (size_t)n1 + (size_t)n2;
-    if (m->aux_count < need) {
-        cudaFree(m->aux); m->aux = nullptr; m->aux_count = 0;
-        BORB_CUDA(cudaMalloc(&m->aux, need * 4));
-        m->aux_count = need;
+    borb_sim3_job B{};
+    B.kf1 = *kf1; B.kf2 = *kf2; B.pts1 = *pts1; B.pts2 = *pts2;
+    std::memcpy(B.T1w, T1w, sizeof(B.T1w)); std::memcpy(B.T2w, T2w, sizeof(B.T2w));
+    std::memcpy(B.S12, S12, sizeof(B.S12)); std::memcpy(B.S21, S21, sizeof(B.S21));
+    B.fx = fx; B.fy = fy; B.cx = cx; B.cy = cy; B.log_scale_factor1 = log_scale_factor1; B.log_scale_factor2 = log_scale_factor2; B.th = th;
+    B.match12 = match12;
+    return sim3_jobs(m, &B, 1, false, n_found);
+}
+
+borb_status borb_search_by_sim3_batch(borb_matcher* m, const borb_sim3_job* jobs, int n_jobs, int32_t* n_found) {
+    if (!m || n_jobs < 0 || (n_jobs > 0 && (!jobs || !n_found))) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+    for (int j = 0; j < n_jobs; j++) {
+        if (!jobs[j].kf1.resident || !jobs[j].kf2.resident) {
+            set_error("job %d: borb_search_by_sim3_batch needs device-resident keyframes (borb_frame_view::resident)", j);
+            return BORB_ERR_INVALID_ARG;
+        }
+        if (!jobs[j].match12) { set_error("job %d: null output", j); return BORB_ERR_INVALID_ARG; }
     }
-    int32_t nm = 0;
-    // KF1's points into KF2 (:1146-1222) and KF2's points into KF1 (:1224-1300); both results stay on the device
-    PointQuery Q{};
-    Q.variant = 2; Q.n = pts1->n; Q.world_pos = pts1->world_pos; Q.desc = pts1->desc; Q.valid = pts1->valid;
-    Q.max_distance = pts1->max_distance; Q.min_distance = pts1->min_distance;
-    Q.Tcw = T1w; Q.chain = 1; Q.T2 = S21; Q.fx = fx; Q.fy = fy; Q.cx = cx; Q.cy = cy; Q.th = th; Q.log_scale = log_scale_factor2;
-    Q.th_dist = 100; Q.argmin = 1; Q.invz_double = 1; Q.to_aux = 1; Q.aux_off = 0;        // TH_HIGH (:1218)
-    const PointJob P{&F2, Q, nullptr};
-    borb_status s = point_query_jobs(m, &P, 1, &nm, false);
-    if (s != BORB_OK) return s;
-    PointQuery R{};
-    R.variant = 2; R.n = pts2->n; R.world_pos = pts2->world_pos; R.desc = pts2->desc; R.valid = pts2->valid;
-    R.max_distance = pts2->max_distance; R.min_distance = pts2->min_distance;
-    R.Tcw = T2w; R.chain = 1; R.T2 = S12; R.fx = fx; R.fy = fy; R.cx = cx; R.cy = cy; R.th = th; R.log_scale = log_scale_factor1;
-    R.th_dist = 100; R.argmin = 1; R.invz_double = 1; R.to_aux = 1; R.aux_off = (size_t)n1;
-    const PointJob PR{&F1, R, nullptr};
-    s = point_query_jobs(m, &PR, 1, &nm, false);
-    if (s != BORB_OK) return s;
-    // agreement test (:1302-1323) on the device
-    Call c(m);
-    const size_t r_out = c.result((size_t)n1 * 4), r_nf = c.result(4);
-    if ((s = c.begin()) != BORB_OK) return s;
-    m->launches += launch_sim3_agree(m->aux, m->aux + n1, n1, n2, (int32_t*)c.res(r_out, false), (int*)c.res(r_nf, false), m->stream);
-    if ((s = c.finish()) != BORB_OK) return s;
-    std::memcpy(match12, c.out(r_out), (size_t)n1 * 4);
-    std::memcpy(n_found, c.out(r_nf), 4);
-    return BORB_OK;
+    return sim3_jobs(m, jobs, n_jobs, true, n_found);
 }
 
 // ---- Tracking::SearchLocalPoints: one camera stream of borb_search_local_points or of borb_search_local_points_batch

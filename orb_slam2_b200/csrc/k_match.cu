@@ -325,38 +325,6 @@ __global__ void __launch_bounds__(32) init_resolve_kernel(ProjArgs A, const borb
     if (lane == 0) *n_matches = nm;
 }
 
-// Order-independent overloads (Fuse x2, the two directions of SearchBySim3): a warp per query point takes the
-// first minimum of its candidate list (dist < bestDist scan == lexicographic min of (distance, list position)).
-// out_match: the feature per query, then the count
-__global__ void __launch_bounds__(256) proj_argmin_kernel(ProjArgs A) {
-    int32_t* __restrict__ best_idx = A.out_match;
-    int* __restrict__ n_found = reinterpret_cast<int*>(A.out_match + A.n_mp);
-    const int lane = threadIdx.x & 31;
-    const int iq = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    if (iq >= A.n_mp) return;
-    const int cnt = A.cand_cnt[iq] & CAND_COUNT_MASK;
-    const uint32_t* c = A.cand + (size_t)iq * A.n;
-    unsigned k1 = 0xFFFFFFFFu;
-    for (int p = lane; p < cnt; p += 32) k1 = min(k1, (((c[p] >> 16) & 0x1FFu) << 16) | (unsigned)p);
-    const unsigned best = warp_min(k1);
-    if (lane == 0) {
-        int out = -1;
-        if (best != 0xFFFFFFFFu && (int)(best >> 16) <= A.th_dist) { out = (int)(c[best & 0xFFFFu] & 0xFFFF); atomicAdd(n_found, 1); }
-        best_idx[iq] = out;
-    }
-}
-
-// SearchBySim3 agreement (:1302-1323): keep i1 -> idx2 only if the reverse search sent idx2 back to i1
-__global__ void __launch_bounds__(256) sim3_agree_kernel(const int32_t* __restrict__ match1, const int32_t* __restrict__ match2, int n1,
-                                                         int n2, int32_t* __restrict__ match12, int* __restrict__ n_found) {
-    const int i1 = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i1 >= n1) return;
-    const int idx2 = match1[i1];
-    int out = -1;
-    if (idx2 >= 0 && idx2 < n2 && match2[idx2] == i1) { out = idx2; atomicAdd(n_found, 1); }
-    match12[i1] = out;
-}
-
 // MapPoint::ComputeDistinctiveDescriptors (src/MapPoint.cc:242-307), batched: a warp per MapPoint, a lane per row of the
 // distance matrix.  The row median (sorted row[(int)(0.5*(N-1))], self-distance included) comes from a 257-bin counting
 // histogram kept in local memory; first minimal median wins (lowest row index).
@@ -927,20 +895,6 @@ int launch_point_projection_batch(const LastArgs* d_last, const ProjArgs* d_jobs
     if (n_jobs == 1) project_points_kernel<<<(one_last.n_last + 255) / 256, 256, 0, s>>>(one_last);
     else project_points_batch_kernel<<<dim3((max_nq + 255) / 256, n_jobs), 256, 0, s>>>(d_last);
     return 1 + launch_projection_batch(d_jobs, one, n_jobs, max_n, max_n_mp, s, last);
-}
-int launch_projection_argmin(const LastArgs& L, const ProjArgs& A, cudaStream_t s) {
-    cudaMemsetAsync(A.out_match + A.n_mp, 0, sizeof(int), s);
-    if (A.n_mp > 0) {
-        project_points_kernel<<<(L.n_last + 255) / 256, 256, 0, s>>>(L);
-        launch_candidates(A, s);
-        proj_argmin_kernel<<<(A.n_mp + 7) / 8, 256, 0, s>>>(A);
-    }
-    return 3;
-}
-int launch_sim3_agree(const int32_t* match1, const int32_t* match2, int n1, int n2, int32_t* match12, int* n_found, cudaStream_t s) {
-    cudaMemsetAsync(n_found, 0, sizeof(int), s);
-    if (n1 > 0) sim3_agree_kernel<<<(n1 + 255) / 256, 256, 0, s>>>(match1, match2, n1, n2, match12, n_found);
-    return 1;
 }
 int launch_bow_match(const KfDev* qs, const KfDev* ts, int n_pairs, int mode, float nnratio, int check_ori, int32_t* match,
                      const size_t* out_off, uint8_t* bins, int32_t* n_matches, int max_t, cudaStream_t s) {

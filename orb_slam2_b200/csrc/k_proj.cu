@@ -1,6 +1,6 @@
 // Windowed projection search shared by every ORBmatcher::SearchByProjection overload, Fuse and SearchBySim3
 // (reference src/ORBmatcher.cc:45-129, 290-403, 825-1100, 1102-1326, 1328-1599) — candidate enumeration and the
-// order-dependent claim resolution; fuse_batch_kernel (below) is the list-free search of both Fuse overloads.
+// order-dependent claim resolution; fuse_batch_kernel (below) is the list-free search of both Fuse overloads and SearchBySim3.
 //
 //   proj_candidates_kernel   Frame::GetFeaturesInArea (src/Frame.cc:327-380) + the per-candidate gates + DescriptorDistance,
 //       a warp per query.  Lanes take different GRID CELLS of the query window (a cell holds ~0.3 features, so a lane per
@@ -20,6 +20,8 @@
 //       LAST = false: best / second-best + ratio test (:98-121), out[query] = feature.
 //       LAST = true : best only, threshold th_dist, out[feature] = query, match events for the rotation histogram (:1426-1466).
 //   init_prefix_kernel / init_replay_kernel   SearchForInitialization (:405-520) of many frame pairs on resident frames (below).
+//   fuse_batch_kernel / sim3_agree_batch_kernel   the order-independent searches, Fuse x2 and both directions of SearchBySim3, with
+//       no candidate list; the agreement test of SearchBySim3 (below).
 // All float tests use _rn intrinsics (no FMA contraction) so comparisons match the reference bit for bit.
 #include "borb_match.h"
 
@@ -247,6 +249,31 @@ __global__ void __launch_bounds__(256) fuse_batch_kernel(const FuseJob* __restri
 
 void launch_fuse_search(const FuseJob* d_jobs, int n_jobs, int max_nq, cudaStream_t s) {
     fuse_batch_kernel<<<dim3((max_nq + 7) / 8, n_jobs), 256, 0, s>>>(d_jobs);
+}
+
+// SearchBySim3 (:1102-1326) runs its two directions as direction jobs of fuse_batch_kernel (inv_sigma2 null, u_right null,
+// th_dist = TH_HIGH), then this agreement test (:1308-1323) for a table of jobs, a thread per KF1 feature on grid (n1 / 256, jobs):
+// i1 keeps idx2 only if the reverse search sent idx2 back to i1.  Each direction is bit-identical to the reference's scan: with the
+// chi2 gates off, fuse_batch_kernel applies exactly the gates of proj_candidates_kernel (area_window, then area_passes without a
+// stereo test: the SearchBySim3 directions stage no u_right) and keeps min((dist << 16) | e) over ascending positions e of
+// cell_idx, which is the (ix, iy, insertion) order of GetFeaturesInArea; so it takes the same first minimum (`dist < bestDist`,
+// :1214, :1294) as a scan of the candidate list in list order, with no list.
+__global__ void __launch_bounds__(256) sim3_agree_batch_kernel(const Sim3AgreeJob* __restrict__ jobs) {
+    const Sim3AgreeJob& J = jobs[blockIdx.y];
+    const int i1 = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i1 >= J.n1) return;
+    const int idx2 = J.match1[i1];
+    int out = -1;
+    if (idx2 >= 0 && idx2 < J.n2 && J.match2[idx2] == i1) { out = idx2; atomicAdd(J.n_found, 1); }
+    J.match12[i1] = out;
+}
+
+int launch_sim3_batch(const LastArgs* d_last, const FuseJob* d_dirs, const Sim3AgreeJob* d_jobs, int n_jobs, int max_nq, int max_n1,
+                      cudaStream_t s) {
+    if (n_jobs <= 0 || max_nq <= 0) return 0;
+    const int n = launch_fuse_batch(d_last, d_dirs, 2 * n_jobs, max_nq, s);
+    sim3_agree_batch_kernel<<<dim3((max_n1 + 255) / 256, n_jobs), 256, 0, s>>>(d_jobs);
+    return n + 1;
 }
 
 size_t resolve_smem_bytes(int n, int n_mp) {

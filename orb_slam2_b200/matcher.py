@@ -96,6 +96,25 @@ class _InitJobC(C.Structure):                      # borb_init_job
                 ("matches12", C.c_void_p)]
 
 
+class _KfProjectionJobC(C.Structure):             # borb_kf_projection_job
+    _fields_ = [("cur", _FrameViewC), ("pts", _WorldPointsViewC), ("Tcw", C.c_float * 12), ("Ow", C.c_float * 3)] + \
+               [(n, C.c_float) for n in ("fx", "fy", "cx", "cy", "log_scale_factor", "th")] + \
+               [("orb_dist", C.c_int32), ("state_cur", C.c_void_p)]
+
+
+class _Sim3ProjectionJobC(C.Structure):           # borb_sim3_projection_job
+    _fields_ = [("kf", _FrameViewC), ("pts", _WorldPointsViewC), ("Tcw", C.c_float * 12), ("Ow", C.c_float * 3)] + \
+               [(n, C.c_float) for n in ("fx", "fy", "cx", "cy", "log_scale_factor")] + \
+               [("th", C.c_int32), ("state_kf", C.c_void_p)]
+
+
+class _Sim3JobC(C.Structure):                      # borb_sim3_job
+    _fields_ = [("kf1", _FrameViewC), ("kf2", _FrameViewC), ("pts1", _WorldPointsViewC), ("pts2", _WorldPointsViewC)] + \
+               [(n, C.c_float * 12) for n in ("T1w", "T2w", "S12", "S21")] + \
+               [(n, C.c_float) for n in ("fx", "fy", "cx", "cy", "log_scale_factor1", "log_scale_factor2", "th")] + \
+               [("match12", C.c_void_p)]
+
+
 def _p(a):
     return a.ctypes.data if a is not None else None
 
@@ -107,6 +126,10 @@ def _per_job(x, n, ndim=0):
 
 def _pose12(Tcw):
     return (C.c_float * 12)(*np.asarray(Tcw, np.float32)[:3, :4].reshape(12).tolist())
+
+
+def _vec3(Ow):
+    return (C.c_float * 3)(*np.asarray(Ow, np.float32).reshape(3).tolist())
 
 
 def _c_arrays(*pairs):
@@ -542,6 +565,76 @@ class ORBmatcher:
         check(self._lib.borb_search_by_projection_last_batch(self._h, jobs, n, int(self.mbCheckOrientation), _p(nm)),
               "borb_search_by_projection_last_batch")
         return [(int(nm[j]), state[:n_cur]) for j, (n_cur, state) in enumerate(outs)]
+
+    def SearchByProjectionKFBatch(self, curs: Sequence[FrameView], points: Sequence[WorldPointsView], poses, K, th, ORBdist):
+        """borb_search_by_projection_kf_batch: SearchByProjection(CurrentFrame, pKF, sAlreadyFound, th, ORBdist) of many relocalising
+        camera streams (device-resident current frames) in one launch sequence.  poses[j] = (Tcw, Ow); K, th and ORBdist are one
+        value for every job or one per job.  Returns [(nmatches, state)] per job, equal to what SearchByProjectionKF returns."""
+        n = len(curs)
+        assert n == len(points) == len(poses)
+        Ks, ths, ods = _per_job(K, n, 1), _per_job(th, n), _per_job(ORBdist, n)
+        jobs = (_KfProjectionJobC * max(n, 1))()
+        keep, outs = [], []
+        for j in range(n):
+            fv, pv, logs, n_cur, k = self._points_call(curs[j], points[j])
+            state = np.full(max(n_cur, 1), -1, np.int32)
+            Tcw, Ow = poses[j]
+            J = jobs[j]
+            J.cur, J.pts, J.Tcw, J.Ow = fv, pv, _pose12(Tcw), _vec3(Ow)
+            J.fx, J.fy, J.cx, J.cy = [float(x) for x in Ks[j]]
+            J.log_scale_factor, J.th, J.orb_dist, J.state_cur = logs, float(ths[j]), int(ods[j]), _p(state)
+            keep.append(k); outs.append((n_cur, state))
+        nm = np.zeros(max(n, 1), np.int32)
+        check(self._lib.borb_search_by_projection_kf_batch(self._h, jobs, n, int(self.mbCheckOrientation), _p(nm)),
+              "borb_search_by_projection_kf_batch")
+        return [(int(nm[j]), state[:n_cur]) for j, (n_cur, state) in enumerate(outs)]
+
+    def SearchByProjectionSim3Batch(self, kfs: Sequence[FrameView], points: Sequence[WorldPointsView], poses, K, th=10):
+        """borb_search_by_projection_sim3_batch: SearchByProjection(pKF, Scw, vpPoints, vpMatched, th) of many loop-closing streams
+        (device-resident keyframes) in one launch sequence.  poses[j] = (Tcw, Ow) with the Sim3 scale divided out; K and th are one
+        value for every job or one per job.  Returns [(nmatches, state)] per job, equal to what SearchByProjectionSim3 returns."""
+        n = len(kfs)
+        assert n == len(points) == len(poses)
+        Ks, ths = _per_job(K, n, 1), _per_job(th, n)
+        jobs = (_Sim3ProjectionJobC * max(n, 1))()
+        keep, outs = [], []
+        for j in range(n):
+            fv, pv, logs, n_kf, k = self._points_call(kfs[j], points[j])
+            state = np.full(max(n_kf, 1), -1, np.int32)
+            Tcw, Ow = poses[j]
+            J = jobs[j]
+            J.kf, J.pts, J.Tcw, J.Ow = fv, pv, _pose12(Tcw), _vec3(Ow)
+            J.fx, J.fy, J.cx, J.cy = [float(x) for x in Ks[j]]
+            J.log_scale_factor, J.th, J.state_kf = logs, int(ths[j]), _p(state)
+            keep.append(k); outs.append((n_kf, state))
+        nm = np.zeros(max(n, 1), np.int32)
+        check(self._lib.borb_search_by_projection_sim3_batch(self._h, jobs, n, _p(nm)), "borb_search_by_projection_sim3_batch")
+        return [(int(nm[j]), state[:n_kf]) for j, (n_kf, state) in enumerate(outs)]
+
+    def SearchBySim3Batch(self, kf1s: Sequence[FrameView], kf2s: Sequence[FrameView], P1s: Sequence[WorldPointsView],
+                          P2s: Sequence[WorldPointsView], poses, sims, K, th=7.5):
+        """borb_search_by_sim3_batch: SearchBySim3(pKF1, pKF2, vpMatches12, s12, R12, t12, th) of many (keyframe, candidate) pairs on
+        device-resident keyframes in three launches.  poses[j] = (T1w, T2w), sims[j] = (S12, S21) as for SearchBySim3; K (pKF1's)
+        and th are one value for every job or one per job.  Returns [(nFound, match12)] per job, equal to what SearchBySim3 returns."""
+        n = len(kf1s)
+        assert n == len(kf2s) == len(P1s) == len(P2s) == len(poses) == len(sims)
+        Ks, ths = _per_job(K, n, 1), _per_job(th, n)
+        jobs = (_Sim3JobC * max(n, 1))()
+        keep, outs = [], []
+        for j in range(n):
+            fv1, pv1, logs1, n1, k1 = self._points_call(kf1s[j], P1s[j])
+            fv2, pv2, logs2, _, k2 = self._points_call(kf2s[j], P2s[j])
+            match = np.full(max(n1, 1), -1, np.int32)
+            J = jobs[j]
+            J.kf1, J.kf2, J.pts1, J.pts2 = fv1, fv2, pv1, pv2
+            J.T1w, J.T2w = _pose12(poses[j][0]), _pose12(poses[j][1])
+            J.S12, J.S21 = _pose12(sims[j][0]), _pose12(sims[j][1])
+            J.fx, J.fy, J.cx, J.cy = [float(x) for x in Ks[j]]
+            J.log_scale_factor1, J.log_scale_factor2, J.th, J.match12 = logs1, logs2, float(ths[j]), _p(match)
+            keep.append((k1, k2)); outs.append((n1, match))
+        nf = np.zeros(max(n, 1), np.int32)
+        check(self._lib.borb_search_by_sim3_batch(self._h, jobs, n, _p(nf)), "borb_search_by_sim3_batch")
+        return [(int(nf[j]), match[:n1]) for j, (n1, match) in enumerate(outs)]
 
     def SearchForInitialization(self, F1: FrameView, F2: FrameView, vbPrevMatched: np.ndarray, windowSize: int = 10):
         """SearchForInitialization(F1, F2, vbPrevMatched, vnMatches12, windowSize) — src/ORBmatcher.cc:405-520.

@@ -112,6 +112,15 @@ FB = M.FrameView(kb, rng.integers(0, 256, (6000, 32), dtype=np.uint8), X.GetScal
 mt.ComputeBoWBatch(voc6, [FR0, FB], 2, want_host=False)
 print("kfdb query batch", [q[0][:3] for q in mt.KfdbQueryBatch([db2, db3], [FR0, FB])])
 print("bowdb batch", [int(r[0].sum()) for r in mt.SearchByBoWDbBatch([db2, db3, db2], [None, None, [0, 5, 5]], [FR0, FB, FB])])
+K_S, I34, Z3 = (525.0, 525.0, 319.5, 239.5), np.eye(4, dtype=np.float32)[:3], np.zeros(3, np.float32)
+def _slots(F, z=5.0):                                                   # one MapPoint per feature, back-projected at depth z
+    k = F.mvKeysUn
+    Pw = np.stack([(k["x"] - K_S[2]) * z / K_S[0], (k["y"] - K_S[3]) * z / K_S[1], np.full(len(k), z)], 1).astype(np.float32)
+    d = np.linalg.norm(Pw, axis=1).astype(np.float32)
+    return M.WorldPointsView(Pw, F.mDescriptors, (d * np.float32(1.2) ** k["octave"]).astype(np.float32), np.full(len(k), 0.1, np.float32),
+                             (Pw / d[:, None]).astype(np.float32), k["angle"].astype(np.float32))
+Pr0, PrB = _slots(FR0), _slots(FB)
+print("pose search batches", mt.SearchBySim3Batch([FR0, FR0], [FR0, FB], [Pr0, Pr0], [Pr0, PrB], [(I34, I34)] * 2, [(I34, I34)] * 2, K_S, 7.5)[0][0], mt.SearchByProjectionKFBatch([FR0, FB], [Pr0, Pr0], [(I34, Z3)] * 2, K_S, 10.0, 100)[0][0], mt.SearchByProjectionSim3Batch([FR0, FB], [PrB, Pr0], [(I34, Z3)] * 2, K_S, 10)[0][0])
 print("init batch", [r[0] for r in mt.SearchForInitializationBatch([FR0, FR0, FB], [FR0, FB, FR0], [np.stack([outs[0][0]["x"], outs[0][0]["y"]], 1)] * 2 + [np.stack([kb["x"], kb["y"]], 1)], [100, 100, 30])])
 
 # place-recognition envelope (tests/bow_envelope.py): the flat 70,000-word vocabulary, the 8192 x 8192 one-node database search,
