@@ -824,6 +824,12 @@ BORB_API borb_status borb_debug_set_fast_mode(borb_extractor* e, int mode);
  * entry = (x + 128) | (y + 128) << 8 | point << 16 for pattern point `point` (= 2 * test + 0/1) at (x, y); the first
  * min(cap, 512 * *n_bins) entries go to dst (may be NULL). */
 BORB_API borb_status borb_debug_brief_slots(uint32_t* dst, int cap, int* n_bins);
+/* Evaluates a device maths function on n host inputs (tests only): fn 0 sinf(a), 1 cosf(a), 2 fastAtan2(a = y, b = x) in degrees,
+ * 3 logf(a), 4 PredictScale(a = max_distance, b = dist, log_scale, n_levels) -> int32.  out: n floats (int32 for fn 4).
+ * These are the functions the descriptor kernel (0-2) and the projection searches (3-4) inline, compiled with them.  sinf/cosf
+ * are defined for 0 <= a < 120 and logf for positive normal a (the inputs those kernels form).  Runs on the current device
+ * on a stream of its own and returns when out is written; b may be NULL for fn 0, 1 and 3. */
+BORB_API borb_status borb_debug_eval_math(int fn, const float* a, const float* b, int n, float log_scale, int n_levels, void* out);
 /* Distance arithmetic of the database SearchByBoW kernel: 2 (default) = three 3:2 compressors + 5 POPC per 256-bit distance,
  * 1 = full carry-save adder tree + 4 POPC, 0 = 8 POPC.  Same results; kept switchable for measurements.  Applies to the
  * relocalisation search (borb_search_by_bow_db*); the loop-closure search (borb_search_by_bow_kf_db_*) always uses mode 2. */

@@ -1037,6 +1037,37 @@ def port_predict_scale(max_distance, dist, log_scale, n_levels):
     return out[:len(mx)]
 
 
+LIBM_SINF, LIBM_COSF, LIBM_LOGF = 0, 1, 2
+
+
+def port_libm(fn, x):
+    """The host libm on float32 inputs (fn LIBM_SINF / LIBM_COSF / LIBM_LOGF), a few threads (orbport_libm)."""
+    lib = _plib()
+    x = _a(x, np.float32)
+    out = np.empty(len(x), np.float32)
+    lib.orbport_libm.restype = None
+    lib.orbport_libm.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int64]
+    lib.orbport_libm(int(fn), _ptr(x), _ptr(out), len(x))
+    return out
+
+
+def port_fast_atan2(y, x):
+    """cv::fastAtan2(y, x) in degrees, element-wise (orbport_fast_atan2, pinned to cv2).  Slices run on a few threads (ctypes
+    releases the GIL): tiny ratios make subnormal products, which are slow on x86."""
+    from concurrent.futures import ThreadPoolExecutor
+    lib = _plib()
+    y = _a(y, np.float32); x = _a(x, np.float32)
+    out = np.empty(len(y), np.float32)
+    lib.orbport_fast_atan2.restype = None
+    lib.orbport_fast_atan2.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
+    cuts = np.linspace(0, len(y), min(16, os.cpu_count() or 1) + 1).astype(np.int64)
+    with ThreadPoolExecutor(len(cuts) - 1) as pool:
+        for _ in pool.map(lambda s: lib.orbport_fast_atan2(_ptr(y[s]), _ptr(x[s]), _ptr(out[s]), len(out[s])),
+                          [slice(a, b) for a, b in zip(cuts[:-1], cuts[1:])]):
+            pass
+    return out
+
+
 def ref_distance_invariance(max_distance, min_distance):
     lib = C.CDLL(MAPREF_SO)
     mx = _a(max_distance, np.float32); mn = _a(min_distance, np.float32)

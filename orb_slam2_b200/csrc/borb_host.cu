@@ -840,6 +840,35 @@ borb_status borb_debug_brief_slots(uint32_t* dst, int cap, int* n_bins) {
     return BORB_OK;
 }
 
+borb_status borb_debug_eval_math(int fn, const float* a, const float* b, int n, float log_scale, int n_levels, void* out) {
+    if (fn < 0 || fn > 4) { set_error("eval_math: no function %d (0..4)", fn); return BORB_ERR_INVALID_ARG; }
+    if (n < 0) { set_error("eval_math: n = %d", n); return BORB_ERR_INVALID_ARG; }
+    const bool binary = fn == 2 || fn == 4;
+    if (!a || !out || (binary && !b)) { set_error("eval_math: NULL input or output"); return BORB_ERR_INVALID_ARG; }
+    if (n == 0) return BORB_OK;
+    struct Buffers {         // released on every return, after the frees have waited for the stream's work
+        cudaStream_t s = nullptr;
+        float *a = nullptr, *b = nullptr;
+        void* out = nullptr;
+        ~Buffers() { cudaFree(a); cudaFree(b); cudaFree(out); if (s) cudaStreamDestroy(s); }
+    } d;
+    const size_t bytes = (size_t)n * sizeof(float);
+    BORB_CUDA(cudaStreamCreateWithFlags(&d.s, cudaStreamNonBlocking));
+    BORB_CUDA(cudaMalloc(&d.a, bytes));
+    BORB_CUDA(cudaMalloc(&d.out, bytes));
+    BORB_CUDA(cudaMemcpyAsync(d.a, a, bytes, cudaMemcpyHostToDevice, d.s));
+    if (binary) {
+        BORB_CUDA(cudaMalloc(&d.b, bytes));
+        BORB_CUDA(cudaMemcpyAsync(d.b, b, bytes, cudaMemcpyHostToDevice, d.s));
+    }
+    if (fn <= 2) launch_describe_math_probe(fn, d.a, d.b, n, static_cast<float*>(d.out), d.s);
+    else launch_match_math_probe(fn, d.a, d.b, n, log_scale, n_levels, d.out, d.s);
+    BORB_CUDA(cudaGetLastError());
+    BORB_CUDA(cudaMemcpyAsync(out, d.out, bytes, cudaMemcpyDeviceToHost, d.s));
+    BORB_CUDA(cudaStreamSynchronize(d.s));
+    return BORB_OK;
+}
+
 borb_status borb_launch_count(const borb_extractor* e, uint64_t* n) {
     if (!e || !n) return BORB_ERR_INVALID_ARG;
     *n = e->launches;

@@ -144,6 +144,11 @@ int launch_fast(const Geometry& g, const Workspace& ws, int n_images, cudaStream
 int launch_quadtree(const Geometry& g, const Workspace& ws, int n_images, cudaStream_t s);
 int launch_blur(const Geometry& g, const Workspace& ws, int n_images, cudaStream_t s);
 int launch_describe(const Geometry& g, const Workspace& ws, int n_images, cudaStream_t s);
+// borb_debug_eval_math probes (device pointers): fn 0-2 run k_describe.cu's sinf / cosf / fastAtan2, fn 3-4 k_match.cu's logf /
+// PredictScale (out is int32 for fn 4)
+int launch_describe_math_probe(int fn, const float* a, const float* b, int n, float* out, cudaStream_t s);
+int launch_match_math_probe(int fn, const float* a, const float* b, int n, float log_scale, int n_levels, void* out,
+                            cudaStream_t s);
 
 struct StereoView {          // device pointers of one side of a stereo pair set
     const uint8_t* pyr;      // pyramid base (image 0)

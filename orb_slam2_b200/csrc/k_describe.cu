@@ -8,8 +8,9 @@
 //       BLURRED level; bit k of byte i = tap(16i+2k... ) i.e. test t -> byte t/8, bit t%8;
 //   operator() tail (:1059-1104) — levels concatenated 0..n-1, pt *= mvScaleFactor[level], size, octave.
 // sinf/cosf: device port (double arithmetic) of the glibc >= 2.28 single-precision kernels the
-// reference binary calls on x86-64 (ARM optimized-routines sincosf); checked exhaustively on the CPU
-// against glibc for every float in [0, 2*pi] (DESIGN.md).  The 512 taps are fetched in the order of the keypoint's
+// reference binary calls on x86-64 (ARM optimized-routines sincosf); the device function itself is compared with glibc
+// for every float in [0, 2*pi], and fastAtan2 over its whole domain, through describe_math_probe_kernel
+// (tests/test_gpu_device_math.py, DESIGN.md).  The 512 taps are fetched in the order of the keypoint's
 // orientation bin (brief_slot_table, borb_internal.h): one gather instruction then touches a few adjacent rows of the
 // patch (~4 128-byte lines) instead of points spread over the whole 37 x 37 window (~20 lines).  Each tap byte goes to
 // its canonical place 2*test + which in the warp's 512 B of shared memory; lane t%32 then reads test t's two bytes as one
@@ -187,6 +188,19 @@ __global__ void __launch_bounds__(256, 8) describe_kernel(const __grid_constant_
 int launch_describe(const Geometry& g, const Workspace& ws, int n_images, cudaStream_t s) {
     dim3 grid((g.sel_image_stride + 7) / 8, n_images);
     describe_kernel<<<grid, 256, 0, s>>>(g, ws.pyr, ws.blur, ws.brief_slots, ws.sel, ws.sel_cnt, ws.kps, ws.desc, ws.nkp);
+    return 1;
+}
+
+// Test probe (borb_debug_eval_math fn 0-2): the very glibc_sincosf / fast_atan2_deg that describe_kernel inlines, compiled in
+// this translation unit with its flags, on arbitrary inputs.  fn 0 sinf(a), 1 cosf(a), 2 fastAtan2(y = a, x = b).
+__global__ void describe_math_probe_kernel(int fn, const float* __restrict__ a, const float* __restrict__ b, int n,
+                                           float* __restrict__ out) {
+    for (long long i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+        out[i] = fn == 2 ? fast_atan2_deg(a[i], b[i]) : glibc_sincosf(a[i], fn);
+}
+
+int launch_describe_math_probe(int fn, const float* a, const float* b, int n, float* out, cudaStream_t s) {
+    describe_math_probe_kernel<<<std::min((n + 255) / 256, 8192), 256, 0, s>>>(fn, a, b, n, out);
     return 1;
 }
 

@@ -15,6 +15,8 @@
 //       a warp per descriptor descends the tree, lanes = children, first-wins argmin (bow_transform_batch_kernel: the same
 //       descent for many resident frames, grid.y = frame).
 //   bow_build_kernel      the BowVector / FeatureVector bookkeeping of transform (:1150-1194) on the device, a CTA per frame.
+//   match_math_probe_kernel  tests only (borb_debug_eval_math): glibc_logf and predict_scale on given inputs, swept over every
+//       input against glibc and MapPoint::PredictScale by tests/test_gpu_device_math.py.
 // All float tests use _rn intrinsics (no FMA contraction) so comparisons match the reference bit for bit.
 //
 // Bound: latency / POPC issue (15 thread-ops/clk/SM measured); the batch (map points, keyframes) supplies parallelism.
@@ -106,8 +108,9 @@ __global__ void __launch_bounds__(1024) grid_sort_kernel(const borb_keypoint* __
 // (candidate enumeration and claim resolution: k_proj.cu)
 
 // glibc (>= 2.28) logf for positive normal finite x — the function MapPoint::PredictScale calls (src/MapPoint.cc:393,410;
-// `log` resolves to the float overload).  ARM optimized-routines algorithm in double; checked on the CPU against glibc for
-// every positive normal float, with and without FMA contraction: 0 mismatches (DESIGN.md).
+// `log` resolves to the float overload).  ARM optimized-routines algorithm in double; the device function itself is compared
+// with glibc for every positive normal float, and predict_scale for every float ratio, through match_math_probe_kernel
+// (tests/test_gpu_device_math.py, DESIGN.md).
 struct LogfTab { double invc[16], logc[16]; double ln2, a0, a1, a2; };
 __device__ const LogfTab d_logf = {
     {0x1.661ec79f8f3bep+0, 0x1.571ed4aaf883dp+0, 0x1.49539f0f010bp+0, 0x1.3c995b0b80385p+0, 0x1.30d190c8864a5p+0, 0x1.25e227b0b8eap+0,
@@ -147,6 +150,23 @@ __device__ __forceinline__ int predict_scale(float max_distance, float dist, flo
     if (nScale < 0) nScale = 0;
     else if (nScale >= n_levels) nScale = n_levels - 1;
     return nScale;
+}
+
+// Test probe (borb_debug_eval_math fn 3-4): the very glibc_logf / predict_scale that project_points_kernel inlines, compiled in
+// this translation unit with its flags.  fn 3 logf(a) (defined for positive normal a); fn 4 PredictScale(max_distance = a,
+// dist = b, log_scale, n_levels) as int32.
+__global__ void match_math_probe_kernel(int fn, const float* __restrict__ a, const float* __restrict__ b, int n, float log_scale,
+                                        int n_levels, void* __restrict__ out) {
+    for (long long i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        if (fn == 3) static_cast<float*>(out)[i] = glibc_logf(a[i]);
+        else static_cast<int*>(out)[i] = predict_scale(a[i], b[i], log_scale, n_levels);
+    }
+}
+
+int launch_match_math_probe(int fn, const float* a, const float* b, int n, float log_scale, int n_levels, void* out,
+                            cudaStream_t s) {
+    match_math_probe_kernel<<<std::min((n + 255) / 256, 8192), 256, 0, s>>>(fn, a, b, n, log_scale, n_levels, out);
+    return 1;
 }
 
 // Projection of query point i with the 3x4 pose, for the three SearchByProjection overloads that take world points and for
