@@ -37,8 +37,9 @@ struct borb_voc {
     size_t bytes = 0;
     VocDev dev;
     cudaStream_t stream = nullptr;
+    std::mutex mu;                  // borb_bow_transform holds it for the whole call: the scratch and the stream are shared by every caller
     uint8_t* scratch = nullptr;     // pinned HOST buffer of borb_bow_transform: descriptors in, (weight, word, node) out - the kernel reads
-    size_t scratch_bytes = 0;       // and writes it in place (UVA), so a call is one launch and one synchronize.  One caller at a time per handle.
+    size_t scratch_bytes = 0;       // and writes it in place (UVA), so a call is one launch and one synchronize
 };
 
 namespace {
@@ -2349,6 +2350,9 @@ extern "C" void borb_voc_adopt_ownership(borb_voc* v) { if (v) v->owns = true; }
 borb_status borb_bow_transform(borb_voc* v, const uint8_t* desc, int n, int levelsup, int32_t* word, double* weight, int32_t* node) {
     if (!v || n < 0 || (n > 0 && (!desc || !word || !weight || !node))) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
     if (n == 0) return BORB_OK;
+    // Tracking (Frame::ComputeBoW) and LocalMapping (KeyFrame::ComputeBoW) transform on one vocabulary, as DBoW2's const transform
+    // allows: one call at a time owns the scratch, from the grow to the copy out
+    std::lock_guard<std::mutex> lk(v->mu);
     BORB_CUDA(cudaSetDevice(v->device));
     const size_t need = (size_t)n * (32 + 4 + 8 + 4) + 1024;
     if (v->scratch_bytes < need) {
@@ -2417,7 +2421,8 @@ borb_status borb_compute_bow(borb_voc* v, const uint8_t* desc, int n, int levels
 }
 
 // Frame::ComputeBoW for many resident frames: borb_compute_bow's descent and bookkeeping both on the device (bow_transform_batch_kernel,
-// bow_build_kernel), two launches and one synchronisation; the vectors stay with the frames for borb_search_by_bow_batch.
+// bow_build_kernel), two launches and one synchronisation; the vectors stay with the frames for borb_search_by_bow_batch.  Of the
+// vocabulary it reads only the immutable blob (v->dev), on the matcher's stream, so it takes no vocabulary lock.
 borb_status borb_frames_compute_bow(borb_matcher* m, borb_voc* v, borb_frame* const* frames, int n_frames, int levelsup,
                                     uint32_t* const* bow_word, double* const* bow_value, int32_t* n_bow, uint32_t* const* fv_node,
                                     int32_t* const* fv_start, uint32_t* const* fv_idx, int32_t* n_nodes) {

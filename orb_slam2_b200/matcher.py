@@ -17,6 +17,7 @@ from . import _lib
 from ._lib import KP_DTYPE, check
 
 TH_HIGH, TH_LOW, HISTO_LENGTH = 100, 50, 30        # src/ORBmatcher.cc:37-39
+BORB_ERR_CAPACITY = 5
 
 
 class _FrameViewC(C.Structure):
@@ -808,18 +809,24 @@ class ORBmatcher:
         sequential calls it replaces."""
         n = len(frames)
         dbs = self._db_jobs(dbs, n)
-        jobs = (_KfdbQueryJobC * max(n, 1))()
-        outs = []
-        for j, (db, F) in enumerate(zip(dbs, frames)):
-            ns = db.size()[0] if db is not None else 0
-            cw = np.zeros(max(ns, 1), np.int32); sc = np.zeros(max(ns, 1), np.float32); fw = np.zeros(max(ns, 1), np.uint32)
-            nsl = np.zeros(1, np.int32)
-            J = jobs[j]
-            J.db = db._h.value if db is not None else None
-            J.frame = F.resident._h.value if (F is not None and F.resident is not None) else None
-            J.common_words, J.score, J.first_word, J.cap, J.n_slots = _p(cw), _p(sc), _p(fw), len(cw), _p(nsl)
-            outs.append((cw, sc, fw, nsl))
-        check(self._lib.borb_kfdb_query_batch(self._h, jobs, n), "borb_kfdb_query_batch")
+        sizes = [db.size()[0] if db is not None else 0 for db in dbs]
+        while True:              # sized again when another thread added keyframes since (refused before any launch)
+            jobs = (_KfdbQueryJobC * max(n, 1))()
+            outs = []
+            for j, (db, F, ns) in enumerate(zip(dbs, frames, sizes)):
+                cw = np.zeros(max(ns, 1), np.int32); sc = np.zeros(max(ns, 1), np.float32); fw = np.zeros(max(ns, 1), np.uint32)
+                nsl = np.zeros(1, np.int32)
+                J = jobs[j]
+                J.db = db._h.value if db is not None else None
+                J.frame = F.resident._h.value if (F is not None and F.resident is not None) else None
+                J.common_words, J.score, J.first_word, J.cap, J.n_slots = _p(cw), _p(sc), _p(fw), len(cw), _p(nsl)
+                outs.append((cw, sc, fw, nsl))
+            st = self._lib.borb_kfdb_query_batch(self._h, jobs, n)
+            grown = [int(o[3][0]) > len(o[0]) for o in outs]
+            if not (st == BORB_ERR_CAPACITY and any(grown)):
+                break
+            sizes = [max(ns, int(o[3][0])) for ns, o in zip(sizes, outs)]
+        check(st, "borb_kfdb_query_batch")
         return [(cw[:int(nsl[0])], sc[:int(nsl[0])], fw[:int(nsl[0])]) for cw, sc, fw, nsl in outs]
 
     def SearchByBoWDbBatch(self, dbs, slots_list, frames: Sequence[FrameView], pairs_cap=None):
@@ -1111,6 +1118,15 @@ class KeyFrameDatabase:
         hm = np.ascontiguousarray(has_mp, np.uint8)
         check(self._lib.borb_kfdb_set_has_mp(self._h, int(slot), _p(hm)), "borb_kfdb_set_has_mp")
 
+    def set_has_mp_batch(self, slots, has_mps) -> None:
+        """borb_kfdb_set_has_mp_batch: the MapPoint masks of several slots in one update that every search sees whole (a repeated
+        slot takes its last mask).  A bad slot or a None mask anywhere refuses the whole batch and changes nothing."""
+        sl = np.ascontiguousarray(slots, np.int32)
+        keep = [np.ascontiguousarray(h, np.uint8) if h is not None else None for h in has_mps]
+        assert len(keep) == len(sl)
+        arr = (C.c_void_p * max(len(keep), 1))(*[h.ctypes.data if h is not None else None for h in keep])
+        check(self._lib.borb_kfdb_set_has_mp_batch(self._h, len(sl), _p(sl), arr), "borb_kfdb_set_has_mp_batch")
+
     def size(self) -> Tuple[int, int]:
         n = C.c_int32(0); b = C.c_uint64(0)
         check(self._lib.borb_kfdb_size(self._h, C.byref(n), C.byref(b)), "borb_kfdb_size")
@@ -1119,12 +1135,15 @@ class KeyFrameDatabase:
     def query(self, mBowVec: Dict[int, float]):
         """Returns (common_words[int32], score[float32], first_word[uint32]) with one entry per slot."""
         w, v = self._bow_arrays(mBowVec)
-        n = self.size()[0]
-        cw = np.zeros(max(n, 1), np.int32); sc = np.zeros(max(n, 1), np.float32); fw = np.zeros(max(n, 1), np.uint32)
-        ns = C.c_int32(0)
-        check(self._lib.borb_kfdb_query(self._m._h, self._h, _p(w), _p(v), len(w), _p(cw), _p(sc), _p(fw), len(cw), C.byref(ns)),
-              "borb_kfdb_query")
-        return cw[:n], sc[:n], fw[:n]
+        ns = C.c_int32(self.size()[0])
+        while True:              # sized again when another thread added keyframes since (refused before any launch)
+            n = ns.value
+            cw = np.zeros(max(n, 1), np.int32); sc = np.zeros(max(n, 1), np.float32); fw = np.zeros(max(n, 1), np.uint32)
+            st = self._lib.borb_kfdb_query(self._m._h, self._h, _p(w), _p(v), len(w), _p(cw), _p(sc), _p(fw), len(cw), C.byref(ns))
+            if not (st == BORB_ERR_CAPACITY and ns.value > len(cw)):
+                break
+        check(st, "borb_kfdb_query")
+        return cw[:ns.value], sc[:ns.value], fw[:ns.value]
 
     def DetectRelocalizationCandidates(self, mBowVec: Dict[int, float], covisibility) -> list:
         """src/KeyFrameDatabase.cc:199-310.  covisibility(slot) -> up to 10 slots (GetBestCovisibilityKeyFrames(10))."""
