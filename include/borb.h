@@ -720,6 +720,26 @@ typedef struct borb_kfdb_query_job {
  * 1 launch whatever n_jobs (0 when no database has a slot), one synchronisation. */
 BORB_API borb_status borb_kfdb_query_batch(borb_matcher* m, const borb_kfdb_query_job* jobs, int n_jobs);
 
+/* KeyFrameDatabase::add (:41-47) of many keyframes straight from their resident frames: LoopClosing::DetectLoop of many camera
+ * streams adds each stream's keyframe with nothing of it crossing PCIe but the MapPoint mask.  Job j leaves its database exactly as
+ * borb_kfdb_add, called in job order, leaves it for a host view of the frame (its mvKeysUn, mDescriptors and FeatureVector, and
+ * has_mp) with the frame's BowVector: the same block bytes, the same slot (jobs on one database get ascending slots in job order),
+ * the same borb_kfdb_size bytes, the same host copy of the row records that borb_kfdb_set_has_mp rewrites later.  The caller's duty,
+ * as for borb_search_by_bow_db_batch: the frame's FeatureVector level (borb_frames_compute_bow's levelsup) must be the database's.
+ * The new slot does not refer to the frame: destroying or recycling the frame afterwards changes nothing.  Argument errors are
+ * refused with BORB_ERR_INVALID_ARG before anything is allocated or launched, the error text starting "job j:": a NULL database,
+ * frame or slot_out, a frame without BoW (recycled frames included), a frame, database and matcher on different devices.  A CUDA
+ * failure frees every block the call allocated and appends no slot.  A frame with 0 features or only stop words is added as
+ * borb_kfdb_add adds empty vectors.  1 launch whatever n_jobs, one synchronisation; the blocks are complete when the call returns.
+ * Every distinct database is locked, in address order, while the slots are appended. */
+typedef struct borb_kfdb_add_job {
+    borb_kfdb* db;
+    const borb_frame* frame;       /* resident, BoW computed by borb_frames_compute_bow */
+    const uint8_t* has_mp;         /* host, frame n entries: MapPoint present && !isBad(); NULL: none */
+    int32_t* slot_out;
+} borb_kfdb_add_job;
+BORB_API borb_status borb_kfdb_add_frames(borb_matcher* m, const borb_kfdb_add_job* jobs, int n_jobs);
+
 typedef struct borb_bow_db_job {
     borb_kfdb* db;
     const borb_frame* frame;       /* resident, BoW computed */
@@ -823,6 +843,14 @@ BORB_API borb_status borb_frames_compute_bow(borb_matcher* m, borb_voc* v, borb_
 BORB_API borb_status borb_matcher_set_timing(borb_matcher* m, int enable);
 BORB_API borb_status borb_matcher_last_kernel_ms(borb_matcher* m, float* ms);
 BORB_API borb_status borb_matcher_launch_count(const borb_matcher* m, uint64_t* n);
+/* What the database holds for a live slot (read-only; tests compare blocks byte for byte).  counts4 = {nn FeatureVector nodes, m rows
+ * (features inside the nodes), n features, n_bow BowVector words}; *block_bytes = the slot's device bytes.  Each non-NULL array gets:
+ * node[nn], start[nn + 1], meta[2 m] (row records in FeatureVector order: feature | good-MapPoint flag << 16 | node index << 17, then
+ * the bits of mvKeysUn[feature].angle), desc[m x 32] (row order), bow_word[n_bow], bow_value[n_bow], host_meta[2 m] (the host copy of
+ * the row records), block[*block_bytes] (the whole device block, padding included).  Call with NULL arrays first to size them. */
+BORB_API borb_status borb_debug_kfdb_read(borb_kfdb* db, int32_t slot, int32_t* counts4, uint64_t* block_bytes, uint32_t* node,
+                                          int32_t* start, uint32_t* meta, uint8_t* desc, uint32_t* bow_word, double* bow_value,
+                                          uint32_t* host_meta, uint8_t* block);
 /* Per-stage intermediates of the last batch, for parity tests (tests/ compare each stage with the
  * oracle).  xys: (x, y, score) int32 triples in level pixel coordinates. */
 BORB_API borb_status borb_debug_candidates(borb_extractor* e, int image, int level, int32_t* xys, int cap, int* n_out);

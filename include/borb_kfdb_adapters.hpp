@@ -61,6 +61,22 @@ inline void kfdb_add(KfdbState<KeyFrameT>& S, KeyFrameT* pKF, const borb_keyfram
     S.slot_of[pKF] = slot;
 }
 
+// KeyFrameDatabase::add (:41-47) of a keyframe whose Frame is still resident (`f`, BoW computed by borb_frames_compute_bow at the
+// database's levelsup): the keyframe's features and BowVector are taken from the device, only has_mp (f's n entries, MapPoint present
+// && !isBad(); nullptr: none) crosses PCIe.  The database ends as kfdb_add with the keyframe's view leaves it.  Many streams at once:
+// borb_kfdb_add_frames with one job per stream, then the slot bookkeeping below per job.
+template <class KeyFrameT>
+inline void kfdb_add_resident(KfdbState<KeyFrameT>& S, KeyFrameT* pKF, const borb_frame* f, const uint8_t* has_mp) {
+    std::lock_guard<std::mutex> lk(S.mu);
+    S.ensure();
+    int32_t slot = -1;
+    const borb_kfdb_add_job job = {S.db, f, has_mp, &slot};
+    check(borb_kfdb_add_frames(thread_matcher(S.device), &job, 1), "borb_kfdb_add_frames");
+    if ((size_t)slot >= S.kf_of_slot.size()) S.kf_of_slot.resize((size_t)slot + 1, nullptr);
+    S.kf_of_slot[slot] = pKF;
+    S.slot_of[pKF] = slot;
+}
+
 template <class KeyFrameT>
 inline void kfdb_erase(KfdbState<KeyFrameT>& S, KeyFrameT* pKF) {          // :49-66
     std::lock_guard<std::mutex> lk(S.mu);

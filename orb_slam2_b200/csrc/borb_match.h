@@ -170,6 +170,34 @@ struct KfStream {                  // one keyframe of the device-resident databa
     const void* pad2[2];
 };
 
+// One keyframe's device block in the database (borb_kfdb_add, borb_kfdb_add_frames): the KfStream and BowDev sections
+//   node[nn] | start[nn + 1] | meta[m] uint2 | desc[m][32] | bow words[n_bow] | bow values[n_bow]
+// each 256-byte aligned, then 256 bytes of tail; every byte outside the sections is 0.
+struct KfdbBlock { size_t node, start, meta, desc, bow_word, bow_value, bytes; };
+__host__ __device__ inline KfdbBlock kfdb_block_layout(int nn, int m, int n_bow) {
+    size_t off = 0;
+    auto put = [&](size_t bytes) { off = (off + 255) & ~size_t(255); const size_t o = off; off += bytes; return o; };
+    KfdbBlock L;
+    L.node = put((size_t)nn * 4); L.start = put((size_t)(nn + 1) * 4); L.meta = put((size_t)m * 8); L.desc = put((size_t)m * 32);
+    L.bow_word = put((size_t)n_bow * 4); L.bow_value = put((size_t)n_bow * 8);
+    L.bytes = off + 256;
+    return L;
+}
+
+struct KfdbInsertJob {            // one keyframe of kfdb_insert_kernel (k_bowdb.cu): a resident frame with BoW -> its database block
+    const uint32_t* fv_node;      // the frame's FeatureVector (nn nodes, m = fv_start[nn] rows) and BowVector
+    const int32_t* fv_start;
+    const uint32_t* fv_idx;
+    const borb_keypoint* keys;
+    const uint8_t* desc;
+    const uint32_t* bow_word;
+    const double* bow_value;
+    const uint8_t* has_mp;        // n entries, may be null
+    int nn, m, n_bow, pad;
+    uint8_t* block;               // kfdb_block_layout(nn, m, n_bow), written whole
+    uint2* meta_out;              // m rows: a copy of the row records for the host (pinned, device-addressable)
+};
+
 // Packed query frame of the database search (k_bowdb.cu), built on the device by bowdb_pack_kernel: header, then 16-byte
 // aligned sections
 //   node[nn] u32 ascending | start[nn+1] i32 | orig[m] u16 | angle[m] f32 | desc[m][32]     (m = features inside nodes)
@@ -341,6 +369,8 @@ int launch_frame_build(const FrameJob* d_jobs, int n_jobs, int max_n, const borb
 int launch_bowdb(const BowDbArgs& A, const BowDbJob& one, int max_smem_frame, long long max_items, int total_kf, int max_nn, int csa, int n_sm,
                  bool kfkf, cudaStream_t s);
 bool bowdb_frame_fits_smem(int frame_bytes);
+// n_jobs database blocks (a job table in device memory) in one launch, a CTA per job
+int launch_kfdb_insert(const KfdbInsertJob* d_jobs, int n_jobs, cudaStream_t s);
 // n_jobs searches (a job table in device memory) in one launch
 int launch_triangulation(const TriJob* d_jobs, int n_jobs, int check_ori, cudaStream_t s);
 // project_points over a LastArgs table (variant 2), then fuse_batch_kernel over a FuseJob table: 2 launches; max_nq = most points of a job

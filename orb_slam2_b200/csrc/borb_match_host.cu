@@ -1668,6 +1668,29 @@ borb_status borb_kfdb_destroy(borb_kfdb* db) {
     return BORB_OK;
 }
 
+// Appends a keyframe whose device block (kfdb_block_layout(nn, m, n_bow), complete) holds the row records `meta` (m x 2 u32, row
+// order) and returns its slot; the caller holds db->mu.  The one place that points a slot's KfStream and BowDev into its block and
+// keeps the host copies of the rows (borb_kfdb_set_has_mp rewrites their flag), for borb_kfdb_add and borb_kfdb_add_frames alike.
+static int32_t kfdb_append_locked(borb_kfdb* db, uint8_t* block, int nn, int m, int n, int n_bow, const uint32_t* meta) {
+    const KfdbBlock L = kfdb_block_layout(nn, m, n_bow);
+    borb_kfdb::Entry e;
+    e.block = block;
+    e.orig.resize(m);
+    e.meta.assign(meta, meta + (size_t)m * 2);
+    for (int r = 0; r < m; r++) e.orig[r] = (uint16_t)(meta[2 * r] & 0xFFFFu);
+    e.stream.node = (const uint32_t*)(block + L.node); e.stream.start = (const int32_t*)(block + L.start);
+    e.stream.meta = (const uint2*)(block + L.meta); e.stream.desc = block + L.desc;
+    e.stream.nn = nn; e.stream.m = m; e.stream.n = n; e.stream.pad = 0;
+    e.d_meta = block + L.meta;
+    e.n = n;
+    e.bow.word = (const uint32_t*)(block + L.bow_word); e.bow.value = (const double*)(block + L.bow_value); e.bow.n = n_bow;
+    e.alive = true;
+    db->entries.push_back(std::move(e));
+    db->dirty = true;
+    db->bytes += L.bytes;
+    return (int32_t)db->entries.size() - 1;
+}
+
 borb_status borb_kfdb_add(borb_kfdb* db, const borb_keyframe_view* kf, const uint32_t* bow_word, const double* bow_value, int n_bow,
                           int32_t* slot_out) {
     if (!db || !kf || !slot_out || n_bow < 0 || (n_bow > 0 && (!bow_word || !bow_value))) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
@@ -1679,46 +1702,28 @@ borb_status borb_kfdb_add(borb_kfdb* db, const borb_keyframe_view* kf, const uin
     const int m = nn > 0 ? kf->fv.start[nn] : 0;
     std::lock_guard<std::mutex> lk(db->mu);
     BORB_CUDA(cudaSetDevice(db->device));
-    // one device block per keyframe: [node | start | orig | angle | hasmp | desc (rows in FeatureVector order) | bow words | bow values]
-    size_t off = 0;
-    auto put = [&](size_t bytes) { off = (off + 255) & ~size_t(255); const size_t o = off; off += bytes; return o; };
-    const size_t o_node = put((size_t)nn * 4), o_start = put((size_t)(nn + 1) * 4), o_meta = put((size_t)m * 8), o_desc = put((size_t)m * 32);
-    const size_t o_bw = put((size_t)n_bow * 4), o_bv = put((size_t)n_bow * 8);
-    const size_t total = off + 256;
-    std::vector<uint8_t> h(total, 0);
-    borb_kfdb::Entry e;
-    e.orig.resize(m);
+    // one device block per keyframe, packed here and uploaded whole (kfdb_insert_kernel writes the same bytes from a resident frame)
+    const KfdbBlock L = kfdb_block_layout(nn, m, n_bow);
+    std::vector<uint8_t> h(L.bytes, 0);
+    uint32_t* meta = reinterpret_cast<uint32_t*>(&h[L.meta]);
     if (nn) {
-        std::memcpy(&h[o_node], kf->fv.node_id, (size_t)nn * 4);
-        std::memcpy(&h[o_start], kf->fv.start, (size_t)(nn + 1) * 4);
-        uint32_t* meta = reinterpret_cast<uint32_t*>(&h[o_meta]);
-        e.meta.resize((size_t)m * 2);
+        std::memcpy(&h[L.node], kf->fv.node_id, (size_t)nn * 4);
+        std::memcpy(&h[L.start], kf->fv.start, (size_t)(nn + 1) * 4);
         int a = 0;                                                     // node index of row r (rows are grouped by node)
         for (int r = 0; r < m; r++) {
             while (a + 1 < nn && r >= kf->fv.start[a + 1]) a++;
             const uint32_t f = kf->fv.feat_idx[r];
-            e.orig[r] = (uint16_t)f;
             meta[2 * r] = f | ((kf->has_mp && kf->has_mp[f]) ? 0x10000u : 0u) | ((uint32_t)a << 17);
             std::memcpy(&meta[2 * r + 1], &kf->keys_un[f].angle, 4);
-            e.meta[2 * r] = meta[2 * r]; e.meta[2 * r + 1] = meta[2 * r + 1];
-            std::memcpy(&h[o_desc + (size_t)r * 32], kf->desc + (size_t)f * 32, 32);
+            std::memcpy(&h[L.desc + (size_t)r * 32], kf->desc + (size_t)f * 32, 32);
         }
     }
-    if (n_bow) { std::memcpy(&h[o_bw], bow_word, (size_t)n_bow * 4); std::memcpy(&h[o_bv], bow_value, (size_t)n_bow * 8); }
-    BORB_CUDA(cudaMalloc(&e.block, total));
-    BORB_CUDA(cudaMemcpy(e.block, h.data(), total, cudaMemcpyHostToDevice));
-    uint8_t* b = e.block;
-    e.stream.node = (const uint32_t*)(b + o_node); e.stream.start = (const int32_t*)(b + o_start); e.stream.meta = (const uint2*)(b + o_meta);
-    e.stream.desc = b + o_desc;
-    e.stream.nn = nn; e.stream.m = m; e.stream.n = kf->n; e.stream.pad = 0;
-    e.d_meta = b + o_meta;
-    e.n = kf->n;
-    e.bow.word = (const uint32_t*)(b + o_bw); e.bow.value = (const double*)(b + o_bv); e.bow.n = n_bow;
-    e.alive = true;
-    db->entries.push_back(std::move(e));
-    db->dirty = true;
-    db->bytes += total;
-    *slot_out = (int32_t)db->entries.size() - 1;
+    if (n_bow) { std::memcpy(&h[L.bow_word], bow_word, (size_t)n_bow * 4); std::memcpy(&h[L.bow_value], bow_value, (size_t)n_bow * 8); }
+    uint8_t* block = nullptr;
+    BORB_CUDA(cudaMalloc(&block, L.bytes));
+    const cudaError_t ce = cudaMemcpy(block, h.data(), L.bytes, cudaMemcpyHostToDevice);
+    if (ce != cudaSuccess) { cudaFree(block); BORB_CUDA(ce); }
+    *slot_out = kfdb_append_locked(db, block, nn, m, kf->n, n_bow, meta);
     return BORB_OK;
 }
 
@@ -2076,6 +2081,87 @@ borb_status borb_kfdb_query_batch(borb_matcher* m, const borb_kfdb_query_job* jo
         q[j] = QueryJob{B.db, B.frame, nullptr, nullptr, 0, B.common_words, B.score, B.first_word, B.cap, B.n_slots};
     }
     return kfdb_query_jobs(m, q.data(), n_jobs, true);
+}
+
+// Every job's block is allocated and written by one launch of kfdb_insert_kernel before any database is locked; the slots are
+// appended in job order under the locks once the blocks are complete, so no search ever sees a partial block.
+borb_status borb_kfdb_add_frames(borb_matcher* m, const borb_kfdb_add_job* jobs, int n_jobs) {
+    if (!m || n_jobs < 0 || (n_jobs > 0 && !jobs)) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+    if (n_jobs == 0) return BORB_OK;
+    for (int j = 0; j < n_jobs; j++) {
+        const borb_kfdb_add_job& B = jobs[j];
+        const borb_status s = check_db_job(m, B.db, B.frame, j);
+        if (s != BORB_OK) return s;
+        if (!B.slot_out) { set_error("job %d: null slot_out", j); return BORB_ERR_INVALID_ARG; }
+    }
+    BORB_CUDA(cudaSetDevice(m->device));
+    std::vector<uint8_t*> blocks(n_jobs, nullptr);
+    auto fail = [&](borb_status s) { for (uint8_t* b : blocks) cudaFree(b); return s; };
+    Call c(m);
+    std::vector<size_t> o_hm(n_jobs, 0), r_meta(n_jobs, 0);
+    for (int j = 0; j < n_jobs; j++)
+        if (jobs[j].has_mp && jobs[j].frame->n > 0) o_hm[j] = c.in(jobs[j].has_mp, (size_t)jobs[j].frame->n);
+    const size_t o_jobs = c.in(nullptr, (size_t)n_jobs * sizeof(KfdbInsertJob));     // filled in place
+    for (int j = 0; j < n_jobs; j++) r_meta[j] = c.result((size_t)jobs[j].frame->n_fv * 8);
+    for (int j = 0; j < n_jobs; j++) {
+        const borb_frame* f = jobs[j].frame;
+        const cudaError_t e = cudaMalloc(&blocks[j], kfdb_block_layout(f->n_nodes, f->n_fv, f->n_bow).bytes);
+        if (e != cudaSuccess) { blocks[j] = nullptr; set_error("job %d: keyframe block allocation failed: %s", j, cudaGetErrorString(e)); return fail(BORB_ERR_CUDA); }
+    }
+    borb_status s;
+    if ((s = c.begin()) != BORB_OK) return fail(s);
+    KfdbInsertJob* hj = c.host<KfdbInsertJob>(o_jobs);
+    for (int j = 0; j < n_jobs; j++) {
+        const borb_frame* f = jobs[j].frame;
+        KfdbInsertJob J{};
+        J.fv_node = f->fv_node; J.fv_start = f->fv_start; J.fv_idx = f->fv_idx; J.keys = f->keys; J.desc = f->desc;
+        J.bow_word = f->bow_word; J.bow_value = f->bow_value;
+        J.has_mp = (jobs[j].has_mp && f->n > 0) ? c.dev(o_hm[j]) : nullptr;
+        J.nn = f->n_nodes; J.m = f->n_fv; J.n_bow = f->n_bow;
+        J.block = blocks[j];
+        // the row records for the host copies are written by the kernel straight into the pinned landing buffer (UVA)
+        J.meta_out = f->n_fv > 0 ? reinterpret_cast<uint2*>(c.res(r_meta[j], true)) : nullptr;
+        hj[j] = J;
+    }
+    if ((s = c.commit()) != BORB_OK) return fail(s);
+    for (int j = 0; j < n_jobs; j++)
+        if ((s = c.wait(jobs[j].frame)) != BORB_OK) return fail(s);
+    m->launches += launch_kfdb_insert((const KfdbInsertJob*)c.dev(o_jobs), n_jobs, m->stream);
+    if ((s = c.finish()) != BORB_OK) return fail(s);
+    std::vector<borb_kfdb*> dbs(n_jobs);
+    for (int j = 0; j < n_jobs; j++) dbs[j] = jobs[j].db;
+    DbLocks lk(std::move(dbs));
+    for (int j = 0; j < n_jobs; j++) {
+        const borb_frame* f = jobs[j].frame;
+        *jobs[j].slot_out = kfdb_append_locked(jobs[j].db, blocks[j], f->n_nodes, f->n_fv, f->n, f->n_bow,
+                                               reinterpret_cast<const uint32_t*>(c.out(r_meta[j])));
+    }
+    return BORB_OK;
+}
+
+borb_status borb_debug_kfdb_read(borb_kfdb* db, int32_t slot, int32_t* counts4, uint64_t* block_bytes, uint32_t* node, int32_t* start,
+                                 uint32_t* meta, uint8_t* desc, uint32_t* bow_word, double* bow_value, uint32_t* host_meta, uint8_t* block) {
+    if (!db) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+    std::lock_guard<std::mutex> lk(db->mu);
+    if (slot < 0 || slot >= (int)db->entries.size() || !db->entries[slot].alive) { set_error("bad keyframe slot"); return BORB_ERR_INVALID_ARG; }
+    const borb_kfdb::Entry& e = db->entries[slot];
+    const int nn = e.stream.nn, m = e.stream.m, nb = e.bow.n;
+    const KfdbBlock L = kfdb_block_layout(nn, m, nb);
+    if (counts4) { counts4[0] = nn; counts4[1] = m; counts4[2] = e.n; counts4[3] = nb; }
+    if (block_bytes) *block_bytes = L.bytes;
+    BORB_CUDA(cudaSetDevice(db->device));
+    auto get = [&](void* dst, size_t off, size_t bytes) -> borb_status {
+        if (dst && bytes) BORB_CUDA(cudaMemcpy(dst, e.block + off, bytes, cudaMemcpyDeviceToHost));
+        return BORB_OK;
+    };
+    borb_status s;
+    if ((s = get(node, L.node, (size_t)nn * 4)) != BORB_OK || (s = get(start, L.start, (size_t)(nn + 1) * 4)) != BORB_OK ||
+        (s = get(meta, L.meta, (size_t)m * 8)) != BORB_OK || (s = get(desc, L.desc, (size_t)m * 32)) != BORB_OK ||
+        (s = get(bow_word, L.bow_word, (size_t)nb * 4)) != BORB_OK || (s = get(bow_value, L.bow_value, (size_t)nb * 8)) != BORB_OK ||
+        (s = get(block, 0, L.bytes)) != BORB_OK)
+        return s;
+    if (host_meta && m > 0) std::memcpy(host_meta, e.meta.data(), (size_t)m * 8);
+    return BORB_OK;
 }
 
 borb_status borb_search_by_bow_db(borb_matcher* m, borb_kfdb* db, const int32_t* slots, int n_kf, const borb_keyframe_view* frame,

@@ -717,4 +717,54 @@ int launch_bowdb(const BowDbArgs& A, const BowDbJob& one, int max_smem_frame, lo
     return 3;
 }
 
+// KeyFrameDatabase::add of a resident frame with its BoW (borb_kfdb_add_frames), a CTA per job: the block that borb_kfdb_add packs
+// on the host, byte for byte (kfdb_block_layout; every byte outside the sections is written 0).  Row r of the FeatureVector holds
+// feature j = fv_idx[r] of node a, the largest a with fv_start[a] <= r; its record is {j | has_mp[j] != 0 << 16 | a << 17, bits of
+// mvKeysUn[j].angle}, and its descriptor is gathered as two uint4, a thread per half, as bowdb_pack does.  The records also go to
+// meta_out, the host's copy.
+constexpr int INSERT_THREADS = 256;
+__global__ void __launch_bounds__(INSERT_THREADS) kfdb_insert_kernel(const KfdbInsertJob* __restrict__ jobs) {
+    const KfdbInsertJob& J = jobs[blockIdx.x];
+    const int tid = threadIdx.x, T = blockDim.x;
+    const int nn = J.nn, m = J.m, nb = J.n_bow;
+    const KfdbBlock L = kfdb_block_layout(nn, m, nb);
+    uint8_t* blk = J.block;
+    auto zero = [&](size_t lo, size_t hi) { for (size_t i = lo + tid; i < hi; i += T) blk[i] = 0; };
+    zero(L.node + (size_t)nn * 4, L.start);
+    zero(L.start + (size_t)(nn + 1) * 4, L.meta);
+    zero(L.meta + (size_t)m * 8, L.desc);
+    zero(L.desc + (size_t)m * 32, L.bow_word);
+    zero(L.bow_word + (size_t)nb * 4, L.bow_value);
+    zero(L.bow_value + (size_t)nb * 8, L.bytes);
+    uint32_t* node = reinterpret_cast<uint32_t*>(blk + L.node);
+    int32_t* start = reinterpret_cast<int32_t*>(blk + L.start);
+    uint2* meta = reinterpret_cast<uint2*>(blk + L.meta);
+    uint4* desc = reinterpret_cast<uint4*>(blk + L.desc);
+    const uint4* src = reinterpret_cast<const uint4*>(J.desc);
+    for (int i = tid; i < nn; i += T) node[i] = J.fv_node[i];
+    for (int i = tid; i <= nn; i += T) start[i] = nn > 0 ? J.fv_start[i] : 0;
+    for (int t = tid; t < 2 * m; t += T) {
+        const int r = t >> 1;
+        const uint32_t j = J.fv_idx[r];
+        desc[t] = src[(size_t)j * 2 + (t & 1)];
+        if ((t & 1) == 0) {
+            int lo = 0, hi = nn;                                  // the row's node: largest a with fv_start[a] <= r
+            while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (J.fv_start[mid] <= r) lo = mid; else hi = mid; }
+            const uint32_t good = (J.has_mp && J.has_mp[j]) ? 0x10000u : 0u;
+            const uint2 rec = make_uint2(j | good | ((uint32_t)lo << 17), __float_as_uint(J.keys[j].angle));
+            meta[r] = rec;
+            J.meta_out[r] = rec;
+        }
+    }
+    uint32_t* bw = reinterpret_cast<uint32_t*>(blk + L.bow_word);
+    double* bv = reinterpret_cast<double*>(blk + L.bow_value);
+    for (int i = tid; i < nb; i += T) { bw[i] = J.bow_word[i]; bv[i] = J.bow_value[i]; }
+}
+
+int launch_kfdb_insert(const KfdbInsertJob* d_jobs, int n_jobs, cudaStream_t s) {
+    if (n_jobs <= 0) return 0;
+    kfdb_insert_kernel<<<n_jobs, INSERT_THREADS, 0, s>>>(d_jobs);
+    return 1;
+}
+
 }  // namespace borb

@@ -70,6 +70,10 @@ class _KfdbQueryJobC(C.Structure):                  # borb_kfdb_query_job
                 ("cap", C.c_int32), ("n_slots", C.c_void_p)]
 
 
+class _KfdbAddJobC(C.Structure):                    # borb_kfdb_add_job
+    _fields_ = [("db", C.c_void_p), ("frame", C.c_void_p), ("has_mp", C.c_void_p), ("slot_out", C.c_void_p)]
+
+
 class _BowDbJobC(C.Structure):                      # borb_bow_db_job
     _fields_ = [("db", C.c_void_p), ("frame", C.c_void_p), ("slots", C.c_void_p), ("n_kf", C.c_int32), ("n_matches", C.c_void_p),
                 ("pair_offset", C.c_void_p), ("pairs", C.c_void_p), ("pairs_cap", C.c_int32), ("n_pairs_total", C.c_void_p)]
@@ -829,6 +833,30 @@ class ORBmatcher:
         check(st, "borb_kfdb_query_batch")
         return [(cw[:int(nsl[0])], sc[:int(nsl[0])], fw[:int(nsl[0])]) for cw, sc, fw, nsl in outs]
 
+    def KfdbAddFramesBatch(self, dbs, frames: Sequence[FrameView], has_mps) -> List[int]:
+        """borb_kfdb_add_frames: KeyFrameDatabase.add of many resident frames whose BoW ComputeBoWBatch computed, in one launch; only
+        the MapPoint masks cross PCIe.  dbs[j] is job j's database (or one database for every job); has_mps[j] = job j's mask (n
+        entries, MapPoint present && !isBad()) or None.  Returns the new slots; each database ends as db.add() in job order leaves it
+        with a host view of the frame and its BowVector.  The frames' FeatureVector level must be the databases' (caller's duty)."""
+        n = len(frames)
+        dbs = self._db_jobs(dbs, n)
+        has_mps = list(has_mps) if has_mps is not None else [None] * n
+        assert len(has_mps) == n
+        jobs = (_KfdbAddJobC * max(n, 1))()
+        slots = np.full(max(n, 1), -1, np.int32)
+        keep = []
+        for j, (db, F, hm) in enumerate(zip(dbs, frames, has_mps)):
+            hm = np.ascontiguousarray(hm, np.uint8) if hm is not None else None
+            keep.append(hm)
+            J = jobs[j]
+            J.db = db._h.value if db is not None else None
+            J.frame = F.resident._h.value if (F is not None and F.resident is not None) else None
+            J.has_mp, J.slot_out = _p(hm), slots.ctypes.data + 4 * j
+        check(self._lib.borb_kfdb_add_frames(self._h, jobs, n), "borb_kfdb_add_frames")
+        for db, F in zip(dbs, frames):
+            db._appended(F.resident.n)
+        return [int(s) for s in slots[:n]]
+
     def SearchByBoWDbBatch(self, dbs, slots_list, frames: Sequence[FrameView], pairs_cap=None):
         """borb_search_by_bow_db_batch: SearchByBoW(KeyFrame*, Frame&) (src/ORBmatcher.cc:159-288) of many resident frames with BoW
         against candidate keyframes of their databases, in one launch sequence.  slots_list[j] = slot list of job j (None: every
@@ -1097,9 +1125,31 @@ class KeyFrameDatabase:
         slot = C.c_int32(-1)
         kc = pKF._c()
         check(self._lib.borb_kfdb_add(self._h, C.byref(kc), _p(w), _p(v), len(w), C.byref(slot)), "borb_kfdb_add")
-        self._seq.append(len(self._seq))
-        self._n.append(len(pKF.mvKeysUn))
+        self._appended(len(pKF.mvKeysUn))
         return slot.value
+
+    def _appended(self, n_features: int) -> None:
+        """The host bookkeeping of a new slot (add() and ORBmatcher.KfdbAddFramesBatch): slots are handed out in call order."""
+        self._seq.append(len(self._seq))
+        self._n.append(n_features)
+
+    def read_slot(self, slot: int) -> dict:
+        """borb_debug_kfdb_read: what the database holds for a live slot — node, start, meta (row records, 2 u32 per row), desc (row
+        order), bow_word, bow_value, host_meta (the host copy of the rows), block (the whole device block) and n (features)."""
+        cnt = np.zeros(4, np.int32); nb = C.c_uint64(0)
+        check(self._lib.borb_debug_kfdb_read(self._h, int(slot), _p(cnt), C.byref(nb), *([None] * 8)), "borb_debug_kfdb_read")
+        nn, m, n, nbow = (int(x) for x in cnt)
+        out = dict(node=np.zeros(max(nn, 1), np.uint32), start=np.zeros(nn + 1, np.int32), meta=np.zeros(max(2 * m, 1), np.uint32),
+                   desc=np.zeros((max(m, 1), 32), np.uint8), bow_word=np.zeros(max(nbow, 1), np.uint32),
+                   bow_value=np.zeros(max(nbow, 1), np.float64), host_meta=np.zeros(max(2 * m, 1), np.uint32),
+                   block=np.zeros(nb.value, np.uint8))
+        check(self._lib.borb_debug_kfdb_read(self._h, int(slot), None, None, *[_p(out[k]) for k in ("node", "start", "meta", "desc", "bow_word",
+                                                                                                 "bow_value", "host_meta", "block")]),
+              "borb_debug_kfdb_read")
+        for k, ln in (("node", nn), ("meta", 2 * m), ("desc", m), ("bow_word", nbow), ("bow_value", nbow), ("host_meta", 2 * m)):
+            out[k] = out[k][:ln]
+        out["n"] = n
+        return out
 
     def erase(self, slot: int) -> None:
         check(self._lib.borb_kfdb_erase(self._h, int(slot)), "borb_kfdb_erase")
