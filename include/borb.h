@@ -467,7 +467,9 @@ BORB_API borb_status borb_search_by_projection_last_batch(borb_matcher* m, const
 /* ORBmatcher::SearchForInitialization(Frame &F1, Frame &F2, vector<cv::Point2f> &vbPrevMatched, vector<int> &vnMatches12,
  * int windowSize) — src/ORBmatcher.cc:405-520 (Tracking::MonocularInitialization, src/Tracking.cc:599).
  * f1/f2: keys_un, desc (and f2's grid bounds) are read; prev_matched = vbPrevMatched as f1->n x 2 floats, updated in
- * place (:513-517); matches12[i1] = index in F2 or -1; n_matches = return value. */
+ * place (:513-517); matches12[i1] = index in F2 or -1; n_matches = return value.  The one-job case of
+ * borb_search_for_initialization_batch on host views: the device scratch is f1->n x 36 bytes plus f2's feature grid, with no
+ * f1->n x f2->n candidate list. */
 BORB_API borb_status borb_search_for_initialization(borb_matcher* m, const borb_frame_view* f1, const borb_frame_view* f2,
                                                     float* prev_matched, int window_size, float nnratio, int check_orientation,
                                                     int32_t* matches12, int32_t* n_matches);

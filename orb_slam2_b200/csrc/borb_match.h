@@ -95,8 +95,8 @@ struct Sim3AgreeJob {             // one SearchBySim3 of sim3_agree_batch_kernel
 
 constexpr int INIT_K = 8;         // window entries per F1 feature kept by init_prefix_kernel
 
-struct InitJob {                  // one SearchForInitialization of borb_search_for_initialization_batch (k_proj.cu)
-    ProjArgs A;                   // F2 = the current frame: keys, descriptors, grid and bounds of the resident frame (bind_resident)
+struct InitJob {                  // one SearchForInitialization of init_prefix / init_replay (k_proj.cu)
+    ProjArgs A;                   // F2 = the current frame: keys, descriptors, grid and bounds (bind_frame_fields)
     const borb_keypoint* keys1;   // F1 = the initial frame
     const uint8_t* desc1;
     int n1;                       // 0: nothing to do (the host wrote the result of a job without features)
@@ -347,8 +347,6 @@ int launch_projection_batch(const ProjArgs* d_jobs, const ProjArgs& one, int n_j
 int launch_point_projection_batch(const LastArgs* d_last, const ProjArgs* d_jobs, const LastArgs& one_last, const ProjArgs& one, int n_jobs,
                                   int max_nq, int max_n, int max_n_mp, bool last, cudaStream_t s);
 void launch_resolve(const ProjArgs& A, bool last, cudaStream_t s);
-int launch_initialization(const ProjArgs& A, const borb_keypoint* keys1, int n1, int32_t* match12, int32_t* ev_idx, uint8_t* ev_bin,
-                          float* prev, int* n_matches, cudaStream_t s);
 // SearchForInitialization of n_jobs jobs in 2 launches: one job by value (`one`), more over the InitJob table d_jobs;
 // max_n1 / max_n2 = the most features of an initial / current frame of a live job
 int launch_init_batch(const InitJob* d_jobs, const InitJob& one, int n_jobs, int max_n1, int max_n2, float nnratio, int check_ori,

@@ -1364,6 +1364,102 @@ borb_status borb_search_local_points_batch(borb_matcher* m, const borb_local_poi
     return local_points_jobs(m, jobs, n_jobs, viewing_cos_limit, nnratio, n_matches, true);
 }
 
+// ---- SearchForInitialization: borb_search_for_initialization is the one-job case of borb_search_for_initialization_batch
+// (init_prefix + init_replay, k_proj.cu, one synchronisation).  The scratch of a job is O(n1), with no n1 x n2 candidate list.
+namespace {
+// Tracking::MonocularInitialization of one or many camera streams.  Each job has two frame sides, F1 (initial) and F2 (current).
+// host == nullptr: the batch, whose jobs read their resident frames in place (keys, descriptors and F2's grid as built), so that only
+// vbPrevMatched crosses PCIe.  Otherwise host = {F1, F2}, the single call's host views, of which only keys_un and desc are staged
+// and F2's grid is built in call scratch.
+borb_status init_jobs(borb_matcher* m, const borb_init_job* jobs, int n_jobs, const borb_frame_view* host, float nnratio,
+                      int check_orientation, int32_t* n_matches) {
+    const bool batch = host == nullptr;
+    struct Job { borb_frame_view F[2]; FrameInfo I[2]; FrameStage fs[2]; bool live = false; size_t prev = 0, pre = 0, cnt = 0, res = 0, rprev = 0; };
+    std::vector<Job> J(n_jobs);
+    for (int j = 0; j < n_jobs; j++) {
+        const borb_init_job& B = jobs[j];
+        Job& o = J[j];
+        if (batch) {
+            if (!B.initial || !B.current) { set_error("job %d: null frame (the batch takes device-resident frames)", j); return BORB_ERR_INVALID_ARG; }
+            o.F[0].resident = B.initial; o.F[1].resident = B.current;
+        } else {
+            o.F[0] = host[0]; o.F[1] = host[1];
+        }
+        for (int k = 0; k < 2; k++) {
+            o.I[k] = frame_info(&o.F[k]);
+            const borb_status s = batch ? check_frame(&o.F[k], o.I[k], m) : BORB_OK;     // the single call checks its views itself
+            if (s != BORB_OK) return job_fail(batch, j, s);
+        }
+        if (o.I[0].n > 0 && (!B.prev_matched || !B.matches12)) { set_error("job %d: null prev_matched or matches12", j); return BORB_ERR_INVALID_ARG; }
+    }
+    int max_n1 = 0, max_n2 = 0;
+    for (int j = 0; j < n_jobs; j++) {                  // a job without features: matches12 -1, prev_matched untouched
+        const int n1 = J[j].I[0].n, n2 = J[j].I[1].n;
+        n_matches[j] = 0;
+        J[j].live = n1 > 0 && n2 > 0;
+        if (!J[j].live) { std::fill_n(jobs[j].matches12, n1, -1); continue; }
+        max_n1 = std::max(max_n1, n1); max_n2 = std::max(max_n2, n2);
+    }
+    if (max_n1 == 0) return BORB_OK;
+    Call c(m);
+    for (int j = 0; j < n_jobs; j++) {
+        Job& o = J[j];
+        if (!o.live) continue;
+        for (int k = 0; k < 2; k++)
+            if (!o.I[k].rf) {                            // of a host view, only what the init kernels read
+                o.fs[k].keys = c.in(o.F[k].keys_un, (size_t)o.I[k].n * sizeof(borb_keypoint));
+                o.fs[k].desc = c.in(o.F[k].desc, (size_t)o.I[k].n * 32);
+            }
+        o.prev = c.in(jobs[j].prev_matched, (size_t)o.I[0].n * 8);
+    }
+    JobTable<InitJob> jt(c, n_jobs);
+    for (int j = 0; j < n_jobs; j++) {
+        Job& o = J[j];
+        if (!o.live) continue;
+        const size_t n1 = (size_t)o.I[0].n;
+        o.pre = c.scratch(n1 * INIT_K * 4);
+        o.cnt = c.scratch(n1 * 4);
+        reserve_grid(c, o.I[1], o.fs[1]);
+        o.res = c.result(n1 * 4 + 4);
+        o.rprev = c.result(n1 * 8);
+    }
+    borb_status s;
+    // in place only for the batch: the kernels read a staged F2 more than once (ZERO_COPY_MAX)
+    if ((s = c.begin(batch && n_jobs == 1)) != BORB_OK) return s;
+    InitJob* hj = jt.host(c);
+    for (int j = 0; j < n_jobs; j++) {
+        const Job& o = J[j];
+        InitJob I{};
+        if (o.live) {                                    // a dead job keeps n1 = 0: both kernels skip it
+            bind_frame_fields(o.I[1], o.fs[1], c, I.A);
+            const borb_frame* f1 = o.I[0].rf;
+            I.keys1 = f1 ? f1->keys : (const borb_keypoint*)c.dev(o.fs[0].keys);
+            I.desc1 = f1 ? f1->desc : c.dev(o.fs[0].desc);
+            I.n1 = o.I[0].n;
+            I.window = (float)jobs[j].window_size;
+            I.prev_in = (const float*)c.dev(o.prev);
+            I.prefix = (uint32_t*)c.dev(o.pre); I.win_count = (int*)c.dev(o.cnt);
+            I.out = (int32_t*)c.res(o.res, true); I.prev_out = (float*)c.res(o.rprev, true);     // straight into the landing buffer
+        }
+        hj[j] = I;
+    }
+    if ((s = c.commit()) != BORB_OK) return s;
+    for (int j = 0; j < n_jobs; j++) {
+        if (!J[j].live) continue;
+        if (J[j].I[0].rf && (s = c.wait(J[j].I[0].rf)) != BORB_OK) return s;
+        if ((s = prepare_frame(m, c, J[j].I[1], hj[j].A)) != BORB_OK) return s;
+    }
+    m->launches += launch_init_batch(jt.dev(c), hj[0], n_jobs, max_n1, max_n2, nnratio, check_orientation, m->stream);
+    if ((s = c.finish()) != BORB_OK) return s;
+    for (int j = 0; j < n_jobs; j++) {
+        if (!J[j].live) continue;
+        read_counted(c.out(J[j].res), J[j].I[0].n, jobs[j].matches12, &n_matches[j]);
+        std::memcpy(jobs[j].prev_matched, c.out(J[j].rprev), (size_t)J[j].I[0].n * 8);
+    }
+    return BORB_OK;
+}
+}  // namespace
+
 borb_status borb_search_for_initialization(borb_matcher* m, const borb_frame_view* f1, const borb_frame_view* f2, float* prev_matched,
                                            int window_size, float nnratio, int check_orientation, int32_t* matches12, int32_t* n_matches) {
     if (!m || !f1 || !f2 || !prev_matched || !matches12 || !n_matches) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
@@ -1374,115 +1470,18 @@ borb_status borb_search_for_initialization(borb_matcher* m, const borb_frame_vie
     if (!f1->keys_un || !f1->desc || !f2->keys_un || !f2->desc || !(f2->max_x > f2->min_x) || !(f2->max_y > f2->min_y)) {
         set_error("incomplete frame view"); return BORB_ERR_INVALID_ARG;
     }
-    const int n1 = f1->n;
-    // the query windows are data the caller already has: vbPrevMatched as centre, windowSize as radius, level 0 only (:421-427)
-    std::vector<float> px(n1), py(n1), rad(n1, (float)window_size);
-    std::vector<int32_t> zero(n1, 0);
-    std::vector<uint8_t> valid(n1);
-    for (int i = 0; i < n1; i++) { px[i] = prev_matched[2 * i]; py[i] = prev_matched[2 * i + 1]; valid[i] = f1->keys_un[i].octave > 0 ? 0 : 1; }
-    Call c(m);
-    const size_t o_k2 = c.in(f2->keys_un, (size_t)f2->n * sizeof(borb_keypoint));
-    const size_t o_d2 = c.in(f2->desc, (size_t)f2->n * 32);
-    const size_t o_k1 = c.in(f1->keys_un, (size_t)n1 * sizeof(borb_keypoint));
-    const size_t o_d1 = c.in(f1->desc, (size_t)n1 * 32);
-    const size_t o_px = c.in(px.data(), (size_t)n1 * 4), o_py = c.in(py.data(), (size_t)n1 * 4), o_rad = c.in(rad.data(), (size_t)n1 * 4);
-    const size_t o_lv = c.in(zero.data(), (size_t)n1 * 4), o_val = c.in(valid.data(), (size_t)n1);
-    const size_t o_prev = c.in(prev_matched, (size_t)n1 * 8);
-    const size_t o_cs = c.scratch((size_t)(GRID_CELLS + 1) * 4), o_ci = c.scratch((size_t)MATCH_MAX_FEATURES * 4 + 16);
-    const size_t o_cand = c.scratch((size_t)n1 * f2->n * 4), o_cc = c.scratch((size_t)n1 * 4);
-    const size_t o_m12 = c.scratch((size_t)n1 * 4), o_evi = c.scratch((size_t)n1 * 4), o_evb = c.scratch((size_t)n1), o_nm = c.scratch(16);
-    borb_status s;
-    if ((s = c.begin()) != BORB_OK || (s = c.commit()) != BORB_OK) return s;
-    ProjArgs A{};
-    A.n = f2->n; A.keys = (const borb_keypoint*)c.dev(o_k2); A.desc = c.dev(o_d2);
-    A.u_right = nullptr; A.occupied = nullptr;
-    A.minX = f2->min_x; A.minY = f2->min_y;
-    A.invW = (float)GRID_COLS / (float)(f2->max_x - f2->min_x);
-    A.invH = (float)GRID_ROWS / (float)(f2->max_y - f2->min_y);
-    A.scale_factors = nullptr;
-    A.cell_start = (const int*)c.dev(o_cs); A.cell_idx = (const int*)c.dev(o_ci);
-    A.n_mp = n1; A.proj_x = (const float*)c.dev(o_px); A.proj_y = (const float*)c.dev(o_py); A.proj_xr = (const float*)c.dev(o_px);
-    A.mp_desc = c.dev(o_d1); A.mp_valid = c.dev(o_val); A.mp_has_obs = nullptr;
-    A.th = 1.f; A.nnratio = nnratio;
-    A.cand = (uint32_t*)c.dev(o_cand); A.cand_cnt = (int*)c.dev(o_cc);
-    A.q_radius = (const float*)c.dev(o_rad); A.q_minl = (const int32_t*)c.dev(o_lv); A.q_maxl = (const int32_t*)c.dev(o_lv);
-    A.mode = 1; A.check_ori = check_orientation; A.th_dist = 50;
-    m->launches += launch_grid_sort(A.keys, A.n, A.minX, A.minY, A.invW, A.invH, (int*)c.dev(o_cs), (int*)c.dev(o_ci), m->stream);
-    m->launches += launch_initialization(A, (const borb_keypoint*)c.dev(o_k1), n1, (int32_t*)c.dev(o_m12), (int32_t*)c.dev(o_evi), c.dev(o_evb),
-                                         (float*)c.dev(o_prev), (int*)c.dev(o_nm), m->stream);
-    // vbPrevMatched is updated on its staged copy: the three results go straight to the caller's arrays
-    BORB_CUDA(cudaMemcpyAsync(matches12, c.dev(o_m12), (size_t)n1 * 4, cudaMemcpyDeviceToHost, m->stream));
-    BORB_CUDA(cudaMemcpyAsync(prev_matched, c.dev(o_prev), (size_t)n1 * 8, cudaMemcpyDeviceToHost, m->stream));
-    BORB_CUDA(cudaMemcpyAsync(n_matches, c.dev(o_nm), 4, cudaMemcpyDeviceToHost, m->stream));
-    return c.finish();
+    borb_frame_view V[2] = {*f1, *f2};
+    V[0].resident = V[1].resident = nullptr;            // the host fields are read, never the resident frame
+    borb_init_job B{};
+    B.prev_matched = prev_matched; B.window_size = window_size; B.matches12 = matches12;
+    return init_jobs(m, &B, 1, V, nnratio, check_orientation, n_matches);
 }
 
-// Tracking::MonocularInitialization of many camera streams: every job reads its two resident frames in place (keys, descriptors and
-// the current frame's grid as built), only vbPrevMatched crosses PCIe, and two launches serve every job (k_proj.cu).
 borb_status borb_search_for_initialization_batch(borb_matcher* m, const borb_init_job* jobs, int n_jobs, float nnratio, int check_orientation,
                                                  int32_t* n_matches) {
     if (!m || n_jobs < 0) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
     if (n_jobs > 0 && (!jobs || !n_matches)) { set_error("job 0: null job table or n_matches"); return BORB_ERR_INVALID_ARG; }
-    struct Job { int n1 = 0, n2 = 0; bool live = false; size_t prev = 0, pre = 0, cnt = 0, res = 0, rprev = 0; };
-    std::vector<Job> J(n_jobs);
-    for (int j = 0; j < n_jobs; j++) {
-        const borb_init_job& B = jobs[j];
-        if (!B.initial || !B.current) { set_error("job %d: null frame (the batch takes device-resident frames)", j); return BORB_ERR_INVALID_ARG; }
-        for (const borb_frame* f : {B.initial, B.current}) {
-            borb_frame_view v{};
-            v.resident = f;
-            const borb_status s = check_frame(&v, frame_info(&v), m);
-            if (s != BORB_OK) return job_fail(true, j, s);
-        }
-        J[j].n1 = B.initial->n; J[j].n2 = B.current->n;
-        if (J[j].n1 > 0 && (!B.prev_matched || !B.matches12)) { set_error("job %d: null prev_matched or matches12", j); return BORB_ERR_INVALID_ARG; }
-    }
-    int max_n1 = 0, max_n2 = 0;
-    for (int j = 0; j < n_jobs; j++) {                  // a job without features gets the single call's result here (prev_matched untouched)
-        n_matches[j] = 0;
-        J[j].live = J[j].n1 > 0 && J[j].n2 > 0;
-        if (!J[j].live) { std::fill_n(jobs[j].matches12, J[j].n1, -1); continue; }
-        max_n1 = std::max(max_n1, J[j].n1); max_n2 = std::max(max_n2, J[j].n2);
-    }
-    if (max_n1 == 0) return BORB_OK;
-    Call c(m);
-    for (int j = 0; j < n_jobs; j++)
-        if (J[j].live) J[j].prev = c.in(jobs[j].prev_matched, (size_t)J[j].n1 * 8);
-    JobTable<InitJob> jt(c, n_jobs);
-    for (int j = 0; j < n_jobs; j++) {
-        if (!J[j].live) continue;
-        J[j].pre = c.scratch((size_t)J[j].n1 * INIT_K * 4);
-        J[j].cnt = c.scratch((size_t)J[j].n1 * 4);
-        J[j].res = c.result((size_t)J[j].n1 * 4 + 4);
-        J[j].rprev = c.result((size_t)J[j].n1 * 8);
-    }
-    borb_status s;
-    if ((s = c.begin(n_jobs == 1)) != BORB_OK) return s;
-    InitJob* hj = jt.host(c);
-    for (int j = 0; j < n_jobs; j++) {
-        InitJob I{};
-        if (J[j].live) {                                 // a dead job keeps n1 = 0: both kernels skip it
-            const borb_init_job& B = jobs[j];
-            bind_resident(B.current, I.A);
-            I.keys1 = B.initial->keys; I.desc1 = B.initial->desc; I.n1 = J[j].n1;
-            I.window = (float)B.window_size;
-            I.prev_in = (const float*)c.dev(J[j].prev);
-            I.prefix = (uint32_t*)c.dev(J[j].pre); I.win_count = (int*)c.dev(J[j].cnt);
-            I.out = (int32_t*)c.res(J[j].res, true); I.prev_out = (float*)c.res(J[j].rprev, true);     // straight into the landing buffer
-        }
-        hj[j] = I;
-    }
-    if ((s = c.commit()) != BORB_OK) return s;
-    for (int j = 0; j < n_jobs; j++)
-        if (J[j].live && ((s = c.wait(jobs[j].initial)) != BORB_OK || (s = c.wait(jobs[j].current)) != BORB_OK)) return s;
-    m->launches += launch_init_batch(jt.dev(c), hj[0], n_jobs, max_n1, max_n2, nnratio, check_orientation, m->stream);
-    if ((s = c.finish()) != BORB_OK) return s;
-    for (int j = 0; j < n_jobs; j++) {
-        if (!J[j].live) continue;
-        read_counted(c.out(J[j].res), J[j].n1, jobs[j].matches12, &n_matches[j]);
-        std::memcpy(jobs[j].prev_matched, c.out(J[j].rprev), (size_t)J[j].n1 * 8);
-    }
-    return BORB_OK;
+    return init_jobs(m, jobs, n_jobs, nullptr, nnratio, check_orientation, n_matches);
 }
 
 borb_status borb_distinctive_descriptors(borb_matcher* m, const uint8_t* desc, const int32_t* offsets, int n_points, int32_t* best_idx) {

@@ -270,81 +270,6 @@ __global__ void __launch_bounds__(256) project_points_batch_kernel(const LastArg
     if (i < L.n_last) project_point(L, i);
 }
 
-// SearchForInitialization (:405-520): one warp replays F1's level-0 features in order.  A candidate i2 is skipped
-// when an earlier feature already holds it with a distance <= ours (vMatchedDistance, :441-442); a better match
-// displaces the earlier owner (:462-466).  vMatchedDistance / vnMatches21 live in shared memory.
-__global__ void __launch_bounds__(32) init_resolve_kernel(ProjArgs A, const borb_keypoint* __restrict__ keys1, int n1,
-                                                          int32_t* __restrict__ match12, int32_t* __restrict__ ev_idx,
-                                                          uint8_t* __restrict__ ev_bin, float* __restrict__ prev, int* __restrict__ n_matches) {
-    extern __shared__ uint32_t smem_init[];
-    uint16_t* matchedDist = reinterpret_cast<uint16_t*>(smem_init);           // 0xFFFF = INT_MAX
-    uint16_t* owner = matchedDist + ((A.n + 1) & ~1);                          // 0xFFFF = -1
-    __shared__ int hist[32];
-    const int lane = threadIdx.x;
-    for (int i = lane; i < A.n; i += 32) { matchedDist[i] = 0xFFFFu; owner[i] = 0xFFFFu; }
-    for (int i = lane; i < n1; i += 32) match12[i] = -1;
-    hist[lane] = 0;
-    __syncwarp();
-    int nm = 0, nev = 0;
-    for (int i1 = 0; i1 < n1; i1++) {
-        const int cnt = A.cand_cnt[i1] & CAND_COUNT_MASK;
-        if (cnt == 0) continue;
-        const uint32_t* c = A.cand + (size_t)i1 * A.n;
-        unsigned k1 = 0xFFFFFFFFu, k2 = 0xFFFFFFFFu;
-        for (int p = lane; p < cnt; p += 32) {
-            const uint32_t e = c[p];
-            const unsigned dist = (e >> 16) & 0x1FFu;
-            if ((unsigned)matchedDist[e & 0xFFFF] <= dist) continue;
-            const unsigned key = (dist << 16) | (unsigned)p;
-            if (key < k1) { k2 = k1; k1 = key; } else if (key < k2) k2 = key;
-        }
-        const unsigned best = warp_min(k1);
-        const unsigned second = warp_min(k1 == best ? k2 : k1);
-        if (best != 0xFFFFFFFFu) {
-            const int bestDist = (int)(best >> 16);
-            const float bd2 = second != 0xFFFFFFFFu ? (float)(int)(second >> 16) : 2147483648.f;      // (float)INT_MAX
-            if (bestDist <= TH_LOW && (float)bestDist < __fmul_rn(bd2, A.nnratio)) {
-                const int i2 = (int)(c[best & 0xFFFFu] & 0xFFFF);
-                const int prevOwner = owner[i2];
-                __syncwarp();                                    // every lane has read the owner before lane 0 replaces it
-                if (prevOwner != 0xFFFF) nm--;
-                nm++;
-                if (lane == 0) {
-                    if (prevOwner != 0xFFFF) match12[prevOwner] = -1;
-                    match12[i1] = i2;
-                    owner[i2] = (uint16_t)i1;
-                    matchedDist[i2] = (uint16_t)bestDist;
-                    if (A.check_ori) {
-                        const int b = rot_bin(keys1[i1].angle, A.keys[i2].angle);
-                        ev_idx[nev] = i1; ev_bin[nev] = (uint8_t)b;
-                        hist[b]++;
-                    }
-                }
-                nev++;
-            }
-        }
-        __syncwarp();
-    }
-    if (A.check_ori) {
-        int i1m, i2m, i3m;
-        three_maxima(hist, i1m, i2m, i3m);
-        int removed = 0;
-        for (int e = lane; e < nev; e += 32) {                   // every F1 feature appears at most once in the histogram
-            const int b = ev_bin[e];
-            if (b != i1m && b != i2m && b != i3m && match12[ev_idx[e]] >= 0) { match12[ev_idx[e]] = -1; removed++; }
-        }
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) removed += __shfl_xor_sync(0xFFFFFFFFu, removed, off);
-        nm -= removed;
-    }
-    __syncwarp();
-    for (int i = lane; i < n1; i += 32) {                        // update vbPrevMatched (:513-517)
-        const int m = match12[i];
-        if (m >= 0) { prev[2 * i] = A.keys[m].x; prev[2 * i + 1] = A.keys[m].y; }
-    }
-    if (lane == 0) *n_matches = nm;
-}
-
 // MapPoint::ComputeDistinctiveDescriptors (src/MapPoint.cc:242-307), batched: a warp per MapPoint, a lane per row of the
 // distance matrix.  The row median (sorted row[(int)(0.5*(N-1))], self-distance included) comes from a 257-bin counting
 // histogram kept in local memory; first minimal median wins (lowest row index).
@@ -885,13 +810,6 @@ int launch_grid_sort(const borb_keypoint* keys, int n, float minX, float minY, f
     allow_max_smem((const void*)grid_sort_kernel);
     grid_sort_kernel<<<1, 1024, K * 4, s>>>(keys, n, minX, minY, invW, invH, K, cell_start, cell_idx);
     return 1;
-}
-int launch_initialization(const ProjArgs& A, const borb_keypoint* keys1, int n1, int32_t* match12, int32_t* ev_idx, uint8_t* ev_bin,
-                          float* prev, int* n_matches, cudaStream_t s) {
-    launch_candidates(A, s);
-    const size_t smem = (size_t)((A.n + 1) & ~1) * 2 + (size_t)A.n * 2 + 16;
-    init_resolve_kernel<<<1, 32, smem, s>>>(A, keys1, n1, match12, ev_idx, ev_bin, prev, n_matches);
-    return 2;
 }
 int launch_kfdb_score(const KfdbQueryJob* d_jobs, int n_jobs, int max_slots, int max_nq, int n_sm, cudaStream_t s) {
     if (n_jobs > 0 && max_slots > 0) {

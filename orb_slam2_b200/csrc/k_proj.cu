@@ -19,7 +19,7 @@
 //       number of queries, the cost.)
 //       LAST = false: best / second-best + ratio test (:98-121), out[query] = feature.
 //       LAST = true : best only, threshold th_dist, out[feature] = query, match events for the rotation histogram (:1426-1466).
-//   init_prefix_kernel / init_replay_kernel   SearchForInitialization (:405-520) of many frame pairs on resident frames (below).
+//   init_prefix_kernel / init_replay_kernel   SearchForInitialization (:405-520) of one or many frame pairs (below).
 //   fuse_batch_kernel / sim3_agree_batch_kernel   the order-independent searches, Fuse x2 and both directions of SearchBySim3, with
 //       no candidate list; the agreement test of SearchBySim3 (below).
 // All float tests use _rn intrinsics (no FMA contraction) so comparisons match the reference bit for bit.
@@ -465,11 +465,11 @@ void launch_resolve(const ProjArgs& A, bool last, cudaStream_t s) {
 }
 
 // ------------------------------------------------------------------------------------------------ SearchForInitialization
-// ORBmatcher::SearchForInitialization (:405-520) of many (initial F1, current F2) pairs of resident frames, two launches for any
-// number of jobs and O(n1 x INIT_K) scratch per job instead of an n1 x n2 candidate list.
+// ORBmatcher::SearchForInitialization (:405-520) of one or many (initial F1, current F2) frame pairs, resident or staged per call,
+// two launches for any number of jobs and O(n1 x INIT_K) scratch per job instead of an n1 x n2 candidate list.
 //   init_prefix_kernel   a warp per (job, F1 feature) on grid (features / 8, jobs), independent across queries.  A feature with
 //       octave > 0 is skipped (:421-423); otherwise its level-0 window GetFeaturesInArea(prev.x, prev.y, windowSize, 0, 0) is walked
-//       on F2's resident grid, each window column as ONE contiguous cell_idx range (as fuse_batch_kernel does), keeping the window's
+//       on F2's grid, each window column as ONE contiguous cell_idx range (as fuse_batch_kernel does), keeping the window's
 //       entry count and its INIT_K smallest keys (dist << 16) | e, with e the entry's position in cell_idx.
 //   init_replay_kernel   a warp per job replays F1's features in order with vMatchedDistance / vnMatches21 in shared memory.  A
 //       query's best and second best are the first two prefix entries that are not excluded (vMatchedDistance[i2] <= dist, :441-442).

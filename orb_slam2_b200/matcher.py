@@ -157,6 +157,12 @@ def _lastframe_c(Last: "LastFrameView"):
     return _LastFrameViewC(len(arrs[0]), *[_p(a) for a in arrs]), arrs
 
 
+def _prev_matched(vbPrevMatched):
+    """vbPrevMatched as an (N,2) float32 copy that the library updates in place (at least one row, so that the pointer is valid)."""
+    prev = np.ascontiguousarray(np.asarray(vbPrevMatched, np.float32).reshape(-1, 2)).copy()
+    return prev if len(prev) else np.zeros((1, 2), np.float32)
+
+
 def _local_points_outputs(nq: int):
     """The output arrays of SearchLocalPoints for nq points (at least one entry each, so that every pointer is valid)."""
     m1 = max(nq, 1)
@@ -651,9 +657,7 @@ class ORBmatcher:
             views.append(_FrameViewC(len(k), _p(k), _p(d), None, None, *[float(x) for x in F.bounds], len(sf), _p(sf)))
             keep += [k, d, sf]
         n1 = views[0].n
-        prev = np.ascontiguousarray(np.asarray(vbPrevMatched, np.float32).reshape(-1, 2)).copy()
-        if len(prev) == 0:
-            prev = np.zeros((1, 2), np.float32)
+        prev = _prev_matched(vbPrevMatched)
         m12 = np.full(max(n1, 1), -1, np.int32)
         nm = C.c_int32(0)
         check(self._lib.borb_search_for_initialization(self._h, C.byref(views[0]), C.byref(views[1]), _p(prev), int(windowSize), self.mfNNratio,
@@ -673,9 +677,7 @@ class ORBmatcher:
         for j in range(n):
             F1, F2 = F1s[j], F2s[j]
             n1 = F1.resident.n if F1.resident is not None else len(F1.mvKeysUn)
-            prev = np.ascontiguousarray(np.asarray(prevs[j], np.float32).reshape(-1, 2)).copy()
-            if len(prev) == 0:
-                prev = np.zeros((1, 2), np.float32)
+            prev = _prev_matched(prevs[j])
             m12 = np.full(max(n1, 1), -1, np.int32)
             jobs[j] = _InitJobC(F1.resident._h if F1.resident is not None else None, F2.resident._h if F2.resident is not None else None,
                                 _p(prev), int(wins[j]), _p(m12))

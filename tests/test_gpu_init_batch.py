@@ -1,5 +1,5 @@
 """GPU parity of borb_search_for_initialization_batch: SearchForInitialization (src/ORBmatcher.cc:405-520) of many camera streams on
-resident frames.  Every job must equal the single call on host views of the same frames (and the oracle restatement) bit for bit;
+resident frames.  Every job must equal the oracle restatement and the single call on host views of the same frames bit for bit;
 the batch is two launches whatever its size, and argument errors are refused before anything is launched."""
 import ctypes as C
 
@@ -91,11 +91,15 @@ def test_two_rounds_follow_the_tracker(M, oracle, views):
     for (F1, F2, _, _, prev), g1, g2, w in zip(jobs, r1, r2, [50, 50, 20, 20, 5, 5]):
         s1 = mt.SearchForInitialization(F1, F2, prev, 100)
         s2 = mt.SearchForInitialization(F1, F2, s1[2], w)
+        o1 = oracle.port_search_for_initialization(F1, F2, prev, 100, 0.9, True)
+        o2 = oracle.port_search_for_initialization(F1, F2, o1[2], w, 0.9, True)
         assert same(g1, s1) and same(g2, s2)
+        assert same(g1, o1) and same(g2, o2)
 
 
-def test_extractor_frames_at_2000_features(M):
-    """The real path: frames made by borb_frames_from_extractor (mono) against the single call on the extractor's host copies."""
+def test_extractor_frames_at_2000_features(M, oracle):
+    """The real path: frames made by borb_frames_from_extractor (mono) against the single call on the extractor's host copies
+    and the oracle port."""
     from orb_slam2_b200 import synth
     from orb_slam2_b200.extractor import ORBextractor
     X = ORBextractor(2000)
@@ -112,6 +116,7 @@ def test_extractor_frames_at_2000_features(M):
         F1 = M.FrameView(host["keys_un"][s], outs[s][1], sf, b)
         F2 = M.FrameView(host["keys_un"][4 + s], outs[4 + s][1], sf, b)
         assert same(got[s], mt.SearchForInitialization(F1, F2, prevs[s], 100))
+        assert same(got[s], oracle.port_search_for_initialization(F1, F2, prevs[s], 100, 0.9, True))
         assert got[s][0] > 50
 
 

@@ -7,7 +7,7 @@ synth.stereo_pair(300, s, 0, 640, 480) and the current frame the right one (a ho
    batch:  one borb_search_for_initialization_batch.
 Both arms must return equal results before anything is timed.  Host clock around the public Python calls (each ends in a
 synchronise) after warm-up: median, 25th and 75th percentile of `--reps`.  Device time per kernel comes from torch.profiler in a run
-of its own; the device scratch of a batch is read off its layout.
+of its own; the device scratch of each arm is read off its layout.
 usage: python tools/bench_mono_init.py [--reps 30] [--out DIR]  -> one JSON line on stdout (and DIR/bench_mono_init.json)."""
 import argparse
 import json
@@ -24,15 +24,17 @@ from tools.bench_loop_closure import spread                                    #
 from tools.bench_track_ref import kernel_times                                 # noqa: E402
 
 K_TUM = (517.306408, 516.469215, 318.643040, 255.313989)
-SINGLE_KERNELS = ("grid_sort_kernel", "proj_candidates_kernel", "init_resolve_kernel")
+SINGLE_KERNELS = ("grid_sort_kernel", "init_prefix_kernel", "init_replay_kernel")
 BATCH_KERNELS = ("init_prefix_kernel", "init_prefix_batch_kernel", "init_replay_kernel", "init_replay_batch_kernel")
 
 
-def scratch_bytes(n1s):
-    """Device scratch of one batch: per job the prefix table (n1 x 8 entries x 4 B) and the window counts (n1 x 4 B), each 256-byte
-    aligned."""
+def scratch_bytes(n1s, grid=False):
+    """Device scratch of one call: per job the prefix table (n1 x 8 entries x 4 B) and the window counts (n1 x 4 B), and with
+    `grid` (the single call, whose current frame is a host view) that frame's grid, cell_start (64 x 48 + 1 entries) and cell_idx
+    (8192 entries + 16 B); each 256-byte aligned."""
     al = lambda b: (b + 255) // 256 * 256
-    return int(sum(al(32 * n) + al(4 * n) for n in n1s))
+    g = al(4 * (64 * 48 + 1)) + al(4 * 8192 + 16) if grid else 0
+    return int(sum(al(32 * n) + al(4 * n) + g for n in n1s))
 
 
 def main(reps, out_dir, ns=(1, 8, 32)):
@@ -57,10 +59,9 @@ def main(reps, out_dir, ns=(1, 8, 32)):
         a, c = single(), batch()
         assert all(x[0] == y[0] and np.array_equal(x[1], y[1]) and np.array_equal(x[2], y[2]) for x, y in zip(a, c))
         n1s = [len(host["keys_un"][s]) for s in range(n)]
-        n2s = [len(host["keys_un"][n_max + s]) for s in range(n)]
         res[str(n)] = {"single_calls": spread(single, reps), "batch": spread(batch, reps), "matches": int(sum(x[0] for x in c)),
                        "batch_scratch_bytes": scratch_bytes(n1s),
-                       "single_candidate_list_bytes": int(max(p * q * 4 for p, q in zip(n1s, n2s)))}
+                       "single_call_scratch_bytes": max(scratch_bytes([p], grid=True) for p in n1s)}
     try:
         res["kernels_us"] = {
             "single_1": kernel_times(lambda: mt.SearchForInitialization(views[0], views[n_max], prevs[0], 100), SINGLE_KERNELS),
