@@ -571,6 +571,24 @@ BORB_API borb_status borb_search_by_sim3_batch(borb_matcher* m, const borb_sim3_
 BORB_API borb_status borb_distinctive_descriptors(borb_matcher* m, const uint8_t* desc, const int32_t* offsets, int n_points,
                                                   int32_t* best_idx);
 
+/* MapPoint::ComputeDistinctiveDescriptors (src/MapPoint.cc:242-307) for n_points MapPoints, read from resident keyframes.
+ * frames[0..n_frames)        resident frames of the observing keyframes: any stream, any matcher on this device, repeats allowed
+ * offsets[n_points + 1]      MapPoint p owns observations offsets[p] .. offsets[p+1]-1, in mObservations order, bad keyframes dropped
+ * obs_frame[o], obs_idx[o]   observation o = row obs_idx[o] of frames[obs_frame[o]]
+ * best_idx[p]                as borb_distinctive_descriptors (relative to offsets[p]; -1 when the point has no observation)
+ * desc_out[p*32 .. +32)      that row: the new mDescriptor; left unchanged where best_idx[p] == -1
+ * Many streams concatenate their points and frames into one call.  best_idx and desc_out are bit-identical to
+ * borb_distinctive_descriptors on the same rows gathered on the host (first minimal median wins, median = sorted_row[(int)(0.5*(N-1))],
+ * self-distance included).  One launch and one synchronisation when any observation exists, none otherwise; the call waits for every
+ * distinct frame of the table.  Only obs_frame / obs_idx (8 bytes per observation), the offsets and the frame table (8 bytes per entry)
+ * go up, and only best_idx and 32 bytes per point come down: a host keeps no copy of a keyframe's descriptors.  A NULL frame, a frame
+ * on another device, obs_frame[o] outside [0, n_frames), obs_idx[o] outside [0, that frame's n), offsets that do not ascend from 0,
+ * more than 65535 observations on one point and NULL outputs with n_points > 0 are refused with BORB_ERR_INVALID_ARG before anything
+ * is uploaded or launched, the error text naming the point ("point p:") or the frame-table entry ("frame f"). */
+BORB_API borb_status borb_distinctive_descriptors_frames(borb_matcher* m, const borb_frame* const* frames, int n_frames,
+                                                         const int32_t* obs_frame, const int32_t* obs_idx, const int32_t* offsets,
+                                                         int n_points, int32_t* best_idx, uint8_t* desc_out);
+
 /* DBoW2::FeatureVector (ordered map NodeId -> feature indices) as CSR: node_id strictly ascending, 0 <= start[0] <=
  * start[1] <= ... <= start[n_nodes], and every feat_idx[r], r < start[n_nodes], below the view's n.  Every entry point that takes a
  * borb_keyframe_view as a host view checks this and refuses a violator with BORB_ERR_INVALID_ARG before anything is launched. */

@@ -89,6 +89,7 @@ _SIGNATURES = {
     "borb_search_for_initialization": (C.c_int, [vp, vp, vp, vp, C.c_int, C.c_float, C.c_int, vp, i32p]),
     "borb_search_for_initialization_batch": (C.c_int, [vp, vp, C.c_int, C.c_float, C.c_int, vp]),
     "borb_distinctive_descriptors": (C.c_int, [vp, vp, vp, C.c_int, vp]),
+    "borb_distinctive_descriptors_frames": (C.c_int, [vp, vp, C.c_int, vp, vp, vp, C.c_int, vp, vp]),
     "borb_kfdb_create": (C.c_int, [C.c_int, C.POINTER(vp)]),
     "borb_kfdb_destroy": (C.c_int, [vp]),
     "borb_kfdb_clear": (C.c_int, [vp]),

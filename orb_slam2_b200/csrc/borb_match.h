@@ -309,6 +309,16 @@ struct TriJob {                   // one SearchForTriangulation of triangulation
     int32_t* n_pairs;
 };
 
+struct DistinctArgs {             // MapPoint::ComputeDistinctiveDescriptors of n_points points (distinctive_kernel, k_match.cu)
+    const uint8_t* const* src;    // row sources: descriptor arrays of 32-byte rows, 16-byte aligned
+    const int32_t* obs_src;       // observation o = row obs_row[o] of src[obs_src[o]]; null: row o of src[0]
+    const int32_t* obs_row;
+    const int32_t* offsets;       // n_points + 1: point p owns observations offsets[p] .. offsets[p+1]-1
+    int n_points;
+    int32_t* best_idx;            // n_points: the chosen observation, relative to offsets[p] (-1: none)
+    uint8_t* desc_out;            // n_points x 32: the chosen row, untouched where best_idx is -1; may be null
+};
+
 struct BowTables {                // a BowVector (word order) and a FeatureVector (CSR); word == null: not written
     uint32_t* word;
     double* value;
@@ -353,7 +363,7 @@ int launch_init_batch(const InitJob* d_jobs, const InitJob& one, int n_jobs, int
                       cudaStream_t s);
 // n_jobs queries (a job table in device memory) in one launch; max_slots / max_nq: the largest n_slots / nq of the jobs
 int launch_kfdb_score(const KfdbQueryJob* d_jobs, int n_jobs, int max_slots, int max_nq, int n_sm, cudaStream_t s);
-int launch_distinctive(const uint8_t* desc, const int32_t* offsets, int n_points, int32_t* best_idx, cudaStream_t s);
+int launch_distinctive(const DistinctArgs& A, cudaStream_t s);
 // n_pairs searches in one launch (tables in device memory): pair p matches qs[p] against ts[p] and writes its output (mode 0: ts[p].n
 // entries, mode 1: qs[p].n) at match + out_off[p], its rotation bins at bins + out_off[p]; max_t = the largest ts[p].n
 int launch_bow_match(const KfDev* qs, const KfDev* ts, int n_pairs, int mode, float nnratio, int check_ori, int32_t* match,

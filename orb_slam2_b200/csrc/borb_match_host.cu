@@ -1492,14 +1492,77 @@ borb_status borb_distinctive_descriptors(borb_matcher* m, const uint8_t* desc, c
         if (offsets[i + 1] < offsets[i] || offsets[i] < 0 || offsets[i + 1] - offsets[i] >= (1 << 16)) { set_error("offsets must ascend; at most 65535 observations per MapPoint"); return BORB_ERR_INVALID_ARG; }
     if (total_desc > 0 && !desc) { set_error("null descriptors"); return BORB_ERR_INVALID_ARG; }
     Call c(m);
+    const size_t o_src = c.in(nullptr, sizeof(const uint8_t*));     // the one row source: the staged rows, filled in place
     const size_t o_d = c.in(desc, (size_t)total_desc * 32);
     const size_t o_o = c.in(offsets, (size_t)(n_points + 1) * 4);
     const size_t r_b = c.result((size_t)n_points * 4);
     borb_status s;
-    if ((s = c.begin()) != BORB_OK || (s = c.commit()) != BORB_OK) return s;
-    m->launches += launch_distinctive(c.dev(o_d), (const int32_t*)c.dev(o_o), n_points, (int32_t*)c.res(r_b, false), m->stream);
+    if ((s = c.begin()) != BORB_OK) return s;
+    *c.host<const uint8_t*>(o_src) = c.dev(o_d);
+    if ((s = c.commit()) != BORB_OK) return s;
+    const DistinctArgs A{(const uint8_t* const*)c.dev(o_src), nullptr, nullptr, (const int32_t*)c.dev(o_o), n_points,
+                         (int32_t*)c.res(r_b, false), nullptr};
+    m->launches += launch_distinctive(A, m->stream);
     if ((s = c.finish()) != BORB_OK) return s;
     std::memcpy(best_idx, c.out(r_b), (size_t)n_points * 4);
+    return BORB_OK;
+}
+
+// The rows are read in place from the resident frames: only the observation tables, the offsets and the frame table go up, and only
+// best_idx and the chosen rows come down.
+borb_status borb_distinctive_descriptors_frames(borb_matcher* m, const borb_frame* const* frames, int n_frames, const int32_t* obs_frame,
+                                                const int32_t* obs_idx, const int32_t* offsets, int n_points, int32_t* best_idx,
+                                                uint8_t* desc_out) {
+    if (!m || n_frames < 0 || n_points < 0 || (n_frames > 0 && !frames) || (n_points > 0 && !offsets)) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+    if (n_points > 0 && (!best_idx || !desc_out)) { set_error("null best_idx or desc_out"); return BORB_ERR_INVALID_ARG; }
+    for (int f = 0; f < n_frames; f++) {
+        if (!frames[f]) { set_error("frame %d: not a device-resident frame", f); return BORB_ERR_INVALID_ARG; }
+        if (frames[f]->device != m->device) { set_error("frame %d and matcher live on different devices", f); return BORB_ERR_INVALID_ARG; }
+    }
+    if (n_points == 0) return BORB_OK;
+    if (offsets[0] != 0) { set_error("point 0: offsets must start at 0 (got %d)", offsets[0]); return BORB_ERR_INVALID_ARG; }
+    for (int p = 0; p < n_points; p++)
+        if (offsets[p + 1] < offsets[p] || offsets[p + 1] - offsets[p] >= (1 << 16)) {
+            set_error("point %d: offsets must ascend; at most 65535 observations per MapPoint (got %d .. %d)", p, offsets[p], offsets[p + 1]);
+            return BORB_ERR_INVALID_ARG;
+        }
+    const int total = offsets[n_points];
+    if (total > 0 && (!obs_frame || !obs_idx)) { set_error("null obs_frame or obs_idx"); return BORB_ERR_INVALID_ARG; }
+    for (int p = 0; p < n_points; p++)
+        for (int o = offsets[p]; o < offsets[p + 1]; o++) {
+            const int f = obs_frame[o];
+            if (f < 0 || f >= n_frames) { set_error("point %d: observation %d names frame %d outside the table's %d", p, o, f, n_frames); return BORB_ERR_INVALID_ARG; }
+            if (obs_idx[o] < 0 || obs_idx[o] >= frames[f]->n) {
+                set_error("point %d: observation %d reads feature %d of frame %d, which has %d", p, o, obs_idx[o], f, frames[f]->n);
+                return BORB_ERR_INVALID_ARG;
+            }
+        }
+    if (total == 0) {                                   // no observation: nothing to launch
+        for (int p = 0; p < n_points; p++) best_idx[p] = -1;
+        return BORB_OK;
+    }
+    Call c(m);
+    const size_t o_src = c.in(nullptr, (size_t)n_frames * sizeof(const uint8_t*));   // the frames' descriptor arrays, filled in place
+    const size_t o_of = c.in(obs_frame, (size_t)total * 4), o_oi = c.in(obs_idx, (size_t)total * 4);
+    const size_t o_o = c.in(offsets, (size_t)(n_points + 1) * 4);
+    const size_t r_b = c.result((size_t)n_points * 4), r_d = c.result((size_t)n_points * 32);
+    borb_status s;
+    if ((s = c.begin()) != BORB_OK) return s;
+    const uint8_t** src = c.host<const uint8_t*>(o_src);
+    for (int f = 0; f < n_frames; f++) src[f] = frames[f]->desc;
+    if ((s = c.commit()) != BORB_OK) return s;
+    std::vector<const borb_frame*> wait(frames, frames + n_frames);
+    std::sort(wait.begin(), wait.end());
+    wait.erase(std::unique(wait.begin(), wait.end()), wait.end());
+    for (const borb_frame* f : wait)
+        if ((s = c.wait(f)) != BORB_OK) return s;
+    const DistinctArgs A{(const uint8_t* const*)c.dev(o_src), (const int32_t*)c.dev(o_of), (const int32_t*)c.dev(o_oi), (const int32_t*)c.dev(o_o),
+                         n_points, (int32_t*)c.res(r_b, false), c.res(r_d, false)};
+    m->launches += launch_distinctive(A, m->stream);
+    if ((s = c.finish()) != BORB_OK) return s;
+    std::memcpy(best_idx, c.out(r_b), (size_t)n_points * 4);
+    for (int p = 0; p < n_points; p++)
+        if (best_idx[p] >= 0) std::memcpy(desc_out + (size_t)p * 32, c.out(r_d) + (size_t)p * 32, 32);
     return BORB_OK;
 }
 

@@ -270,31 +270,37 @@ __global__ void __launch_bounds__(256) project_points_batch_kernel(const LastArg
     if (i < L.n_last) project_point(L, i);
 }
 
+// Row o of the observations of DistinctArgs: through the (source, row) lookup, or row o of the single source src0.
+__device__ __forceinline__ const uint4* distinct_row(const DistinctArgs& A, const uint8_t* src0, int o) {
+    const uint8_t* r = A.obs_src ? A.src[A.obs_src[o]] + (size_t)A.obs_row[o] * 32 : src0 + (size_t)o * 32;
+    return reinterpret_cast<const uint4*>(r);
+}
+
 // MapPoint::ComputeDistinctiveDescriptors (src/MapPoint.cc:242-307), batched: a warp per MapPoint, a lane per row of the
 // distance matrix.  The row median (sorted row[(int)(0.5*(N-1))], self-distance included) comes from a 257-bin counting
-// histogram kept in local memory; first minimal median wins (lowest row index).
-__global__ void __launch_bounds__(128) distinctive_kernel(const uint8_t* __restrict__ desc, const int32_t* __restrict__ offsets,
-                                                          int n_points, int32_t* __restrict__ best_idx) {
+// histogram kept in local memory; first minimal median wins (lowest row index).  The rows are the staged host rows of
+// borb_distinctive_descriptors (one source, read in order) or rows of resident frames (borb_distinctive_descriptors_frames).
+__global__ void __launch_bounds__(128) distinctive_kernel(const DistinctArgs A) {
     const int lane = threadIdx.x & 31;
     const int pt = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    if (pt >= n_points) return;
-    const int o0 = offsets[pt], N = offsets[pt + 1] - o0;
-    if (N <= 0) { if (lane == 0) best_idx[pt] = -1; return; }
-    const uint32_t* D = reinterpret_cast<const uint32_t*>(desc) + (size_t)o0 * 8;
+    if (pt >= A.n_points) return;
+    const int o0 = A.offsets[pt], N = A.offsets[pt + 1] - o0;
+    if (N <= 0) { if (lane == 0) A.best_idx[pt] = -1; return; }
+    const uint8_t* src0 = A.obs_src ? nullptr : A.src[0];
     const int k = (int)(0.5 * (double)(N - 1));
     unsigned bestKey = 0xFFFFFFFFu;                              // median << 20 | row
     for (int i = lane; i < N; i += 32) {
         uint16_t hist[257];
 #pragma unroll 1
         for (int b = 0; b < 257; b++) hist[b] = 0;
-        uint32_t a[8];
-#pragma unroll
-        for (int w = 0; w < 8; w++) a[w] = D[(size_t)i * 8 + w];
+        const uint4* ra = distinct_row(A, src0, o0 + i);
+        const uint4 a0 = ra[0], a1 = ra[1];
 #pragma unroll 1
         for (int j = 0; j < N; j++) {
-            int d = 0;
-#pragma unroll
-            for (int w = 0; w < 8; w++) d += __popc(a[w] ^ D[(size_t)j * 8 + w]);
+            const uint4* rb = distinct_row(A, src0, o0 + j);
+            const uint4 b0 = rb[0], b1 = rb[1];
+            const int d = __popc(a0.x ^ b0.x) + __popc(a0.y ^ b0.y) + __popc(a0.z ^ b0.z) + __popc(a0.w ^ b0.w) +
+                          __popc(a1.x ^ b1.x) + __popc(a1.y ^ b1.y) + __popc(a1.z ^ b1.z) + __popc(a1.w ^ b1.w);
             hist[d]++;
         }
         int cum = 0, median = 256;
@@ -306,7 +312,10 @@ __global__ void __launch_bounds__(128) distinctive_kernel(const uint8_t* __restr
         bestKey = min(bestKey, ((unsigned)median << 20) | (unsigned)i);
     }
     bestKey = warp_min(bestKey);
-    if (lane == 0) best_idx[pt] = (int)(bestKey & 0xFFFFFu);
+    const int best = (int)(bestKey & 0xFFFFFu);
+    if (lane == 0) A.best_idx[pt] = best;
+    if (A.desc_out && lane < 8)
+        reinterpret_cast<uint32_t*>(A.desc_out)[(size_t)pt * 8 + lane] = reinterpret_cast<const uint32_t*>(distinct_row(A, src0, o0 + best))[lane];
 }
 
 // KeyFrameDatabase query (src/KeyFrameDatabase.cc:76-197, 199-310): for every keyframe of the device-resident database,
@@ -823,8 +832,8 @@ int launch_kfdb_score(const KfdbQueryJob* d_jobs, int n_jobs, int max_slots, int
     }
     return 1;
 }
-int launch_distinctive(const uint8_t* desc, const int32_t* offsets, int n_points, int32_t* best_idx, cudaStream_t s) {
-    if (n_points > 0) distinctive_kernel<<<(n_points + 3) / 4, 128, 0, s>>>(desc, offsets, n_points, best_idx);
+int launch_distinctive(const DistinctArgs& A, cudaStream_t s) {
+    if (A.n_points > 0) distinctive_kernel<<<(A.n_points + 3) / 4, 128, 0, s>>>(A);
     return 1;
 }
 int launch_point_projection_batch(const LastArgs* d_last, const ProjArgs* d_jobs, const LastArgs& one_last, const ProjArgs& one, int n_jobs,

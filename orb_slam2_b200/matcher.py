@@ -698,6 +698,26 @@ class ORBmatcher:
         check(self._lib.borb_distinctive_descriptors(self._h, _p(desc), _p(off), len(groups), _p(best)), "borb_distinctive_descriptors")
         return best[:len(groups)]
 
+    def ComputeDistinctiveDescriptorsFrames(self, frames, groups) -> Tuple[np.ndarray, np.ndarray]:
+        """borb_distinctive_descriptors_frames: ComputeDistinctiveDescriptors of many MapPoints (any number of streams) read from
+        resident keyframes, no keyframe row crossing PCIe.  frames = ResidentFrames, or FrameViews carrying one; groups[p] = (frame
+        indices, feature indices) of MapPoint p's non-bad observations in mObservations order.  Returns (best[p], descriptors
+        (n_points,32)): best as ComputeDistinctiveDescriptors on the gathered rows, and the chosen row (zeros where best is -1)."""
+        rfs = [F.resident if isinstance(F, FrameView) else F for F in frames]
+        handles = (C.c_void_p * max(len(rfs), 1))(*[rf._h.value if rf is not None else None for rf in rfs])
+        fi = [np.asarray(f, np.int32).reshape(-1) for f, _ in groups]
+        ki = [np.asarray(k, np.int32).reshape(-1) for _, k in groups]
+        assert all(len(a) == len(b) for a, b in zip(fi, ki))
+        off = np.zeros(len(groups) + 1, np.int32)
+        off[1:] = np.cumsum([len(a) for a in fi])
+        obs_f = np.ascontiguousarray(np.concatenate(fi)) if off[-1] > 0 else np.zeros(1, np.int32)
+        obs_k = np.ascontiguousarray(np.concatenate(ki)) if off[-1] > 0 else np.zeros(1, np.int32)
+        best = np.full(max(len(groups), 1), -1, np.int32)
+        desc = np.zeros((max(len(groups), 1), 32), np.uint8)
+        check(self._lib.borb_distinctive_descriptors_frames(self._h, handles, len(rfs), _p(obs_f), _p(obs_k), _p(off), len(groups), _p(best),
+                                                            _p(desc)), "borb_distinctive_descriptors_frames")
+        return best[:len(groups)], desc[:len(groups)]
+
     def Fuse(self, pKF: FrameView, P: WorldPointsView, Tcw: np.ndarray, Ow: np.ndarray, K: Tuple[float, float, float, float], bf: float,
              th: float = 3.0, Scw: bool = False) -> Tuple[int, np.ndarray]:
         """Search part of Fuse(pKF, vpMapPoints, th) — src/ORBmatcher.cc:825-970 — or, with Scw=True, of
