@@ -327,13 +327,13 @@ struct BowTables {                // a BowVector (word order) and a FeatureVecto
     uint32_t* idx;
 };
 
-struct BowFrameJob {              // one frame of borb_frames_compute_bow (bow_transform_batch_kernel, bow_build_kernel)
-    const uint8_t* desc;          // the resident frame's descriptors
+struct BowFrameJob {              // one frame of a BoW call (bow_transform_batch_kernel, bow_build_kernel)
+    const uint8_t* desc;          // a resident frame's descriptors, or staged host ones
     int n;
-    int32_t* word;                // scratch: word id, word weight, node id per feature (the descent's output)
-    double* weight;
+    int32_t* word;                // word id, word weight, node id per feature (the descent's output): scratch, or the results of
+    double* weight;               // a descent-only call
     int32_t* node;
-    BowTables dst;                // the frame's storage
+    BowTables dst;                // a resident frame's storage, or result slots
     BowTables copy;               // the same tables again, for the host (may be unset)
     int32_t* counts;              // n_bow, n_nodes, fv_start[n_nodes]
 };
@@ -388,9 +388,7 @@ void launch_fuse_search(const FuseJob* d_jobs, int n_jobs, int max_nq, cudaStrea
 // 2j + 1), then sim3_agree_batch_kernel over d_jobs; max_nq = most points of a direction, max_n1 = most KF1 features of a job
 int launch_sim3_batch(const LastArgs* d_last, const FuseJob* d_dirs, const Sim3AgreeJob* d_jobs, int n_jobs, int max_nq, int max_n1,
                       cudaStream_t s);
-int launch_bow_transform(const VocDev& V, const uint8_t* desc, int n, int levelsup, int32_t* word, double* weight, int32_t* node,
-                         cudaStream_t s);
-// descent + bookkeeping for n_frames frames (a job table in device memory): 2 launches
-int launch_bow_frames(const VocDev& V, const BowFrameJob* d_jobs, int n_frames, int max_n, int levelsup, cudaStream_t s);
+// descent + bookkeeping for n_frames frames (a job table the kernels can read): 2 launches, descent_only: 1
+int launch_bow_frames(const VocDev& V, const BowFrameJob* d_jobs, int n_frames, int max_n, int levelsup, bool descent_only, cudaStream_t s);
 
 }  // namespace borb

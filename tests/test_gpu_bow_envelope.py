@@ -90,15 +90,24 @@ def test_transform_and_compute_bow_equal_port(oracle, vocs, mt, name):
 
 
 def test_compute_bow_sizes_equal_port(oracle, vocs, mt):
-    a, pv, vt, _ = vocs["weights"]
+    """Every ComputeBoW size up to 8192 features; past it the descent alone still equals the port, and borb_compute_bow refuses
+    the frame (bow_build_kernel's keys of 8193 features would need 256 KB of shared memory)."""
+    a, pv, vt, va = vocs["weights"]
     sets = [BE.compute_set(n) for n in BE.COMPUTE_SIZES] + [BE.compute_set(n, True) for n in (1, 1025, 8192)]
     frames = [resident(mt, _keys(len(d), i), d) for i, d in enumerate(sets)]
+    big = BE.compute_set(10000)
     for levelsup in (0, 1, 2):
         got = mt.ComputeBoWBatch(vt, frames, levelsup)
         for d, g in zip(sets, got):
             want = BE.port_transform(oracle, pv, d, levelsup)[:2]
             same_bow(g, want)
             same_bow(vt.ComputeBoW(d, levelsup), want)
+        want_raw = pv.transform_raw(big, levelsup)
+        for voc in (vt, va):
+            assert all(np.array_equal(g, w) for g, w in zip(voc.transform_raw(big, levelsup), want_raw)), levelsup
+    with pytest.raises(BorbError) as ei:
+        vt.ComputeBoW(BE.compute_set(BE.MATCH_MAX_FEATURES + 1), 0)
+    assert ei.value.status == 1 and f"limit {BE.MATCH_MAX_FEATURES}" in str(ei.value), str(ei.value)
 
 
 def test_child_rank_limit_is_refused_naming_the_node():

@@ -102,16 +102,18 @@ def bow_race(M, oracle, voc, pv, descs, sizes_of):
 
 
 def test_shared_vocabulary_fixed_scratch(M, oracle, descriptor_sets):
-    """Six threads transform on one vocabulary whose scratch was sized beforehand by the largest set, so nothing is reallocated
-    during the race: without the vocabulary's lock the calls overwrite each other's descriptors and results in the one staging
-    buffer."""
+    """Six threads transform on one vocabulary whose buffers were sized beforehand by both calls on the largest set, so nothing is
+    reallocated during the race: without the vocabulary's lock the calls overwrite each other's descriptors and results in the
+    one set of buffers."""
+    from orb_slam2_b200.matcher import bow_and_featvec
     pv = oracle.PortVocabulary.random(10, 4, 5)
     voc = voc_of(M, pv)
     descs = [d for _, d in descriptor_sets]
     big = max(range(len(descs)), key=lambda t: len(descs[t]))
     sizes = lambda t, r: min(len(descs[t]), 200 + ((7 * t + 3 * r) % 10) * 200)
-    single = voc.transform_raw(descs[big], LEVELSUP)                      # sizes the scratch for every call below
-    assert same_raw(single, pv.transform_raw(descs[big], LEVELSUP))
+    raw = pv.transform_raw(descs[big], LEVELSUP)
+    assert same_raw(voc.transform_raw(descs[big], LEVELSUP), raw)          # these two size the buffers for every call below
+    assert same_bow(voc.ComputeBoW(descs[big], LEVELSUP), bow_and_featvec(*raw))
     errors, mismatched, total, want = bow_race(M, oracle, voc, pv, descs, sizes)
     assert not errors, errors
     assert not mismatched, f"{len(mismatched)} of {total} calls differ from the port, e.g. {mismatched[:6]}"
@@ -132,7 +134,7 @@ def test_shared_vocabulary_growing_scratch(M, oracle, descriptor_sets):
 
 
 def test_shared_vocabulary_host_and_resident_paths(M, oracle, descriptor_sets):
-    """One thread runs the host path (borb_compute_bow, the only user of the vocabulary's scratch) while the others run
+    """One thread runs the host path (borb_compute_bow, on the vocabulary's buffers and stream) while the others run
     ComputeBoWBatch on their own resident frames with their own matchers; both paths equal the port."""
     from orb_slam2_b200.matcher import bow_and_featvec
     pv = oracle.PortVocabulary.random(10, 4, 5)
