@@ -145,8 +145,8 @@ borb_status build_geometry(borb_extractor* e, int w, int h, std::vector<int16_t>
     const int L = e->cfg.n_levels;
     g.nlevels = L; g.w = w; g.h = h;
     g.fast_mode = e->fast_mode;
-    g.ini_th = e->cfg.ini_th_fast < 0 ? 0 : (e->cfg.ini_th_fast > 255 ? 255 : e->cfg.ini_th_fast);
-    g.min_th = e->cfg.min_th_fast < 0 ? 0 : (e->cfg.min_th_fast > 255 ? 255 : e->cfg.min_th_fast);
+    g.ini_th = e->cfg.ini_th_fast;          // in [0, 255]: borb_extractor_create refuses anything else
+    g.min_th = e->cfg.min_th_fast;
     for (int i = 0; i < 16; i++) g.umax[i] = e->umax[i];
     unsigned pyr_off = 0, cand_off = 0;
     int blk = 0, sel_off = 0, btile = 0;
@@ -596,6 +596,16 @@ borb_status borb_extractor_create(const borb_extractor_cfg* cfg, int device, bor
     *out = nullptr;
     if (cfg->n_levels < 1 || cfg->n_levels > BORB_MAX_LEVELS || cfg->n_features < 1 || !(cfg->scale_factor > 1.0f)) {
         set_error("bad extractor cfg (n_features=%d scale=%f levels=%d)", cfg->n_features, cfg->scale_factor, cfg->n_levels);
+        return BORB_ERR_INVALID_ARG;
+    }
+    // cv::FAST outside [0, 255] gives results that depend on the OpenCV build (its SIMD body wraps the threshold to a
+    // byte, its scalar tail does not), so there is no reference behaviour to reproduce there
+    if (cfg->ini_th_fast < 0 || cfg->ini_th_fast > 255) {
+        set_error("ini_th_fast %d outside [0, 255]", cfg->ini_th_fast);
+        return BORB_ERR_INVALID_ARG;
+    }
+    if (cfg->min_th_fast < 0 || cfg->min_th_fast > 255) {
+        set_error("min_th_fast %d outside [0, 255]", cfg->min_th_fast);
         return BORB_ERR_INVALID_ARG;
     }
     int ndev = 0;

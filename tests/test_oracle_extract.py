@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 from orb_slam2_b200 import synth
+from tests import extract_config as XC
 
 SHAPES = [(synth.KITTI, 2000), (synth.TUM, 1000), (synth.EUROC, 1200)]
 
@@ -105,14 +106,19 @@ def _cells_cv2(level_img, ini_th=20, min_th=7):
 
 @pytest.mark.parametrize("shape", [synth.KITTI, synth.TUM, (179, 134), (719, 217)])
 def test_whole_level_candidates_equal_per_cell_cv2(oracle, shape):
+    """At the default thresholds and at every pair of tests/extract_config.py (0, 127/128, 255, ini == min, ini < min); at
+    the TUM shape also on that module's exact-score dot images."""
     w, h = shape
-    for img in (synth.mono_frame(6, 0, 0, w, h), synth.white_noise(2, w, h),
-                (synth.mono_frame(7, 0, 0, w, h) // 8 + 100).astype(np.uint8)):   # low contrast: fallback cells
-        P = oracle.PortExtractor(1000)
-        P(img)
-        got = [tuple(r) for r in P.candidates(0).tolist()]
-        want = _cells_cv2(img)
-        assert got == want
+    imgs = (synth.mono_frame(6, 0, 0, w, h), synth.white_noise(2, w, h),
+            (synth.mono_frame(7, 0, 0, w, h) // 8 + 100).astype(np.uint8))   # low contrast: fallback cells
+    for ini, mn in [(20, 7)] + XC.THRESHOLD_PAIRS:
+        dots = [XC.threshold_dots(ini, mn, b)[0] for b in (True, False)] if shape == XC.THRESHOLD_SIZE else []
+        for img in list(imgs) + dots:
+            P = oracle.PortExtractor(1000, 1.2, 8, ini, mn)
+            P(img)
+            got = [tuple(r) for r in P.candidates(0).tolist()]
+            want = _cells_cv2(img, ini, mn)
+            assert got == want, (ini, mn)
 
 
 @pytest.mark.parametrize("N", [5, 60, 434, 869])

@@ -71,8 +71,9 @@ def _cv_fast(img, th):
     return [(int(k.pt[0]), int(k.pt[1]), int(k.response)) for k in det.detect(img, None)]
 
 
-@pytest.mark.parametrize("th", [20, 7, 12, 1])
+@pytest.mark.parametrize("th", range(256))
 def test_fast_matches_cv2(lib, th):
+    """Every threshold the extractor accepts (0..255): the reject's constants change at 0, 127/128 and 255."""
     for (w, h) in [(37, 38), (36, 35), (200, 120), (7, 7), (8, 30)]:
         for seed in range(3):
             base = synth.white_noise(seed, w, h) if seed else synth.mono_frame(9, 0, 0, max(w, 64), max(h, 64))[:h, :w].copy()
