@@ -265,7 +265,8 @@ BORB_API borb_status borb_frames_from_extractor(borb_matcher* m, borb_extractor*
                                                 float* u_right, float* depth_out, int cap, float* bounds4, borb_frame** frames);
 BORB_API borb_status borb_frame_info(const borb_frame* f, int32_t* n, int32_t* n_levels, int32_t* has_u_right);
 /* Read-only introspection of a resident frame (tests, debugging): waits for the frame to be complete and copies mvKeysUn (n),
- * mDescriptors (n x 32), mvuRight / mvDepth (n; BORB_ERR_INVALID_ARG on a monocular frame) and the feature grid of
+ * mDescriptors (n x 32), mvuRight / mvDepth (n; BORB_ERR_INVALID_ARG on a monocular frame, and for mvDepth on a frame made by
+ * borb_frame_create, whose view carries no depth) and the feature grid of
  * Frame::AssignFeaturesToGrid flattened: cell_start[64*48 + 1], cell c = x*48 + y holding cell_idx[cell_start[c] ..
  * cell_start[c+1]) in insertion order; cell_idx needs room for n entries (cell_start[64*48] are written: features whose
  * PosInGrid fails are in no cell).  Any pointer may be NULL. */
@@ -898,6 +899,10 @@ BORB_API borb_status borb_debug_eval_math(int fn, const float* a, const float* b
  * 1 = full carry-save adder tree + 4 POPC, 0 = 8 POPC.  Same results; kept switchable for measurements.  Applies to the
  * relocalisation search (borb_search_by_bow_db*); the loop-closure search (borb_search_by_bow_kf_db_*) always uses mode 2. */
 BORB_API borb_status borb_debug_set_bow_csa(int mode);
+/* Fills every buffer the library reuses or recycles with `byte` (0..255) before a call writes it, -1 (the default) stops: matcher
+ * and vocabulary staging, arena and landing buffers, resident frame and keyframe blocks, the extractor workspace (DESIGN.md, "Buffer
+ * reuse").  Process-wide; for tests that pin results to the unpoisoned run.  Other values give BORB_ERR_INVALID_ARG. */
+BORB_API borb_status borb_debug_set_poison(int byte);
 /* Work-item size of the same kernel: keyframes per item = target / (bucket width)^2, clamped to [1, 32] (default 2560); a negative
  * target selects the static item-to-warp schedule instead of the atomic work counter. */
 BORB_API borb_status borb_debug_set_bow_item_target(int target);

@@ -21,6 +21,8 @@ void set_error(const char* fmt, ...) {
     tl_error = buf;
 }
 
+std::atomic<int> g_poison{-1};
+
 bool allow_max_smem(const void* func) {
     static std::mutex mu;
     static std::vector<std::pair<const void*, int>> done;
@@ -273,6 +275,48 @@ borb_status ensure(borb_extractor* e, int w, int h, int n_images) {
     return BORB_OK;
 }
 
+// borb_debug_set_poison: an extraction step fills the per-image buffers it rewrites, on the handle's stream before its upload, so
+// that no result can depend on what an earlier step left there.  Not filled, because they are carried from step to step on
+// purpose: tabs (resize tables) and fast_tiles / fast_tmaps (FAST tile tables), built once per geometry; brief_slots (rBRIEF tap
+// order); the rectification maps d_map; pair_idx, uploaded only when pair_cache changes.  u_right, depth, sad, st_bins and
+// st_recs are the stereo association's (poison_stereo): borb_stereo_match and borb_frames_from_extractor read the association
+// of the previous extraction.
+borb_status poison_extract(borb_extractor* e) {
+    const int p = poison_byte();
+    if (p < 0) return BORB_OK;
+    const Geometry& g = e->geom;
+    Workspace& ws = e->ws;
+    const size_t n = (size_t)ws.max_images;
+    cudaStream_t s = e->stream;
+    if (ws.stage) BORB_CUDA(cudaMemsetAsync(ws.stage, p, ws.stage_bytes, s));
+    BORB_CUDA(cudaMemsetAsync(ws.pyr, p, n * g.pyr_image_stride + 256, s));       // the slack included
+    BORB_CUDA(cudaMemsetAsync(ws.blur, p, n * g.pyr_image_stride + 256, s));
+    BORB_CUDA(cudaMemsetAsync(ws.cand, p, n * g.cand_image_stride * sizeof(uint32_t), s));
+    BORB_CUDA(cudaMemsetAsync(ws.pnode, p, n * g.cand_image_stride * sizeof(int), s));
+    BORB_CUDA(cudaMemsetAsync(ws.cand_cnt, p, n * g.nlevels * sizeof(int), s));
+    BORB_CUDA(cudaMemsetAsync(ws.sel, p, n * g.sel_image_stride * sizeof(uint32_t), s));
+    BORB_CUDA(cudaMemsetAsync(ws.sel_cnt, p, n * g.nlevels * sizeof(int), s));
+    BORB_CUDA(cudaMemsetAsync(ws.kps, p, n * g.sel_image_stride * sizeof(borb_keypoint), s));
+    BORB_CUDA(cudaMemsetAsync(ws.desc, p, n * g.sel_image_stride * 32, s));
+    BORB_CUDA(cudaMemsetAsync(ws.nkp, p, n * sizeof(int), s));
+    return BORB_OK;
+}
+
+// borb_debug_set_poison: each stereo association fills its own outputs and scratch at its start (see poison_extract).
+borb_status poison_stereo(borb_extractor* e) {
+    const int p = poison_byte();
+    if (p < 0) return BORB_OK;
+    Workspace& ws = e->ws;
+    const size_t n = (size_t)ws.max_images * e->geom.sel_image_stride;
+    cudaStream_t s = e->stream;
+    BORB_CUDA(cudaMemsetAsync(ws.u_right, p, n * sizeof(float), s));
+    BORB_CUDA(cudaMemsetAsync(ws.depth, p, n * sizeof(float), s));
+    BORB_CUDA(cudaMemsetAsync(ws.sad, p, n * sizeof(int), s));
+    BORB_CUDA(cudaMemsetAsync(ws.st_bins, p, (size_t)ws.max_images * stereo_bins_bytes_per_pair(), s));
+    BORB_CUDA(cudaMemsetAsync(ws.st_recs, p, ws.st_recs_bytes, s));
+    return BORB_OK;
+}
+
 void drain_timing(borb_extractor* e);
 void begin_step(borb_extractor* e) {
     if (!e->timing) return;
@@ -369,6 +413,7 @@ borb_status upload_slots(borb_extractor* e, const uint8_t* const* slots, int n, 
             e->ws.stage = nullptr; e->ws.stage_bytes = 0;
             BORB_CUDA(cudaMalloc(&e->ws.stage, need));
             e->ws.stage_bytes = need;
+            if (poison_byte() >= 0) BORB_CUDA(cudaMemsetAsync(e->ws.stage, poison_byte(), need, e->stream));
         }
         return BORB_OK;
     };
@@ -496,6 +541,8 @@ borb_status enqueue_stereo(borb_extractor* eL, borb_extractor* eR, int n_pairs, 
         BORB_CUDA(cudaMalloc(&e->ws.st_recs, rec_bytes));
         e->ws.st_recs_bytes = rec_bytes;
     }
+    const borb_status pst = poison_stereo(e);
+    if (pst != BORB_OK) return pst;
     StereoView L{eL->ws.pyr, eL->ws.kps, eL->ws.desc, eL->ws.nkp, eL->geom.pyr_image_stride, eL->geom.sel_image_stride};
     StereoView R{eR->ws.pyr, eR->ws.kps, eR->ws.desc, eR->ws.nkp, eR->geom.pyr_image_stride, eR->geom.sel_image_stride};
     mark(e, 6);
@@ -557,6 +604,12 @@ const std::vector<uint32_t>& brief_slot_table() {
 using namespace borb;
 
 extern "C" {
+
+borb_status borb_debug_set_poison(int byte) {
+    if (byte < -1 || byte > 255) { set_error("poison byte %d outside [-1, 255]", byte); return BORB_ERR_INVALID_ARG; }
+    g_poison.store(byte, std::memory_order_relaxed);
+    return BORB_OK;
+}
 
 const char* borb_last_error(void) { return tl_error.c_str(); }
 const char* borb_status_str(borb_status s) {
@@ -689,6 +742,7 @@ borb_status borb_extract_batch_enqueue(borb_extractor* e, const uint8_t* const* 
     int gw = w, gh = h;
     if ((st = rectified_size(e, w, h, &gw, &gh)) != BORB_OK) return st;
     if ((st = ensure(e, gw, gh, n)) != BORB_OK) return st;
+    if ((st = poison_extract(e)) != BORB_OK) return st;
     begin_step(e);
     mark(e, 0);
     if ((st = upload_slots(e, gray, n, w, h, stride)) != BORB_OK) return st;
@@ -729,6 +783,7 @@ borb_status borb_extract_batch_device(borb_extractor* e, const uint8_t* d_gray, 
     int gw = w, gh = h;
     if ((st = rectified_size(e, w, h, &gw, &gh)) != BORB_OK) return st;
     if ((st = ensure(e, gw, gh, n)) != BORB_OK) return st;
+    if ((st = poison_extract(e)) != BORB_OK) return st;
     begin_step(e);
     mark(e, 0);
     if ((st = upload_device(e, d_gray, n, w, h, pitch, image_stride)) != BORB_OK) return st;
@@ -960,6 +1015,7 @@ borb_status borb_stereo_frames_enqueue(borb_extractor* e, const uint8_t* const* 
     int gw = w, gh = h;
     if ((st = rectified_size(e, w, h, &gw, &gh)) != BORB_OK) return st;
     if ((st = ensure(e, gw, gh, 2 * n_pairs)) != BORB_OK) return st;
+    if ((st = poison_extract(e)) != BORB_OK) return st;
     begin_step(e);
     mark(e, 0);
     {
@@ -998,6 +1054,7 @@ borb_status borb_stereo_frames_device_enqueue(borb_extractor* e, const uint8_t* 
     int gw = w, gh = h;
     if ((st = rectified_size(e, w, h, &gw, &gh)) != BORB_OK) return st;
     if ((st = ensure(e, gw, gh, 2 * n_pairs)) != BORB_OK) return st;
+    if ((st = poison_extract(e)) != BORB_OK) return st;
     begin_step(e);
     mark(e, 0);
     if ((st = upload_device(e, d_gray, 2 * n_pairs, w, h, pitch, image_stride, true)) != BORB_OK) return st;

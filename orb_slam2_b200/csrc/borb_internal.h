@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <atomic>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -10,6 +11,10 @@
 #include "../../include/borb.h"
 
 namespace borb {
+
+// borb_debug_set_poison: -1 = off (default), 0..255 = the byte that fills reused and recycled buffers before each call writes them
+extern std::atomic<int> g_poison;
+inline int poison_byte() { return g_poison.load(std::memory_order_relaxed); }
 
 constexpr int EDGE = 19;          // EDGE_THRESHOLD   (ORBextractor.cc:74)
 constexpr int PATCH = 31;         // PATCH_SIZE       (:72)

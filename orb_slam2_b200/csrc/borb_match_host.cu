@@ -82,6 +82,11 @@ public:
         if ((s = grow_pinned(b_->h_stage, b_->h_bytes, in_end_)) != BORB_OK) return s;
         if (res_bytes_ && (s = grow_pinned(b_->h_out, b_->h_out_bytes, res_bytes_ + 4096)) != BORB_OK) return s;
         BORB_CUDA(cudaStreamSynchronize(b_->stream));   // the staging buffer may still feed an earlier copy
+        if (const int p = poison_byte(); p >= 0) {      // borb_debug_set_poison: everything this call has not written yet
+            std::memset(b_->h_stage, p, in_end_);        // the alignment gaps between the inputs included
+            std::memset(b_->h_out, p, res_bytes_);
+            BORB_CUDA(cudaMemsetAsync(b_->arena + in_end_, p, off_ - in_end_, b_->stream));
+        }
         for (const Item& it : items_)
             if (it.src) std::memcpy(b_->h_stage + it.off, it.src, it.bytes);
         begun_ = true;
@@ -508,13 +513,19 @@ borb_status frame_alloc(int device, int n, int n_levels, bool stereo, borb_frame
         f->bow_value = (double*)(f->block + o_bv); f->bow_word = (uint32_t*)(f->block + o_bw); f->fv_node = (uint32_t*)(f->block + o_fn);
         f->fv_start = (int32_t*)(f->block + o_fs); f->fv_idx = (uint32_t*)(f->block + o_fi);
     }
-    f->has_bow = false;                 // a new frame, or a recycled block that still holds another frame's vectors
+    f->has_bow = false;                // a new frame, or a recycled block that still holds another frame's vectors
     f->n_bow = f->n_nodes = f->n_fv = 0;
     // u_right / depth storage always exists; the pointers are nulled for a monocular frame
     f->u_right = stereo ? f->ur_store : nullptr;
     f->depth = stereo ? f->depth_store : nullptr;
     f->n = n; f->n_levels = n_levels;
     *out = f;
+    return BORB_OK;
+}
+// borb_debug_set_poison: the whole block of a frame handed out by frame_alloc, new or recycled, on the stream that then writes it
+borb_status poison_frame(const borb_frame* f, cudaStream_t s) {
+    const int p = poison_byte();
+    if (p >= 0) BORB_CUDA(cudaMemsetAsync(f->block, p, f->block_bytes, s));
     return BORB_OK;
 }
 }  // namespace
@@ -530,6 +541,7 @@ borb_status borb_frame_create(borb_matcher* m, const borb_frame_view* v, borb_fr
     BORB_CUDA(cudaSetDevice(m->device));
     borb_frame* f = nullptr;
     if ((s = frame_alloc(m->device, I.n, I.n_levels, v->u_right != nullptr, &f)) != BORB_OK) return s;
+    f->depth = nullptr;                 // a view carries mvuRight but no mvDepth: nothing is written to depth_store
     f->min_x = I.min_x; f->min_y = I.min_y; f->max_x = I.max_x; f->max_y = I.max_y;
     Call c(m);
     const size_t o_k = c.in(v->keys_un, (size_t)I.n * sizeof(borb_keypoint)), o_d = c.in(v->desc, (size_t)I.n * 32);
@@ -537,6 +549,7 @@ borb_status borb_frame_create(borb_matcher* m, const borb_frame_view* v, borb_fr
     const size_t o_s = c.in(v->scale_factors, (size_t)I.n_levels * 4);
     if ((s = c.begin()) != BORB_OK || (s = c.commit()) != BORB_OK) { borb_frame_destroy(f); return s; }
     cudaStream_t q = m->stream;
+    if ((s = poison_frame(f, q)) != BORB_OK) return s;
     if (I.n > 0) {
         BORB_CUDA(cudaMemcpyAsync(f->keys, c.dev(o_k), (size_t)I.n * sizeof(borb_keypoint), cudaMemcpyDeviceToDevice, q));
         BORB_CUDA(cudaMemcpyAsync(f->desc, c.dev(o_d), (size_t)I.n * 32, cudaMemcpyDeviceToDevice, q));
@@ -631,6 +644,8 @@ borb_status borb_frames_from_extractor(borb_matcher* m, borb_extractor* e, const
     if (!m->ev_a) { BORB_CUDA(cudaEventCreateWithFlags(&m->ev_a, cudaEventDisableTiming)); BORB_CUDA(cudaEventCreateWithFlags(&m->ev_b, cudaEventDisableTiming)); }
     BORB_CUDA(cudaEventRecord(m->ev_a, e->stream));
     BORB_CUDA(cudaStreamWaitEvent(q, m->ev_a, 0));
+    for (int i = 0; i < n_frames; i++)
+        if ((s = poison_frame(frames[i], q)) != BORB_OK) return fail(s);
     if (mode == 2 && !depth_on_device)
         for (int i = 0; i < n_frames; i++)
             BORB_CUDA(cudaMemcpy2DAsync(c.dev(o_depth) + (size_t)i * depth_img_bytes, (size_t)w * px, depth[i], (size_t)depth_stride_bytes, (size_t)w * px, h,
@@ -663,6 +678,7 @@ borb_status borb_debug_frame_read(const borb_frame* f, borb_keypoint* keys, uint
                                   int32_t* cell_idx) {
     if (!f) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
     if ((u_right || depth) && !f->u_right) { set_error("a monocular frame has no mvuRight / mvDepth"); return BORB_ERR_INVALID_ARG; }
+    if (depth && !f->depth) { set_error("a frame made by borb_frame_create has no mvDepth"); return BORB_ERR_INVALID_ARG; }
     BORB_CUDA(cudaSetDevice(f->device));
     BORB_CUDA(cudaEventSynchronize(f->ready));
     const size_t n = (size_t)f->n;
@@ -1886,7 +1902,8 @@ borb_status borb_kfdb_add(borb_kfdb* db, const borb_keyframe_view* kf, const uin
     if (n_bow) { std::memcpy(&h[L.bow_word], bow_word, (size_t)n_bow * 4); std::memcpy(&h[L.bow_value], bow_value, (size_t)n_bow * 8); }
     uint8_t* block = nullptr;
     BORB_CUDA(cudaMalloc(&block, L.bytes));
-    const cudaError_t ce = cudaMemcpy(block, h.data(), L.bytes, cudaMemcpyHostToDevice);
+    cudaError_t ce = poison_byte() >= 0 ? cudaMemset(block, poison_byte(), L.bytes) : cudaSuccess;   // borb_debug_set_poison
+    if (ce == cudaSuccess) ce = cudaMemcpy(block, h.data(), L.bytes, cudaMemcpyHostToDevice);
     if (ce != cudaSuccess) { cudaFree(block); BORB_CUDA(ce); }
     *slot_out = kfdb_append_locked(db, block, nn, m, kf->n, n_bow, meta);
     return BORB_OK;
@@ -1946,6 +1963,10 @@ static borb_status kfdb_sync_table(borb_kfdb* db) {
         db->table_cap = n + n / 2 + 64;
         BORB_CUDA(cudaMalloc(&db->d_table, db->table_cap * sizeof(BowDev)));
         BORB_CUDA(cudaMalloc(&db->d_stream, db->table_cap * sizeof(KfStream)));
+        if (const int p = poison_byte(); p >= 0) {      // borb_debug_set_poison: the entries past the live slots are never written
+            BORB_CUDA(cudaMemset(db->d_table, p, db->table_cap * sizeof(BowDev)));
+            BORB_CUDA(cudaMemset(db->d_stream, p, db->table_cap * sizeof(KfStream)));
+        }
     }
     std::vector<BowDev> t(n);
     std::vector<KfStream> st(n);
@@ -2272,6 +2293,8 @@ borb_status borb_kfdb_add_frames(borb_matcher* m, const borb_kfdb_add_job* jobs,
         const borb_frame* f = jobs[j].frame;
         const cudaError_t e = cudaMalloc(&blocks[j], kfdb_block_layout(f->n_nodes, f->n_fv, f->n_bow).bytes);
         if (e != cudaSuccess) { blocks[j] = nullptr; set_error("job %d: keyframe block allocation failed: %s", j, cudaGetErrorString(e)); return fail(BORB_ERR_CUDA); }
+        if (poison_byte() >= 0)                          // borb_debug_set_poison, ahead of kfdb_insert_kernel on the same stream
+            BORB_CUDA(cudaMemsetAsync(blocks[j], poison_byte(), kfdb_block_layout(f->n_nodes, f->n_fv, f->n_bow).bytes, m->stream));
     }
     borb_status s;
     if ((s = c.begin()) != BORB_OK) return fail(s);
