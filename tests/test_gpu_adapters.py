@@ -62,6 +62,13 @@ from tests import test_oracle_match_envelope as TE      # noqa: E402
 
 test_envelope_port_equals_reference = TE.test_port_equals_reference
 
+# the float decision-boundary cases through the adapters: their host arithmetic (the forward / backward decision from the two
+# poses, the Scw decomposition, S21 from s12, R12, t12) meets the boundaries as well as the kernels do
+from tests import test_oracle_proj_geometry as TG      # noqa: E402
+
+test_proj_geometry_port_equals_reference = TG.test_port_equals_reference
+test_proj_geometry_dense_port_equals_reference = TG.test_dense_port_equals_reference
+
 
 def test_adapters_reproduce_the_reference_golden_vectors(O):
     """tests/golden/match_ref.npz = outputs of the verbatim src/ORBmatcher.cc; the adapter library, driven through the same

@@ -38,14 +38,14 @@ def _cur(c):
 
 def run_gpu(mt, c, method, resident):
     """One method of case c on the CUDA library, in the form of proj_geometry.run_port's result."""
-    _set(mt)
+    _set(mt, ori=c.get("ori", False))
     F = c["F"].make_resident(mt) if resident and "F" in c else c.get("F")
     if method == "local":
         r = mt.SearchLocalPoints(F, c["P"], c["Tcw"], c["Ow"], c["K"], c["bf"], c["th"], has_obs=c["has_obs"], viewingCosLimit=c["vcl"])
         return r, r["nmatches"], r["match"]
     if method == "last":
         Cur = _cur(c).make_resident(mt) if resident else _cur(c)
-        return mt.SearchByProjectionLast(Cur, G.last_view(c), c["Tcw"], c["K"], c["bf"], c["th"])
+        return mt.SearchByProjectionLast(Cur, G.last_view(c), c["Tcw"], c["K"], c["bf"], c["th"], c.get("fwd", False), c.get("bwd", False))
     if method == "kf":
         return mt.SearchByProjectionKF(F, c["P"], c["Tcw"], c["Ow"], c["K"], c["th"], 100)
     if method == "sim3proj":
@@ -53,11 +53,14 @@ def run_gpu(mt, c, method, resident):
     if method in ("fuse", "fuse_kf"):
         T = G.scw(c) if method == "fuse" else c["Tcw"]
         return mt.Fuse(F, c["P"], T, c["Ow"], c["K"], c["bf"], c["th"], Scw=method == "fuse")
+    if method == "sim3" and "kind" in c:
+        KF1, KF2 = (c["KF1"].make_resident(mt), c["KF2"].make_resident(mt)) if resident else (c["KF1"], c["KF2"])
+        return mt.SearchBySim3(KF1, KF2, c["P1"], c["P2"], c["T1w"], c["T2w"], c["S12"], c["S21"], c["K"], c["th"])
     if method == "sim3":
         _, _, P1, P2, T1, T2, S12, S21, K, th = G.sim3_args(c)
         return mt.SearchBySim3(F, F, P1, P2, T1, T2, S12, S21, K, th)
     if method == "proj":
-        _set(mt, c["ratio"])
+        _set(mt, c["ratio"], c.get("ori", False))
         return mt.SearchByProjection(F, c["mps"], c["th"])
     if method == "tri":
         return mt.SearchForTriangulation(c["kf1"], c["kf2"], c["F12"], c["ep"], c["only_stereo"])
@@ -138,16 +141,74 @@ def test_projection_batch(M, mt, oracle):
 
 
 def test_last_frame_batch(M, mt, oracle):
-    """borb_search_by_projection_last_batch: every LastFrame case in one call, next to a LastFrame without points."""
-    _set(mt)
-    cs = _by("last")[None]
+    """borb_search_by_projection_last_batch: every LastFrame case in one call, each with its own forward / backward flags (the
+    three modes mixed), next to a LastFrame without points."""
+    groups = _by("last", lambda c: c.get("ori", False))
+    assert sorted(groups) == [False, True]
+    assert {(c.get("fwd", False), c.get("bwd", False)) for c in groups[False]} == {(True, False), (False, True), (False, False)}
+    for ori, cs in groups.items():
+        _last_frame_batch(M, mt, oracle, cs, ori)
+
+
+def _last_frame_batch(M, mt, oracle, cs, ori):
+    _set(mt, ori=ori)
     L0 = G.last_view(cs[0])
     empty = M.LastFrameView(L0.mvKeysUn[:0], L0.world_pos[:0], L0.descriptors[:0], L0.valid[:0], L0.has_obs[:0])
     curs = [_cur(c).make_resident(mt) for c in cs + cs[:1]]
     got = mt.SearchByProjectionLastBatch(curs, [G.last_view(c) for c in cs] + [empty], [c["Tcw"] for c in cs + cs[:1]], G.K_CAM, G.BF,
-                                         [c["th"] for c in cs + cs[:1]])
+                                         [c["th"] for c in cs + cs[:1]], forward=[c.get("fwd", False) for c in cs + cs[:1]],
+                                         backward=[c.get("bwd", False) for c in cs + cs[:1]])
     for j, c in enumerate(cs):
         assert _equal("last", got[j], G.run_port(oracle, c, "last")), (c["cls"], c["member"])
+    assert got[-1][0] == 0 and (got[-1][1] == -1).all()
+
+
+def test_keyframe_projection_batch(mt, oracle):
+    """borb_search_by_projection_kf_batch: every SearchByProjection(CurrentFrame, KeyFrame) case in one call, next to a keyframe
+    without points."""
+    for ori, cs in _by("kf", lambda c: c.get("ori", False)).items():
+        _set(mt, ori=ori)
+        curs = [c["F"].make_resident(mt) for c in cs + cs[:1]]
+        points = [c["P"] for c in cs] + [_empty_points(cs[0]["P"])]
+        got = mt.SearchByProjectionKFBatch(curs, points, [(c["Tcw"], c["Ow"]) for c in cs + cs[:1]], G.K_CAM, [c["th"] for c in cs + cs[:1]],
+                                           100)
+        for j, c in enumerate(cs):
+            assert _equal("kf", got[j], G.run_port(oracle, c, "kf")), (c["cls"], c["member"])
+        assert got[-1][0] == 0 and (got[-1][1] == -1).all()
+
+
+def test_sim3_projection_batch(mt, oracle):
+    """borb_search_by_projection_sim3_batch: every SearchByProjection(pKF, Scw) case in one call, next to a job without points."""
+    _set(mt)
+    cs = _by("sim3proj")[None]
+    kfs = [c["F"].make_resident(mt) for c in cs + cs[:1]]
+    points = [c["P"] for c in cs] + [_empty_points(cs[0]["P"])]
+    got = mt.SearchByProjectionSim3Batch(kfs, points, [(c["Tcw"], c["Ow"]) for c in cs + cs[:1]], G.K_CAM, [int(c["th"]) for c in cs + cs[:1]])
+    for j, c in enumerate(cs):
+        assert _equal("sim3proj", got[j], G.run_port(oracle, c, "sim3proj")), (c["cls"], c["member"])
+    assert got[-1][0] == 0 and (got[-1][1] == -1).all()
+
+
+def test_sim3_batch(mt, oracle):
+    """borb_search_by_sim3_batch: every SearchBySim3 case — the identity Sim3 of the world-point cases and the scaled, rotated
+    similarities of the sim3_* cases — in one call, next to a keyframe pair without MapPoints."""
+    _set(mt)
+    cs = _by("sim3")[None]
+    assert any("kind" in c for c in cs) and any("kind" not in c for c in cs)
+
+    def job(c):
+        if "kind" in c:
+            return c["KF1"], c["KF2"], c["P1"], c["P2"], (c["T1w"], c["T2w"]), (c["S12"], c["S21"]), c["th"]
+        F, _, P1, P2, T1, T2, S12, S21, _, th = G.sim3_args(c)
+        return F, F, P1, P2, (T1, T2), (S12, S21), th
+    jobs = [job(c) for c in cs]
+    none = lambda P: dataclasses.replace(P, valid=np.zeros(len(P.world_pos), np.uint8))
+    e = jobs[0]
+    jobs.append((e[0], e[1], none(e[2]), none(e[3]), e[4], e[5], e[6]))
+    got = mt.SearchBySim3Batch([j[0].make_resident(mt) for j in jobs], [j[1].make_resident(mt) for j in jobs], [j[2] for j in jobs],
+                               [j[3] for j in jobs], [j[4] for j in jobs], [j[5] for j in jobs], G.K_CAM, [j[6] for j in jobs])
+    for j, c in enumerate(cs):
+        assert _equal("sim3", got[j], G.run_port(oracle, c, "sim3")), (c["cls"], c["member"])
     assert got[-1][0] == 0 and (got[-1][1] == -1).all()
 
 
@@ -168,12 +229,26 @@ def test_fuse_batch(mt, oracle, scw):
 def test_triangulation_batch(mt, oracle):
     """borb_search_for_triangulation_batch: every SearchForTriangulation case in one call, next to a job whose keyframe features
     all have MapPoints (nothing to triangulate)."""
-    _set(mt)
-    cs = _by("tri")[None]
-    full = dataclasses.replace(cs[0]["kf1"], has_mp=np.ones(len(cs[0]["kf1"].mvKeysUn), np.uint8), _keep=[])
-    kf1s = [c["kf1"] for c in cs] + [full]
-    kf2s = [c["kf2"] for c in cs + cs[:1]]
-    got = mt.SearchForTriangulationBatch(kf1s, kf2s, [c["F12"] for c in cs + cs[:1]], [c["ep"] for c in cs + cs[:1]])
-    for j, c in enumerate(cs):
-        assert _equal("tri", got[j], G.run_port(oracle, c, "tri")), (c["cls"], c["member"])
-    assert len(got[-1]) == 0
+    for ori, cs in _by("tri", lambda c: c["ori"]).items():
+        _set(mt, ori=ori)
+        full = dataclasses.replace(cs[0]["kf1"], has_mp=np.ones(len(cs[0]["kf1"].mvKeysUn), np.uint8), _keep=[])
+        kf1s = [c["kf1"] for c in cs] + [full]
+        kf2s = [c["kf2"] for c in cs + cs[:1]]
+        got = mt.SearchForTriangulationBatch(kf1s, kf2s, [c["F12"] for c in cs + cs[:1]], [c["ep"] for c in cs + cs[:1]])
+        for j, c in enumerate(cs):
+            assert _equal("tri", got[j], G.run_port(oracle, c, "tri")), (c["cls"], c["member"])
+        assert len(got[-1]) == 0
+
+
+@pytest.mark.parametrize("cls", G.dense_classes())
+def test_dense_variants_equal_port(mt, oracle, cls):
+    """Both members of every world-point class inside a natural ~1000-point call (proj_geometry.dense_case), every method, on
+    host views and on resident frames."""
+    for c in G.cases():
+        if c["cls"] != cls or "kind" in c:
+            continue
+        d = G.dense_case(oracle, c)
+        for method in G.methods(d):
+            want = G.run_port(oracle, d, method)
+            for resident in (False, True):
+                assert _equal(method, run_gpu(mt, d, method, resident), want), (cls, c["member"], method, resident)

@@ -77,6 +77,27 @@ def test_reference_pose_arithmetic_is_restated(O):
             assert np.array_equal(bits(O.ref_camera_center(c["Tcw"])), bits(c["Ow"])), c["cls"]
     S12, S21 = O.ref_sim3_mats(1.0, np.eye(3, dtype=np.float32), np.zeros(3, np.float32))
     assert np.array_equal(bits(S12), bits(G.S12_ID)) and np.array_equal(bits(S21), bits(G.S21_ID))
+    for sim in (G.SIM_A, G.SIM_B):
+        S12, S21 = O.ref_sim3_mats(*sim)
+        mine = G.sim3_mats(*sim)
+        assert np.array_equal(bits(S12), bits(mine[0])) and np.array_equal(bits(S21), bits(mine[1]))
+    for c in G.cases():
+        if c.get("kind") == "sim3":
+            assert all(np.array_equal(bits(a), bits(b)) for a, b in zip(O.ref_sim3_mats(*c["sim"]), (c["S12"], c["S21"]))), c["cls"]
+
+
+def test_forward_backward_is_restated(O):
+    """The forward / backward flags the cases hand to the port and to the CUDA library are the reference's own decision
+    (ORBmatcher.cc:1338-1349) on the case's two poses."""
+    n = 0
+    for c in G.cases():
+        if "Tlast" in c:
+            assert O.ref_forward_backward(c["Tcw"], c["Tlast"], G.MB, False) == (c["fwd"], c["bwd"]), (c["cls"], c["member"])
+            assert G.forward_backward(c["Tcw"], c["Tlast"]) == (c["fwd"], c["bwd"])
+            n += 1
+    assert n == 2 * (len(G.LEVEL_PAIRS) + 2)
+    flags = {(c["fwd"], c["bwd"]) for c in G.cases() if "Tlast" in c}
+    assert flags == {(True, False), (False, True), (False, False)}
 
 
 def test_pairs_sit_on_their_bounds():
@@ -97,3 +118,84 @@ def test_pairs_sit_on_their_bounds():
     y = [cs["tri_dsqr", m]["kf1"].mvKeysUn["y"][0] for m in (0, 1)]
     o = cs["tri_dsqr", 0]["kf2"].mvKeysUn["octave"][0]
     assert [np.float32(v * v) < np.float32(np.float32(3.84) * G.SIGMA2[o]) for v in y] != [True, False]
+    # tlc.z == mb exactly in the rejected members of fwd_bwd_mb_*, one step beyond it in the kept ones
+    tlc = {k: G.cam_point(c["Tlast"], G.camera_centre(c["Tcw"]))[2] for k, c in cs.items() if k[0].startswith("fwd_bwd_mb")}
+    assert tlc["fwd_bwd_mb_fwd", 1] == G.MB and tlc["fwd_bwd_mb_fwd", 0] == G.step(G.MB, 1)
+    assert tlc["fwd_bwd_mb_bwd", 1] == -G.MB and tlc["fwd_bwd_mb_bwd", 0] == -G.step(G.MB, 1)
+    # PredictScale: the ratio of the lower member is sf^2 as the float pyramid holds it, the upper member's one step above
+    a, b = G.predict_scale_pair()
+    assert np.float32(a / dist) == np.float32(G.SCALE[2] / G.SCALE[0]) and G.predict_scale(a, dist) == G.PS_LEVEL
+    assert G.predict_scale(b, dist) == G.PS_LEVEL + 1
+    # SearchBySim3: dist3D is the norm of the chained camera-frame point, and the kept member sits on the bound
+    d3, (mn, _), (_, mx) = G.sim3_dist_pairs()
+    for side in (12, 21):
+        c = cs[f"sim3_min_dist_{side}", 0]
+        P, T, S = (c["P1"], c["T1w"], c["S21"]) if side == 12 else (c["P2"], c["T2w"], c["S12"])
+        pc = G.sim3_chain(T, S, P.world_pos[0])
+        assert G.norm3(pc) == d3 and np.float32(np.float32(0.8) * P.min_distance[0]) == d3 and P.min_distance[0] == mn
+        other = G.norm3(G.cam_point(T, P.world_pos[0])) / d3         # the chain's other point: outside [0.8, 1.2] times as far
+        assert not 0.5 < other < 1.5, other
+        c = cs[f"sim3_max_dist_{side}", 0]
+        P = c["P1"] if side == 12 else c["P2"]
+        assert np.float32(np.float32(1.2) * P.max_distance[0]) == d3 and P.max_distance[0] == mx
+    for side, key in ((12, ("P1", "T1w", "S21")), (21, ("P2", "T2w", "S12"))):
+        z = [G.sim3_chain(cs[f"sim3_depth_{side}", m][key[1]], cs[f"sim3_depth_{side}", m][key[2]], cs[f"sim3_depth_{side}", m][key[0]].world_pos[0])
+             for m in (0, 1)]
+        z_other = [G.cam_point(cs[f"sim3_depth_{side}", m][key[1]], cs[f"sim3_depth_{side}", m][key[0]].world_pos[0])[2] for m in (0, 1)]
+        assert z[0][2] > 0 > z[1][2] and min(z_other) > 0
+
+
+def test_level_pairs_straddle_their_windows():
+    """Each level_* pair puts the kept member's key octave inside the window of its mode and the rejected member's outside,
+    restated from GetFeaturesInArea (Frame.cc:327-380) with the windows of ORBmatcher.cc:1385-1390."""
+    def inside(mode, o, ko):
+        lo, hi = {"fwd": (o, -1), "bwd": (0, o), "none": (o - 1, o + 1)}[mode]
+        if not (lo > 0 or hi >= 0):
+            return True
+        return ko >= lo and (hi < 0 or ko <= hi)
+    assert {o for members in G.LEVEL_PAIRS.values() for _, o, _ in members} == {0, 3, 7}
+    for cls, (kept, rejected) in G.LEVEL_PAIRS.items():
+        assert inside(*kept) and not inside(*rejected), cls
+        assert all(0 <= ko < G.N_LEVELS for _, _, ko in (kept, rejected))
+
+
+def test_rotation_boundaries_are_placed():
+    """rot = -0.0 is bin 0 and rot = -2^-149 is bin 12 (360.0f*(1/30), not wrapped); the x.5 pair has the product exactly 0.5
+    (bin 1, half away from zero) and one step below it (bin 0), where floor(x + 0.5f) would give 1."""
+    b = G.rot_boundaries()
+    assert [G.rot_bin(*a) for a in b["zero"]] == [0, 12]
+    assert [G.rot_bin(*a) for a in b["half"]] == [1, 0]
+    lo, hi = G.rot_half_pair()
+    assert np.float32(hi * G.FACTOR) == 0.5 and np.floor(np.float32(np.float32(lo * G.FACTOR) + np.float32(0.5))) == 1
+    for bins in G.ROT_BINS.values():
+        counts = sorted(np.bincount(bins, minlength=30), reverse=True)
+        assert counts[:4] == [3, 3, 2, 1] and bins.count(0 if bins[0] == 0 else 1) == 3
+
+
+def test_area_edge_keys_lie_in_the_window_edge_cell():
+    """The key each area_edge_* pair keeps sits in the window's edge cell on its side, so a window one cell narrower there
+    would lose the match (Frame.cc:332-344 and PosInGrid, restated)."""
+    for c in G.cases():
+        if not c["cls"].startswith("area_edge") or c["member"] != 0:
+            continue
+        _, _, axis, side = G.AREA_EDGES[c["cls"]]
+        k = c["F"].mvKeysUn[0]
+        cell = G.grid_cell(c["F"], k["x"], k["y"])
+        win = G.area_window(c["F"], c["mps"].mTrackProjX[0], c["mps"].mTrackProjY[0], G.AREA_R)
+        edge = win[2 * axis + (1 if side > 0 else 0)]
+        assert cell is not None and cell[axis] == edge, (c["cls"], cell, win)
+
+
+DENSE = G.dense_classes()
+
+
+@pytest.mark.parametrize("cls", DENSE)
+def test_dense_port_equals_reference(O, cls):
+    """Both members of every world-point class inside a natural ~1000-point call: the port equals the verbatim build on every
+    method, and the verbatim build still decides the boundary point differently between the two members."""
+    pair = {c["member"]: G.dense_case(O, c) for c in G.cases() if c["cls"] == cls and "kind" not in c}
+    for c in pair.values():
+        assert len(c["P"].world_pos) > 500
+        for method in G.methods(c):
+            port_equals_reference(O, c, method)
+    assert G.decided(O, pair[0]) is True and G.decided(O, pair[1]) is False, cls
