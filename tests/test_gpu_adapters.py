@@ -69,6 +69,12 @@ from tests import test_oracle_proj_geometry as TG      # noqa: E402
 test_proj_geometry_port_equals_reference = TG.test_port_equals_reference
 test_proj_geometry_dense_port_equals_reference = TG.test_dense_port_equals_reference
 
+# the descriptor-distance gate cases through the adapters: the thresholds, nnratio products and claims they pass to the C ABI
+# (TH_LOW / TH_HIGH / ORBdist per overload, mfNNratio, the MapPoint and vbMatched masks) meet the same boundaries
+from tests import test_oracle_match_gates as TM      # noqa: E402
+
+test_match_gates_port_equals_reference = TM.test_port_equals_reference
+
 
 def test_adapters_reproduce_the_reference_golden_vectors(O):
     """tests/golden/match_ref.npz = outputs of the verbatim src/ORBmatcher.cc; the adapter library, driven through the same
