@@ -281,7 +281,7 @@ __device__ inline void bitonic_sort_u64(uint64_t* k, int K) {
         }
 }
 
-struct FrameJob {                 // one frame of borb_frames_from_extractor (k_frame.cu)
+struct FrameJob {                 // one frame of borb_frames_from_extractor (k_frame.cu); a grid-only row sets keys, the grid, n and the bounds
     const borb_keypoint* src_keys;   // the extractor's mvKeys of that image
     const uint8_t* src_desc;
     const float* src_ur;             // stereo: the extractor's mvuRight / mvDepth of the pair
@@ -347,8 +347,6 @@ struct VocDev {                   // views into the packed blob
     const int32_t* child_ids;     // n_nodes - 1
 };
 
-int launch_grid_sort(const borb_keypoint* keys, int n, float minX, float minY, float invW, float invH, int* cell_start, int* cell_idx,
-                     cudaStream_t s);
 void launch_candidates(const ProjArgs& A, cudaStream_t s);
 // candidates and resolve (last: resolve<true>) of n_jobs jobs: one job runs the by-value kernels on `one` (the host copy of job 0),
 // more run the *_batch_kernels over the ProjArgs table d_jobs (unused for one job)
@@ -371,6 +369,8 @@ int launch_bow_match(const KfDev* qs, const KfDev* ts, int n_pairs, int mode, fl
 void host_image_bounds(int w, int h, const borb_camera& c, float* b4);
 int launch_frame_build(const FrameJob* d_jobs, int n_jobs, int max_n, const borb_camera& cam, int mode, int depth_type, float depth_factor, int w,
                        int h, int out_cap, borb_keypoint* keys_out, float* ur_out, float* depth_out, cudaStream_t s);
+// Frame::AssignFeaturesToGrid of n_jobs frames (a FrameJob table the kernel can read) in one launch; max_n = the most keys of a job
+int launch_grid_sort(const FrameJob* d_jobs, int n_jobs, int max_n, cudaStream_t s);
 // pack + match + finalize over A.jobs (3 launches): one = a host copy of job 0 (what the match kernel reads of a single job),
 // max_smem_frame = largest frame_bytes of the jobs with frame_in_smem, max_items = an upper bound of the work items of all jobs,
 // total_kf = sum of their n_kf; kfkf: the jobs are SearchByBoW(KeyFrame*, KeyFrame*) of a database slot against candidates

@@ -27,6 +27,7 @@
 // Bound: not HBM (96 MB of keyframe records per 2000-keyframe sweep) but the integer pipes and the per-item / per-batch
 // bookkeeping around the column loop (ham256<MODE>: 8 POPC, 4 POPC + carry-save tree, or 5 POPC + three 3:2 compressors).
 #include "borb_match.h"
+#include "match_rules.cuh"
 
 namespace borb {
 
@@ -37,19 +38,18 @@ constexpr int BDB_CTAS = 1;
 constexpr int BDB_QCAP = 64;                  // pending-row ring per warp
 constexpr int BDB_CLAIM_WORDS = MATCH_MAX_FEATURES / 32;
 constexpr int BDB_WARP_BYTES = BDB_CLAIM_WORDS * 4 + 32 * 24 + BDB_QCAP * 48;   // claim bits | keyframe runs of the batch | pending rows (descriptor halves, meta)
-constexpr int HISTO_LENGTH = 30;
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// 256-bit Hamming distance.  MODE 0: 8 POPC.  MODE 1: full carry-save adder tree, 4 POPC + 17 LOP3.  MODE 2 (default): three
-// 3:2 compressors, 5 POPC + 6 LOP3.  POPC issues at a quarter of LOP3's rate (16 vs 64 results per clock per SM on sm_90,
-// CUDA C++ Programming Guide throughput table): per distance MODE 0 is all POPC, MODE 1 shifts most of the work to LOP3,
+// 256-bit Hamming distance.  MODE 0: 8 POPC (descriptor_distance).  MODE 1: full carry-save adder tree, 4 POPC + 17 LOP3.  MODE 2
+// (default): three 3:2 compressors, 5 POPC + 6 LOP3.  POPC issues at a quarter of LOP3's rate (16 vs 64 results per clock per SM on
+// sm_90, CUDA C++ Programming Guide throughput table): per distance MODE 0 is all POPC, MODE 1 shifts most of the work to LOP3,
 // MODE 2 balances the two.
 template <int MODE>
 __device__ __forceinline__ int ham256(const uint4 a0, const uint4 a1, const uint4 b0, const uint4 b1) {
+    if (MODE == 0) return descriptor_distance(a0, a1, b0, b1);
     const uint32_t x0 = a0.x ^ b0.x, x1 = a0.y ^ b0.y, x2 = a0.z ^ b0.z, x3 = a0.w ^ b0.w;
     const uint32_t x4 = a1.x ^ b1.x, x5 = a1.y ^ b1.y, x6 = a1.z ^ b1.z, x7 = a1.w ^ b1.w;
-    if (MODE == 0) return __popc(x0) + __popc(x1) + __popc(x2) + __popc(x3) + __popc(x4) + __popc(x5) + __popc(x6) + __popc(x7);
     const uint32_t s1 = x0 ^ x1 ^ x2, c1 = (x0 & x1) | (x2 & (x0 ^ x1));
     const uint32_t s2 = x3 ^ x4 ^ x5, c2 = (x3 & x4) | (x5 & (x3 ^ x4));
     const uint32_t s3 = s1 ^ s2 ^ x6, c3 = (s1 & s2) | (x6 & (s1 ^ s2));
@@ -60,27 +60,6 @@ __device__ __forceinline__ int ham256(const uint4 a0, const uint4 a1, const uint
     const uint32_t twos = s5 ^ c4, c6 = s5 & c4;
     const uint32_t fours = c5 ^ c6, eights = c5 & c6;
     return __popc(ones) + 2 * __popc(twos) + 4 * __popc(fours) + 8 * __popc(eights);
-}
-
-__device__ __forceinline__ int rot_bin(float a1, float a2) {         // :234-241
-    float rot = __fsub_rn(a1, a2);
-    if (rot < 0.0f) rot = __fadd_rn(rot, 360.0f);
-    int bin = (int)roundf(__fmul_rn(rot, 1.0f / HISTO_LENGTH));
-    if (bin == HISTO_LENGTH) bin = 0;
-    return bin;
-}
-
-__device__ __forceinline__ void three_maxima(const int* cnt, int& ind1, int& ind2, int& ind3) {   // ORBmatcher::ComputeThreeMaxima :1601-1642
-    int max1 = 0, max2 = 0, max3 = 0;
-    ind1 = ind2 = ind3 = -1;
-    for (int i = 0; i < HISTO_LENGTH; i++) {
-        const int s = cnt[i];
-        if (s > max1) { max3 = max2; max2 = max1; max1 = s; ind3 = ind2; ind2 = ind1; ind1 = i; }
-        else if (s > max2) { max3 = max2; max2 = s; ind3 = ind2; ind2 = i; }
-        else if (s > max3) { max3 = s; ind3 = i; }
-    }
-    if ((float)max2 < 0.1f * (float)max1) { ind2 = -1; ind3 = -1; }
-    else if ((float)max3 < 0.1f * (float)max1) { ind3 = -1; }
 }
 
 }  // namespace

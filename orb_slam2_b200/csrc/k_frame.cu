@@ -73,7 +73,10 @@ __global__ void __launch_bounds__(256) frame_build_kernel(const FrameJob* __rest
     if (ur_out && i < out_cap) { ur_out[o] = ur; depth_out[o] = dp; }
 }
 
-// Frame::AssignFeaturesToGrid for a batch of frames: one CTA per job (same algorithm as grid_sort_kernel, k_match.cu)
+// Frame::AssignFeaturesToGrid for a table of frames, one CTA per job: the frames of borb_frames_from_extractor, and the host views
+// and borb_frame_create frames of the matcher calls (borb_match_host.cu), whose rows set only keys, n, the bounds and the grid.
+// Sorts (cell, feature index) keys in shared memory; writes cell_start[GRID_CELLS+1] and cell_idx[] in (cell, insertion) order —
+// the layout of Frame::mGrid[x][y] (cell = x*48 + y).
 __global__ void __launch_bounds__(1024) grid_sort_jobs_kernel(const FrameJob* __restrict__ jobs) {
     extern __shared__ uint32_t skeys[];
     const FrameJob J = jobs[blockIdx.x];
@@ -125,11 +128,15 @@ int launch_frame_build(const FrameJob* d_jobs, int n_jobs, int max_n, const borb
         frame_build_kernel<<<grid, 256, 0, s>>>(d_jobs, cam, mode, depth_type, depth_factor, w, h, out_cap, keys_out, ur_out, depth_out);
         launches++;
     }
+    return launches + launch_grid_sort(d_jobs, n_jobs, max_n, s);
+}
+
+int launch_grid_sort(const FrameJob* d_jobs, int n_jobs, int max_n, cudaStream_t s) {
     int K = 32;
     while (K < max_n) K <<= 1;
     allow_max_smem((const void*)grid_sort_jobs_kernel);
     grid_sort_jobs_kernel<<<n_jobs, 1024, (size_t)K * 4, s>>>(d_jobs);
-    return launches + 1;
+    return 1;
 }
 
 }  // namespace borb

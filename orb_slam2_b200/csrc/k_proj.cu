@@ -24,44 +24,14 @@
 //       no candidate list; the agreement test of SearchBySim3 (below).
 // All float tests use _rn intrinsics (no FMA contraction) so comparisons match the reference bit for bit.
 #include "borb_match.h"
+#include "match_rules.cuh"
 
 namespace borb {
 
 namespace {
 
-constexpr int HISTO_LENGTH = 30;
 constexpr int SORT_CAP = 128;               // lists up to this length are sorted; longer ones keep position order (flagged)
 constexpr int RES_K = 4;                    // list entries per query staged in shared memory by the resolve kernel
-
-__device__ __forceinline__ int ham_words(const uint32_t* __restrict__ a, const uint32_t* __restrict__ b) {
-    int d = 0;
-#pragma unroll
-    for (int i = 0; i < 8; i++) d += __popc(a[i] ^ b[i]);
-    return d;
-}
-
-__device__ __forceinline__ int rot_bin(float a1, float a2) {
-    float rot = __fsub_rn(a1, a2);
-    if (rot < 0.0f) rot = __fadd_rn(rot, 360.0f);
-    int bin = (int)roundf(__fmul_rn(rot, 1.0f / HISTO_LENGTH));
-    if (bin == HISTO_LENGTH) bin = 0;
-    return bin;
-}
-
-__device__ void three_maxima(const int* cnt, int& ind1, int& ind2, int& ind3) {        // ORBmatcher::ComputeThreeMaxima (:1601-1642)
-    int max1 = 0, max2 = 0, max3 = 0;
-    ind1 = ind2 = ind3 = -1;
-    for (int i = 0; i < HISTO_LENGTH; i++) {
-        const int s = cnt[i];
-        if (s > max1) { max3 = max2; max2 = max1; max1 = s; ind3 = ind2; ind2 = ind1; ind1 = i; }
-        else if (s > max2) { max3 = max2; max2 = s; ind3 = ind2; ind2 = i; }
-        else if (s > max3) { max3 = s; ind3 = i; }
-    }
-    if ((float)max2 < 0.1f * (float)max1) { ind2 = -1; ind3 = -1; }
-    else if ((float)max3 < 0.1f * (float)max1) { ind3 = -1; }
-}
-
-__device__ __forceinline__ unsigned warp_min(unsigned v) { return __reduce_min_sync(0xFFFFFFFFu, v); }
 
 // The cell window of GetFeaturesInArea(x, y, rs) (Frame.cc:327-380) on A's grid: columns c0x..c1x, rows c0y..c1y; false when
 // it is empty.  A NaN centre (a point at the camera centre, Frame::isInFrustum) has an empty window: the reference's
@@ -154,7 +124,7 @@ __device__ __forceinline__ void candidates_body(const ProjArgs& A) {
             // ---- 2. a lane per list entry: 256-bit distance
             for (int e = lane; e < count; e += 32) {
                 const int idx = (int)out[e];
-                const int dist = ham_words(dm, reinterpret_cast<const uint32_t*>(A.desc + (size_t)idx * 32));
+                const int dist = descriptor_distance(dm, reinterpret_cast<const uint32_t*>(A.desc + (size_t)idx * 32));
                 out[e] = (uint32_t)idx | ((uint32_t)dist << 16) | ((uint32_t)A.keys[idx].octave << 25);
             }
             __syncwarp();
@@ -233,7 +203,7 @@ __global__ void __launch_bounds__(256) fuse_batch_kernel(const FuseJob* __restri
                             if ((double)__fmul_rn(e2, inv) > 5.99) continue;
                         }
                     }
-                    const int dist = ham_words(dm, reinterpret_cast<const uint32_t*>(A.desc + (size_t)idx * 32));
+                    const int dist = descriptor_distance(dm, reinterpret_cast<const uint32_t*>(A.desc + (size_t)idx * 32));
                     best = min(best, ((unsigned)dist << 16) | (unsigned)e);
                 }
             }
@@ -497,7 +467,7 @@ __device__ __forceinline__ void init_window(const ProjArgs& A, float x, float y,
         for (int e = A.cell_start[ix * GRID_ROWS + c0y] + lane; e < e1; e += 32) {
             const int idx = A.cell_idx[e];
             if (!area_passes(A.keys[idx], nullptr, idx, x, y, x, rs, 0, 0)) continue;
-            f(e, idx, ham_words(dq, reinterpret_cast<const uint32_t*>(A.desc + (size_t)idx * 32)));
+            f(e, idx, descriptor_distance(dq, reinterpret_cast<const uint32_t*>(A.desc + (size_t)idx * 32)));
         }
     }
 }

@@ -19,18 +19,9 @@
 //
 // Bound: L2-resident gathers; algorithmic bytes ~0.5 MB per pair (SURVEY §8d).
 #include "borb_internal.h"
+#include "match_rules.cuh"
 
 namespace borb {
-
-namespace {
-
-__device__ __forceinline__ int hamming256(const uint4 a0, const uint4 a1, const uint4* __restrict__ b) {
-    const uint4 b0 = b[0], b1 = b[1];
-    return __popc(a0.x ^ b0.x) + __popc(a0.y ^ b0.y) + __popc(a0.z ^ b0.z) + __popc(a0.w ^ b0.w) +
-           __popc(a1.x ^ b1.x) + __popc(a1.y ^ b1.y) + __popc(a1.z ^ b1.z) + __popc(a1.w ^ b1.w);
-}
-
-}  // namespace
 
 constexpr int SBIN_SHIFT = 3;      // 8 image rows per bin
 constexpr int SBIN_MAX = 512;      // bins per pair (images up to 4096 rows)
@@ -148,7 +139,8 @@ __global__ void __launch_bounds__(256, 6) stereo_match_kernel(const __grid_const
             if (row < minr || row > maxr) continue;
             if (rc.octave < levelL - 1 || rc.octave > levelL + 1) continue;
             if (rc.x >= minU && rc.x <= maxU) {
-                const int dist = hamming256(a0, a1, reinterpret_cast<const uint4*>(dR + (size_t)rc.iR * 32));
+                const uint4* b = reinterpret_cast<const uint4*>(dR + (size_t)rc.iR * 32);
+                const int dist = descriptor_distance(a0, a1, b[0], b[1]);
                 const unsigned key = ((unsigned)dist << 16) | (unsigned)rc.iR;
                 best = min(best, key);
             }

@@ -85,3 +85,37 @@ def test_mono_and_stereo_frames_from_extractor(oracle):
     # monocular frames: no mvuRight
     fm, hm = M.frames_from_extractor(mt, X, [1], [len(res[0]["mvKeysRight"])], K, mode=0)
     assert np.array_equal(hm["keys_un"][0], res[0]["mvKeysRight"]) and fm[0].mvuRight is None
+
+
+def test_host_view_grids_share_one_launch(oracle):
+    """One grid_sort_jobs_kernel builds every feature grid: a matcher call builds the grids of all its host views in one launch,
+    and borb_frame_create builds the grid borb_frames_from_extractor builds for the same keypoints."""
+    import ctypes as C
+    from orb_slam2_b200 import matcher as M
+    from orb_slam2_b200.extractor import ORBextractor
+    mt = M.ORBmatcher(0.75, True)
+
+    def launches():
+        n = C.c_uint64(0)
+        assert mt._lib.borb_matcher_launch_count(mt._h, C.byref(n)) == 0
+        return n.value
+
+    # SearchBySim3 on two host keyframes: the resident batch's launches plus one for both grids, and the same matches
+    KF1, KF2, P1, P2, T1w, T2w, S12, S21, K = mf.sim3_case(mf.two_views(oracle, 7), 21)
+    c0 = launches()
+    host = mt.SearchBySim3(KF1, KF2, P1, P2, T1w, T2w, S12, S21, K, 7.5)
+    n_host = launches() - c0
+    R1, R2 = KF1.make_resident(mt), KF2.make_resident(mt)
+    c0 = launches()
+    batch = mt.SearchBySim3Batch([R1], [R2], [P1], [P2], [(T1w, T2w)], [(S12, S21)], K, 7.5)[0]
+    assert n_host == launches() - c0 + 1
+    o = oracle.port_search_by_sim3(KF1, KF2, P1, P2, T1w, T2w, S12, S21, K, 7.5)
+    assert host[0] == batch[0] == o[0] > 100 and np.array_equal(host[1], batch[1]) and np.array_equal(host[1], o[1])
+    # borb_frame_create on the keypoints borb_frames_from_extractor undistorted, within its bounds
+    X = ORBextractor(1000)
+    outs = X.extract_batch([synth.mono_frame(50, 0, 0, 640, 480)])
+    frames, h = M.frames_from_extractor(mt, X, [0], [len(outs[0][0])], TUM1_K, TUM1_DIST, mode=0)
+    created = M.FrameView(h["keys_un"][0], outs[0][1], X.GetScaleFactors(), tuple(float(x) for x in h["bounds"])).make_resident(mt)
+    a, b = frames[0].resident.read(stereo=False), created.resident.read(stereo=False)
+    assert len(a["cell_idx"]) > 500
+    assert np.array_equal(a["cell_start"], b["cell_start"]) and np.array_equal(a["cell_idx"], b["cell_idx"])

@@ -24,7 +24,7 @@ from tools.bench_loop_closure import spread                                    #
 from tools.bench_track_ref import kernel_times                                 # noqa: E402
 
 K_TUM = (517.306408, 516.469215, 318.643040, 255.313989)
-SINGLE_KERNELS = ("grid_sort_kernel", "init_prefix_kernel", "init_replay_kernel")
+SINGLE_KERNELS = ("grid_sort_jobs_kernel", "init_prefix_kernel", "init_replay_kernel")
 BATCH_KERNELS = ("init_prefix_kernel", "init_prefix_batch_kernel", "init_replay_kernel", "init_replay_batch_kernel")
 
 

@@ -38,7 +38,7 @@ K_TUM = (517.306408, 516.469215, 318.643040, 255.313989)
 K_EUROC = (458.654, 457.296, 367.215, 248.375)
 PROJ_KERNELS = ("project_points_kernel", "project_points_batch_kernel", "proj_candidates_kernel", "proj_candidates_batch_kernel",
                 "proj_resolve_kernel", "proj_resolve_batch_kernel")
-SIM3_KERNELS = ("grid_sort_kernel", "project_points_batch_kernel", "fuse_batch_kernel", "sim3_agree_batch_kernel")
+SIM3_KERNELS = ("grid_sort_jobs_kernel", "project_points_batch_kernel", "fuse_batch_kernel", "sim3_agree_batch_kernel")
 
 
 def same(a, b):
