@@ -3,6 +3,7 @@
 #include <algorithm>
 #include <atomic>
 #include <cassert>
+#include <climits>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -247,7 +248,18 @@ template <class T> struct JobTable {
     T* host(const Call& c) { return n > 1 ? c.host<T>(off) : &one; }               // after begin()
     const T* dev(const Call& c) const { return n > 1 ? (const T*)c.dev(off) : nullptr; }
 };
-borb_status check_frame(const borb_frame_view* F, const FrameInfo& I, const borb_matcher* m) {
+// A host view's octaves index the level tables in the kernels (mvInvLevelSigma2 in Fuse, mvScaleFactors / mvLevelSigma2 in
+// SearchForTriangulation) and are packed into 7 bits of a projection search's candidate entries, where the ratio test compares
+// them; so every octave must lie in [0, n_levels), as the extractor makes them.
+borb_status check_octaves(const borb_keypoint* k, int n, int n_levels, const char* what) {
+    for (int i = 0; i < n; i++)
+        if (k[i].octave < 0 || k[i].octave >= n_levels) {
+            set_error("%s keypoint %d: octave %d outside [0, %d)", what, i, k[i].octave, n_levels);
+            return BORB_ERR_INVALID_ARG;
+        }
+    return BORB_OK;
+}
+borb_status check_frame(const borb_frame_view* F, const FrameInfo& I, const borb_matcher* m, const char* what = "frame") {
     if (I.n < 0 || I.n > MATCH_MAX_FEATURES) { set_error("frame has %d features (limit %d)", I.n, MATCH_MAX_FEATURES); return BORB_ERR_INVALID_ARG; }
     if (I.rf) {
         if (I.rf->device != m->device) { set_error("resident frame and matcher live on different devices"); return BORB_ERR_INVALID_ARG; }
@@ -255,7 +267,7 @@ borb_status check_frame(const borb_frame_view* F, const FrameInfo& I, const borb
     }
     if (I.n > 0 && (!F->keys_un || !F->desc)) { set_error("incomplete frame view"); return BORB_ERR_INVALID_ARG; }
     if (I.n_levels < 1 || !F->scale_factors || !(I.max_x > I.min_x) || !(I.max_y > I.min_y)) { set_error("incomplete frame view"); return BORB_ERR_INVALID_ARG; }
-    return BORB_OK;
+    return check_octaves(F->keys_un, I.n, I.n_levels, what);
 }
 // error text of a check shared by the single calls and the batches: the batches prefix it with the job index
 borb_status job_fail(bool batch, int j, borb_status s) {
@@ -281,9 +293,13 @@ void read_counted(const uint8_t* r, int n, int32_t* out, int32_t* count) {
 // indices, and the staging sizes its uploads from start[n_nodes].
 borb_status check_kf(const borb_keyframe_view* v, const char* what) {
     if (!v || v->n < 0 || v->n > MATCH_MAX_FEATURES || (v->n > 0 && (!v->keys_un || !v->desc)) ||
-        (v->n_levels < 0 && (v->scale_factors || v->level_sigma2))) {
+        (v->n_levels < 1 && (v->scale_factors || v->level_sigma2))) {
         set_error("%s: bad keyframe view (n=%d, limit %d)", what, v ? v->n : -1, MATCH_MAX_FEATURES);
         return BORB_ERR_INVALID_ARG;
+    }
+    if (v->n_levels > 0) {                  // every view with level tables (the searches without them read no octave)
+        const borb_status s = check_octaves(v->keys_un, v->n, v->n_levels, what);
+        if (s != BORB_OK) return s;
     }
     const borb_featvec_view& fv = v->fv;
     if (fv.n_nodes < 0 || (fv.n_nodes > 0 && (!fv.node_id || !fv.start || !fv.feat_idx))) {
@@ -763,15 +779,17 @@ borb_status projection_jobs(borb_matcher* m, const borb_frame_view* frames, cons
     int max_n = 1, max_n_mp = 0;
     for (int j = 0; j < n_jobs; j++) {
         const borb_mappoint_view* P = &points[j];
-        n_matches[j] = 0;
         if (batch && !frames[j].resident) { set_error("job %d: borb_search_by_projection_batch needs device-resident frames (borb_frame_view::resident)", j); return BORB_ERR_INVALID_ARG; }
         if (batch && !match_feat[j]) { set_error("job %d: null output", j); return BORB_ERR_INVALID_ARG; }
         const FrameInfo I = J[j].I = frame_info(&frames[j]);
         borb_status s = check_mappoints(&frames[j], I, P, m);
         if (s != BORB_OK) return job_fail(batch, j, s);
         J[j].live = P->n > 0 && I.n > 0;
-        if (!J[j].live) { std::fill_n(match_feat[j], P->n, -1); continue; }
-        max_n = std::max(max_n, I.n); max_n_mp = std::max(max_n_mp, P->n);
+    }
+    for (int j = 0; j < n_jobs; j++) {                  // every job has passed its checks: a refused call writes nothing
+        n_matches[j] = 0;
+        if (!J[j].live) { std::fill_n(match_feat[j], points[j].n, -1); continue; }
+        max_n = std::max(max_n, J[j].I.n); max_n_mp = std::max(max_n_mp, points[j].n);
     }
     if (max_n_mp == 0) return BORB_OK;
     Call c(m);
@@ -970,16 +988,15 @@ borb_status point_query_jobs(borb_matcher* m, const PointJob* jobs, int n_jobs, 
     int max_n = 1, max_nq = 0;
     for (int j = 0; j < n_jobs; j++) {
         const PointQuery& Q = jobs[j].Q;
-        n_matches[j] = 0;
         if (batch && !jobs[j].F->resident) { set_error("job %d: %s needs device-resident frames (borb_frame_view::resident)", j, batch); return BORB_ERR_INVALID_ARG; }
         if (batch && !jobs[j].state) { set_error("job %d: null output", j); return BORB_ERR_INVALID_ARG; }
         const FrameInfo I = J[j].I = frame_info(jobs[j].F);
         borb_status s = check_query(jobs[j].F, I, Q, m);
         if (s != BORB_OK) return job_fail(batch != nullptr, j, s);
-        std::fill_n(jobs[j].state, I.n, -1);
         J[j].live = I.n > 0 && Q.n > 0;
         if (J[j].live) { max_n = std::max(max_n, I.n); max_nq = std::max(max_nq, Q.n); }
     }
+    for (int j = 0; j < n_jobs; j++) { n_matches[j] = 0; std::fill_n(jobs[j].state, J[j].I.n, -1); }   // every job passed its checks
     if (max_nq == 0) return BORB_OK;
     Call c(m);
     HostGrids g;
@@ -1087,7 +1104,6 @@ borb_status fuse_jobs(borb_matcher* m, const borb_fuse_job* jobs, int n_jobs, bo
     int max_nq = 0;
     for (int j = 0; j < n_jobs; j++) {
         const borb_fuse_job& B = jobs[j];
-        n_found[j] = 0;
         if (!B.scw_variant && !B.inv_level_sigma2) { set_error("Fuse(pKF, vpMapPoints, th) needs mvInvLevelSigma2"); return job_fail(batch, j, BORB_ERR_INVALID_ARG); }
         PointQuery& Q = J[j].Q;
         Q.variant = 2; Q.n = B.pts.n; Q.world_pos = B.pts.world_pos; Q.desc = B.pts.desc; Q.valid = B.pts.valid;
@@ -1103,10 +1119,10 @@ borb_status fuse_jobs(borb_matcher* m, const borb_fuse_job* jobs, int n_jobs, bo
         const FrameInfo I = J[j].I = frame_info(&J[j].kf);
         const borb_status s = check_query(&J[j].kf, I, Q, m);
         if (s != BORB_OK) return job_fail(batch, j, s);
-        std::fill_n(B.best_idx, Q.n, -1);
         J[j].live = I.n > 0 && Q.n > 0;
         if (J[j].live) max_nq = std::max(max_nq, Q.n);
     }
+    for (int j = 0; j < n_jobs; j++) { n_found[j] = 0; std::fill_n(jobs[j].best_idx, J[j].Q.n, -1); }   // every job passed its checks
     if (max_nq == 0) return BORB_OK;
     Call c(m);
     HostGrids g;
@@ -1196,7 +1212,6 @@ borb_status sim3_jobs(borb_matcher* m, const borb_sim3_job* jobs, int n_jobs, bo
     int max_nq = 0, max_n1 = 0;
     for (int j = 0; j < n_jobs; j++) {
         const borb_sim3_job& B = jobs[j];
-        n_found[j] = 0;
         Dir& d12 = D[2 * (size_t)j];
         Dir& d21 = D[2 * (size_t)j + 1];
         d12.kf = B.kf2; d12.Q = sim3_direction(B, B.pts1, B.T1w, B.S21, B.log_scale_factor2);
@@ -1212,10 +1227,10 @@ borb_status sim3_jobs(borb_matcher* m, const borb_sim3_job* jobs, int n_jobs, bo
         borb_status s = check_query(&d12.kf, d12.I, d12.Q, m);
         if (s == BORB_OK) s = check_query(&d21.kf, d21.I, d21.Q, m);
         if (s != BORB_OK) return job_fail(batch, j, s);
-        std::fill_n(B.match12, n1, -1);
         live[j] = n1 > 0 && n2 > 0;
         if (live[j]) { max_nq = std::max(max_nq, std::max(n1, n2)); max_n1 = std::max(max_n1, n1); }
     }
+    for (int j = 0; j < n_jobs; j++) { n_found[j] = 0; std::fill_n(jobs[j].match12, D[2 * (size_t)j + 1].I.n, -1); }   // every job passed its checks
     if (max_nq == 0) return BORB_OK;
     const size_t nd = D.size();
     Call c(m);
@@ -1322,9 +1337,9 @@ struct LocalOff { FrameStage fs; size_t sel0; int nq; bool gather; size_t wp, md
 // Resets the job's outputs (not in view, no match) and appends its valid points to sel.  Only the points that reach isInFrustum
 // travel (src/Tracking.cc:1171-1175 skips the already-matched and the bad ones): a KITTI-scale local map lists ten thousand points
 // of which a fraction is valid, and the reference has no limit on the list.
-borb_status select_local(const borb_local_points_job& B, std::vector<int32_t>& sel, LocalOff& o) {
-    const borb_worldpoints_view& P = B.pts;
-    for (int i = 0; i < P.n; i++) {
+// the outputs of a point the search does not reach; written once every job of the call has passed its checks
+void clear_local(const borb_local_points_job& B) {
+    for (int i = 0; i < B.pts.n; i++) {
         B.in_view[i] = 0; B.match_feat[i] = -1;
         if (B.proj_x) B.proj_x[i] = 0.f;
         if (B.proj_y) B.proj_y[i] = 0.f;
@@ -1332,6 +1347,9 @@ borb_status select_local(const borb_local_points_job& B, std::vector<int32_t>& s
         if (B.level) B.level[i] = 0;
         if (B.view_cos) B.view_cos[i] = 0.f;
     }
+}
+borb_status select_local(const borb_local_points_job& B, std::vector<int32_t>& sel, LocalOff& o) {
+    const borb_worldpoints_view& P = B.pts;
     o.sel0 = sel.size();
     for (int i = 0; i < P.n; i++)
         if (!P.valid || P.valid[i]) sel.push_back(i);
@@ -1433,7 +1451,6 @@ borb_status local_points_jobs(borb_matcher* m, const borb_local_points_job* jobs
     int max_nq = 0, max_n = 1, max_n_mp = 0;
     for (int j = 0; j < n_jobs; j++) {
         const borb_local_points_job& B = jobs[j];
-        n_matches[j] = 0;
         if (batch && !B.frame.resident) { set_error("job %d: borb_search_local_points_batch needs device-resident frames (borb_frame_view::resident)", j); return BORB_ERR_INVALID_ARG; }
         if (batch && (!B.in_view || !B.match_feat)) { set_error("job %d: null output", j); return BORB_ERR_INVALID_ARG; }
         const FrameInfo I = J[j].I = frame_info(&B.frame);
@@ -1445,6 +1462,7 @@ borb_status local_points_jobs(borb_matcher* m, const borb_local_points_job* jobs
         max_nq = std::max(max_nq, nq);
         if (J[j].search) { max_n = std::max(max_n, I.n); max_n_mp = std::max(max_n_mp, nq); }
     }
+    for (int j = 0; j < n_jobs; j++) { n_matches[j] = 0; clear_local(jobs[j]); }   // every job passed its checks
     if (max_nq == 0) return BORB_OK;
     Call c(m);
     HostGrids g;
@@ -1611,13 +1629,21 @@ borb_status init_jobs(borb_matcher* m, const borb_init_job* jobs, int n_jobs, co
 borb_status borb_search_for_initialization(borb_matcher* m, const borb_frame_view* f1, const borb_frame_view* f2, float* prev_matched,
                                            int window_size, float nnratio, int check_orientation, int32_t* matches12, int32_t* n_matches) {
     if (!m || !f1 || !f2 || !prev_matched || !matches12 || !n_matches) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
-    *n_matches = 0;
     if (f1->n < 0 || f1->n > MATCH_MAX_FEATURES || f2->n < 0 || f2->n > MATCH_MAX_FEATURES) { set_error("feature count outside [0,%d]", MATCH_MAX_FEATURES); return BORB_ERR_INVALID_ARG; }
+    if (f1->n > 0 && f2->n > 0) {
+        if (!f1->keys_un || !f1->desc || !f2->keys_un || !f2->desc || !(f2->max_x > f2->min_x) || !(f2->max_y > f2->min_y)) {
+            set_error("incomplete frame view"); return BORB_ERR_INVALID_ARG;
+        }
+        // a negative F1 octave would skip the reference's level test (GetFeaturesInArea with bCheckLevels false).  The search reads
+        // no level table, so a view without one (n_levels < 1) has only the sign of its octaves checked
+        const auto levels = [](int n) { return n > 0 ? n : INT_MAX; };
+        borb_status s = check_octaves(f1->keys_un, f1->n, levels(f1->n_levels), "initial frame");
+        if (s == BORB_OK) s = check_octaves(f2->keys_un, f2->n, levels(f2->n_levels), "current frame");
+        if (s != BORB_OK) return s;
+    }
+    *n_matches = 0;
     for (int i = 0; i < f1->n; i++) matches12[i] = -1;
     if (f1->n == 0 || f2->n == 0) return BORB_OK;
-    if (!f1->keys_un || !f1->desc || !f2->keys_un || !f2->desc || !(f2->max_x > f2->min_x) || !(f2->max_y > f2->min_y)) {
-        set_error("incomplete frame view"); return BORB_ERR_INVALID_ARG;
-    }
     borb_frame_view V[2] = {*f1, *f2};
     V[0].resident = V[1].resident = nullptr;            // the host fields are read, never the resident frame
     borb_init_job B{};
@@ -1802,7 +1828,6 @@ borb_status borb_search_by_bow_batch(borb_matcher* m, const borb_bow_job* jobs, 
     std::vector<BowJob> J(n_jobs);
     for (int j = 0; j < n_jobs; j++) {
         const borb_bow_job& B = jobs[j];
-        n_matches[j] = 0;
         borb_status s = check_resident_bow(B.frame, m, j, "frame");
         if (s != BORB_OK) return s;
         if (!B.match) { set_error("job %d: null output", j); return BORB_ERR_INVALID_ARG; }
@@ -1811,6 +1836,7 @@ borb_status borb_search_by_bow_batch(borb_matcher* m, const borb_bow_job* jobs, 
         } else if ((s = check_kf(&B.kf, "keyframe")) != BORB_OK) return job_fail(true, j, s);
         J[j] = BowJob{KfSide{&B.kf, B.kf_frame}, KfSide{&NO_VIEW, B.frame}, B.match};
     }
+    std::fill_n(n_matches, n_jobs, 0);                  // every job passed its checks
     return bow_jobs(m, J, 0, nnratio, check_orientation, n_matches);
 }
 
@@ -2447,7 +2473,6 @@ borb_status triangulation_jobs(borb_matcher* m, const borb_triangulation_job* jo
     for (int j = 0; j < n_jobs; j++) {
         const borb_triangulation_job& B = jobs[j];
         if (!B.pairs || !B.n_pairs || B.cap < 0) { set_error("job %d: null output or negative capacity", j); return BORB_ERR_INVALID_ARG; }
-        *B.n_pairs = 0;
         borb_status s = BORB_OK;
         if (B.kf1_frame) s = check_resident_bow(B.kf1_frame, m, j, "kf1_frame");
         else if ((s = check_kf(&B.kf1, batch ? "kf1" : "borb_search_for_triangulation(kf1)")) != BORB_OK) return job_fail(batch, j, s);
@@ -2465,6 +2490,7 @@ borb_status triangulation_jobs(borb_matcher* m, const borb_triangulation_job* jo
         Q.live = Q.s1.n() > 0 && Q.s1.nn() > 0 && Q.s2.n() > 0 && Q.s2.nn() > 0;
         Q.cap = std::min(B.cap, Q.s1.n());           // a job has at most one pair per kf1 feature
     }
+    for (int j = 0; j < n_jobs; j++) *jobs[j].n_pairs = 0;      // every job passed its checks
     std::vector<int> live;
     for (int j = 0; j < n_jobs; j++) if (J[j].live) live.push_back(j);
     const int nl = (int)live.size();

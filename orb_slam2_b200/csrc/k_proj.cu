@@ -34,14 +34,14 @@ constexpr int SORT_CAP = 128;               // lists up to this length are sorte
 constexpr int RES_K = 4;                    // list entries per query staged in shared memory by the resolve kernel
 
 // The cell window of GetFeaturesInArea(x, y, rs) (Frame.cc:327-380) on A's grid: columns c0x..c1x, rows c0y..c1y; false when
-// it is empty.  A NaN centre (a point at the camera centre, Frame::isInFrustum) has an empty window: the reference's
-// (int)floor(NaN) is INT_MIN on x86, while the device conversion gives 0, which would make the window cell (0, 0).
+// it is empty.  The edges are converted as on x86 (x86_int): an edge that is NaN (a NaN centre, e.g. a point at the camera
+// centre in Frame::isInFrustum), infinite or past +-2^31 (a huge radius, or a narrow frame whose invW is huge) is INT_MIN, so
+// such a far edge empties the window and such a near edge clamps to 0, as the reference's (int)floor / (int)ceil do.
 __device__ __forceinline__ bool area_window(const ProjArgs& A, float x, float y, float rs, int& c0x, int& c1x, int& c0y, int& c1y) {
-    if (!(x == x) || !(y == y)) return false;
-    c0x = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(x, A.minX), rs), A.invW)));
-    c1x = min(GRID_COLS - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(x, A.minX), rs), A.invW)));
-    c0y = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(y, A.minY), rs), A.invH)));
-    c1y = min(GRID_ROWS - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(y, A.minY), rs), A.invH)));
+    c0x = max(0, x86_int(floorf(__fmul_rn(__fsub_rn(__fsub_rn(x, A.minX), rs), A.invW))));
+    c1x = min(GRID_COLS - 1, x86_int(ceilf(__fmul_rn(__fadd_rn(__fsub_rn(x, A.minX), rs), A.invW))));
+    c0y = max(0, x86_int(floorf(__fmul_rn(__fsub_rn(__fsub_rn(y, A.minY), rs), A.invH))));
+    c1y = min(GRID_ROWS - 1, x86_int(ceilf(__fmul_rn(__fadd_rn(__fsub_rn(y, A.minY), rs), A.invH))));
     return !(c0x >= GRID_COLS || c1x < 0 || c0y >= GRID_ROWS || c1y < 0);
 }
 

@@ -1,7 +1,8 @@
-// Device rules every ORBmatcher search shares (reference src/ORBmatcher.cc), written once for k_match.cu, k_proj.cu, k_bowdb.cu
-// and k_stereo.cu.  Device code only.  All float steps use _rn intrinsics (no FMA contraction) so results match the reference bit
+// Device rules every ORBmatcher search shares (reference src/ORBmatcher.cc), written once for k_match.cu, k_proj.cu, k_bowdb.cu,
+// k_stereo.cu and k_frame.cu.  Device code only.  All float steps use _rn intrinsics (no FMA contraction) so results match the reference bit
 // for bit.
 #pragma once
+#include <climits>
 #include <cstdint>
 
 namespace borb {
@@ -9,6 +10,11 @@ namespace borb {
 namespace {
 
 constexpr int HISTO_LENGTH = 30;                 // ORBmatcher::HISTO_LENGTH (:39)
+
+// (int)v as the reference computes it on x86 (cvttss2si): NaN, +-inf and every value outside [-2^31, 2^31) give INT_MIN.  The
+// device conversion saturates instead (+inf and large values INT_MAX, NaN 0), which would put a NaN key into grid column 0 and
+// turn a window edge past 2^31 into the last grid column.
+__device__ __forceinline__ int x86_int(float v) { return (v >= -2147483648.f && v < 2147483648.f) ? (int)v : INT_MIN; }
 
 // ORBmatcher::DescriptorDistance (:1646-1662) of two 256-bit descriptors given as 8 words each
 __device__ __forceinline__ int descriptor_distance(const uint32_t* __restrict__ a, const uint32_t* __restrict__ b) {
