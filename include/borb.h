@@ -764,6 +764,30 @@ typedef struct borb_kfdb_add_job {
 } borb_kfdb_add_job;
 BORB_API borb_status borb_kfdb_add_frames(borb_matcher* m, const borb_kfdb_add_job* jobs, int n_jobs);
 
+/* TemplatedVocabulary::score (Thirdparty/DBoW2/DBoW2/TemplatedVocabulary.h; ScoringObject.cpp:23-71) between BowVectors that are
+ * already on the device: LoopClosing::DetectLoop's minScore (src/LoopClosing.cc:121-140) of many camera streams with no host
+ * BowVector.  A BowVector is a resident frame's (borb_frames_compute_bow) or a database slot's, whether or not the keyframe has
+ * been added to a database yet.  score[t] = (float)score(query, targets[t]), bit-identical to DBoW2's L1 score cast to float: v1 is
+ * the query, v2 the target, the terms are added in ascending word order, and two vectors that share no word give -0.0f.  Frames and
+ * slots mix freely on either side, from any number of databases; repeats are allowed, and so is a query that is also one of its own
+ * targets.  Argument errors are refused with BORB_ERR_INVALID_ARG before anything is uploaded, the error text starting "job j:" or,
+ * for a reference, "job j query:" / "job j target t:": NULL pointers, n_targets < 0, a reference with neither frame nor database,
+ * a frame without BoW (recycled frames included), a frame or database on another device than the matcher, a slot that is out of
+ * range or erased.  The slots are resolved and read under the databases' locks (taken in address order), so a concurrent
+ * borb_kfdb_add, _erase or _set_has_mp is seen whole.  1 launch whatever n_jobs (0 when no job has a target), one
+ * synchronisation. */
+typedef struct borb_bow_ref {           /* one BowVector resident on the device */
+    const borb_frame* frame;            /* a resident frame whose BoW borb_frames_compute_bow computed, or NULL ... */
+    borb_kfdb* db; int32_t slot;        /* ... then a live slot of a database */
+} borb_bow_ref;
+typedef struct borb_bow_score_job {
+    borb_bow_ref query;                 /* v1 of score(): LoopClosing's mpCurrentKF->mBowVec */
+    const borb_bow_ref* targets;        /* v2 of each score(): the covisible keyframes */
+    int32_t n_targets;
+    float* score;                       /* n_targets: float score = mpVoc->score(v1, v2) (LoopClosing.cc:133) */
+} borb_bow_score_job;
+BORB_API borb_status borb_bow_score_batch(borb_matcher* m, const borb_bow_score_job* jobs, int n_jobs);
+
 typedef struct borb_bow_db_job {
     borb_kfdb* db;
     const borb_frame* frame;       /* resident, BoW computed */

@@ -103,6 +103,7 @@ _SIGNATURES = {
     "borb_search_by_bow_db_pairs": (C.c_int, [vp, vp, vp, C.c_int, vp, C.c_float, C.c_int, vp, vp, vp, C.c_int, i32p]),
     "borb_kfdb_query_batch": (C.c_int, [vp, vp, C.c_int]),
     "borb_kfdb_add_frames": (C.c_int, [vp, vp, C.c_int]),
+    "borb_bow_score_batch": (C.c_int, [vp, vp, C.c_int]),
     "borb_debug_kfdb_read": (C.c_int, [vp, C.c_int32, vp, C.POINTER(C.c_uint64), vp, vp, vp, vp, vp, vp, vp, vp]),
     "borb_search_by_bow_db_batch": (C.c_int, [vp, vp, C.c_int, C.c_float, C.c_int]),
     "borb_search_by_bow_kf_db_batch": (C.c_int, [vp, vp, C.c_int, C.c_float, C.c_int]),

@@ -8,6 +8,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <optional>
 #include <string>
 
 #include "borb_match.h"
@@ -28,6 +29,7 @@ struct CallBuffers {
 
 struct borb_matcher : CallBuffers {
     uint64_t launches = 0;
+    int n_sm = 1;                   // the device's multiprocessor count (sizes the persistent grids)
     std::vector<int32_t> sel;       // indices of the valid queries of the current call
     cudaEvent_t ev_a = nullptr, ev_b = nullptr;   // cross-stream ordering with an extractor handle (borb_frames_from_extractor)
     bool timing = false;            // borb_matcher_set_timing: CUDA events around the kernels of the database search
@@ -491,8 +493,10 @@ borb_status borb_matcher_create(int device, borb_matcher** out) {
     borb_matcher* m = new borb_matcher();
     m->device = device;
     cudaError_t e = cudaSetDevice(device);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&m->n_sm, cudaDevAttrMultiProcessorCount, device);
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking);
     if (e != cudaSuccess) { set_error("CUDA init failed: %s", cudaGetErrorString(e)); delete m; return BORB_ERR_CUDA; }
+    if (m->n_sm < 1) m->n_sm = 1;
     *out = m;
     return BORB_OK;
 }
@@ -1744,11 +1748,24 @@ borb_status borb_distinctive_descriptors_frames(borb_matcher* m, const borb_fram
 // borb_search_by_bow_batch (TrackReferenceKeyFrame of many camera streams: a keyframe against its own resident frame with BoW) are
 // jobs of one launch of bow_match_kernel and one synchronisation.
 namespace {
-borb_status check_resident_bow(const borb_frame* f, const borb_matcher* m, int j, const char* what) {
-    if (!f) { set_error("job %d: %s is not a device-resident frame", j, what); return BORB_ERR_INVALID_ARG; }
-    if (f->device != m->device) { set_error("job %d: %s and matcher live on different devices", j, what); return BORB_ERR_INVALID_ARG; }
-    if (!f->has_bow) { set_error("job %d: %s has no BoW (borb_frames_compute_bow)", j, what); return BORB_ERR_INVALID_ARG; }
-    if (f->n > MATCH_MAX_FEATURES) { set_error("job %d: %s has %d features (limit %d)", j, what, f->n, MATCH_MAX_FEATURES); return BORB_ERR_INVALID_ARG; }
+// Where an argument error lies, as its text names it: "job j", or for a BowVector reference of borb_bow_score_batch "job j query"
+// (ref == QUERY_REF) or "job j target t" (ref = t).
+constexpr int NO_REF = -2, QUERY_REF = -1;
+std::string job_at(int j, int ref = NO_REF) {
+    std::string s = "job " + std::to_string(j);
+    if (ref == QUERY_REF) s += " query";
+    else if (ref >= 0) s += " target " + std::to_string(ref);
+    return s;
+}
+
+borb_status check_resident_bow(const borb_frame* f, const borb_matcher* m, int j, const char* what, int ref = NO_REF) {
+    if (!f) { set_error("%s: %s is not a device-resident frame", job_at(j, ref).c_str(), what); return BORB_ERR_INVALID_ARG; }
+    if (f->device != m->device) { set_error("%s: %s and matcher live on different devices", job_at(j, ref).c_str(), what); return BORB_ERR_INVALID_ARG; }
+    if (!f->has_bow) { set_error("%s: %s has no BoW (borb_frames_compute_bow)", job_at(j, ref).c_str(), what); return BORB_ERR_INVALID_ARG; }
+    if (f->n > MATCH_MAX_FEATURES) {
+        set_error("%s: %s has %d features (limit %d)", job_at(j, ref).c_str(), what, f->n, MATCH_MAX_FEATURES);
+        return BORB_ERR_INVALID_ARG;
+    }
     return BORB_OK;
 }
 
@@ -2059,44 +2076,63 @@ struct DbLocks {
         for (borb_kfdb* db : dbs) { borb_status st = kfdb_sync_table(db); if (st != BORB_OK) return st; }
         return BORB_OK;
     }
+    void unlock() { held.clear(); }
 };
 
-// One query of the database score: the BowVector comes from the host (word / value) or from a resident frame.
+// A job of borb_bow_score_batch, resolved under the database locks: the query and the targets as device BowVectors, and the
+// resident frames among them, whose ready events the launch waits on.
+struct BowTable {
+    BowDev query;
+    std::vector<BowDev> targets;
+    std::vector<const borb_frame*> frames;
+};
+
+// One query of the database score: the BowVector comes from the host (word / value) or from a resident frame, and is scored
+// against every slot of db; or, with a table, the table's query is scored against its targets (db, frame and word unused).
 struct QueryJob {
     borb_kfdb* db;
     const borb_frame* frame;
     const uint32_t* word; const double* value; int n_bow;
-    int32_t* common; float* score; uint32_t* first_word;
+    int32_t* common; float* score; uint32_t* first_word;      // common, first_word and n_slots may be null with a table
     int cap; int32_t* n_slots;
+    const BowTable* table = nullptr;
 };
 
-// Shared body of borb_kfdb_query and borb_kfdb_query_batch: one launch of kfdb_score_kernel for every job (none when no database
-// has a slot) and one synchronisation.  The arguments are checked by the callers.
-borb_status kfdb_query_jobs(borb_matcher* m, const QueryJob* q, int n_jobs, bool batch) {
+// Shared body of borb_kfdb_query, borb_kfdb_query_batch and borb_bow_score_batch: one launch of kfdb_score_kernel for every job
+// (none when no job has a slot or a target) and one synchronisation.  The arguments are checked by the callers.  held: the
+// databases' locks, taken by a caller that resolved its tables under them (released once the kernel is enqueued); without it, the
+// jobs' databases are locked here.
+borb_status kfdb_query_jobs(borb_matcher* m, const QueryJob* q, int n_jobs, bool batch, DbLocks* held = nullptr) {
     std::vector<int> ns(n_jobs);
-    std::vector<size_t> o_w(n_jobs, 0), o_v(n_jobs, 0), ho(n_jobs, 0);
+    std::vector<size_t> o_w(n_jobs, 0), o_v(n_jobs, 0), o_t(n_jobs, 0), ho(n_jobs, 0);
     int max_slots = 0, max_nq = 0;
     Call c(m);
     {
-        std::vector<borb_kfdb*> dbs(n_jobs);
-        for (int j = 0; j < n_jobs; j++) dbs[j] = q[j].db;
-        DbLocks lk(std::move(dbs));
+        std::optional<DbLocks> own;
+        if (!held) {
+            std::vector<borb_kfdb*> dbs(n_jobs);
+            for (int j = 0; j < n_jobs; j++) dbs[j] = q[j].db;
+            own.emplace(std::move(dbs));
+        }
+        DbLocks& lk = held ? *held : *own;
         for (int j = 0; j < n_jobs; j++) {
-            ns[j] = (int)q[j].db->entries.size();
-            *q[j].n_slots = ns[j];
+            ns[j] = q[j].table ? (int)q[j].table->targets.size() : (int)q[j].db->entries.size();
+            if (q[j].n_slots) *q[j].n_slots = ns[j];
         }
         for (int j = 0; j < n_jobs; j++)
             if (q[j].cap < ns[j]) { set_error("output capacity %d < %d database slots", q[j].cap, ns[j]); return job_fail(batch, j, BORB_ERR_CAPACITY); }
         for (int j = 0; j < n_jobs; j++) {
             max_slots = std::max(max_slots, ns[j]);
-            max_nq = std::max(max_nq, q[j].frame ? q[j].frame->n_bow : q[j].n_bow);
+            max_nq = std::max(max_nq, q[j].table ? q[j].table->query.n : q[j].frame ? q[j].frame->n_bow : q[j].n_bow);
         }
         if (max_slots == 0) return BORB_OK;
         BORB_CUDA(cudaSetDevice(m->device));
-        borb_status s = lk.sync();
-        if (s != BORB_OK) return s;
-        for (int j = 0; j < n_jobs; j++)
-            if (!q[j].frame) { o_w[j] = c.in(q[j].word, (size_t)q[j].n_bow * 4); o_v[j] = c.in(q[j].value, (size_t)q[j].n_bow * 8); }
+        borb_status s;
+        if (std::any_of(q, q + n_jobs, [](const QueryJob& x) { return !x.table; }) && (s = lk.sync()) != BORB_OK) return s;
+        for (int j = 0; j < n_jobs; j++) {
+            if (q[j].table) o_t[j] = c.in(q[j].table->targets.data(), (size_t)ns[j] * sizeof(BowDev));
+            else if (!q[j].frame) { o_w[j] = c.in(q[j].word, (size_t)q[j].n_bow * 4); o_v[j] = c.in(q[j].value, (size_t)q[j].n_bow * 8); }
+        }
         const size_t o_jobs = c.in(nullptr, (size_t)n_jobs * sizeof(KfdbQueryJob));     // filled in place
         for (int j = 0; j < n_jobs; j++) ho[j] = c.result((size_t)ns[j] * 12);
         if ((s = c.begin()) != BORB_OK) return s;
@@ -2105,24 +2141,35 @@ borb_status kfdb_query_jobs(borb_matcher* m, const QueryJob* q, int n_jobs, bool
             // the three result arrays are written by the kernel straight into the pinned landing buffer (device-addressable, UVA)
             uint8_t* o = c.res(ho[j], true);
             KfdbQueryJob J{};
-            J.table = q[j].db->d_table; J.n_slots = ns[j];
-            if (q[j].frame) { J.qword = q[j].frame->bow_word; J.qvalue = q[j].frame->bow_value; J.nq = q[j].frame->n_bow; }
-            else { J.qword = (const uint32_t*)c.dev(o_w[j]); J.qvalue = (const double*)c.dev(o_v[j]); J.nq = q[j].n_bow; }
+            J.n_slots = ns[j];
+            if (const BowTable* T = q[j].table) {
+                J.table = (const BowDev*)c.dev(o_t[j]);
+                J.qword = T->query.word; J.qvalue = T->query.value; J.nq = T->query.n;
+            } else {
+                J.table = q[j].db->d_table;
+                if (q[j].frame) { J.qword = q[j].frame->bow_word; J.qvalue = q[j].frame->bow_value; J.nq = q[j].frame->n_bow; }
+                else { J.qword = (const uint32_t*)c.dev(o_w[j]); J.qvalue = (const double*)c.dev(o_v[j]); J.nq = q[j].n_bow; }
+            }
             J.common = (int32_t*)o; J.score = (float*)(o + (size_t)ns[j] * 4); J.first_word = (uint32_t*)(o + (size_t)ns[j] * 8);
             hj[j] = J;
         }
         if ((s = c.commit()) != BORB_OK) return s;
-        for (int j = 0; j < n_jobs; j++)
+        for (int j = 0; j < n_jobs; j++) {
             if (q[j].frame && (s = c.wait(q[j].frame)) != BORB_OK) return s;
-        m->launches += launch_kfdb_score((const KfdbQueryJob*)c.dev(o_jobs), n_jobs, max_slots, max_nq, q[0].db->n_sm, m->stream);
+            if (q[j].table)
+                for (const borb_frame* f : q[j].table->frames)
+                    if ((s = c.wait(f)) != BORB_OK) return s;
+        }
+        m->launches += launch_kfdb_score((const KfdbQueryJob*)c.dev(o_jobs), n_jobs, max_slots, max_nq, m->n_sm, m->stream);
+        lk.unlock();
     }
     const borb_status s = c.finish();
     if (s != BORB_OK) return s;
     for (int j = 0; j < n_jobs; j++) {
         const uint8_t* o = c.out(ho[j]);
-        std::memcpy(q[j].common, o, (size_t)ns[j] * 4);
-        std::memcpy(q[j].score, o + (size_t)ns[j] * 4, (size_t)ns[j] * 4);
-        std::memcpy(q[j].first_word, o + (size_t)ns[j] * 8, (size_t)ns[j] * 4);
+        if (q[j].common) std::memcpy(q[j].common, o, (size_t)ns[j] * 4);
+        if (ns[j]) std::memcpy(q[j].score, o + (size_t)ns[j] * 4, (size_t)ns[j] * 4);
+        if (q[j].first_word) std::memcpy(q[j].first_word, o + (size_t)ns[j] * 8, (size_t)ns[j] * 4);
     }
     return BORB_OK;
 }
@@ -2322,6 +2369,57 @@ borb_status borb_kfdb_query_batch(borb_matcher* m, const borb_kfdb_query_job* jo
         q[j] = QueryJob{B.db, B.frame, nullptr, nullptr, 0, B.common_words, B.score, B.first_word, B.cap, B.n_slots};
     }
     return kfdb_query_jobs(m, q.data(), n_jobs, true);
+}
+
+// The frames are checked first; the slots are resolved to their BowVectors under the databases' locks, which are held until the
+// kernel is enqueued (a concurrent erase synchronises the device before it frees a block).
+borb_status borb_bow_score_batch(borb_matcher* m, const borb_bow_score_job* jobs, int n_jobs) {
+    if (!m || n_jobs < 0 || (n_jobs > 0 && !jobs)) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+    if (n_jobs == 0) return BORB_OK;
+    std::vector<borb_kfdb*> dbs;
+    auto check_ref = [&](const borb_bow_ref& r, int j, int ref) {
+        if (r.frame) return check_resident_bow(r.frame, m, j, "frame", ref);
+        if (!r.db) { set_error("%s: neither a frame nor a database", job_at(j, ref).c_str()); return BORB_ERR_INVALID_ARG; }
+        if (r.db->device != m->device) { set_error("%s: database and matcher live on different devices", job_at(j, ref).c_str()); return BORB_ERR_INVALID_ARG; }
+        dbs.push_back(r.db);
+        return BORB_OK;
+    };
+    for (int j = 0; j < n_jobs; j++) {
+        const borb_bow_score_job& B = jobs[j];
+        if (B.n_targets < 0) { set_error("job %d: n_targets %d < 0", j, B.n_targets); return BORB_ERR_INVALID_ARG; }
+        if (B.n_targets > 0 && (!B.targets || !B.score)) { set_error("job %d: null targets or score", j); return BORB_ERR_INVALID_ARG; }
+        borb_status s = check_ref(B.query, j, QUERY_REF);
+        for (int t = 0; t < B.n_targets && s == BORB_OK; t++) s = check_ref(B.targets[t], j, t);
+        if (s != BORB_OK) return s;
+    }
+    DbLocks lk(std::move(dbs));
+    std::vector<BowTable> T(n_jobs);
+    auto resolve = [&](const borb_bow_ref& r, int j, int ref, BowTable& tab, BowDev& out) {
+        if (r.frame) {
+            out = BowDev{r.frame->bow_word, r.frame->bow_value, r.frame->n_bow};
+            tab.frames.push_back(r.frame);
+            return BORB_OK;
+        }
+        if (r.slot < 0 || r.slot >= (int)r.db->entries.size() || !r.db->entries[r.slot].alive) {
+            set_error("%s: slot %d is not a live keyframe", job_at(j, ref).c_str(), r.slot);
+            return BORB_ERR_INVALID_ARG;
+        }
+        out = r.db->entries[r.slot].bow;
+        return BORB_OK;
+    };
+    std::vector<QueryJob> q(n_jobs);
+    for (int j = 0; j < n_jobs; j++) {
+        const borb_bow_score_job& B = jobs[j];
+        BowTable& tab = T[j];
+        tab.targets.resize(B.n_targets);
+        borb_status s = resolve(B.query, j, QUERY_REF, tab, tab.query);
+        for (int t = 0; t < B.n_targets && s == BORB_OK; t++) s = resolve(B.targets[t], j, t, tab, tab.targets[t]);
+        if (s != BORB_OK) return s;
+        std::sort(tab.frames.begin(), tab.frames.end());
+        tab.frames.erase(std::unique(tab.frames.begin(), tab.frames.end()), tab.frames.end());
+        q[j] = QueryJob{nullptr, nullptr, nullptr, nullptr, 0, nullptr, B.score, nullptr, B.n_targets, nullptr, &tab};
+    }
+    return kfdb_query_jobs(m, q.data(), n_jobs, true, &lk);
 }
 
 // Every job's block is allocated and written by one launch of kfdb_insert_kernel before any database is locked; the slots are

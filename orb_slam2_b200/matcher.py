@@ -74,6 +74,14 @@ class _KfdbAddJobC(C.Structure):                    # borb_kfdb_add_job
     _fields_ = [("db", C.c_void_p), ("frame", C.c_void_p), ("has_mp", C.c_void_p), ("slot_out", C.c_void_p)]
 
 
+class _BowRefC(C.Structure):                        # borb_bow_ref
+    _fields_ = [("frame", C.c_void_p), ("db", C.c_void_p), ("slot", C.c_int32)]
+
+
+class _BowScoreJobC(C.Structure):                   # borb_bow_score_job
+    _fields_ = [("query", _BowRefC), ("targets", C.c_void_p), ("n_targets", C.c_int32), ("score", C.c_void_p)]
+
+
 class _BowDbJobC(C.Structure):                      # borb_bow_db_job
     _fields_ = [("db", C.c_void_p), ("frame", C.c_void_p), ("slots", C.c_void_p), ("n_kf", C.c_int32), ("n_matches", C.c_void_p),
                 ("pair_offset", C.c_void_p), ("pairs", C.c_void_p), ("pairs_cap", C.c_int32), ("n_pairs_total", C.c_void_p)]
@@ -874,6 +882,31 @@ class ORBmatcher:
         for db, F in zip(dbs, frames):
             db._appended(F.resident.n)
         return [int(s) for s in slots[:n]]
+
+    @staticmethod
+    def _bow_ref(x) -> "_BowRefC":
+        """A BowVector on the device: a FrameView bound to a resident frame, or a (KeyFrameDatabase, slot) pair."""
+        if isinstance(x, FrameView):
+            return _BowRefC(x.resident._h.value if x.resident is not None else None, None, 0)
+        db, slot = x
+        return _BowRefC(None, db._h.value if db is not None else None, int(slot))
+
+    def BowScoreBatch(self, jobs) -> List[np.ndarray]:
+        """borb_bow_score_batch: TemplatedVocabulary::score(v1, v2) cast to float, as LoopClosing::DetectLoop takes it for minScore
+        (src/LoopClosing.cc:121-140), between BowVectors already on the device, in one launch.  jobs = [(query, targets)], each
+        BowVector a FrameView whose BoW ComputeBoWBatch computed or a (KeyFrameDatabase, slot) pair.  Returns one float32 array
+        per job: score(query, targets[t])."""
+        n = len(jobs)
+        cj = (_BowScoreJobC * max(n, 1))()
+        keep, outs = [], []
+        for j, (query, targets) in enumerate(jobs):
+            refs = (_BowRefC * max(len(targets), 1))(*[self._bow_ref(t) for t in targets])
+            sc = np.zeros(max(len(targets), 1), np.float32)
+            cj[j].query, cj[j].targets, cj[j].n_targets, cj[j].score = self._bow_ref(query), C.addressof(refs), len(targets), _p(sc)
+            keep.append(refs)
+            outs.append(sc[:len(targets)])
+        check(self._lib.borb_bow_score_batch(self._h, cj, n), "borb_bow_score_batch")
+        return outs
 
     def SearchByBoWDbBatch(self, dbs, slots_list, frames: Sequence[FrameView], pairs_cap=None):
         """borb_search_by_bow_db_batch: SearchByBoW(KeyFrame*, Frame&) (src/ORBmatcher.cc:159-288) of many resident frames with BoW

@@ -111,6 +111,7 @@ FR0 = M.FrameView(outs[0][0], outs[0][1], X.GetScaleFactors(), (0.0, 0.0, 640.0,
 FB = M.FrameView(kb, rng.integers(0, 256, (6000, 32), dtype=np.uint8), X.GetScaleFactors(), (0.0, 0.0, 640.0, 480.0)).make_resident(mt)
 mt.ComputeBoWBatch(voc6, [FR0, FB], 2, want_host=False)
 print("kfdb query batch", [q[0][:3] for q in mt.KfdbQueryBatch([db2, db3], [FR0, FB])])
+print("bow score batch", [s[:3] for s in mt.BowScoreBatch([(FR0, [(db2, 0), FB, (db3, 2)]), ((db3, 1), [FR0, (db2, 5)])])])
 print("bowdb batch", [int(r[0].sum()) for r in mt.SearchByBoWDbBatch([db2, db3, db2], [None, None, [0, 5, 5]], [FR0, FB, FB])])
 K_S, I34, Z3 = (525.0, 525.0, 319.5, 239.5), np.eye(4, dtype=np.float32)[:3], np.zeros(3, np.float32)
 def _slots(F, z=5.0):                                                   # one MapPoint per feature, back-projected at depth z
