@@ -263,6 +263,41 @@ BORB_API borb_status borb_frames_from_extractor(borb_matcher* m, borb_extractor*
                                                 const int32_t* n_keys, const borb_camera* cam, int mode, const void* const* depth,
                                                 int depth_type, float depth_factor, int depth_stride_bytes, borb_keypoint* keys_un,
                                                 float* u_right, float* depth_out, int cap, float* bounds4, borb_frame** frames);
+
+/* The host members of one Frame (include/Frame.h:120-176) as its constructor fills them, written by borb_frame_from_extractors.
+ * Every array may be NULL (not copied); the per-feature arrays hold `cap` entries.  `n`, `n_right` and `bounds` are outputs. */
+typedef struct borb_frame_host {
+    int32_t cap;
+    borb_keypoint* keys;           /* mvKeys */
+    uint8_t* desc;                 /* mDescriptors, N x 32 */
+    borb_keypoint* keys_right;     /* mvKeysRight (stereo) */
+    uint8_t* desc_right;           /* mDescriptorsRight (stereo), n_right x 32 */
+    borb_keypoint* keys_un;        /* mvKeysUn */
+    float* u_right;                /* mvuRight (stereo and RGB-D) */
+    float* depth;                  /* mvDepth (stereo and RGB-D) */
+    int32_t* cell_start;           /* mGrid flattened as in borb_debug_frame_read: 64*48 + 1 entries, cell c = x*48 + y */
+    int32_t* cell_idx;             /* cell_start[64*48] entries (at most N) */
+    int32_t n;                     /* N */
+    int32_t n_right;               /* mvKeysRight.size() (stereo; 0 otherwise) */
+    float bounds[4];               /* mnMinX, mnMinY, mnMaxX, mnMaxY (Frame::ComputeImageBounds, src/Frame.cc:436-464) */
+} borb_frame_host;
+
+/* One Frame constructor (src/Frame.cc:61-117 stereo, :119-178 RGB-D, :180-233 monocular) after its extractions were enqueued on
+ * the frame's extractor handles, image 0 of each handle's last batch (borb_extract_batch_enqueue of one image per handle, no
+ * synchronisation needed; two handles' streams overlap):
+ *   mode 0 monocular (right = NULL); 1 stereo: `left` / `right` are mpORBextractorLeft / mpORBextractorRight, nfeatures may
+ *   differ, and the call runs Frame::ComputeStereoMatches (:466-640) with bf = cam->bf and b = mb = mbf/fx > 0 on the left handle,
+ *   as borb_stereo_match2 does; 2 RGB-D (right = NULL): depth = one depth map as in borb_frames_from_extractor.
+ * Then UndistortKeyPoints, ComputeStereoFromRGBD and AssignFeaturesToGrid run on the device into the resident frame *out.  The
+ * keypoint counts stay on the device until the end: the work is sized by the handles' capacities, and the kernels write every
+ * host member `host` asks for, only the N (or N_right) elements the counts give, straight into pinned memory.  So the call waits
+ * for the device once, for its results.  (The first stereo call on a left handle also waits once to install its pair table.)
+ * Refused before any launch: BORB_ERR_STATE when a handle has no extracted batch; BORB_ERR_INVALID_ARG for bad arguments, a
+ * handle pair that borb_stereo_match2 refuses, or a handle whose capacity (borb_extractor_capacity) exceeds
+ * BORB_MATCH_MAX_FEATURES; BORB_ERR_CAPACITY when host->cap is below a handle's capacity. */
+BORB_API borb_status borb_frame_from_extractors(borb_matcher* m, borb_extractor* left, borb_extractor* right, const borb_camera* cam,
+                                                int mode, float b, const void* depth, int depth_type, float depth_factor,
+                                                int depth_stride_bytes, borb_frame_host* host, borb_frame** out);
 BORB_API borb_status borb_frame_info(const borb_frame* f, int32_t* n, int32_t* n_levels, int32_t* has_u_right);
 /* Read-only introspection of a resident frame (tests, debugging): waits for the frame to be complete and copies mvKeysUn (n),
  * mDescriptors (n x 32), mvuRight / mvDepth (n; BORB_ERR_INVALID_ARG on a monocular frame, and for mvDepth on a frame made by

@@ -572,6 +572,30 @@ borb_status finish_timing(borb_extractor* e) {
 
 }  // namespace
 
+borb_status check_stereo_pair(const borb_extractor* left, const borb_extractor* right) {
+    if (!left->have_geom || !right->have_geom || left->last_n_images < 1 || right->last_n_images < 1) { set_error("stereo match before extract"); return BORB_ERR_STATE; }
+    if (left->device != right->device || left->geom.w != right->geom.w || left->geom.h != right->geom.h ||
+        left->geom.nlevels != right->geom.nlevels) {
+        set_error("left/right extractors differ in device or geometry");
+        return BORB_ERR_INVALID_ARG;
+    }
+    // the match kernel reads both pyramids and both keypoint sets with one scale table (level offsets, pitches, row bands)
+    for (int l = 0; l < left->geom.nlevels; l++)
+        if (left->geom.lv[l].scale != right->geom.lv[l].scale) {
+            set_error("left/right extractors differ in scale factor at level %d (%g vs %g)", l, (double)left->geom.lv[l].scale,
+                      (double)right->geom.lv[l].scale);
+            return BORB_ERR_INVALID_ARG;
+        }
+    return BORB_OK;
+}
+
+borb_status enqueue_stereo_pair(borb_extractor* left, borb_extractor* right, float bf, float b) {
+    begin_step(left);
+    const borb_status st = enqueue_stereo(left, right, 1, nullptr, nullptr, bf, b);
+    if (st == BORB_OK) mark(left, 8);
+    return st;
+}
+
 // Plain double math is enough here: the order only groups the taps, every order gives the same descriptor.
 const std::vector<uint32_t>& brief_slot_table() {
     static const std::vector<uint32_t> table = [] {
@@ -981,23 +1005,12 @@ borb_status borb_stereo_match(borb_extractor* e, int n_pairs, const int* left_id
 
 borb_status borb_stereo_match2(borb_extractor* left, borb_extractor* right, float bf, float b, float* u_right, float* depth, int cap) {
     if (!left || !right || !(b > 0.f)) { set_error("bad arguments"); return BORB_ERR_INVALID_ARG; }
-    if (!left->have_geom || !right->have_geom || left->last_n_images < 1 || right->last_n_images < 1) { set_error("stereo match before extract"); return BORB_ERR_STATE; }
-    if (left->device != right->device || left->geom.w != right->geom.w || left->geom.h != right->geom.h ||
-        left->geom.nlevels != right->geom.nlevels) {
-        set_error("left/right extractors differ in device or geometry");
-        return BORB_ERR_INVALID_ARG;
-    }
-    // the match kernel reads both pyramids and both keypoint sets with one scale table (level offsets, pitches, row bands)
-    for (int l = 0; l < left->geom.nlevels; l++)
-        if (left->geom.lv[l].scale != right->geom.lv[l].scale) {
-            set_error("left/right extractors differ in scale factor at level %d (%g vs %g)", l, (double)left->geom.lv[l].scale,
-                      (double)right->geom.lv[l].scale);
-            return BORB_ERR_INVALID_ARG;
-        }
+    borb_status st = check_stereo_pair(left, right);
+    if (st != BORB_OK) return st;
     BORB_CUDA(cudaSetDevice(left->device));
     BORB_CUDA(cudaStreamSynchronize(right->stream));   // right results must be complete before left's stream reads them
     begin_step(left);
-    borb_status st = enqueue_stereo(left, right, 1, nullptr, nullptr, bf, b);
+    st = enqueue_stereo(left, right, 1, nullptr, nullptr, bf, b);
     if (st != BORB_OK) return st;
     if ((st = download_stereo(left, 1, u_right, depth, cap)) != BORB_OK) return st;
     mark(left, 8);

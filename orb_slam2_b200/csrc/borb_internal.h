@@ -166,6 +166,11 @@ struct StereoView {          // device pointers of one side of a stereo pair set
 int launch_stereo(const Geometry& g, const StereoView& L, const StereoView& R, const int* d_pair_idx, int n_pairs,
                   float bf, float b, float* d_u_right, float* d_depth, int* d_sad, int out_stride, int* d_bins, void* d_recs,
                   int rec_stride, cudaStream_t s);
+// borb_stereo_match2's state and geometry checks of a (left, right) handle pair
+borb_status check_stereo_pair(const borb_extractor* left, const borb_extractor* right);
+// Frame::ComputeStereoMatches of image 0 of `left` against image 0 of `right` on the left handle's stream, results left in the
+// left handle's workspace as pair 0; the right handle's extraction must be complete
+borb_status enqueue_stereo_pair(borb_extractor* left, borb_extractor* right, float bf, float b);
 int stereo_rec_stride(const Geometry& g);   // records per pair for right images of geometry g
 size_t stereo_bins_bytes_per_pair();
 size_t stereo_rec_bytes();

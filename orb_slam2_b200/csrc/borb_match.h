@@ -371,6 +371,17 @@ int launch_frame_build(const FrameJob* d_jobs, int n_jobs, int max_n, const borb
                        int h, int out_cap, borb_keypoint* keys_out, float* ur_out, float* depth_out, cudaStream_t s);
 // Frame::AssignFeaturesToGrid of n_jobs frames (a FrameJob table the kernel can read) in one launch; max_n = the most keys of a job
 int launch_grid_sort(const FrameJob* d_jobs, int n_jobs, int max_n, cudaStream_t s);
+// Copies whose lengths are device-side counts (an extraction's keypoint count, a grid's size), written by host_copy_kernel straight
+// into mapped pinned memory: only the bytes of the counted elements cross PCIe and the host needs no count beforehand.
+struct HostCopy {
+    const void* src;
+    void* dst;
+    const int* count;     // elements: *count, or `fixed` when null
+    int fixed;
+    int elem_words;       // 32-bit words per element
+};
+struct HostCopies { HostCopy seg[8]; int n; };
+int launch_host_copy(const HostCopies& c, cudaStream_t s);
 // pack + match + finalize over A.jobs (3 launches): one = a host copy of job 0 (what the match kernel reads of a single job),
 // max_smem_frame = largest frame_bytes of the jobs with frame_in_smem, max_items = an upper bound of the work items of all jobs,
 // total_kf = sum of their n_kf; kfkf: the jobs are SearchByBoW(KeyFrame*, KeyFrame*) of a database slot against candidates

@@ -32,6 +32,7 @@ struct borb_matcher : CallBuffers {
     int n_sm = 1;                   // the device's multiprocessor count (sizes the persistent grids)
     std::vector<int32_t> sel;       // indices of the valid queries of the current call
     cudaEvent_t ev_a = nullptr, ev_b = nullptr;   // cross-stream ordering with an extractor handle (borb_frames_from_extractor)
+    cudaEvent_t ev_r = nullptr;     // borb_frame_from_extractors: the right handle's extraction before the left stream's association
     bool timing = false;            // borb_matcher_set_timing: CUDA events around the kernels of the database search
     cudaEvent_t t0 = nullptr, t1 = nullptr;
     float last_ms = 0.f;
@@ -505,6 +506,7 @@ borb_status borb_matcher_destroy(borb_matcher* m) {
     if (!m) return BORB_OK;
     free_call_buffers(*m);
     if (m->ev_a) { cudaEventDestroy(m->ev_a); cudaEventDestroy(m->ev_b); }
+    if (m->ev_r) cudaEventDestroy(m->ev_r);
     if (m->t0) { cudaEventDestroy(m->t0); cudaEventDestroy(m->t1); }
     delete m;
     return BORB_OK;
@@ -609,17 +611,89 @@ borb_status borb_frame_destroy(borb_frame* f) {
     return BORB_OK;
 }
 
+namespace {
+// What borb_frame_from_extractors adds to the one-frame build of image 0: the extractors' own keypoints and descriptors and the
+// feature grid, copied into the same result region as mvKeysUn / mvuRight / mvDepth.
+struct FrameHostCopies {
+    borb_frame_host* host;
+    const borb_extractor* right;    // stereo: mvKeysRight / mDescriptorsRight come from image 0 of this handle
+    int n_right;
+};
+
+borb_status check_frames_args(borb_matcher* m, borb_extractor* e, const borb_camera* cam, int mode, const void* depth, int depth_type) {
+    depth_type &= 3;
+    if (mode < 0 || mode > 2 || (mode == 2 && !depth) || (depth_type != 0 && depth_type != 1)) { set_error("bad mode / depth arguments"); return BORB_ERR_INVALID_ARG; }
+    if (!e->have_geom || e->last_n_images < 1) { set_error("no extracted batch on this extractor handle"); return BORB_ERR_STATE; }
+    if (e->device != m->device) { set_error("extractor and matcher live on different devices"); return BORB_ERR_INVALID_ARG; }
+    (void)cam;
+    return BORB_OK;
+}
+
+borb_status build_frames(borb_matcher* m, borb_extractor* e, const int32_t* images, int n_frames, const int32_t* n_keys,
+                         const borb_camera* cam, int mode, const void* const* depth, int depth_type, float depth_factor,
+                         int depth_stride_bytes, borb_keypoint* keys_un, float* u_right, float* depth_out, int cap,
+                         float* bounds4, borb_frame** frames, const FrameHostCopies* hc);
+}  // namespace
+
 borb_status borb_frames_from_extractor(borb_matcher* m, borb_extractor* e, const int32_t* images, int n_frames, const int32_t* n_keys,
                                        const borb_camera* cam, int mode, const void* const* depth, int depth_type, float depth_factor,
                                        int depth_stride_bytes, borb_keypoint* keys_un, float* u_right, float* depth_out, int cap,
                                        float* bounds4, borb_frame** frames) {
     if (!m || !e || !cam || !frames || n_frames < 0 || (n_frames > 0 && (!images || !n_keys))) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }
+    borb_status s = check_frames_args(m, e, cam, mode, depth, depth_type);
+    if (s != BORB_OK) return s;
+    if ((keys_un || u_right || depth_out) && cap < 0) { set_error("negative capacity"); return BORB_ERR_INVALID_ARG; }
+    return build_frames(m, e, images, n_frames, n_keys, cam, mode, depth, depth_type, depth_factor, depth_stride_bytes, keys_un, u_right,
+                        depth_out, cap, bounds4, frames, nullptr);
+}
+
+borb_status borb_frame_from_extractors(borb_matcher* m, borb_extractor* left, borb_extractor* right, const borb_camera* cam, int mode,
+                                       float b, const void* depth, int depth_type, float depth_factor, int depth_stride_bytes,
+                                       borb_frame_host* host, borb_frame** out) {
+    if (!m) { set_error("null argument: m"); return BORB_ERR_INVALID_ARG; }
+    if (!left) { set_error("null argument: left"); return BORB_ERR_INVALID_ARG; }
+    if (!cam) { set_error("null argument: cam"); return BORB_ERR_INVALID_ARG; }
+    if (!host) { set_error("null argument: host"); return BORB_ERR_INVALID_ARG; }
+    if (!out) { set_error("null argument: out"); return BORB_ERR_INVALID_ARG; }
+    *out = nullptr;
+    host->n = host->n_right = 0;
+    if (host->cap < 0) { set_error("host->cap is negative (%d)", host->cap); return BORB_ERR_INVALID_ARG; }
+    if ((mode == 1) != (right != nullptr)) { set_error("right: a stereo frame (mode 1) takes a right handle, other modes none"); return BORB_ERR_INVALID_ARG; }
+    if (right == left) { set_error("right: the same handle as left"); return BORB_ERR_INVALID_ARG; }
+    if (mode == 1 && !(b > 0.f)) { set_error("b: mb = mbf/fx must be positive (%g)", (double)b); return BORB_ERR_INVALID_ARG; }
+    borb_status s = check_frames_args(m, left, cam, mode, depth, depth_type);
+    if (s != BORB_OK) return s;
+    if (right && (s = check_stereo_pair(left, right)) != BORB_OK) return s;
+    // the frame is built before its keypoint counts reach the host: everything is sized by the handles' capacities (one image each)
+    const int bound = left->geom.sel_image_stride, bound_r = right ? right->geom.sel_image_stride : 0;
+    if (bound > MATCH_MAX_FEATURES || bound_r > MATCH_MAX_FEATURES) {
+        set_error("left/right: up to %d / %d keypoints per image (limit %d per frame)", bound, bound_r, MATCH_MAX_FEATURES);
+        return BORB_ERR_INVALID_ARG;
+    }
+    if (host->cap < bound || host->cap < bound_r) {
+        set_error("host->cap %d: the handles return up to %d / %d keypoints (borb_extractor_capacity)", host->cap, bound, bound_r);
+        return BORB_ERR_CAPACITY;
+    }
+    BORB_CUDA(cudaSetDevice(m->device));
+    if (right) {    // the association on the left stream reads the right handle's extraction: ordered by an event, not by the host
+        if (!m->ev_r) BORB_CUDA(cudaEventCreateWithFlags(&m->ev_r, cudaEventDisableTiming));
+        BORB_CUDA(cudaEventRecord(m->ev_r, right->stream));
+        BORB_CUDA(cudaStreamWaitEvent(left->stream, m->ev_r, 0));
+        if ((s = enqueue_stereo_pair(left, right, cam->bf, b)) != BORB_OK) return s;
+    }
+    const int32_t image = 0;
+    const FrameHostCopies hc{host, right, bound_r};
+    return build_frames(m, left, &image, 1, &bound, cam, mode, mode == 2 ? &depth : nullptr, depth_type, depth_factor, depth_stride_bytes,
+                        host->keys_un, host->u_right, host->depth, bound, host->bounds, out, &hc);
+}
+
+namespace {
+borb_status build_frames(borb_matcher* m, borb_extractor* e, const int32_t* images, int n_frames, const int32_t* n_keys,
+                         const borb_camera* cam, int mode, const void* const* depth, int depth_type, float depth_factor,
+                         int depth_stride_bytes, borb_keypoint* keys_un, float* u_right, float* depth_out, int cap,
+                         float* bounds4, borb_frame** frames, const FrameHostCopies* hc) {
     const bool depth_on_device = (depth_type & 4) != 0;
     depth_type &= 3;
-    if (mode < 0 || mode > 2 || (mode == 2 && !depth) || (depth_type != 0 && depth_type != 1)) { set_error("bad mode / depth arguments"); return BORB_ERR_INVALID_ARG; }
-    if (!e->have_geom || e->last_n_images < 1) { set_error("no extracted batch on this extractor handle"); return BORB_ERR_STATE; }
-    if (e->device != m->device) { set_error("extractor and matcher live on different devices"); return BORB_ERR_INVALID_ARG; }
-    if ((keys_un || u_right || depth_out) && cap < 0) { set_error("negative capacity"); return BORB_ERR_INVALID_ARG; }
     const Geometry& g = e->geom;
     const int w = g.w, h = g.h, nl = g.nlevels;
     float b4[4];
@@ -654,6 +728,18 @@ borb_status borb_frames_from_extractor(borb_matcher* m, borb_extractor* e, const
     // the requested outputs; the kernel writes depth_out wherever it writes u_right
     const size_t kb = keys_un ? (size_t)n_frames * ocap * sizeof(borb_keypoint) : 0, fb = (u_right || depth_out) ? (size_t)n_frames * ocap * 4 : 0;
     const size_t r_k = c.result(kb), r_u = c.result(fb), r_d = c.result(fb);
+    // borb_frame_from_extractors: one frame, image 0, sized by the handles' capacities; its counts, mvKeys / mDescriptors (and the
+    // right image's) and the grid join the results, and every result is written straight into the landing buffer by the kernels,
+    // only as many elements as the device-side counts say
+    borb_frame_host* H = hc ? hc->host : nullptr;
+    const bool direct = H != nullptr;
+    const size_t n0 = (size_t)n_keys[0], nr = hc ? (size_t)hc->n_right : 0;
+    const bool want_grid = H && (H->cell_start || H->cell_idx);
+    const size_t xk = H && H->keys ? n0 * sizeof(borb_keypoint) : 0, xd = H && H->desc ? n0 * 32 : 0;
+    const size_t xkr = H && H->keys_right ? nr * sizeof(borb_keypoint) : 0, xdr = H && H->desc_right ? nr * 32 : 0;
+    const size_t xcs = want_grid ? (size_t)(GRID_CELLS + 1) * 4 : 0, xci = H && H->cell_idx ? n0 * 4 : 0;
+    const size_t r_xk = c.result(xk), r_xd = c.result(xd), r_xkr = c.result(xkr), r_xdr = c.result(xdr), r_xcs = c.result(xcs), r_xci = c.result(xci);
+    const size_t r_cnt = c.result(H ? 2 * sizeof(int32_t) : 0);
     if ((s = c.begin()) != BORB_OK) return fail(s);
     FrameJob* hj = c.host<FrameJob>(o_jobs);
     const float invW = (float)GRID_COLS / (float)(b4[2] - b4[0]), invH = (float)GRID_ROWS / (float)(b4[3] - b4[1]);
@@ -683,13 +769,54 @@ borb_status borb_frames_from_extractor(borb_matcher* m, borb_extractor* e, const
             BORB_CUDA(cudaMemcpy2DAsync(c.dev(o_depth) + (size_t)i * depth_img_bytes, (size_t)w * px, depth[i], (size_t)depth_stride_bytes, (size_t)w * px, h,
                                         cudaMemcpyHostToDevice, q));
     for (int i = 0; i < n_frames; i++) BORB_CUDA(cudaMemcpyAsync(frames[i]->sf, c.dev(o_sf), (size_t)nl * 4, cudaMemcpyDeviceToDevice, q));
+    // the frame's keypoint count is the extraction's, read on the device
+    if (H) BORB_CUDA(cudaMemcpyAsync(c.dev(o_jobs) + offsetof(FrameJob, n), e->ws.nkp, sizeof(int), cudaMemcpyDeviceToDevice, q));
     m->launches += launch_frame_build((const FrameJob*)c.dev(o_jobs), n_frames, max_n, *cam, mode, depth_type, depth_factor, w, h, ocap,
-                                      keys_un ? (borb_keypoint*)c.res(r_k, false) : nullptr, fb ? (float*)c.res(r_u, false) : nullptr,
-                                      (float*)c.res(r_d, false), q);
+                                      keys_un ? (borb_keypoint*)c.res(r_k, direct) : nullptr, fb ? (float*)c.res(r_u, direct) : nullptr,
+                                      (float*)c.res(r_d, direct), q);
+    if (H) {
+        const int* cnt_r = hc->right ? hc->right->ws.nkp : nullptr;
+        HostCopies hcp{};
+        auto seg = [&](size_t r, size_t bytes, const void* src, const int* count, int fixed, int elem_words) {
+            if (bytes) hcp.seg[hcp.n++] = HostCopy{src, c.res(r, true), count, fixed, elem_words};
+        };
+        seg(r_cnt, 4, e->ws.nkp, nullptr, 1, 1);
+        seg(r_cnt + 4, hc->right ? 4 : 0, cnt_r, nullptr, 1, 1);
+        seg(r_xk, xk, e->ws.kps, e->ws.nkp, 0, sizeof(borb_keypoint) / 4);
+        seg(r_xd, xd, e->ws.desc, e->ws.nkp, 0, 8);
+        seg(r_xkr, xkr, hc->right ? (const void*)hc->right->ws.kps : nullptr, cnt_r, 0, sizeof(borb_keypoint) / 4);
+        seg(r_xdr, xdr, hc->right ? (const void*)hc->right->ws.desc : nullptr, cnt_r, 0, 8);
+        seg(r_xcs, xcs, frames[0]->cell_start, nullptr, GRID_CELLS + 1, 1);
+        seg(r_xci, xci, frames[0]->cell_idx, frames[0]->cell_start + GRID_CELLS, 0, 1);
+        m->launches += launch_host_copy(hcp, q);
+    }
     for (int i = 0; i < n_frames; i++) BORB_CUDA(cudaEventRecord(frames[i]->ready, q));
     BORB_CUDA(cudaEventRecord(m->ev_b, q));
     BORB_CUDA(cudaStreamWaitEvent(e->stream, m->ev_b, 0));
+    if (hc && hc->right) BORB_CUDA(cudaStreamWaitEvent(hc->right->stream, m->ev_b, 0));
     if ((s = c.finish()) != BORB_OK) return s;
+    if (H) {    // the one wait is over: the counts are known
+        const int32_t* cnt = (const int32_t*)c.out(r_cnt);
+        const int n = cnt[0], n_r = hc->right ? cnt[1] : 0;
+        if (n < 0 || (size_t)n > n0 || n_r < 0 || (size_t)n_r > nr) { set_error("keypoint counts %d / %d beyond the handles' capacities", n, n_r); return fail(BORB_ERR_STATE); }
+        frames[0]->n = n;
+        H->n = n; H->n_right = n_r;
+        if (keys_un) std::memcpy(keys_un, c.out(r_k), (size_t)n * sizeof(borb_keypoint));
+        if (u_right) std::memcpy(u_right, c.out(r_u), (size_t)n * 4);
+        if (depth_out) std::memcpy(depth_out, c.out(r_d), (size_t)n * 4);
+        if (xk) std::memcpy(H->keys, c.out(r_xk), (size_t)n * sizeof(borb_keypoint));
+        if (xd) std::memcpy(H->desc, c.out(r_xd), (size_t)n * 32);
+        if (xkr) std::memcpy(H->keys_right, c.out(r_xkr), (size_t)n_r * sizeof(borb_keypoint));
+        if (xdr) std::memcpy(H->desc_right, c.out(r_xdr), (size_t)n_r * 32);
+        if (want_grid) {
+            const int32_t* cs = (const int32_t*)c.out(r_xcs);
+            const int in_grid = cs[GRID_CELLS];
+            if (in_grid < 0 || in_grid > n) { set_error("grid of %d entries for %d features", in_grid, n); return fail(BORB_ERR_STATE); }
+            if (H->cell_start) std::memcpy(H->cell_start, cs, xcs);
+            if (H->cell_idx && in_grid > 0) std::memcpy(H->cell_idx, c.out(r_xci), (size_t)in_grid * 4);
+        }
+        return BORB_OK;
+    }
     if (ocap > 0) {
         if (keys_un) std::memcpy(keys_un, c.out(r_k), kb);
         if (u_right) std::memcpy(u_right, c.out(r_u), fb);
@@ -697,6 +824,7 @@ borb_status borb_frames_from_extractor(borb_matcher* m, borb_extractor* e, const
     }
     return BORB_OK;
 }
+}  // namespace
 
 borb_status borb_frame_info(const borb_frame* f, int32_t* n, int32_t* n_levels, int32_t* has_u_right) {
     if (!f) { set_error("null argument"); return BORB_ERR_INVALID_ARG; }

@@ -133,6 +133,21 @@ int launch_frame_build(const FrameJob* d_jobs, int n_jobs, int max_n, const borb
     return launches + launch_grid_sort(d_jobs, n_jobs, max_n, s);
 }
 
+// One segment per blockIdx.y (borb_frame_from_extractors: the counts, mvKeys, mDescriptors and the right image's, the grid).
+__global__ void __launch_bounds__(256) host_copy_kernel(HostCopies c) {
+    const HostCopy g = c.seg[blockIdx.y];
+    const size_t words = (size_t)(g.count ? *g.count : g.fixed) * (size_t)g.elem_words;
+    const uint32_t* __restrict__ src = reinterpret_cast<const uint32_t*>(g.src);
+    uint32_t* __restrict__ dst = reinterpret_cast<uint32_t*>(g.dst);
+    for (size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x; k < words; k += (size_t)gridDim.x * blockDim.x) dst[k] = src[k];
+}
+
+int launch_host_copy(const HostCopies& c, cudaStream_t s) {
+    if (c.n <= 0) return 0;
+    host_copy_kernel<<<dim3(16, c.n), 256, 0, s>>>(c);
+    return 1;
+}
+
 int launch_grid_sort(const FrameJob* d_jobs, int n_jobs, int max_n, cudaStream_t s) {
     int K = 32;
     while (K < max_n) K <<= 1;

@@ -146,6 +146,18 @@ class ORBextractor:
         self._last_n = n
         return [(kps[i, :cnt[i]].copy(), desc[i, :cnt[i]].copy()) for i in range(n)]
 
+    def extract_enqueue(self, image: np.ndarray) -> None:
+        """borb_extract_batch_enqueue of one CV_8UC1 image with no host copies: the keypoints stay on the device for
+        matcher.frame_from_extractors (the Frame constructors' ExtractORB, src/Frame.cc:247-253)."""
+        image = np.ascontiguousarray(image, np.uint8)
+        assert image.ndim == 2, "CV_8UC1 expected"
+        self._set_format(1)
+        h, w = image.shape
+        ptrs = (C.c_void_p * 1)(image.ctypes.data)
+        check(self._lib.borb_extract_batch_enqueue(self._h, ptrs, 1, w, h, image.strides[0], None, None, 0, None),
+              "borb_extract_batch_enqueue")
+        self._last_n = 1
+
     # ---- mvImagePyramid (ORBextractor.h:85) of image `image` of the last call
     def pyramid(self, level: int, image: int = 0) -> np.ndarray:
         w, h = C.c_int32(), C.c_int32()

@@ -320,6 +320,52 @@ def frames_from_extractor(matcher: "ORBmatcher", extractor, images, n_keys, K, d
                      depth=[dp[i, :nk[i]] for i in range(nf)], bounds=b4)
 
 
+class _FrameHostC(C.Structure):
+    _fields_ = [("cap", C.c_int32)] + [(n, C.c_void_p) for n in ("keys", "desc", "keys_right", "desc_right", "keys_un", "u_right", "depth",
+                                                                  "cell_start", "cell_idx")] + \
+               [("n", C.c_int32), ("n_right", C.c_int32), ("bounds", C.c_float * 4)]
+
+
+def frame_from_extractors(matcher: "ORBmatcher", left, right, K, dist=(0, 0, 0, 0, 0), bf: float = 0.0, fx: Optional[float] = None,
+                          mode: int = 0, depth=None, depth_factor: float = 1.0):
+    """borb_frame_from_extractors: one Frame constructor after left.extract_enqueue (and right.extract_enqueue for a stereo frame,
+    mode 1; mb = bf/fx as float32, src/Frame.cc:114).  mode 2 takes one (h, w) float32 (metres) or uint16 (raw) depth map.
+    Returns (frame, host): frame is a FrameView bound to the resident frame, host holds every member the constructor fills —
+    mvKeys, mDescriptors, mvKeysRight, mDescriptorsRight, mvKeysUn, mvuRight, mvDepth, the grid as cell_start / cell_idx
+    (borb_debug_frame_read's layout) and bounds."""
+    lib = _lib.load()
+    w, h = left._shape()
+    cap = max(left.capacity(w, h), right.capacity(w, h) if right is not None else 0, 1)
+    a = dict(keys=np.zeros(cap, KP_DTYPE), desc=np.zeros((cap, 32), np.uint8), keys_right=np.zeros(cap, KP_DTYPE),
+             desc_right=np.zeros((cap, 32), np.uint8), keys_un=np.zeros(cap, KP_DTYPE), u_right=np.zeros(cap, np.float32),
+             depth=np.zeros(cap, np.float32), cell_start=np.zeros(64 * 48 + 1, np.int32), cell_idx=np.zeros(cap, np.int32))
+    hs = _FrameHostC(cap, *[_p(a[k]) for k in ("keys", "desc", "keys_right", "desc_right", "keys_un", "u_right", "depth", "cell_start",
+                                               "cell_idx")])
+    d5 = list(dist) + [0.0] * (5 - len(dist))
+    cam = _CameraC(*[float(x) for x in K], *[float(x) for x in d5], float(bf))
+    b = float(np.float32(bf) / np.float32(fx if fx is not None else K[0]))
+    dptr, dtype_flag, stride = None, 0, 0
+    if mode == 2:
+        dmap = np.ascontiguousarray(depth)
+        dtype_flag = 1 if dmap.dtype == np.uint16 else 0
+        dmap = np.ascontiguousarray(dmap, np.uint16 if dtype_flag else np.float32)
+        dptr, stride = dmap.ctypes.data, dmap.strides[0]
+    out = C.c_void_p()
+    check(lib.borb_frame_from_extractors(matcher._h, left._h, right._h if right is not None else None, C.byref(cam), int(mode), b, dptr,
+                                         dtype_flag, float(np.float32(depth_factor)), int(stride), C.byref(hs), C.byref(out)),
+          "borb_frame_from_extractors")
+    n, nr = hs.n, hs.n_right
+    rf = ResidentFrame.__new__(ResidentFrame)
+    rf._lib, rf._h, rf.n = lib, out, n
+    bounds = tuple(float(x) for x in hs.bounds)
+    host = dict(mvKeys=a["keys"][:n], mDescriptors=a["desc"][:n], mvKeysRight=a["keys_right"][:nr], mDescriptorsRight=a["desc_right"][:nr],
+                mvKeysUn=a["keys_un"][:n], mvuRight=a["u_right"][:n], mvDepth=a["depth"][:n], cell_start=a["cell_start"],
+                cell_idx=a["cell_idx"][:a["cell_start"][-1]], bounds=bounds)
+    F = FrameView(mvKeysUn=host["mvKeysUn"], mDescriptors=host["mDescriptors"], mvScaleFactors=left.GetScaleFactors(), bounds=bounds,
+                  mvuRight=host["mvuRight"] if mode else None, resident=rf)
+    return F, host
+
+
 def dataclass_replace_resident(F):
     import dataclasses
     return dataclasses.replace(F, resident=None)

@@ -15,6 +15,16 @@ print("stereo", len(out[0]["mvKeys"]), int((out[0]["mvuRight"] >= 0).sum()))
 G2 = ORBextractor(500)
 k, d = G2(synth.white_noise(1, 400, 300))
 print("noise", len(k))
+# one Frame constructor of each kind on the frame's own handles (borb_frame_from_extractors)
+XL, XR = ORBextractor(1000), ORBextractor(1200)
+XL.extract_enqueue(L); XR.extract_enqueue(R)
+Fs, hs = M.frame_from_extractors(M.ORBmatcher(0.8, True), XL, XR, (525.0, 525.0, 319.5, 239.5), bf=40.0, mode=1)
+XL.extract_enqueue(L)
+Fd, hd = M.frame_from_extractors(M.ORBmatcher(0.8, True), XL, None, (525.0, 525.0, 319.5, 239.5), (0.26, -0.95, 0.0, 0.0, 1.16), bf=40.0,
+                                 mode=2, depth=np.full(L.shape, 6000, np.uint16), depth_factor=1.0 / 5000.0)
+XL.extract_enqueue(R)
+Fm, hm = M.frame_from_extractors(M.ORBmatcher(0.8, True), XL, None, (525.0, 525.0, 319.5, 239.5))
+print("frame ctors", len(hs["mvKeys"]), int((hs["mvuRight"] >= 0).sum()), int((hd["mvDepth"] > 0).sum()), len(hm["cell_idx"]))
 # geometry edges (tests/extract_geometry.py): the smallest accepted frame, a frame whose level-0 pitch is exactly its width + 8
 # (no slack after the padding), and a level 0 one candidate over the quadtree's on-chip limit
 from tests import extract_geometry as EG
