@@ -1,8 +1,8 @@
 // TEST INFRASTRUCTURE ONLY (oracle/).  Force-included (-include) ahead of /root/reference/src/Frame.cc so that it compiles
-// VERBATIM against the reference's REAL include/Frame.h (oracle/Makefile target `ref`, library _ref/libframeref.so): the include
+// VERBATIM against the reference's REAL include/Frame.h (oracle/Makefile target `ref`, libraries _ref/libframeref.so and _ref/libframector.so): the include
 // guards of the headers Frame.h pulls in are pre-defined, and plain-data stand-ins with the members Frame.cc touches take
-// their place.  Frame.cc then provides, unmodified: ComputeStereoMatches (:466-640), AssignFeaturesToGrid / PosInGrid /
-// GetFeaturesInArea (:230-245, :327-392) and isInFrustum (:269-325).
+// their place.  Frame.cc then provides, unmodified: the three constructors (:61-228), ComputeStereoMatches (:466-640),
+// AssignFeaturesToGrid / PosInGrid / GetFeaturesInArea (:230-245, :327-392) and isInFrustum (:269-325).
 #pragma once
 #define MAPPOINT_H
 #define KEYFRAME_H
@@ -48,13 +48,22 @@ public:
     int PredictScale(const float& currentDist, Frame* pF);                 // :402-417, defined in frameref_wrap.cpp
 };
 
+// The extractor of a Frame constructor (framector_run in framector_wrap.cpp): operator() replays the keypoints and descriptors
+// that the verbatim src/ORBextractor.cc (liborbref.so) found on the same image, and the pyramid and scale tables are that run's.  As the real
+// extractor does (ORBextractor.cc:1065-1068), an image without keypoints gives an empty descriptor matrix.
 class ORBextractor {
 public:
     std::vector<cv::Mat> mvImagePyramid;
     std::vector<float> mvScaleFactor, mvInvScaleFactor, mvLevelSigma2, mvInvLevelSigma2;
-    void operator()(const cv::Mat&, const cv::Mat&, std::vector<cv::KeyPoint>&, cv::Mat&) {}     // never run by the oracle
+    float scaleFactor = 1.2f;                       // ORBextractor::scaleFactor (a double set from the float argument)
+    std::vector<cv::KeyPoint> replayKeys;
+    cv::Mat replayDesc;
+    void operator()(const cv::Mat&, const cv::Mat&, std::vector<cv::KeyPoint>& keys, cv::Mat& desc) {
+        keys = replayKeys;
+        if (replayKeys.empty()) desc.release(); else desc = replayDesc.clone();
+    }
     int GetLevels() { return (int)mvScaleFactor.size(); }
-    float GetScaleFactor() { return mvScaleFactor.size() > 1 ? mvScaleFactor[1] : 1.f; }
+    float GetScaleFactor() { return scaleFactor; }
     std::vector<float> GetScaleFactors() { return mvScaleFactor; }
     std::vector<float> GetInverseScaleFactors() { return mvInvScaleFactor; }
     std::vector<float> GetScaleSigmaSquares() { return mvLevelSigma2; }

@@ -1126,6 +1126,83 @@ def port_rgbd_frame(keys, K4, dist, bf, depth):
     return dict(keys_un=ku[:n], u_right=ur[:n], depth=dp[:n], bounds=b4, count=cnt)
 
 
+# The reference's three Frame constructors, run unmodified (oracle/_ref/libframector.so, oracle/framector_wrap.cpp).
+FRAMECTOR_SO = os.path.join(HERE, "_ref", "libframector.so")
+FRAME_KINDS = {"mono": 0, "stereo": 1, "rgbd": 2}
+
+
+def have_framector() -> bool:
+    return os.path.exists(FRAMECTOR_SO)
+_REF_EXTRACTORS = {}
+
+
+def ref_extractor(nfeatures, scale_factor=1.2, nlevels=8):
+    """A RefExtractor per configuration, shared by the callers of this process: liborbref.so gives every handle an arena it never
+    unmaps, and a process can hold at most 256 of them."""
+    key = (int(nfeatures), float(np.float32(scale_factor)), int(nlevels))
+    if key not in _REF_EXTRACTORS:
+        _REF_EXTRACTORS[key] = RefExtractor(*key)
+    return _REF_EXTRACTORS[key]
+
+
+def ref_frame(kind, left, right=None, nfeatures=(2000, 2000), scale_factor=1.2, nlevels=8, K=(0, 0, 0, 0), dist=(0, 0, 0, 0), bf=0.0,
+              th_depth=0.0, depth=None, mb=None, fresh=True):
+    """One of the reference's own Frame constructors (src/Frame.cc:61-228, libframector.so framector_run), run unmodified on the
+    keypoints, descriptors, pyramid and scale tables that the verbatim ORBextractor.cc (RefExtractor) finds on `left` (and
+    `right` for a stereo frame).  kind: "mono" / "stereo" / "rgbd" (or 0 / 1 / 2); nfeatures: (left, right) extractor sizes;
+    K = (fx, fy, cx, cy); dist as Tracking builds mDistCoef (4 or 5 entries); depth: the (h, w) float32 map Tracking hands the
+    RGB-D constructor.  mb pre-fills the storage the constructor reads before it assigns mb (default float32(bf)/float32(fx)).
+    fresh sets Frame::mbInitialComputations first, as in a new process; fresh=False continues the previous call's statics.
+    Returns a dict of every member the constructor sets, the grid flattened as ref_assign_grid does, and the statics."""
+    kind = FRAME_KINDS.get(kind, kind)
+    lib = C.CDLL(FRAMECTOR_SO)
+    left = np.ascontiguousarray(left, np.uint8)
+    h, w = left.shape
+    sides = [left] + ([np.ascontiguousarray(right, np.uint8)] if kind == 1 else [])
+    nf = tuple(nfeatures) if np.ndim(nfeatures) else (nfeatures, nfeatures)
+    ext, kd, pyr, tabs = [], [], [], []
+    for s, img in enumerate(sides):
+        E = ref_extractor(nf[s], scale_factor, nlevels)        # each result is copied out before the handle runs again
+        k, d = E(img)
+        ext.append(E); kd.append((np.ascontiguousarray(k), np.ascontiguousarray(d, np.uint8)))
+        pyr.append([np.ascontiguousarray(E.level(l), np.uint8) for l in range(nlevels)])
+        tabs.append(np.ascontiguousarray(np.concatenate([E.scale, E.inv_scale, E.sigma2, E.inv_sigma2]), np.float32))
+    if kind != 1:
+        kd.append((np.zeros(0, KP_DTYPE), np.zeros((0, 32), np.uint8))); pyr.append(pyr[0]); tabs.append(tabs[0])
+    lw = np.array([p.shape[1] for p in pyr[0]], np.int32); lh = np.array([p.shape[0] for p in pyr[0]], np.int32)
+    PL = (C.c_void_p * nlevels)(*[p.ctypes.data for p in pyr[0]])
+    PR = (C.c_void_p * nlevels)(*[p.ctypes.data for p in pyr[1]])
+    K4 = np.ascontiguousarray(K, np.float32); D = np.ascontiguousarray(dist, np.float32)
+    dmap = np.ascontiguousarray(depth, np.float32) if kind == 2 else None
+    if dmap is not None:
+        assert dmap.shape == (h, w)
+    b = np.float32(bf) / np.float32(K4[0]) if mb is None else np.float32(mb)
+    (kl, dl), (kr, dr) = kd
+    cap = max(len(kl), len(kr), 1)
+    i_out = np.zeros(9, np.int64); f_out = np.zeros(17, np.float32); sc = np.zeros(4 * nlevels, np.float32)
+    keys = np.zeros(cap, KP_DTYPE); desc = np.zeros((cap, 32), np.uint8); keys_r = np.zeros(cap, KP_DTYPE); desc_r = np.zeros((cap, 32), np.uint8)
+    keys_un = np.zeros(cap, KP_DTYPE); ur = np.zeros(cap, np.float32); dp = np.zeros(cap, np.float32)
+    cs = np.zeros(GRID_CELLS + 1, np.int32); ci = np.zeros(cap, np.int32)
+    fn = lib.framector_run
+    fn.restype = C.c_int
+    fn.argtypes = [C.c_int] * 4 + [C.c_void_p, C.c_void_p, C.c_int] * 2 + [C.c_void_p] * 4 + [C.c_int, C.c_void_p, C.c_void_p, C.c_float,
+                                                                                                C.c_void_p, C.c_void_p, C.c_int] + \
+        [C.c_float] * 3 + [C.c_void_p] * 13
+    fn(kind, int(bool(fresh)), w, h, _ptr(kl), _ptr(dl), len(kl), _ptr(kr), _ptr(dr), len(kr), PL, PR, _ptr(lw), _ptr(lh), nlevels,
+       _ptr(tabs[0]), _ptr(tabs[1]), float(np.float32(scale_factor)), _ptr(K4), _ptr(D), len(D), float(bf), float(th_depth), float(b),
+       _ptr(dmap), _ptr(i_out), _ptr(f_out), _ptr(sc), _ptr(keys), _ptr(desc), _ptr(keys_r), _ptr(desc_r), _ptr(keys_un), _ptr(ur),
+       _ptr(dp), _ptr(cs), _ptr(ci))
+    mnId, N, Nr, in_grid, levels, n_un, n_ur, n_dp, init_left = (int(x) for x in i_out)
+    L = nlevels
+    return dict(mnId=mnId, N=N, mvKeys=keys[:N], mDescriptors=desc[:N], mvKeysRight=keys_r[:Nr], mDescriptorsRight=desc_r[:Nr],
+                mvKeysUn=keys_un[:n_un], mvuRight=ur[:n_ur], mvDepth=dp[:n_dp], cell_start=cs, cell_idx=ci[:in_grid],
+                bounds=f_out[0:4].copy(), grid_inv=f_out[4:6].copy(), fx=f_out[6], fy=f_out[7], cx=f_out[8], cy=f_out[9],
+                invfx=f_out[10], invfy=f_out[11], mb=f_out[12], mbf=f_out[13], mThDepth=f_out[14], mfScaleFactor=f_out[15],
+                mfLogScaleFactor=f_out[16], mnScaleLevels=levels, mvScaleFactors=sc[0:L].copy(), mvInvScaleFactors=sc[L:2 * L].copy(),
+                mvLevelSigma2=sc[2 * L:3 * L].copy(), mvInvLevelSigma2=sc[3 * L:].copy(), mbInitialComputations=bool(init_left),
+                extractor_keys=kd, extractor_tables=tabs[0], pyramid=pyr[0], pyramid_right=pyr[1] if kind == 1 else None)
+
+
 def port_depth_to_float(raw, factor):
     lib = _plib()
     raw = _a(raw, np.uint16)

@@ -345,10 +345,12 @@ def frame_from_extractors(matcher: "ORBmatcher", left, right, K, dist=(0, 0, 0, 
     cam = _CameraC(*[float(x) for x in K], *[float(x) for x in d5], float(bf))
     b = float(np.float32(bf) / np.float32(fx if fx is not None else K[0]))
     dptr, dtype_flag, stride = None, 0, 0
-    if mode == 2:
-        dmap = np.ascontiguousarray(depth)
+    if mode == 2:       # a map whose rows are contiguous keeps its row stride (a padded cv::Mat's step)
+        dmap = np.asarray(depth)
         dtype_flag = 1 if dmap.dtype == np.uint16 else 0
-        dmap = np.ascontiguousarray(dmap, np.uint16 if dtype_flag else np.float32)
+        dt = np.uint16 if dtype_flag else np.float32
+        if dmap.dtype != dt or dmap.ndim != 2 or dmap.strides[1] != dmap.itemsize or dmap.strides[0] < dmap.shape[1] * dmap.itemsize:
+            dmap = np.ascontiguousarray(dmap, dt)
         dptr, stride = dmap.ctypes.data, dmap.strides[0]
     out = C.c_void_p()
     check(lib.borb_frame_from_extractors(matcher._h, left._h, right._h if right is not None else None, C.byref(cam), int(mode), b, dptr,
