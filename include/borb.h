@@ -954,17 +954,10 @@ BORB_API borb_status borb_debug_brief_slots(uint32_t* dst, int cap, int* n_bins)
  * are defined for 0 <= a < 120 and logf for positive normal a (the inputs those kernels form).  Runs on the current device
  * on a stream of its own and returns when out is written; b may be NULL for fn 0, 1 and 3. */
 BORB_API borb_status borb_debug_eval_math(int fn, const float* a, const float* b, int n, float log_scale, int n_levels, void* out);
-/* Distance arithmetic of the database SearchByBoW kernel: 2 (default) = three 3:2 compressors + 5 POPC per 256-bit distance,
- * 1 = full carry-save adder tree + 4 POPC, 0 = 8 POPC.  Same results; kept switchable for measurements.  Applies to the
- * relocalisation search (borb_search_by_bow_db*); the loop-closure search (borb_search_by_bow_kf_db_*) always uses mode 2. */
-BORB_API borb_status borb_debug_set_bow_csa(int mode);
 /* Fills every buffer the library reuses or recycles with `byte` (0..255) before a call writes it, -1 (the default) stops: matcher
  * and vocabulary staging, arena and landing buffers, resident frame and keyframe blocks, the extractor workspace (DESIGN.md, "Buffer
  * reuse").  Process-wide; for tests that pin results to the unpoisoned run.  Other values give BORB_ERR_INVALID_ARG. */
 BORB_API borb_status borb_debug_set_poison(int byte);
-/* Work-item size of the same kernel: keyframes per item = target / (bucket width)^2, clamped to [1, 32] (default 2560); a negative
- * target selects the static item-to-warp schedule instead of the atomic work counter. */
-BORB_API borb_status borb_debug_set_bow_item_target(int target);
 /* Kernel launches issued by this handle since creation (bench.py's gpu_launches). */
 BORB_API borb_status borb_launch_count(const borb_extractor* e, uint64_t* n);
 /* Device time (ms, CUDA events on the handle's stream) of each stage of the last batch:

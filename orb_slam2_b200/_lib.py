@@ -143,8 +143,6 @@ _SIGNATURES = {
     "borb_matcher_set_timing": (C.c_int, [vp, C.c_int]),
     "borb_matcher_last_kernel_ms": (C.c_int, [vp, f32p]),
     "borb_matcher_launch_count": (C.c_int, [vp, C.POINTER(C.c_uint64)]),
-    "borb_debug_set_bow_csa": (C.c_int, [C.c_int]),
-    "borb_debug_set_bow_item_target": (C.c_int, [C.c_int]),
     "borb_debug_set_poison": (C.c_int, [C.c_int]),
     "borb_debug_set_fast_mode": (C.c_int, [vp, C.c_int]),
     "borb_debug_brief_slots": (C.c_int, [vp, C.c_int, i32p]),

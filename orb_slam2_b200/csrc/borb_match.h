@@ -230,7 +230,7 @@ struct BowDbJob {
         const uint2* q_meta;      // SearchByBoW(KeyFrame*, KeyFrame*): the query slot's KfStream rows (fv_node / fv_start / desc are
     };                            // its stream's, desc in row order, fv_idx unused)
     const uint8_t* desc;          // n x 32, 16-byte aligned
-    int nn, m, n, item_target;    // item_target: keyframes per work item = item_target / nt^2, clamped to 1..32
+    int nn, m, n;
     uint8_t* frame_block;         // FrameBlockHdr + sections, 128-byte aligned, frame_bytes = frame_block_layout(nn, m, n).bytes
     int frame_bytes, frame_in_smem;
     // the keyframes
@@ -252,7 +252,6 @@ struct BowDbJob {
 struct BowDbArgs {                // the launch sequence of the database search over a job table in device memory
     const BowDbJob* jobs;
     int n_jobs;
-    int static_sched;             // 1: item i of every job -> warp i mod (warps), 0: atomic work counter per job
     float nnratio;
     int check_ori;
 };
@@ -385,7 +384,7 @@ int launch_host_copy(const HostCopies& c, cudaStream_t s);
 // pack + match + finalize over A.jobs (3 launches): one = a host copy of job 0 (what the match kernel reads of a single job),
 // max_smem_frame = largest frame_bytes of the jobs with frame_in_smem, max_items = an upper bound of the work items of all jobs,
 // total_kf = sum of their n_kf; kfkf: the jobs are SearchByBoW(KeyFrame*, KeyFrame*) of a database slot against candidates
-int launch_bowdb(const BowDbArgs& A, const BowDbJob& one, int max_smem_frame, long long max_items, int total_kf, int max_nn, int csa, int n_sm,
+int launch_bowdb(const BowDbArgs& A, const BowDbJob& one, int max_smem_frame, long long max_items, int total_kf, int max_nn, int n_sm,
                  bool kfkf, cudaStream_t s);
 bool bowdb_frame_fits_smem(int frame_bytes);
 // n_jobs database blocks (a job table in device memory) in one launch, a CTA per job

@@ -1,7 +1,6 @@
 // Host side of the matcher / vocabulary entry points of the C ABI (include/borb.h): snapshots arrive as plain host
 // arrays, are staged into one device arena per call, and every result is produced by the CUDA kernels in k_match.cu.
 #include <algorithm>
-#include <atomic>
 #include <cassert>
 #include <climits>
 #include <cmath>
@@ -2182,12 +2181,6 @@ static borb_status kfdb_sync_table(borb_kfdb* db) {
     return BORB_OK;
 }
 
-static std::atomic<int> g_bow_csa{2};
-static std::atomic<int> g_bow_item_target{8192};   // keyframes per work item = target / nt^2 (tuning knob of the measurement scripts)
-static std::atomic<int> g_bow_static{0};
-borb_status borb_debug_set_bow_item_target(int t) { g_bow_static.store(t < 0 ? 1 : 0); if (t < 0) t = -t; g_bow_item_target.store(t < 1 ? 1 : t); return BORB_OK; }
-borb_status borb_debug_set_bow_csa(int mode) { g_bow_csa.store(mode < 0 ? 0 : (mode > 2 ? 2 : mode)); return BORB_OK; }
-
 namespace {
 
 // Every distinct database of a call, locked in address order (two concurrent batches over the same databases cannot deadlock),
@@ -2405,7 +2398,7 @@ borb_status bowdb_jobs(borb_matcher* m, const SearchJob* J, int n_jobs, float nn
                 const KfDev f = p.f.bind(c);
                 D.fv_node = f.node; D.fv_start = f.start; D.fv_idx = f.idx; D.keys = f.keys; D.desc = f.desc;
             }
-            D.nn = p.nn; D.m = p.m; D.n = p.n; D.item_target = g_bow_item_target.load();
+            D.nn = p.nn; D.m = p.m; D.n = p.n;
             D.frame_block = c.dev(p.o_fb); D.frame_bytes = p.h.bytes; D.frame_in_smem = bowdb_frame_fits_smem(p.h.bytes) ? 1 : 0;
             D.table = S.db->d_stream; D.slots = S.slots ? (const int32_t*)c.dev(p.o_sl) : nullptr;
             D.n_kf = S.n_kf; D.kf_base = kf_base; kf_base += S.n_kf;
@@ -2427,11 +2420,10 @@ borb_status bowdb_jobs(borb_matcher* m, const SearchJob* J, int n_jobs, float nn
             if (J[j].frame && (s = c.wait(J[j].frame)) != BORB_OK) return s;
         }
         BowDbArgs A{};
-        A.jobs = (const BowDbJob*)c.dev(o_jobs); A.n_jobs = nw; A.static_sched = g_bow_static.load();
+        A.jobs = (const BowDbJob*)c.dev(o_jobs); A.n_jobs = nw;
         A.nnratio = nnratio; A.check_ori = check_ori;
         if (m->timing) BORB_CUDA(cudaEventRecord(m->t0, m->stream));
-        m->launches += launch_bowdb(A, hj[0], max_smem_frame, max_items, total_kf, max_nn, g_bow_csa.load(), J[work[0]].db->n_sm, kfkf,
-                                   m->stream);
+        m->launches += launch_bowdb(A, hj[0], max_smem_frame, max_items, total_kf, max_nn, J[work[0]].db->n_sm, kfkf, m->stream);
         if (m->timing) BORB_CUDA(cudaEventRecord(m->t1, m->stream));
         for (int j : work)
             if (J[j].dense) BORB_CUDA(cudaMemcpyAsync(J[j].dense, c.dev(P[j].o_dense), (size_t)J[j].n_kf * P[j].n * 4, cudaMemcpyDeviceToHost, m->stream));

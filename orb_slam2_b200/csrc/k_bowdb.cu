@@ -25,7 +25,7 @@
 // (node, frame feature) order — deterministic output.
 //
 // Bound: not HBM (96 MB of keyframe records per 2000-keyframe sweep) but the integer pipes and the per-item / per-batch
-// bookkeeping around the column loop (ham256<MODE>: 8 POPC, 4 POPC + carry-save tree, or 5 POPC + three 3:2 compressors).
+// bookkeeping around the column loop (ham256: 5 POPC + three 3:2 compressors per distance).
 #include "borb_match.h"
 #include "match_rules.cuh"
 
@@ -41,25 +41,16 @@ constexpr int BDB_WARP_BYTES = BDB_CLAIM_WORDS * 4 + 32 * 24 + BDB_QCAP * 48;   
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// 256-bit Hamming distance.  MODE 0: 8 POPC (descriptor_distance).  MODE 1: full carry-save adder tree, 4 POPC + 17 LOP3.  MODE 2
-// (default): three 3:2 compressors, 5 POPC + 6 LOP3.  POPC issues at a quarter of LOP3's rate (16 vs 64 results per clock per SM on
-// sm_90, CUDA C++ Programming Guide throughput table): per distance MODE 0 is all POPC, MODE 1 shifts most of the work to LOP3,
-// MODE 2 balances the two.
-template <int MODE>
+// 256-bit Hamming distance: three 3:2 compressors, 5 POPC + 6 LOP3.  POPC issues at a quarter of LOP3's rate (16 vs 64 results
+// per clock per SM on sm_90, CUDA C++ Programming Guide throughput table), so this balances the two pipes where 8 POPC
+// (descriptor_distance) is all POPC and a full carry-save adder tree (4 POPC + 17 LOP3) shifts most of the work to LOP3.
 __device__ __forceinline__ int ham256(const uint4 a0, const uint4 a1, const uint4 b0, const uint4 b1) {
-    if (MODE == 0) return descriptor_distance(a0, a1, b0, b1);
     const uint32_t x0 = a0.x ^ b0.x, x1 = a0.y ^ b0.y, x2 = a0.z ^ b0.z, x3 = a0.w ^ b0.w;
     const uint32_t x4 = a1.x ^ b1.x, x5 = a1.y ^ b1.y, x6 = a1.z ^ b1.z, x7 = a1.w ^ b1.w;
     const uint32_t s1 = x0 ^ x1 ^ x2, c1 = (x0 & x1) | (x2 & (x0 ^ x1));
     const uint32_t s2 = x3 ^ x4 ^ x5, c2 = (x3 & x4) | (x5 & (x3 ^ x4));
     const uint32_t s3 = s1 ^ s2 ^ x6, c3 = (s1 & s2) | (x6 & (s1 ^ s2));
-    if (MODE == 2) return (__popc(s3) + __popc(x7)) + 2 * (__popc(c1) + __popc(c2) + __popc(c3));
-    // full tree: 8 words -> bit planes of weight 1, 2, 4, 8
-    const uint32_t ones = s3 ^ x7, c4 = s3 & x7;
-    const uint32_t s5 = c1 ^ c2 ^ c3, c5 = (c1 & c2) | (c3 & (c1 ^ c2));
-    const uint32_t twos = s5 ^ c4, c6 = s5 & c4;
-    const uint32_t fours = c5 ^ c6, eights = c5 & c6;
-    return __popc(ones) + 2 * __popc(twos) + 4 * __popc(fours) + 8 * __popc(eights);
+    return (__popc(s3) + __popc(x7)) + 2 * (__popc(c1) + __popc(c2) + __popc(c3));
 }
 
 }  // namespace
@@ -68,9 +59,9 @@ struct KfRun { const uint2* meta; const uint4* desc; int rs, off; };     // rows
 
 // The items of one job, taken by this CTA's warps until the job's work counter is exhausted.  fb: the job's frame block, in
 // shared memory (FSM) or in global memory; ws: the warp's scratch.
-template <int CSA, bool FSM>
+template <bool FSM>
 __device__ __forceinline__ void bowdb_job_items(const BowDbArgs& A, const BowDbJob& J, const uint8_t* fb, uint8_t* ws) {
-    const int lane = threadIdx.x & 31, wrp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
     const unsigned lt_mask = (1u << lane) - 1u;
     const FrameBlockHdr* H = reinterpret_cast<const FrameBlockHdr*>(fb);
     const int mf = H->m, np = H->np;
@@ -90,15 +81,10 @@ __device__ __forceinline__ void bowdb_job_items(const BowDbArgs& A, const BowDbJ
     int4* qm = reinterpret_cast<int4*>(qd1 + BDB_QCAP);
 
     const int items = pstart[np];
-    const int warps_total = gridDim.x * (blockDim.x >> 5);
-    int it_static = blockIdx.x + gridDim.x * wrp;                 // static schedule: consecutive (similar-cost) items go to different SMs
     while (true) {
         int it = 0;
-        if (A.static_sched) { it = it_static; it_static += warps_total; }
-        else {
-            if (lane == 0) it = atomicAdd(J.ctr, 1);
-            it = __shfl_sync(0xFFFFFFFFu, it, 0);
-        }
+        if (lane == 0) it = atomicAdd(J.ctr, 1);
+        it = __shfl_sync(0xFFFFFFFFu, it, 0);
         if (it >= items) break;
         int lo = 0, hi = np;                                      // largest p with pstart[p] <= it
         while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (pstart[mid] <= it) lo = mid; else hi = mid; }
@@ -156,7 +142,7 @@ __device__ __forceinline__ void bowdb_job_items(const BowDbArgs& A, const BowDbJ
                 unsigned k1v = 0xFFFFFFFFu, k2v = 0xFFFFFFFFu;
 #pragma unroll 2
                 for (int c = 0; c < nt; c++) {
-                    const int d = ham256<CSA>(q0, q1, fd[2 * c], fd[2 * c + 1]);
+                    const int d = ham256(q0, q1, fd[2 * c], fd[2 * c + 1]);
                     const unsigned key = ((unsigned)d << 16) | (unsigned)c;
                     k2v = min(k2v, max(k1v, key));                 // second smallest so far (k1v <= k2v always)
                     k1v = min(k1v, key);
@@ -183,7 +169,7 @@ __device__ __forceinline__ void bowdb_job_items(const BowDbArgs& A, const BowDbJ
                         unsigned m1 = 0xFFFFFFFFu, m2 = 0xFFFFFFFFu;
                         for (int col = lane; col < nt; col += 32) {
                             if (is_claimed((unsigned)col)) continue;
-                            const int d = ham256<CSA>(r0v, r1v, fd[2 * col], fd[2 * col + 1]);
+                            const int d = ham256(r0v, r1v, fd[2 * col], fd[2 * col + 1]);
                             const unsigned key = ((unsigned)d << 16) | (unsigned)col;
                             if (key < m1) { m2 = m1; m1 = key; } else if (key < m2) m2 = key;
                         }
@@ -258,7 +244,7 @@ __device__ __forceinline__ void bowdb_job_items(const BowDbArgs& A, const BowDbJ
 // candidate feature | bin << 16, the bin of query angle - candidate angle (:607), so the relocalisation finalize culls and compacts it.
 template <bool FSM>
 __device__ __forceinline__ void bowkf_job_items(const BowDbArgs& A, const BowDbJob& J, const uint8_t* fb, uint8_t* ws) {
-    const int lane = threadIdx.x & 31, wrp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
     const FrameBlockHdr* H = reinterpret_cast<const FrameBlockHdr*>(fb);
     const int mf = H->m, np = H->np;
     const uint32_t* fnode = reinterpret_cast<const uint32_t*>(fb + H->off_node);
@@ -272,15 +258,10 @@ __device__ __forceinline__ void bowkf_job_items(const BowDbArgs& A, const BowDbJ
     uint32_t* claim = reinterpret_cast<uint32_t*>(ws);            // claimed columns when the bucket is wider than 32
 
     const int items = pstart[np];
-    const int warps_total = gridDim.x * (blockDim.x >> 5);
-    int it_static = blockIdx.x + gridDim.x * wrp;
     while (true) {
         int it = 0;
-        if (A.static_sched) { it = it_static; it_static += warps_total; }
-        else {
-            if (lane == 0) it = atomicAdd(J.ctr, 1);
-            it = __shfl_sync(0xFFFFFFFFu, it, 0);
-        }
+        if (lane == 0) it = atomicAdd(J.ctr, 1);
+        it = __shfl_sync(0xFFFFFFFFu, it, 0);
         if (it >= items) break;
         int lo = 0, hi = np;                                      // largest p with pstart[p] <= it
         while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (pstart[mid] <= it) lo = mid; else hi = mid; }
@@ -330,7 +311,7 @@ __device__ __forceinline__ void bowkf_job_items(const BowDbArgs& A, const BowDbJ
                 unsigned k1v = 0xFFFFFFFFu, k2v = 0xFFFFFFFFu;
                 for (int c = 0; c < nc; c++) {
                     if (!good(c)) continue;                                        // warp-uniform
-                    const int d = ham256<2>(q0, q1, cd[2 * c], cd[2 * c + 1]);
+                    const int d = ham256(q0, q1, cd[2 * c], cd[2 * c + 1]);
                     const unsigned key = ((unsigned)d << 16) | (unsigned)c;
                     k2v = min(k2v, max(k1v, key));
                     k1v = min(k1v, key);
@@ -350,7 +331,7 @@ __device__ __forceinline__ void bowkf_job_items(const BowDbArgs& A, const BowDbJ
                         unsigned m1 = 0xFFFFFFFFu, m2 = 0xFFFFFFFFu;
                         for (int col = lane; col < nc; col += 32) {
                             if (is_claimed((unsigned)col) || !good(col)) continue;
-                            const int d = ham256<2>(r0v, r1v, cd[2 * col], cd[2 * col + 1]);
+                            const int d = ham256(r0v, r1v, cd[2 * col], cd[2 * col + 1]);
                             const unsigned key = ((unsigned)d << 16) | (unsigned)col;
                             if (key < m1) { m2 = m1; m1 = key; } else if (key < m2) m2 = key;
                         }
@@ -388,19 +369,19 @@ __device__ __forceinline__ void bowkf_job_items(const BowDbArgs& A, const BowDbJ
 // that do not fit next to the warp scratch are read through L1 from global memory (FSM = false), in the same launch.
 // KFKF selects the items of SearchByBoW(KeyFrame*, KeyFrame*) (bowkf_job_items) instead of those of (KeyFrame*, Frame&).
 enum { ONE_SMEM = 0, ONE_GLOBAL = 1, TABLE = 2 };
-template <int CSA, bool FSM, bool KFKF>
+template <bool FSM, bool KFKF>
 __device__ __forceinline__ void job_items(const BowDbArgs& A, const BowDbJob& J, const uint8_t* fb, uint8_t* ws) {
     if constexpr (KFKF) bowkf_job_items<FSM>(A, J, fb, ws);
-    else bowdb_job_items<CSA, FSM>(A, J, fb, ws);
+    else bowdb_job_items<FSM>(A, J, fb, ws);
 }
-template <int CSA, int KIND, bool KFKF>
+template <int KIND, bool KFKF>
 __device__ __forceinline__ void bowdb_match(const BowDbArgs& A, int smem_frame, const BowDbJob& J0) {
     extern __shared__ __align__(128) uint8_t sm[];
     __shared__ __align__(8) unsigned long long bar;
     __shared__ BowDbJob sJ;
     __shared__ int s_job, s_next, s_left, s_loads;     // the job cursor (the next job to look at, jobs not looked at) and the block loads so far
     const int tid = threadIdx.x;
-    if (KIND == ONE_GLOBAL) { job_items<CSA, false, KFKF>(A, J0, J0.frame_block, sm + (size_t)(tid >> 5) * BDB_WARP_BYTES); return; }
+    if (KIND == ONE_GLOBAL) { job_items<false, KFKF>(A, J0, J0.frame_block, sm + (size_t)(tid >> 5) * BDB_WARP_BYTES); return; }
     if (KIND == ONE_SMEM) {
         if (tid == 0) {
             asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(&bar)));
@@ -421,20 +402,20 @@ __device__ __forceinline__ void bowdb_match(const BowDbArgs& A, int smem_frame, 
             "BOWDB_DONE1:\n"
             "}\n" ::"r"(smem_u32(&bar))
             : "memory");
-        job_items<CSA, true, KFKF>(A, J0, sm, sm + (((size_t)smem_frame + 127) & ~size_t(127)) + (size_t)(tid >> 5) * BDB_WARP_BYTES);
+        job_items<true, KFKF>(A, J0, sm, sm + (((size_t)smem_frame + 127) & ~size_t(127)) + (size_t)(tid >> 5) * BDB_WARP_BYTES);
         return;
     }
     if (tid == 0) {
         asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(&bar)));
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        s_next = A.static_sched ? 0 : (int)((long long)blockIdx.x * A.n_jobs / gridDim.x); s_left = A.n_jobs; s_loads = 0;
+        s_next = (int)((long long)blockIdx.x * A.n_jobs / gridDim.x); s_left = A.n_jobs; s_loads = 0;
     }
     while (true) {
         if (tid == 0) {
             int pick = -1, next = s_next, left = s_left;
             for (; left > 0 && pick < 0; left--) {
                 const int* c = A.jobs[next].ctr;
-                if (A.static_sched || *(volatile const int*)c < *(volatile const int*)(c + 1)) pick = next;
+                if (*(volatile const int*)c < *(volatile const int*)(c + 1)) pick = next;
                 next = next + 1 == A.n_jobs ? 0 : next + 1;
             }
             s_next = next; s_left = left; s_job = pick;
@@ -461,22 +442,21 @@ __device__ __forceinline__ void bowdb_match(const BowDbArgs& A, int smem_frame, 
                 "BOWDB_DONE:\n"
                 "}\n" ::"r"(smem_u32(&bar)), "r"((uint32_t)s_loads & 1u)
                 : "memory");
-            job_items<CSA, true, KFKF>(A, sJ, sm, ws);
+            job_items<true, KFKF>(A, sJ, sm, ws);
         } else {
-            job_items<CSA, false, KFKF>(A, sJ, sJ.frame_block, ws);
+            job_items<false, KFKF>(A, sJ, sJ.frame_block, ws);
         }
         __syncthreads();                                          // every warp is done with this job's block
         if (tid == 0 && sJ.frame_in_smem) s_loads++;
     }
 }
-template <int CSA, int KIND>
+template <int KIND>
 __global__ void __launch_bounds__(32 * BDB_WARPS, BDB_CTAS) bowdb_match_kernel(BowDbArgs A, int smem_frame, const __grid_constant__ BowDbJob J0) {
-    bowdb_match<CSA, KIND, false>(A, smem_frame, J0);
+    bowdb_match<KIND, false>(A, smem_frame, J0);
 }
-// One distance arithmetic (MODE 2, the default) only: borb_debug_set_bow_csa applies to bowdb_match_kernel.
 template <int KIND>
 __global__ void __launch_bounds__(32 * BDB_WARPS, BDB_CTAS) bowkf_match_kernel(BowDbArgs A, int smem_frame, const __grid_constant__ BowDbJob J0) {
-    bowdb_match<2, KIND, true>(A, smem_frame, J0);
+    bowdb_match<KIND, true>(A, smem_frame, J0);
 }
 
 // Rotation-consistency cull and compaction, a 128-thread CTA per keyframe.  table_out row: one u32 per frame position
@@ -579,13 +559,14 @@ bool bowdb_frame_fits_smem(int frame_bytes) { return bowdb_warps(frame_bytes, tr
 
 // The query frame's block (FrameBlockHdr + sections), one CTA per job: the FeatureVector's node and start arrays; orig, angle and
 // desc of every feature inside a node in FeatureVector order; and the work list - the non-empty nodes stable-sorted widest first
-// (the long items start first), keyframes per item cs = clamp(item_target / nt^2, 1, 32) so that an item is a few hundred
+// (the long items start first), keyframes per item cs = clamp(BDB_ITEM_TARGET / nt^2, 1, 32) so that an item is a few hundred
 // column-loop iterations whatever the bucket width (a keyframe's bucket of the node is about as full as the frame's), and the
 // item prefix pstart.  Also resets the job's work counter and pair cursor and stores its item count next to them.
 // Shared memory: 8 B per sort key (next power of two >= nn, at least 32).
 // KFKF: the query is a database slot; its stream rows are already in FeatureVector order, with the feature index and angle in
 // q_meta, so row r is copied as it is.
 constexpr int PACK_THREADS = 512;
+constexpr int BDB_ITEM_TARGET = 8192;
 template <bool KFKF>
 __device__ __forceinline__ void bowdb_pack(const BowDbJob* __restrict__ jobs) {
     extern __shared__ __align__(16) uint64_t pk_sm[];
@@ -640,7 +621,7 @@ __device__ __forceinline__ void bowdb_pack(const BowDbJob* __restrict__ jobs) {
     for (int p = c0; p < c1; p++) {
         const int a = (int)(uint32_t)keys[p];
         const long long nt = J.fv_start[a + 1] - J.fv_start[a];
-        long long cs = J.item_target / (nt * nt);
+        long long cs = BDB_ITEM_TARGET / (nt * nt);
         cs = cs < 1 ? 1 : (cs > 32 ? 32 : cs);                            // one 32-lane batch of keyframes per item at most
         pnode[p] = a; pcs[p] = (int32_t)cs;
         items += (int)((J.n_kf + cs - 1) / cs);
@@ -662,7 +643,7 @@ __device__ __forceinline__ void bowdb_pack(const BowDbJob* __restrict__ jobs) {
 __global__ void __launch_bounds__(PACK_THREADS) bowdb_pack_kernel(const BowDbJob* __restrict__ jobs) { bowdb_pack<false>(jobs); }
 __global__ void __launch_bounds__(PACK_THREADS) bowkf_pack_kernel(const BowDbJob* __restrict__ jobs) { bowdb_pack<true>(jobs); }
 
-int launch_bowdb(const BowDbArgs& A, const BowDbJob& one, int max_smem_frame, long long max_items, int total_kf, int max_nn, int csa, int n_sm,
+int launch_bowdb(const BowDbArgs& A, const BowDbJob& one, int max_smem_frame, long long max_items, int total_kf, int max_nn, int n_sm,
                  bool kfkf, cudaStream_t s) {
     int K = 32;
     while (K < max_nn) K <<= 1;
@@ -679,17 +660,7 @@ int launch_bowdb(const BowDbArgs& A, const BowDbJob& one, int max_smem_frame, lo
     const int kind = A.n_jobs > 1 ? TABLE : (one.frame_in_smem ? ONE_SMEM : ONE_GLOBAL);
     void (*kern)(BowDbArgs, int, BowDbJob) = nullptr;
     if (kfkf) kern = kind == TABLE ? bowkf_match_kernel<TABLE> : (kind == ONE_SMEM ? bowkf_match_kernel<ONE_SMEM> : bowkf_match_kernel<ONE_GLOBAL>);
-    else switch (csa * 3 + kind) {
-        case 0: kern = bowdb_match_kernel<0, ONE_SMEM>; break;
-        case 1: kern = bowdb_match_kernel<0, ONE_GLOBAL>; break;
-        case 2: kern = bowdb_match_kernel<0, TABLE>; break;
-        case 3: kern = bowdb_match_kernel<1, ONE_SMEM>; break;
-        case 4: kern = bowdb_match_kernel<1, ONE_GLOBAL>; break;
-        case 5: kern = bowdb_match_kernel<1, TABLE>; break;
-        case 6: kern = bowdb_match_kernel<2, ONE_SMEM>; break;
-        case 7: kern = bowdb_match_kernel<2, ONE_GLOBAL>; break;
-        default: kern = bowdb_match_kernel<2, TABLE>; break;
-    }
+    else kern = kind == TABLE ? bowdb_match_kernel<TABLE> : (kind == ONE_SMEM ? bowdb_match_kernel<ONE_SMEM> : bowdb_match_kernel<ONE_GLOBAL>);
     allow_max_smem((const void*)kern);
     kern<<<(int)ctas, 32 * warps, smem, s>>>(A, fsm ? max_smem_frame : 0, one);
     bowdb_finalize_kernel<<<total_kf, FIN_THREADS, 0, s>>>(A);

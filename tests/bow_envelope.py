@@ -35,6 +35,7 @@ BDB_QCAP = 64                      # k_bowdb.cu:38 — pending-row ring per warp
 BDB_CLAIM_WORDS = MATCH_MAX_FEATURES // 32
 BDB_WARP_BYTES = BDB_CLAIM_WORDS * 4 + 32 * 24 + BDB_QCAP * 48     # k_bowdb.cu:40
 BDB_SMEM_BUDGET = 226 * 1024       # k_bowdb.cu:423
+BDB_ITEM_TARGET = 8192             # k_bowdb.cu:569 — keyframes per work item = clamp(BDB_ITEM_TARGET / nt^2, 1, 32)
 FIN_THREADS, FIN_REG = 128, 16     # k_bowdb.cu:337-338 — a row stays in registers up to FIN_THREADS * FIN_REG positions
 TH_LOW = 50                        # ORBmatcher.cc:15
 HISTO_LENGTH = 30

@@ -586,7 +586,5 @@ NOT_COVERED = {
     "borb_debug_set_fast_mode": "ablation switch of fast_kernel; only mode 0 produces keypoints",
     "borb_debug_brief_slots": "host table, no device memory",
     "borb_debug_eval_math": "allocates fresh buffers per call and writes every output element (tests/test_gpu_device_math.py)",
-    "borb_debug_set_bow_csa": "configuration switch of the database search; same results in every mode",
-    "borb_debug_set_bow_item_target": "configuration switch of the database search; same results for every target",
     "borb_debug_set_poison": "the switch itself (tests/test_poison_catalogue.py checks its arguments)",
 }

@@ -1,14 +1,12 @@
 """GPU: the place-recognition envelope (tests/bow_envelope.py) through the CUDA library, bit for bit against the port:
 borb_bow_transform, borb_compute_bow and borb_frames_compute_bow on every vocabulary shape (text loader and array upload);
 borb_kfdb_query and _batch on every query size; borb_search_by_bow_db, _pairs and _batch on every search case and on batches of
-2 * n_SM + 1 small jobs and of mixed shared / global frame blocks with empty jobs — each database search under the three Hamming
-modes and four scheduling settings (item targets 1, 8192 and 2^20, and the static schedule)."""
+2 * n_SM + 1 small jobs and of mixed shared / global frame blocks with empty jobs."""
 import functools
 
 import numpy as np
 import pytest
 
-from orb_slam2_b200 import _lib
 from orb_slam2_b200 import matcher as M
 from orb_slam2_b200._lib import BorbError
 from tests import bow_envelope as BE
@@ -16,9 +14,6 @@ from tests import bow_envelope as BE
 pytestmark = pytest.mark.gpu
 
 SCALE = (1.2 ** np.arange(8)).astype(np.float32)
-CSA_MODES = [0, 1, 2]
-ITEM_TARGETS = [1, 8192, 2 ** 20, -8192]          # negative: the static schedule with target 8192
-DEFAULT_CSA, DEFAULT_TARGET = 2, 8192             # borb_match_host.cu:1652-1653
 
 
 @pytest.fixture(scope="module")
@@ -30,20 +25,6 @@ def mt():
 def n_sm():
     import torch
     return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def knobs():
-    """Every (Hamming mode, item target) setting; both knobs are restored when the generator is closed."""
-    lib = _lib.load()
-    try:
-        for csa in CSA_MODES:
-            for tgt in ITEM_TARGETS:
-                _lib.check(lib.borb_debug_set_bow_csa(csa), "set_bow_csa")
-                _lib.check(lib.borb_debug_set_bow_item_target(tgt), "set_bow_item_target")
-                yield csa, tgt
-    finally:
-        lib.borb_debug_set_bow_csa(DEFAULT_CSA)
-        lib.borb_debug_set_bow_item_target(DEFAULT_TARGET)
 
 
 @pytest.fixture(scope="module")
@@ -177,7 +158,7 @@ def _db_of(mt, kfs):
 
 
 @pytest.mark.parametrize("name", BE.SEARCH_NAMES)
-def test_database_search_equals_port_in_every_mode(oracle, mt, name):
+def test_database_search_equals_port(oracle, mt, name):
     c = BE.search_case(name)
     port = _port_search(name)
     want_nm = np.array([n for n, _ in port], np.int32)
@@ -185,11 +166,10 @@ def test_database_search_equals_port_in_every_mode(oracle, mt, name):
     n_f = len(c["F"].mvKeysUn)
     db = _db_of(mt, c["kfs"])
     slots = np.arange(len(c["kfs"]), dtype=np.int32)
-    for csa, tgt in knobs():
-        nm, dn = db.SearchByBoW(slots, c["F"])
-        assert np.array_equal(nm, want_nm) and np.array_equal(dn, want), (csa, tgt)
-        nm, off, pairs = db.SearchByBoWPairs(None, c["F"])
-        assert np.array_equal(nm, want_nm) and np.array_equal(BE.dense_from_pairs(nm, off, pairs, n_f), want), (csa, tgt)
+    nm, dn = db.SearchByBoW(slots, c["F"])
+    assert np.array_equal(nm, want_nm) and np.array_equal(dn, want)
+    nm, off, pairs = db.SearchByBoWPairs(None, c["F"])
+    assert np.array_equal(nm, want_nm) and np.array_equal(BE.dense_from_pairs(nm, off, pairs, n_f), want)
     assert want_nm.sum() > 0
 
 
@@ -254,17 +234,15 @@ def test_table_batch_of_2_nsm_plus_1_small_jobs(mt, batch_world):
     W = batch_world
     n = 2 * W["n_sm"] + 1
     jobs = [(j % 12, [j % 12, (j + 1) % 12, (j + 5) % 12][: 1 + j % 3]) for j in range(n)]
-    for csa, tgt in knobs():
-        got = mt.SearchByBoWDbBatch(W["db"], [sl for _, sl in jobs], [W["frames"][f] for f, _ in jobs])
-        _check_jobs(W, jobs, got, (csa, tgt))
+    got = mt.SearchByBoWDbBatch(W["db"], [sl for _, sl in jobs], [W["frames"][f] for f, _ in jobs])
+    _check_jobs(W, jobs, got, "table")
 
 
 def test_mixed_batch_with_empty_jobs(mt, batch_world):
     """Shared-memory and global frame blocks in one launch, with n_kf == 0 jobs in the middle and at the end."""
     W = batch_world
     jobs = [(0, [0, 3, 12]), (12, [12, 0, 1, 12]), (5, []), (1, [1]), (12, [4, 12]), (7, list(range(13))), (2, [])]
-    for csa, tgt in knobs():
-        got = mt.SearchByBoWDbBatch(W["db"], [sl for _, sl in jobs], [W["frames"][f] for f, _ in jobs])
-        _check_jobs(W, jobs, got, (csa, tgt))
-        assert len(got[2][0]) == 0 and len(got[6][0]) == 0
+    got = mt.SearchByBoWDbBatch(W["db"], [sl for _, sl in jobs], [W["frames"][f] for f, _ in jobs])
+    _check_jobs(W, jobs, got, "mixed")
+    assert len(got[2][0]) == 0 and len(got[6][0]) == 0
     assert W["port"][12, 12][0] > 100

@@ -137,53 +137,48 @@ def _pairs_to_dense(nm, off, pairs, n_f):
 
 
 @pytest.mark.parametrize("levelsup", [1, 2, 3, 4])
-@pytest.mark.parametrize("csa", [2, 1, 0])
-def test_search_by_bow_pairs_all_bucket_shapes(oracle, levelsup, csa):
+def test_search_by_bow_pairs_all_bucket_shapes(oracle, levelsup):
     """The compact database search against the restated SearchByBoW for every bucket geometry of the kernel: levelsup 1 = ~1000
     single-feature nodes, 2 = ~100 nodes of ~8, 3 = 10 nodes of ~80 (multi-tile matrix), 4 = one node with every feature
-    (direct evaluation); with and without the orientation cull; the three distance-arithmetic modes (5-POPC hybrid, full carry-save tree, plain POPC)."""
-    from orb_slam2_b200 import _lib, matcher as M
+    (direct evaluation); with and without the orientation cull."""
+    from orb_slam2_b200 import matcher as M
     from orb_slam2_b200.extractor import ORBextractor
-    _lib.check(_lib.load().borb_debug_set_bow_csa(csa), "set_bow_csa")
-    try:
-        pv = oracle.PortVocabulary.random(10, 4, 5)
-        e = pv.export()
-        voc = M.ORBVocabulary.from_arrays(e["parent"], e["is_leaf"], e["desc"], e["weight"], e["k"], e["L"])
-        X = ORBextractor(800)
-        rng = np.random.default_rng(17 + levelsup)
-        base = [synth.mono_frame(300 + i // 3, 0, 0, 640, 480) for i in range(9)]
-        imgs = [np.clip(b.astype(np.int32) + rng.integers(-6, 7, b.shape), 0, 255).astype(np.uint8) for b in base]
-        outs = X.extract_batch(imgs)
-        kfs, bows = [], []
-        for k, d in outs:
-            bow, fv = voc.transform(d, levelsup)
-            kfs.append(M.KeyFrameView(mvKeysUn=k, mDescriptors=d, mFeatVec=fv, has_mp=(rng.random(len(k)) < 0.6).astype(np.uint8)))
-            bows.append(bow)
-        qk, qd = X(np.clip(base[4].astype(np.int32) + rng.integers(-8, 9, base[4].shape), 0, 255).astype(np.uint8))
-        qbow, qfv = voc.transform(qd, levelsup)
-        F = M.KeyFrameView(mvKeysUn=qk, mDescriptors=qd, mFeatVec=qfv)
-        for ori in (True, False):
-            mt = M.ORBmatcher(0.75, ori)
-            db = M.KeyFrameDatabase(mt)
-            for kf, bow in zip(kfs, bows):
-                db.add(kf, bow)
-            nm, off, pairs = db.SearchByBoWPairs(None, F)
-            dense = _pairs_to_dense(nm, off, pairs, len(qk))
-            nm_d, dense_d = db.SearchByBoW(np.arange(len(kfs), dtype=np.int32), F)
-            assert np.array_equal(nm, nm_d) and np.array_equal(dense, dense_d)
-            for s in range(len(kfs)):
-                n_o, m_o = oracle.port_search_by_bow(kfs[s], F, 0.75, ori)
-                assert nm[s] == n_o and np.array_equal(dense[s], m_o), (levelsup, ori, s)
-            assert nm.max() > 10
-            # counts only, a slot subset with a repeat, and an erased slot
-            nm2, _, none = db.SearchByBoWPairs([3, 4, 4, 0], F, want_pairs=False)
-            assert none is None and np.array_equal(nm2, nm[[3, 4, 4, 0]])
-            db.erase(2)
-            nm3, off3, pairs3 = db.SearchByBoWPairs(None, F)
-            assert nm3[2] == 0 and np.array_equal(np.delete(nm3, 2), np.delete(nm, 2))
-            assert np.array_equal(_pairs_to_dense(nm3, off3, pairs3, len(qk))[[0, 1, 3, 8]], dense[[0, 1, 3, 8]])
-    finally:
-        _lib.check(_lib.load().borb_debug_set_bow_csa(2), "set_bow_csa")
+    pv = oracle.PortVocabulary.random(10, 4, 5)
+    e = pv.export()
+    voc = M.ORBVocabulary.from_arrays(e["parent"], e["is_leaf"], e["desc"], e["weight"], e["k"], e["L"])
+    X = ORBextractor(800)
+    rng = np.random.default_rng(17 + levelsup)
+    base = [synth.mono_frame(300 + i // 3, 0, 0, 640, 480) for i in range(9)]
+    imgs = [np.clip(b.astype(np.int32) + rng.integers(-6, 7, b.shape), 0, 255).astype(np.uint8) for b in base]
+    outs = X.extract_batch(imgs)
+    kfs, bows = [], []
+    for k, d in outs:
+        bow, fv = voc.transform(d, levelsup)
+        kfs.append(M.KeyFrameView(mvKeysUn=k, mDescriptors=d, mFeatVec=fv, has_mp=(rng.random(len(k)) < 0.6).astype(np.uint8)))
+        bows.append(bow)
+    qk, qd = X(np.clip(base[4].astype(np.int32) + rng.integers(-8, 9, base[4].shape), 0, 255).astype(np.uint8))
+    qbow, qfv = voc.transform(qd, levelsup)
+    F = M.KeyFrameView(mvKeysUn=qk, mDescriptors=qd, mFeatVec=qfv)
+    for ori in (True, False):
+        mt = M.ORBmatcher(0.75, ori)
+        db = M.KeyFrameDatabase(mt)
+        for kf, bow in zip(kfs, bows):
+            db.add(kf, bow)
+        nm, off, pairs = db.SearchByBoWPairs(None, F)
+        dense = _pairs_to_dense(nm, off, pairs, len(qk))
+        nm_d, dense_d = db.SearchByBoW(np.arange(len(kfs), dtype=np.int32), F)
+        assert np.array_equal(nm, nm_d) and np.array_equal(dense, dense_d)
+        for s in range(len(kfs)):
+            n_o, m_o = oracle.port_search_by_bow(kfs[s], F, 0.75, ori)
+            assert nm[s] == n_o and np.array_equal(dense[s], m_o), (levelsup, ori, s)
+        assert nm.max() > 10
+        # counts only, a slot subset with a repeat, and an erased slot
+        nm2, _, none = db.SearchByBoWPairs([3, 4, 4, 0], F, want_pairs=False)
+        assert none is None and np.array_equal(nm2, nm[[3, 4, 4, 0]])
+        db.erase(2)
+        nm3, off3, pairs3 = db.SearchByBoWPairs(None, F)
+        assert nm3[2] == 0 and np.array_equal(np.delete(nm3, 2), np.delete(nm, 2))
+        assert np.array_equal(_pairs_to_dense(nm3, off3, pairs3, len(qk))[[0, 1, 3, 8]], dense[[0, 1, 3, 8]])
 
 
 def test_config4_real_size_2000_keyframes(oracle):

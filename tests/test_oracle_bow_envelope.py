@@ -128,6 +128,13 @@ def test_database_search_equals_reference(O, name):
     _hits.setdefault("search", set()).update(BE.search_coverage(c, port, port_all))
 
 
+def test_search_cases_reach_both_item_size_clamps():
+    """The frames' node widths nt give work items of one keyframe, of 32 keyframes, and of sizes in between."""
+    nt = np.concatenate([np.diff(BE.search_case(name)["F"].mFeatVec.start) for name in BE.SEARCH_NAMES]).astype(np.int64)
+    cs = np.clip(BE.BDB_ITEM_TARGET // nt[nt > 0] ** 2, 1, 32)
+    assert (cs == 1).any() and (cs == 32).any() and ((cs > 1) & (cs < 32)).any(), sorted(set(cs.tolist()))
+
+
 def test_coverage_reaches_every_class():
     """Runs after the case tests of this module: every class of BE.CLASSES is reached by some case."""
     got = set().union(*_hits.values()) if _hits else set()

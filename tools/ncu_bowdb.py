@@ -33,25 +33,10 @@ db.query(qbow)
 nm, off, pairs = db.SearchByBoWPairs(None, F)
 cap = int(nm.sum()) + 1024
 so = _lib.load()
-res = {}
-for csa in (2, 1, 0):
-    so.borb_debug_set_bow_csa(csa)
-    so.borb_matcher_set_timing(mt._h, 1)
-    ts = []
-    for _ in range(reps):
-        db.SearchByBoWPairs(None, F, pairs_cap=cap)
-        f = C.c_float(0); so.borb_matcher_last_kernel_ms(mt._h, C.byref(f)); ts.append(round(f.value, 5))
-    so.borb_matcher_set_timing(mt._h, 0)
-    res[{2: "hybrid5", 1: "csa4", 0: "popc8"}[csa]] = ts
-so.borb_debug_set_bow_csa(2)
-for tgt in (640, 1280, 2560, 5120, 10240, 40960, -1280, -2560, -5120, -10240):
-    so.borb_debug_set_bow_item_target(tgt)
-    so.borb_matcher_set_timing(mt._h, 1)
-    ts = []
-    for _ in range(reps):
-        db.SearchByBoWPairs(None, F, pairs_cap=cap)
-        f = C.c_float(0); so.borb_matcher_last_kernel_ms(mt._h, C.byref(f)); ts.append(round(f.value, 5))
-    so.borb_matcher_set_timing(mt._h, 0)
-    res[f"target{tgt}"] = ts[1:]
-so.borb_debug_set_bow_item_target(2560)
-print(json.dumps({"pairs": int(nm.sum()), "kernel_ms": res}))
+so.borb_matcher_set_timing(mt._h, 1)
+ts = []
+for _ in range(reps):
+    db.SearchByBoWPairs(None, F, pairs_cap=cap)
+    f = C.c_float(0); so.borb_matcher_last_kernel_ms(mt._h, C.byref(f)); ts.append(round(f.value, 5))
+so.borb_matcher_set_timing(mt._h, 0)
+print(json.dumps({"pairs": int(nm.sum()), "kernel_ms": ts}))
